@@ -571,6 +571,18 @@ YAMS_B200_API yams_status_t yams_b200_debug_stage1_scores(yams_b200_corpus* c, c
                                                           int engine, uint64_t row_start, uint64_t row_stride,
                                                           uint64_t nrows, float* out);
 
+/* diagnostics: the same rows and engines in FILTER mode, the candidate lists of the search's corpus pass.  Row i is
+ * listed for query q when its stage-1 score is > tau[q] (and, with allowed lists in the format of yams_b200_search, the row
+ * is in query q's set).  out_counts[q] = rows that passed (NOT capped at cap); out_cands[q * cap + j], j < min(count, cap),
+ * = (float score, uint32 row index) pairs, 8 bytes each, in no particular order (HOST). YAMS_ERR_UNSUPPORTED when the
+ * engine cannot take the shape. */
+YAMS_B200_API yams_status_t yams_b200_debug_stage1_candidates(yams_b200_corpus* c, const float* queries, uint32_t nq,
+                                                              int engine, uint64_t row_start, uint64_t row_stride,
+                                                              uint64_t nrows, const float* tau, uint32_t cap,
+                                                              const int64_t* allowed_rowids,
+                                                              const uint64_t* allowed_offsets, uint32_t* out_counts,
+                                                              void* out_cands);
+
 /* diagnostics: the per-query stage-1 error bound eps[q] of the last search / debug_stage1_scores call (HOST out) */
 YAMS_B200_API yams_status_t yams_b200_debug_last_eps(yams_b200_corpus* c, uint32_t nq, float* out);
 

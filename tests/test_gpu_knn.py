@@ -240,30 +240,6 @@ def test_partial_topk_merge_like_allgather(Y, oracle):
         c.close()
 
 
-@pytest.mark.parametrize("shape", [(1000, 128, 16), (5000, 768, 300), (777, 72, 5), (40000, 64, 257)])
-def test_tcgen05_engine_matches_cuda_core_engine(Y, oracle, shape):
-    """Dense stage-1 scores: tensor-core engine vs CUDA-core engine vs the oracle's double-precision cosine."""
-    O = oracle
-    n, d, nq = shape
-    rows32 = O.gen_rows_f32(42, 0, n, d)
-    rows16 = O.f16_from_float(rows32).reshape(n, d)
-    c = Y.Corpus(d, Y.F16, Y.COSINE)
-    c.append(rows16.view(np.float16))
-    q = O.gen_rows_f32(43, 0, nq, d) * np.float32(3.0)            # non-unit queries: 1/|q| folding
-    cc = c.debug_stage1_scores(q, 0)
-    tc = c.debug_stage1_scores(q, 1)
-    assert np.isfinite(tc).all()
-    assert np.abs(cc - tc).max() < 1e-3, np.abs(cc - tc).max()
-    up = O.f16_to_float(rows16).reshape(n, d).astype(np.float64)
-    qn = q.astype(np.float64)
-    want = (up @ qn.T).T / (np.linalg.norm(up, axis=1)[None, :] * np.linalg.norm(qn, axis=1)[:, None])
-    assert np.abs(tc - want).max() < 1e-3
-    # strided rows (the sampling pass)
-    ts = c.debug_stage1_scores(q[:3], 1, row_start=0, row_stride=7, nrows=n // 7)
-    assert np.abs(ts - want[:3, 0:7 * (n // 7):7]).max() < 1e-3
-    c.close()
-
-
 @pytest.mark.parametrize("nq", [1, 3, 17, 40, 100])
 def test_small_query_batches_through_tensor_engine(Y, oracle, nq):
     """Query tiles the batch does not fill: the padding columns must never reach the candidate lists (Q=1 once wrote

@@ -102,6 +102,61 @@ def test_certificate_catches_near_ties(Y, oracle, dtype, n):
     c.close()
 
 
+@pytest.mark.parametrize("dtype", ["f16", "f32"])
+@pytest.mark.parametrize("nq", [65, 257])
+def test_certificate_catches_near_ties_in_wide_query_tiles(Y, oracle, dtype, nq):
+    """The near-tie query above inside 256-column query tiles: in the last live column of the only tile (nq = 65), and in
+    the last column of the first tile and the only column of the second (nq = 257).  Exactly those queries leave the fast
+    path; every query's ids and scores equal the reference's, bit for bit."""
+    O = oracle
+    n, d, k = 100_000, 128, 10
+    rng = np.random.default_rng(11)
+    q_adv = O.gen_rows_f32(77, 0, 1, d)[0]
+    rows32, _ = near_tie_corpus(O, n, d, q_adv, 300, 1e-4, 42, rng)
+    if dtype == "f16":
+        rows = O.f16_from_float(rows32).reshape(n, d)
+        c = Y.Corpus(d, Y.F16, Y.COSINE)
+        c.append(rows.view(np.float16))
+    else:
+        rows = rows32
+        c = Y.Corpus(d, Y.F32, Y.COSINE)
+        c.append(rows)
+    adv = [64] if nq == 65 else [255, 256]
+    queries = O.gen_rows_f32(43, 0, nq, d)
+    queries[adv] = q_adv
+    got = c.search(queries, k, threshold=-1.0)
+    assert c.last_timings()["engine"] == "wgmma"
+    rc, wr, ws, wc = O.exact_scan_cosine_batch(rows, queries, k)
+    assert rc == 0 and np.array_equal(got[2], wc) and np.array_equal(got[0], wr) and np.array_equal(got[1], ws)
+    assert list(np.nonzero(got[3] & Y.FLAG_FALLBACK_PATH)[0]) == adv
+    assert c.last_timings()["resolved_exhaustively"] == len(adv)
+    c.close()
+
+
+@pytest.mark.parametrize("dtype", ["f16", "f32"])
+def test_l2_certificate_catches_near_ties(Y, oracle, dtype):
+    """300 rows on a 2^-14 grid around one query (tests/ref_checks.l2_near_tie_case): their squared distances lie far
+    inside the stage-1 error bound.  The L2 certificate (|q|^2 - bound - eps > dist_k^2) must send that query, and only
+    that one, to the exhaustive levels, and every answer must equal the reference build's own l2_distance ranked by
+    (distance, rowid): ids in order, distances bit for bit (d % 16 == 0: the reference's AVX summation order)."""
+    O = oracle
+    rows, held, queries = ref_checks.l2_near_tie_case(O, dtype)
+    ref = ref_checks.load()["l2_near_tie"][dtype]
+    assert ref_checks.digest(held, queries) == ref["inputs"]           # the stored answers belong to these inputs
+    n, d = held.shape
+    k = 10
+    c = Y.Corpus(d, Y.F16 if dtype == "f16" else Y.F32, Y.L2)
+    c.append(rows)
+    rid, dist, cnt, flags = c.search(queries, k)
+    assert c.last_timings()["engine"] == "wgmma"
+    for qi in range(len(queries)):
+        assert list(rid[qi]) == ref["rowids"][qi][:k], qi
+        assert np.array_equal(dist[qi], ref_checks.unpack_f32(ref["dist"][qi])[:k]), qi
+    assert flags[-1] & Y.FLAG_FALLBACK_PATH and not np.any(flags[:-1] & Y.FLAG_FALLBACK_PATH)
+    assert c.last_timings()["resolved_exhaustively"] == 1
+    c.close()
+
+
 @pytest.mark.parametrize("n", [20_000, 150_000])
 def test_corpus_of_duplicates_takes_the_full_exact_pass(Y, oracle, n):
     """More identical rows than exhaustive level 1 re-scores (4096): only the exact score of every row can answer.
@@ -227,14 +282,17 @@ def test_l2_corpus_through_the_tensor_engine(Y, oracle, cfg):
         wr, wd = O.vec0_exact(rows, queries[qi], k=k)
         assert cnt[qi] == k
         assert np.allclose(dist[qi], wd, rtol=1e-5, atol=1e-6), qi
-        if list(rid[qi]) != list(wr):                               # float summation order may swap near-equal neighbours
+        if d % 16 == 0:
+            # the reference BUILD's own l2_distance (AVX order) of the oracle's 15 nearest rows is stored: ranked by
+            # (distance, rowid), its first k are the answer -- ids in order, distances bit for bit
+            near, _ = O.vec0_exact(rows, queries[qi], k=15)
+            ref = ref_checks.unpack_f32(ref_checks.load()["l2_corpus"][ref_checks.key(list(cfg))][qi])
+            order = np.lexsort((near, ref))[:k]
+            assert list(rid[qi]) == list(near[order]), qi
+            assert np.array_equal(dist[qi], ref[order]), qi
+        elif list(rid[qi]) != list(wr):                             # float summation order may swap near-equal neighbours
             allr, alld = O.vec0_exact(rows, queries[qi], k=k + 5)
             assert set(rid[qi]) <= set(allr), qi
-        if d % 16 == 0:                                             # bit-equal to the reference BUILD's own l2_distance (AVX order)
-            near, _ = O.vec0_exact(rows, queries[qi], k=15)         # the reference's distances of these rows are stored
-            want = dict(zip(near.tolist(), ref_checks.unpack_f32(ref_checks.load()["l2_corpus"][ref_checks.key(list(cfg))][qi])))
-            for j in range(k):
-                assert np.float32(want[int(rid[qi, j])]) == dist[qi, j], (qi, j)
     assert list(rid[1][:2]) == [7, n // 2] and dist[1][0] == 0.0
     assert np.all(np.diff(dist, axis=1) >= 0)
     ex = c.search_exhaustive(queries[:3], k)

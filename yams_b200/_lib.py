@@ -57,6 +57,7 @@ CHUNK_REF_DTYPE = np.dtype([("hash", "S64"), ("offset", "<u8"), ("size", "<u4"),
 assert CHUNK_REF_DTYPE.itemsize == 80
 CHUNK_DTYPE = np.dtype([("offset", "<u8"), ("size", "<u8"), ("digest", "u1", (32,))])
 assert CHUNK_DTYPE.itemsize == C.sizeof(ChunkDesc) == 48
+CAND_DTYPE = np.dtype([("score", "<f4"), ("row", "<u4")])   # one stage-1 candidate list entry
 
 # every symbol include/yams_b200.h declares: name -> (restype, argtypes)
 _descpp = C.POINTER(C.POINTER(ChunkDesc))
@@ -125,6 +126,8 @@ SYMBOLS = {
     "yams_b200_vec_distance_l1": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, f32p]),
     "yams_b200_synth_bytes_device": (C.c_int, [C.c_uint64, C.c_uint64, C.c_uint64, C.c_void_p]),
     "yams_b200_debug_stage1_scores": (C.c_int, [C.c_void_p, f32p, C.c_uint32, C.c_int, C.c_uint64, C.c_uint64, C.c_uint64, f32p]),
+    "yams_b200_debug_stage1_candidates": (C.c_int, [C.c_void_p, f32p, C.c_uint32, C.c_int, C.c_uint64, C.c_uint64, C.c_uint64, f32p,
+                                                    C.c_uint32, i64p, u64p, u32p, C.c_void_p]),
     "yams_b200_synth_rows_device": (C.c_int, [C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint32, C.c_void_p]),
     "yams_b200_simeon_default_config": (None, [C.POINTER(SimeonConfig)]),
     "yams_b200_simeon_yams_config": (None, [C.POINTER(SimeonConfig), C.c_uint32]),
@@ -493,6 +496,28 @@ class Corpus:
         _check(lib().yams_b200_debug_stage1_scores(self._h, q.ctypes.data_as(f32p), q.shape[0], engine, row_start, row_stride,
                                                    nrows, out.ctypes.data_as(f32p)), "debug_stage1_scores")
         return out
+
+    def debug_stage1_candidates(self, queries, engine: int, tau, cap: int, row_start: int = 0, row_stride: int = 1, nrows: int = 0,
+                                allowed=None):
+        """Stage 1 in filter mode -> (counts u32[Q] (not capped), lists CAND_DTYPE[Q, cap]); entry j < min(counts[q], cap) of
+        lists[q] is a row whose stage-1 score exceeded tau[q] (and is in allowed[q], a list of rowids, when given)."""
+        q = np.ascontiguousarray(queries, dtype=np.float32)
+        nq = q.shape[0]
+        t = np.ascontiguousarray(tau, dtype=np.float32).reshape(nq)
+        nrows = nrows or len(self)
+        counts = np.zeros(nq, dtype=np.uint32)
+        lists = np.empty((nq, max(cap, 1)), dtype=CAND_DTYPE)
+        al_p = of_p = None
+        if allowed is not None:
+            offs = np.zeros(nq + 1, dtype=np.uint64)
+            offs[1:] = np.cumsum([len(a) for a in allowed])
+            al = np.ascontiguousarray(np.concatenate([np.asarray(a, dtype=np.int64) for a in allowed]) if int(offs[-1])
+                                      else np.zeros(1, dtype=np.int64), dtype=np.int64)
+            al_p, of_p = al.ctypes.data_as(i64p), offs.ctypes.data_as(u64p)
+        _check(lib().yams_b200_debug_stage1_candidates(self._h, q.ctypes.data_as(f32p), nq, engine, row_start, row_stride, nrows,
+                                                       t.ctypes.data_as(f32p), cap, al_p, of_p, counts.ctypes.data_as(u32p),
+                                                       lists.ctypes.data), "debug_stage1_candidates")
+        return counts, lists[:, :cap]
 
     def debug_last_eps(self, nq: int) -> np.ndarray:
         out = np.empty(nq, dtype=np.float32)

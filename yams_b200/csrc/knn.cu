@@ -99,7 +99,8 @@ __device__ __forceinline__ void atomic_max_nonneg(float* addr, float v) {
 // sequential double accumulation; rows with a non-finite element or |row|^2 <= 1e-12 get 0.
 // L2 corpora (vec0 surface, no skip rules) keep |row|^2 in the same slot instead: stage 1 ranks by 2 q.r - |row|^2.
 // stats[0] = max |row|, stats[1] = max |row - tf32(row)| (fp32 corpora read by the tf32 tensor-core engine),
-// stats[2] = max of that residual relative to |row|: the inputs of the stage-1 error bound (DESIGN.md §4.2)
+// stats[2] = max of that residual relative to |row|, stats[3] = max 1/|row| of the rows cosine scores: the inputs of the
+// stage-1 error bound (DESIGN.md §4.2)
 __global__ void row_stats_kernel(const void* __restrict__ rows, int dtype, uint32_t d, uint64_t first, uint64_t n,
                                  float* __restrict__ inv_norm, int metric, float* __restrict__ stats) {
     uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -122,7 +123,10 @@ __global__ void row_stats_kernel(const void* __restrict__ rows, int dtype, uint3
         float nrm = (float)sqrt(ss), rs = (float)sqrt(res);
         atomic_max_nonneg(&stats[0], nrm * 1.0000002f);
         atomic_max_nonneg(&stats[1], rs * 1.0000002f);
-        if (ss > 1e-12) atomic_max_nonneg(&stats[2], (rs / nrm) * 1.0000002f);
+        if (ss > 1e-12) {
+            atomic_max_nonneg(&stats[2], (rs / nrm) * 1.0000002f);
+            atomic_max_nonneg(&stats[3], (float)(1.0 / sqrt(ss)) * 1.0000002f);
+        }
     }
 }
 
@@ -306,7 +310,8 @@ __global__ void __launch_bounds__(CC_THREADS, 2) stage1_cc_kernel(Stage1Args a, 
             uint32_t q = q0 + tx * 4 + j;
             if (q >= a.nq) continue;
             float s;
-            if (a.metric == YAMS_B200_L2) s = fmaf(2.f, acc[i][j], -inr);           // 2 q.r - |r|^2 (slot holds |r|^2)
+            // L2: 2 q.r - |r|^2 (slot holds |r|^2; +inf marks a non-finite row, whose dot product may be NaN)
+            if (a.metric == YAMS_B200_L2) s = inr < INFINITY ? fmaf(2.f, acc[i][j], -inr) : -INFINITY;
             else s = inr > 0.f ? acc[i][j] * inr * a.qinv[q] : -INFINITY;
             if (FILTER) {
                 bool pass = s > a.tau[q];
@@ -1328,11 +1333,12 @@ static yams_status_t corpus_finish_append(Corpus* c, uint64_t n_new, const int64
                                                                        c->inv_norm.as<float>(), c->metric, c->stats.as<float>());
     YB_CUDA(cudaGetLastError());
     float h_stats[4] = {0, 0, 0, 0};
-    YB_CUDA(cudaMemcpyAsync(h_stats, c->stats.p, 12, cudaMemcpyDeviceToHost, c->st));
+    YB_CUDA(cudaMemcpyAsync(h_stats, c->stats.p, 16, cudaMemcpyDeviceToHost, c->st));
     YB_CUDA(cudaStreamSynchronize(c->st));
     c->r_max = h_stats[0];
     c->dr_abs_max = h_stats[1];
     c->dr_rel_max = h_stats[2];
+    c->inv_max = h_stats[3];
     c->last_rowid = last;
     c->rowids_dense = dense;
     c->n += n_new;
@@ -1373,6 +1379,7 @@ static void fill_stage1_common(Corpus* c, Stage1Args& a, uint32_t nq) {
     a.r_max = c->r_max;
     a.dr_abs_max = c->dr_abs_max;
     a.dr_rel_max = c->dr_rel_max;
+    a.inv_max = c->inv_max;
 }
 
 // Enqueues the whole pipeline for the nq queries already prepared on the device (prepare_queries) and writes the padded
@@ -1488,6 +1495,7 @@ static yams_status_t scan_enqueue(Corpus* c, const ScanPlan& p, int64_t* d_out_r
     // error bound of the engine(s) that produced the ranking
     if (cc_used || !tensor_used)
         eps_cc_kernel<<<(nq + 255) / 256, 256, 0, st>>>(d_qnorm, nq, c->dim, c->metric, c->r_max, c->eps.as<float>(), tensor_used ? 1 : 0);
+    c->last_ms[4] = tensor_used ? 1.f : 0.f;   // the engine that ran: wgmma declines shapes it does not take (nq > 4096)
     YB_CUDA(cudaEventRecord(c->ev[1], st));
     // ---- stage 2: exact re-scoring, ordering, certificate ----
     if ((rc = c->outbuf.reserve((size_t)nq * Kp * sizeof(Exact))) != YAMS_OK) return rc;
@@ -1817,7 +1825,7 @@ yams_status_t yams_b200_corpus_clear(yams_b200_corpus* c) {
     c->last_rowid = INT64_MIN;
     c->rowids_dense = true;
     c->pending.active = false;
-    c->r_max = c->dr_abs_max = c->dr_rel_max = 0.f;
+    c->r_max = c->dr_abs_max = c->dr_rel_max = c->inv_max = 0.f;
     if (c->stats.p) YB_CUDA(cudaMemsetAsync(c->stats.p, 0, 16, c->st));
     return YAMS_OK;
 }
@@ -1872,6 +1880,27 @@ static yams_status_t finish_scan(yams_b200_corpus* c, const ScanPlan& p, int64_t
     if (out_resolved) *out_resolved = n_bad;
     return resolve_uncertain(c, p, bad.data(), n_bad, d_or, d_os, d_oc, d_of);
 }
+// candidate sets as a bit matrix [nq][mask_ld * 32] of allowed corpus rows (allowed_offsets[nq + 1] into allowed_rowids)
+static yams_status_t upload_mask(yams_b200_corpus* c, uint32_t nq, const int64_t* allowed_rowids, const uint64_t* allowed_offsets,
+                                 const uint32_t** out_mask, uint64_t* out_mask_ld) {
+    yams_status_t rc;
+    const uint64_t total = allowed_offsets[nq];
+    const uint64_t mask_ld = (c->n + 31) / 32;
+    const size_t mb = (size_t)nq * mask_ld * 4;
+    if ((rc = c->mask.reserve(mb + (size_t)total * 8 + (size_t)(nq + 1) * 8 + 64)) != YAMS_OK) return rc;
+    uint32_t* dm = c->mask.as<uint32_t>();
+    int64_t* d_allowed = reinterpret_cast<int64_t*>(c->mask.as<uint8_t>() + ((mb + 7) & ~(size_t)7));
+    uint64_t* d_offs = reinterpret_cast<uint64_t*>(d_allowed + total);
+    YB_CUDA(cudaMemsetAsync(dm, 0, mb, c->st));
+    if (total) YB_CUDA(cudaMemcpyAsync(d_allowed, allowed_rowids, (size_t)total * 8, cudaMemcpyHostToDevice, c->st));
+    YB_CUDA(cudaMemcpyAsync(d_offs, allowed_offsets, (size_t)(nq + 1) * 8, cudaMemcpyHostToDevice, c->st));
+    dim3 grid(64, nq);
+    build_mask_kernel<<<grid, 256, 0, c->st>>>(d_allowed, d_offs, nq, c->rowids.as<int64_t>(), c->n, dm, mask_ld);
+    *out_mask = dm;
+    *out_mask_ld = mask_ld;
+    return YAMS_OK;
+}
+
 static yams_status_t enqueue_status_readback(yams_b200_corpus* c, uint32_t nq) {
     YB_CUDA(cudaMemcpyAsync(c->h_pin.p, c->status.p, sizeof(ScanStatus) + (size_t)nq * 4, cudaMemcpyDeviceToHost, c->st));
     return YAMS_OK;
@@ -1940,20 +1969,7 @@ yams_status_t yams_b200_search(yams_b200_corpus* c, const float* queries, uint32
         lists.total = total;
         plan.direct = &lists;
     } else if (allowed_offsets && c->n) {
-        uint64_t total = allowed_offsets[nq];
-        uint64_t mask_ld = (c->n + 31) / 32;
-        size_t mb = (size_t)nq * mask_ld * 4;
-        if ((rc = c->mask.reserve(mb + (size_t)total * 8 + (size_t)(nq + 1) * 8 + 64)) != YAMS_OK) return rc;
-        uint32_t* dm = c->mask.as<uint32_t>();
-        int64_t* d_allowed = reinterpret_cast<int64_t*>(c->mask.as<uint8_t>() + ((mb + 7) & ~(size_t)7));
-        uint64_t* d_offs = reinterpret_cast<uint64_t*>(d_allowed + total);
-        YB_CUDA(cudaMemsetAsync(dm, 0, mb, c->st));
-        if (total) YB_CUDA(cudaMemcpyAsync(d_allowed, allowed_rowids, (size_t)total * 8, cudaMemcpyHostToDevice, c->st));
-        YB_CUDA(cudaMemcpyAsync(d_offs, allowed_offsets, (size_t)(nq + 1) * 8, cudaMemcpyHostToDevice, c->st));
-        dim3 grid(64, nq);
-        build_mask_kernel<<<grid, 256, 0, c->st>>>(d_allowed, d_offs, nq, c->rowids.as<int64_t>(), c->n, dm, mask_ld);
-        plan.d_mask = dm;
-        plan.mask_ld = mask_ld;
+        if ((rc = upload_mask(c, nq, allowed_rowids, allowed_offsets, &plan.d_mask, &plan.mask_ld)) != YAMS_OK) return rc;
     }
     if ((rc = scan_enqueue(c, plan, d_or, d_os, d_oc, d_of)) != YAMS_OK) return rc;
     cudaEventRecord(c->ev[2], c->st);
@@ -1974,7 +1990,6 @@ yams_status_t yams_b200_search(yams_b200_corpus* c, const float* queries, uint32
     cudaEventElapsedTime(&c->last_ms[0], c->ev[0], c->ev[1]);
     cudaEventElapsedTime(&c->last_ms[1], c->ev[1], c->ev[2]);
     cudaEventElapsedTime(&c->last_ms[2], c->ev[0], c->ev[2]);
-    c->last_ms[4] = plan.use_tensor ? 1.f : 0.f;
     uint32_t resolved = 0;
     rc = finish_scan(c, plan, d_or, d_os, d_oc, d_of, &resolved);
     c->last_ms[6] = (float)resolved;
@@ -2128,7 +2143,6 @@ yams_status_t yams_b200_search_device(yams_b200_corpus* c, const float* d_querie
     if ((rc = scan_enqueue(c, plan, d_out_rowids, d_out_scores, nullptr, nullptr)) != YAMS_OK) return rc;
     YB_CUDA(cudaEventRecord(c->ev[2], c->st));
     if ((rc = enqueue_status_readback(c, nq)) != YAMS_OK) return rc;
-    c->last_ms[4] = plan.use_tensor ? 1.f : 0.f;
     c->pending.active = true;
     c->pending.nq = nq;
     c->pending.k = k;
@@ -2231,6 +2245,47 @@ yams_status_t yams_b200_debug_stage1_scores(yams_b200_corpus* c, const float* qu
     }
     if (rc != YAMS_OK) return rc;
     YB_CUDA(cudaMemcpyAsync(out, c->dense.p, (size_t)nq * nrows * 4, cudaMemcpyDeviceToHost, c->st));
+    YB_CUDA(cudaStreamSynchronize(c->st));
+    return YAMS_OK;
+}
+
+// diagnostics: the same rows and engines in FILTER mode -- the candidate lists the search builds from per-query thresholds
+// (and candidate sets) -> out_counts[q] (raw, may exceed cap), out_cands[q * cap + j] = (float score, uint32 row) (HOST)
+yams_status_t yams_b200_debug_stage1_candidates(yams_b200_corpus* c, const float* queries, uint32_t nq, int engine,
+                                                uint64_t row_start, uint64_t row_stride, uint64_t nrows, const float* tau, uint32_t cap,
+                                                const int64_t* allowed_rowids, const uint64_t* allowed_offsets, uint32_t* out_counts,
+                                                void* out_cands) {
+    YB_ARG(c && queries && tau && out_counts && (out_cands || cap == 0) && nq > 0 && nrows > 0 && row_stride > 0, "bad argument");
+    YB_ARG(!allowed_rowids || allowed_offsets, "allowed_offsets missing");
+    YB_ARG(!allowed_offsets || allowed_rowids || allowed_offsets[nq] == 0, "allowed_rowids missing");
+    std::lock_guard<std::mutex> corpus_lock(c->mu);
+    YB_ARG(row_start + (nrows - 1) * row_stride < c->n, "rows out of range");
+    yams_status_t rc;
+    YB_BIND(c);
+    c->pending.active = false;
+    if ((rc = prepare_queries(c, queries, false, nq)) != YAMS_OK) return rc;
+    const size_t cb = (size_t)nq * cap * sizeof(Cand);
+    if ((rc = c->eps.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
+    if ((rc = c->tau.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
+    if ((rc = c->cands.reserve(cb + 8)) != YAMS_OK) return rc;
+    YB_CUDA(cudaMemcpyAsync(c->tau.p, tau, (size_t)nq * 4, cudaMemcpyHostToDevice, c->st));
+    YB_CUDA(cudaMemsetAsync(c->counts.p, 0, (size_t)nq * 4, c->st));
+    YB_CUDA(cudaMemsetAsync(c->cands.p, 0xFF, cb, c->st));
+    Stage1Args a{};
+    fill_stage1_common(c, a, nq);
+    a.row_start = row_start; a.row_stride = row_stride; a.nrows = nrows;
+    a.tau = c->tau.as<float>(); a.cands = c->cands.as<Cand>(); a.cap = cap; a.counts = c->counts.as<uint32_t>();
+    if (allowed_offsets && (rc = upload_mask(c, nq, allowed_rowids, allowed_offsets, &a.mask, &a.mask_ld)) != YAMS_OK) return rc;
+    if (engine == 1) {
+        rc = stage1_wgmma(c, a, true, c->st);
+    } else {
+        rc = stage1_cuda_core(a, true, c->st);
+        eps_cc_kernel<<<(nq + 255) / 256, 256, 0, c->st>>>(reinterpret_cast<double*>(c->misc.as<uint8_t>()), nq, c->dim, c->metric, c->r_max,
+                                                           c->eps.as<float>(), 0);
+    }
+    if (rc != YAMS_OK) return rc;
+    YB_CUDA(cudaMemcpyAsync(out_counts, c->counts.p, (size_t)nq * 4, cudaMemcpyDeviceToHost, c->st));
+    if (cb) YB_CUDA(cudaMemcpyAsync(out_cands, c->cands.p, cb, cudaMemcpyDeviceToHost, c->st));
     YB_CUDA(cudaStreamSynchronize(c->st));
     return YAMS_OK;
 }

@@ -25,8 +25,9 @@ struct Corpus {
     DevBuf rows;       // n x dim elements
     DevBuf rowids;     // n x int64
     DevBuf inv_norm;   // n x float. cosine: 1/|row| (double math), 0 for rows the reference skips; L2: |row|^2
-    DevBuf stats;      // 3 floats: max |row|, max |row - tf32(row)|, max of that residual relative to |row| (row_stats_kernel)
-    float r_max = 0.f, dr_abs_max = 0.f, dr_rel_max = 0.f;   // host copies of stats (upper bounds; removals keep them)
+    DevBuf stats;      // 4 floats: max |row|, max |row - tf32(row)|, max of that residual relative to |row|, max 1/|row|
+                       // (row_stats_kernel)
+    float r_max = 0.f, dr_abs_max = 0.f, dr_rel_max = 0.f, inv_max = 0.f;   // host copies of stats (upper bounds; removals keep them)
     // search workspace
     DevBuf q32, q16, qinv, tau, counts, cands, sample_scores, sel, outbuf, dense, mask, misc, dout;
     DevBuf status;     // ScanStatus + bad[nq] + bad2[nq] of the call in flight
@@ -80,7 +81,7 @@ struct Stage1Args {
     // exactness certificate) are prepared by the first call of a search and reused by the following ones
     bool skip_qprep;
     float* eps;             // nq floats, written by the engine's query preparation
-    float r_max, dr_abs_max, dr_rel_max;   // corpus norm statistics (Corpus)
+    float r_max, dr_abs_max, dr_rel_max, inv_max;   // corpus norm statistics (Corpus)
 };
 
 yams_status_t stage1_cuda_core(const Stage1Args& a, bool filter, cudaStream_t st);

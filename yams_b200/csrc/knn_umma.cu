@@ -335,13 +335,19 @@ stage1_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
 // With x = the scaled query, y = what the tensor core multiplies (fp16-rounded / tf32-truncated x), dq = |x - y|, and the
 // rows r read as r' (exact for fp16 rows; tf32-truncated for fp32 rows, residual norms tracked per corpus):
 //   |x.r - y.r'| <= dq |r'| + |x| |r - r'|            (Cauchy-Schwarz with the ACTUAL rounding residuals)
-//   cosine (|x| = 1, score = x.r / |r|):  eps = 1.25 (dq + dr_rel_max) + 2^-23 (d + 4)
-//   L2 (score = 2 x.r - |r|^2)         :  eps = 2.5 (dq Rmax + |x| dr_abs_max) + 2^-22 (d + 4) |x| Rmax + 2^-22 Rmax^2
-// The 1.25 covers the second-order term and the fp32 accumulation inside the tensor core is the 2^-23 (d + 4) term.
+//   cosine (|x| = 1, score = x.r / |r|):  eps = 1.25 (dq + dr_rel_max) + 2^-23 (d + 4) Y R1
+//   L2 (score = 2 x.r - |r|^2)         :  eps = 2.5 (dq Rmax + |x| dr_abs_max) + 2^-22 (d + 4) Y R2 + 2^-22 Rmax^2
+// The 1.25 covers the second-order term and the fp32 accumulation inside the tensor core is the 2^-23 (d + 4) term.  The
+// tensor core truncates products on alignment to the block's largest one.  With fp16 subnormal operands the error measured
+// on an H100 reaches ~2^-13 of the largest true product, as if products were sized by exponent fields, where a subnormal
+// counts as 2^-14.  So the accumulation term takes every fp16 operand element as at least 2^-14 (no floor for tf32),
+// f = d 2^-28: Y = sqrt((|x| + dq)^2 + f) >= |y| with the floor,
+// R1 = sqrt(1 + f max(1/|r|)^2) >= |r with the floor| / |r|, R2 = sqrt(Rmax^2 + f).  Both factors are 1 + O(1e-6) unless
+// the corpus holds rows of norm ~1e-3 or less, whose 1/|r| amplifies the accumulator's absolute error.
 template <bool TF32>
 __global__ void __launch_bounds__(128) queries_prep_kernel(const float* __restrict__ q32, const float* __restrict__ qinv, uint32_t nq,
                                                            uint32_t d, void* __restrict__ out, int metric, float r_max, float dr_abs_max,
-                                                           float dr_rel_max, float* __restrict__ eps) {
+                                                           float dr_rel_max, float inv_max, float* __restrict__ eps) {
     const uint32_t q = blockIdx.x;
     const float scale = qinv[q];   // 1 for L2
     float ss = 0.f, xx = 0.f;
@@ -372,9 +378,13 @@ __global__ void __launch_bounds__(128) queries_prep_kernel(const float* __restri
         const float dq = sqrtf(red[0][0] + red[0][1] + red[0][2] + red[0][3]) * 1.000001f;
         const float xn = sqrtf(red[1][0] + red[1][1] + red[1][2] + red[1][3]) * 1.000001f;
         const float u = 1.1920929e-07f;   // 2^-23
+        const float f = TF32 ? 0.f : (float)d * 3.7252903e-09f;                  // d 2^-28
+        const float yf = sqrtf((xn + dq) * (xn + dq) + f) * 1.000001f;
         float e;
-        if (metric == YAMS_B200_L2) e = 2.5f * (dq * r_max + xn * dr_abs_max) + 2.f * u * (float)(d + 4) * xn * r_max + 2.f * u * r_max * r_max + 1e-30f;
-        else e = 1.25f * (dq + xn * dr_rel_max) + u * (float)(d + 4) + 1e-7f;
+        if (metric == YAMS_B200_L2)
+            e = 2.5f * (dq * r_max + xn * dr_abs_max) + 2.f * u * (float)(d + 4) * yf * (sqrtf(r_max * r_max + f) * 1.000001f) +
+                2.f * u * r_max * r_max + 1e-30f;
+        else e = 1.25f * (dq + xn * dr_rel_max) + u * (float)(d + 4) * yf * (sqrtf(1.f + f * inv_max * inv_max) * 1.000001f) + 1e-7f;
         eps[q] = e;
     }
 }
@@ -450,8 +460,9 @@ yams_status_t stage1_wgmma(Corpus* c, const Stage1Args& a, bool filter, cudaStre
     if (!a.skip_qprep) {
         if (!a.eps) return YAMS_ERR_UNSUPPORTED;
         if (tf32) queries_prep_kernel<true><<<a.nq, 128, 0, st>>>(a.q32, a.qinv, a.nq, a.dim, d_q16, a.metric, a.r_max, a.dr_abs_max,
-                                                                   a.dr_rel_max, a.eps);
-        else queries_prep_kernel<false><<<a.nq, 128, 0, st>>>(a.q32, a.qinv, a.nq, a.dim, d_q16, a.metric, a.r_max, 0.f, 0.f, a.eps);
+                                                                   a.dr_rel_max, a.inv_max, a.eps);
+        else queries_prep_kernel<false><<<a.nq, 128, 0, st>>>(a.q32, a.qinv, a.nq, a.dim, d_q16, a.metric, a.r_max, 0.f, 0.f, a.inv_max,
+                                                               a.eps);
     }
 
 
