@@ -492,7 +492,8 @@ YAMS_B200_API void yams_b200_simeon_destroy(yams_b200_encoder* e);
 /* [0] stage-1 scan ms, [1] rescoring+select ms, [2] total device ms, [3] h2d+d2h ms of the last
  * yams_b200_search on this corpus; [4] = which stage-1 kernel ran (0 cuda-core, 1 wgmma);
  * [5] = duration of the full-corpus filtered scan launch alone (the dominant kernel);
- * [6] = queries of that call the certificate sent to the exhaustive levels */
+ * [6] = queries of that call the certificate sent to the exhaustive levels, [7] = of those, the queries level 1 could not
+ * certify either, answered by the full exact pass */
 YAMS_B200_API yams_status_t yams_b200_search_last_timings(yams_b200_corpus* c, float out_ms[8]);
 
 typedef struct yams_vector_scan_v1 {
@@ -575,13 +576,42 @@ YAMS_B200_API yams_status_t yams_b200_debug_stage1_scores(yams_b200_corpus* c, c
  * listed for query q when its stage-1 score is > tau[q] (and, with allowed lists in the format of yams_b200_search, the row
  * is in query q's set).  out_counts[q] = rows that passed (NOT capped at cap); out_cands[q * cap + j], j < min(count, cap),
  * = (float score, uint32 row index) pairs, 8 bytes each, in no particular order (HOST). YAMS_ERR_UNSUPPORTED when the
- * engine cannot take the shape. */
+ * engine cannot take the shape.  engine = 2 is the gather engine of small ascending candidate sets: it scores every entry of
+ * the allowed lists (each at most cap long) and ignores tau and the row range; out_counts[q] = list length, out_cands[q * cap
+ * + j] = list entry j, (-inf, 0xFFFFFFFF) for a rowid that is unknown or repeats the previous entry. */
 YAMS_B200_API yams_status_t yams_b200_debug_stage1_candidates(yams_b200_corpus* c, const float* queries, uint32_t nq,
                                                               int engine, uint64_t row_start, uint64_t row_stride,
                                                               uint64_t nrows, const float* tau, uint32_t cap,
                                                               const int64_t* allowed_rowids,
                                                               const uint64_t* allowed_offsets, uint32_t* out_counts,
                                                               void* out_cands);
+
+/* diagnostics: the search's top-K selection on caller-supplied scores (HOST in and out).  Input per query q, either
+ *   dense (dense != NULL): dense[q * ld + i], i < len, row index row_start + i * row_stride; the device copy starts
+ *                          dense_shift (0..3) floats past a 16-byte boundary, or
+ *   lists: cands[q * cap + j] (float score, uint32 row) pairs, j < min(counts[q], cap), counts[q] may exceed cap; tau
+ *          (nullable) bounds the scores of rows that never reached a list.
+ * tau_only = 0: out_sel[q * K + j] = the K best (score desc, row asc) pairs, out_n[q] their number, out_bound[q] = an upper
+ *               bound of every unselected score (K-th score when the input is longer than K, else tau[q] or -inf; +inf when
+ *               counts[q] > cap); K <= 4096.
+ * tau_only = 1: out_bound[q] = the K-th best score - tau_margin (-inf when fewer than K); fast_tau as in the threshold
+ *               calibration of the corpus pass (K <= 16, len >= 4096: the K-th of the 256 per-thread maxima). */
+YAMS_B200_API yams_status_t yams_b200_debug_select(yams_b200_corpus* c, uint32_t nq, const float* dense, uint64_t ld,
+                                                   uint64_t len, uint64_t row_start, uint64_t row_stride, uint32_t dense_shift,
+                                                   const void* cands, const uint32_t* counts, uint32_t cap, const float* tau,
+                                                   uint32_t K, int tau_only, float tau_margin, int fast_tau, void* out_sel,
+                                                   uint32_t* out_n, float* out_bound);
+
+/* diagnostics: the search's final ordering and exactness certificate on caller-supplied exact scores (HOST in and out).
+ * exact[q * Kp + i], i < (ex_n ? ex_n[q] : Kp): (float sim, uint32 row) pairs, NaN sim = no entry, row indexes this corpus's
+ * rowid table; bound[q], eps[q], qnorm[q] (double, L2) are the certificate inputs; level 0 or 1 as in the exhaustive chain
+ * (level 1 always flags the fallback).  Out: the k best by (sim desc, row asc) as rowids / scores (L2: negated sims = distances),
+ * padded with -1 and -inf (L2: +inf), counts, flags, and the queries the certificate queued (out_queued[nq], in queue order). */
+YAMS_B200_API yams_status_t yams_b200_debug_final(yams_b200_corpus* c, uint32_t nq, uint32_t Kp, uint32_t k, const void* exact,
+                                                  const uint32_t* ex_n, const float* bound, const float* eps,
+                                                  const double* qnorm, float threshold, int metric, int level,
+                                                  int64_t* out_rowids, float* out_scores, uint32_t* out_counts,
+                                                  uint64_t* out_flags, uint32_t* out_queued, uint32_t* out_n_queued);
 
 /* diagnostics: the per-query stage-1 error bound eps[q] of the last search / debug_stage1_scores call (HOST out) */
 YAMS_B200_API yams_status_t yams_b200_debug_last_eps(yams_b200_corpus* c, uint32_t nq, float* out);

@@ -58,6 +58,7 @@ assert CHUNK_REF_DTYPE.itemsize == 80
 CHUNK_DTYPE = np.dtype([("offset", "<u8"), ("size", "<u8"), ("digest", "u1", (32,))])
 assert CHUNK_DTYPE.itemsize == C.sizeof(ChunkDesc) == 48
 CAND_DTYPE = np.dtype([("score", "<f4"), ("row", "<u4")])   # one stage-1 candidate list entry
+EXACT_DTYPE = np.dtype([("sim", "<f4"), ("row", "<u4")])    # one exactly re-scored survivor (NaN sim: none)
 
 # every symbol include/yams_b200.h declares: name -> (restype, argtypes)
 _descpp = C.POINTER(C.POINTER(ChunkDesc))
@@ -139,6 +140,11 @@ SYMBOLS = {
     "yams_b200_pq_codes": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, u64p]),
     "yams_b200_pq_destroy": (None, [C.c_void_p]),
     "yams_b200_debug_last_eps": (C.c_int, [C.c_void_p, C.c_uint32, f32p]),
+    "yams_b200_debug_select": (C.c_int, [C.c_void_p, C.c_uint32, f32p, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint32,
+                                         C.c_void_p, u32p, C.c_uint32, f32p, C.c_uint32, C.c_int, C.c_float, C.c_int, C.c_void_p,
+                                         u32p, f32p]),
+    "yams_b200_debug_final": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, u32p, f32p, f32p,
+                                        C.POINTER(C.c_double), C.c_float, C.c_int, C.c_int, i64p, f32p, u32p, u64p, u32p, u32p]),
     "yams_b200_device_count": (C.c_int, []),
     "yams_b200_last_error": (C.c_char_p, []),
 }
@@ -519,6 +525,56 @@ class Corpus:
                                                        lists.ctypes.data), "debug_stage1_candidates")
         return counts, lists[:, :cap]
 
+    def debug_select(self, K: int, dense=None, row_start: int = 0, row_stride: int = 1, dense_shift: int = 0, cands=None,
+                     counts=None, tau=None, tau_only: bool = False, tau_margin: float = 0.0, fast_tau: bool = False):
+        """The scan's top-K selection on given scores: dense f32[Q, L] (row index row_start + i * row_stride, device copy
+        dense_shift floats past a 16-byte boundary) or lists CAND_DTYPE[Q, cap] with counts u32[Q] (may exceed cap) and an
+        optional tau f32[Q].  -> (sel CAND_DTYPE[Q, K], n u32[Q], bound f32[Q]), or with tau_only the thresholds f32[Q]."""
+        if dense is not None:
+            d = np.ascontiguousarray(dense, dtype=np.float32)
+            nq, L = d.shape
+            dp, ld = d.ctypes.data_as(f32p), L
+            cp = cntp = None
+            cap = 0
+        else:
+            cl = np.ascontiguousarray(cands, dtype=CAND_DTYPE)
+            nq, cap = cl.shape
+            cnt = np.ascontiguousarray(counts, dtype=np.uint32).reshape(nq)
+            dp, ld, L = None, 0, 0
+            cp, cntp = cl.ctypes.data, cnt.ctypes.data_as(u32p)
+        t = np.ascontiguousarray(tau, dtype=np.float32).reshape(nq) if tau is not None else None
+        sel = np.empty((nq, max(K, 1)), dtype=CAND_DTYPE)
+        n = np.zeros(nq, dtype=np.uint32)
+        bound = np.empty(nq, dtype=np.float32)
+        _check(lib().yams_b200_debug_select(self._h, nq, dp, ld, L, row_start, row_stride, dense_shift, cp, cntp, cap,
+                                            t.ctypes.data_as(f32p) if t is not None else None, K, int(tau_only), tau_margin,
+                                            int(fast_tau), sel.ctypes.data, n.ctypes.data_as(u32p), bound.ctypes.data_as(f32p)),
+               "debug_select")
+        return bound if tau_only else (sel[:, :K], n, bound)
+
+    def debug_final(self, exact, k: int, bound, eps, qnorm=None, threshold: float = -1.0, metric: Optional[int] = None,
+                    level: int = 0, ex_n=None):
+        """The scan's final ordering + exactness certificate on given survivors exact EXACT_DTYPE[Q, Kp] (rows index this
+        corpus) -> (rowids i64[Q, k], scores f32[Q, k], counts u32[Q], flags u64[Q], queued queries u32[m])."""
+        ex = np.ascontiguousarray(exact, dtype=EXACT_DTYPE)
+        nq, Kp = ex.shape
+        b = np.ascontiguousarray(bound, dtype=np.float32).reshape(nq)
+        e = np.ascontiguousarray(eps, dtype=np.float32).reshape(nq)
+        qn = np.ascontiguousarray(qnorm if qnorm is not None else np.ones(nq), dtype=np.float64).reshape(nq)
+        en = np.ascontiguousarray(ex_n, dtype=np.uint32).reshape(nq) if ex_n is not None else None
+        out_r = np.empty((nq, k), dtype=np.int64)
+        out_s = np.empty((nq, k), dtype=np.float32)
+        out_c = np.empty(nq, dtype=np.uint32)
+        out_f = np.empty(nq, dtype=np.uint64)
+        queued = np.empty(nq, dtype=np.uint32)
+        nqd = C.c_uint32(0)
+        _check(lib().yams_b200_debug_final(self._h, nq, Kp, k, ex.ctypes.data, en.ctypes.data_as(u32p) if en is not None else None,
+                                           b.ctypes.data_as(f32p), e.ctypes.data_as(f32p), qn.ctypes.data_as(C.POINTER(C.c_double)),
+                                           threshold, self.metric if metric is None else metric, level, out_r.ctypes.data_as(i64p),
+                                           out_s.ctypes.data_as(f32p), out_c.ctypes.data_as(u32p), out_f.ctypes.data_as(u64p),
+                                           queued.ctypes.data_as(u32p), C.byref(nqd)), "debug_final")
+        return out_r, out_s, out_c, out_f, queued[:nqd.value].copy()
+
     def debug_last_eps(self, nq: int) -> np.ndarray:
         out = np.empty(nq, dtype=np.float32)
         _check(lib().yams_b200_debug_last_eps(self._h, nq, out.ctypes.data_as(f32p)), "debug_last_eps")
@@ -535,7 +591,7 @@ class Corpus:
         ms = (C.c_float * 8)()
         lib().yams_b200_search_last_timings(self._h, ms)
         return {"stage1_ms": ms[0], "stage2_ms": ms[1], "total_ms": ms[2], "scan_kernel_ms": ms[5],
-                "engine": "wgmma" if ms[4] else "cuda-core", "resolved_exhaustively": int(ms[6])}
+                "engine": "wgmma" if ms[4] else "cuda-core", "resolved_exhaustively": int(ms[6]), "resolved_full_pass": int(ms[7])}
 
     def close(self):
         if self._h:

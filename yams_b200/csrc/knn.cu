@@ -804,6 +804,7 @@ struct CertArgs {
     const double* qnorm;      // per query (L2)
     float threshold;
     int metric;
+    double l2_margin;         // L2: dist_k^2 factor covering the float rounding of the reference's distances (l2_cert_margin)
     ScanStatus* status;       // nullable: no certificate (results already exhaustive)
     int level;                // 0: failures go to bad[], 1: to bad2[]
     uint32_t nq_total;        // capacity of each list
@@ -878,8 +879,8 @@ __global__ void __launch_bounds__(SEL_THREADS) final_kernel(const Exact* __restr
                     if (valid >= k) {
                         const float dk = -fkey_inv((uint32_t)(buf[k - 1] >> 32));
                         const double qq = cert.qnorm[q] * cert.qnorm[q];
-                        // distances are floats of a float sum: allow their own rounding (d * 2^-24 relative, generously)
-                        const double dk2 = (double)dk * (double)dk * 1.0001 + 1e-30;
+                        // distances are floats of a float sum: allow their own rounding
+                        const double dk2 = (double)dk * (double)dk * cert.l2_margin + 1e-30;
                         certified = qq - (double)bd - (double)e > dk2;
                     }
                 } else {
@@ -1011,7 +1012,9 @@ __global__ void gather_score_kernel(const void* __restrict__ rows, int dtype, ui
         }
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-        out.score = s * inv_norm[a] * qinv[q];
+        // rows the reference skips (inv_norm 0) score -inf like in the other engines: their s may be inf or NaN
+        const float inr = inv_norm[a];
+        out.score = inr > 0.f ? s * inr * qinv[q] : -INFINITY;
         out.row = (uint32_t)a;
     }
     if (lane == 0) cands[(uint64_t)q * cap + j] = out;
@@ -1296,6 +1299,18 @@ static uint32_t survivors_for(uint32_t k) {
     return std::min<uint32_t>(kp, SEL_MAXK);
 }
 
+// dist_k^2 factor of the L2 certificate (final_kernel).  The reference's float distance of a row with exact squared distance
+// D^2 sums d terms fl(fl(q_i - r_i)^2): one term meets three roundings before the sum and one per later addition, t of them
+// in all -- d + 2 for the scalar loop, d/8 + 9 for the AVX order (d/8 - 1 lane additions, 7 across lanes).  So the float sum
+// is >= D^2 (1-u)^t and its rounded square root s >= sqrt(D^2 (1-u)^t) (1-u).  A row whose D^2 exceeds dist_k^2 (1-u)^-(t+2)
+// therefore has a distance > dist_k.  The factor never drops below the 1 + 1e-4 the certificate used before it depended on d
+// (enough up to d ~ 1670 in the scalar order).
+static double l2_cert_margin(uint32_t d) {
+    const double u = 0x1p-24;
+    const double t = (d >= 16 && d % 16 == 0) ? d / 8.0 + 9.0 : d + 2.0;
+    return std::max(1.0001, pow(1.0 - u, -(t + 2.0)) * (1.0 + 1e-12));
+}
+
 static yams_status_t corpus_reserve(Corpus* c, uint64_t n_total) {
     yams_status_t rc;
     if ((rc = c->rows.reserve((size_t)n_total * c->dim * c->elem() + 256, true, c->st)) != YAMS_OK) return rc;
@@ -1364,6 +1379,22 @@ struct ScanPlan {
     bool use_tensor = false;
 };
 
+// stage 1 of the direct path: cands[q * cap + j] = (score, row) of list entry j (cap >= the longest list)
+static yams_status_t gather_scores(Corpus* c, const DirectLists& L, uint32_t nq, const float* q32, const float* qinv, Cand* cands,
+                                   uint32_t cap, cudaStream_t st) {
+    if (L.total) {
+        const unsigned grid = (unsigned)((L.total * 32 + 255) / 256);
+        const bool v8 = c->dtype == YAMS_B200_F16 && c->dim % 8 == 0, v4 = c->dtype == YAMS_B200_F32 && c->dim % 4 == 0;
+#define YB_GATHER(V)                                                                                                              \
+    gather_score_kernel<V><<<grid, 256, 0, st>>>(c->rows.p, c->dtype, c->dim, c->inv_norm.as<float>(), c->rowids.as<int64_t>(), c->n, \
+                                                 q32, qinv, L.d_allowed, L.d_offsets, nq, L.total, cands, cap)
+        if (v8) YB_GATHER(8); else if (v4) YB_GATHER(4); else YB_GATHER(0);
+#undef YB_GATHER
+    }
+    YB_CUDA(cudaGetLastError());
+    return YAMS_OK;
+}
+
 static ScanStatus* status_of(Corpus* c) { return c->status.as<ScanStatus>(); }
 
 static void fill_stage1_common(Corpus* c, Stage1Args& a, uint32_t nq) {
@@ -1426,16 +1457,9 @@ static yams_status_t scan_enqueue(Corpus* c, const ScanPlan& p, int64_t* d_out_r
         const uint32_t cap = std::max<uint32_t>(direct->max_len, 1);
         if ((rc = c->cands.reserve((size_t)nq * cap * sizeof(Cand))) != YAMS_OK) return rc;
         list_lengths_kernel<<<(nq + 255) / 256, 256, 0, st>>>(direct->d_offsets, nq, d_counts);
+        if (direct->total) YB_CUDA(cudaEventRecord(c->ev_scan[0], st));
+        if ((rc = gather_scores(c, *direct, nq, a.q32, a.qinv, c->cands.as<Cand>(), cap, st)) != YAMS_OK) return rc;
         if (direct->total) {
-            const unsigned grid = (unsigned)((direct->total * 32 + 255) / 256);
-            const bool v8 = c->dtype == YAMS_B200_F16 && c->dim % 8 == 0, v4 = c->dtype == YAMS_B200_F32 && c->dim % 4 == 0;
-#define YB_GATHER(V)                                                                                                              \
-    gather_score_kernel<V><<<grid, 256, 0, st>>>(c->rows.p, c->dtype, c->dim, c->inv_norm.as<float>(), c->rowids.as<int64_t>(), n, \
-                                                 a.q32, a.qinv, direct->d_allowed, direct->d_offsets, nq, direct->total,           \
-                                                 c->cands.as<Cand>(), cap)
-            YB_CUDA(cudaEventRecord(c->ev_scan[0], st));
-            if (v8) YB_GATHER(8); else if (v4) YB_GATHER(4); else YB_GATHER(0);
-#undef YB_GATHER
             YB_CUDA(cudaEventRecord(c->ev_scan[1], st));
             c->scan_timed = true;
         }
@@ -1505,7 +1529,7 @@ static yams_status_t scan_enqueue(Corpus* c, const ScanPlan& p, int64_t* d_out_r
                                                                   p.threshold, d_ex, c->metric, nullptr, p.d_mask, p.mask_ld);
     CertArgs cert{};
     cert.bound = d_bound; cert.eps = c->eps.as<float>(); cert.qnorm = d_qnorm; cert.threshold = p.threshold;
-    cert.metric = c->metric; cert.status = status_of(c); cert.level = 0; cert.nq_total = nq;
+    cert.metric = c->metric; cert.l2_margin = l2_cert_margin(c->dim); cert.status = status_of(c); cert.level = 0; cert.nq_total = nq;
     final_kernel<<<nq, SEL_THREADS, 0, st>>>(d_ex, nullptr, Kp, k, c->rowids.as<int64_t>(), l2 ? 1 : 0, d_out_rowids, d_out_scores,
                                              d_out_counts, d_out_flags, l2 ? INFINITY : -INFINITY, nullptr, cert);
     YB_CUDA(cudaGetLastError());
@@ -1568,7 +1592,7 @@ static yams_status_t exact_all_rows(Corpus* c, const ScanPlan& p, uint32_t q, in
 //   level 2: whatever level 1 cannot certify either (more than ~4000 rows within eps of the k-th score: a corpus of
 //            duplicates) is answered by the exact score of every row.
 static yams_status_t resolve_uncertain(Corpus* c, const ScanPlan& p, const uint32_t* bad, uint32_t n_bad, int64_t* d_out_rowids,
-                                       float* d_out_scores, uint32_t* d_out_counts, uint64_t* d_out_flags) {
+                                       float* d_out_scores, uint32_t* d_out_counts, uint64_t* d_out_flags, uint32_t* out_full) {
     yams_status_t rc;
     cudaStream_t st = c->st;
     const uint64_t n = c->n;
@@ -1613,7 +1637,8 @@ static yams_status_t resolve_uncertain(Corpus* c, const ScanPlan& p, const uint3
                                                                       p.threshold, d_ex1, c->metric, d_qmap, p.d_mask, p.mask_ld);
         CertArgs cert{};
         cert.bound = d_bound1; cert.eps = c->eps2.as<float>(); cert.qnorm = d_qnorm; cert.threshold = p.threshold;
-        cert.metric = c->metric; cert.status = status_of(c); cert.level = 1; cert.nq_total = p.nq;
+        cert.metric = c->metric; cert.l2_margin = l2_cert_margin(c->dim); cert.status = status_of(c); cert.level = 1;
+        cert.nq_total = p.nq;
         final_kernel<<<g, SEL_THREADS, 0, st>>>(d_ex1, d_sel1_n, K1, k, c->rowids.as<int64_t>(), l2 ? 1 : 0, d_out_rowids, d_out_scores,
                                                 d_out_counts, d_out_flags, l2 ? INFINITY : -INFINITY, d_qmap, cert);
         YB_CUDA(cudaGetLastError());
@@ -1625,6 +1650,7 @@ static yams_status_t resolve_uncertain(Corpus* c, const ScanPlan& p, const uint3
     YB_CUDA(cudaStreamSynchronize(st));
     if (n_bad2) {
         n_bad2 = std::min(n_bad2, p.nq);
+        *out_full = n_bad2;
         std::vector<uint32_t> bad2(n_bad2);
         const uint32_t* d_list2 = reinterpret_cast<const uint32_t*>(status_of(c) + 1) + p.nq;
         YB_CUDA(cudaMemcpyAsync(bad2.data(), d_list2, (size_t)n_bad2 * 4, cudaMemcpyDeviceToHost, st));
@@ -1872,13 +1898,17 @@ static yams_status_t finish_scan(yams_b200_corpus* c, const ScanPlan& p, int64_t
                                  uint32_t* out_resolved) {
     const ScanStatus* hs = c->h_pin.as<ScanStatus>();
     if (out_resolved) *out_resolved = 0;
+    c->last_ms[7] = 0.f;
     YB_ARG(hs->n_invalid == 0, "exact vector search requires a finite, non-zero query embedding");
     uint32_t n_bad = std::min(hs->n_bad, p.nq);
     if (n_bad == 0) return YAMS_OK;
     std::vector<uint32_t> bad(reinterpret_cast<const uint32_t*>(hs + 1), reinterpret_cast<const uint32_t*>(hs + 1) + n_bad);
     std::sort(bad.begin(), bad.end());
     if (out_resolved) *out_resolved = n_bad;
-    return resolve_uncertain(c, p, bad.data(), n_bad, d_or, d_os, d_oc, d_of);
+    uint32_t full = 0;
+    yams_status_t rc = resolve_uncertain(c, p, bad.data(), n_bad, d_or, d_os, d_oc, d_of, &full);
+    c->last_ms[7] = (float)full;   // queries answered by the full exact pass (level 2)
+    return rc;
 }
 // candidate sets as a bit matrix [nq][mask_ld * 32] of allowed corpus rows (allowed_offsets[nq + 1] into allowed_rowids)
 static yams_status_t upload_mask(yams_b200_corpus* c, uint32_t nq, const int64_t* allowed_rowids, const uint64_t* allowed_offsets,
@@ -1898,6 +1928,22 @@ static yams_status_t upload_mask(yams_b200_corpus* c, uint32_t nq, const int64_t
     build_mask_kernel<<<grid, 256, 0, c->st>>>(d_allowed, d_offs, nq, c->rowids.as<int64_t>(), c->n, dm, mask_ld);
     *out_mask = dm;
     *out_mask_ld = mask_ld;
+    return YAMS_OK;
+}
+
+// candidate sets as ascending device lists for the direct path (gather_score_kernel); they live in c->mask until the scan is done
+static yams_status_t upload_direct_lists(yams_b200_corpus* c, uint32_t nq, const int64_t* allowed_rowids, const uint64_t* allowed_offsets,
+                                         DirectLists* lists) {
+    yams_status_t rc;
+    const uint64_t total = allowed_offsets[nq];
+    if ((rc = c->mask.reserve((size_t)total * 8 + (size_t)(nq + 1) * 8 + 64)) != YAMS_OK) return rc;
+    int64_t* d_allowed = c->mask.as<int64_t>();
+    uint64_t* d_offs = reinterpret_cast<uint64_t*>(d_allowed + total);
+    if (total) YB_CUDA(cudaMemcpyAsync(d_allowed, allowed_rowids, (size_t)total * 8, cudaMemcpyHostToDevice, c->st));
+    YB_CUDA(cudaMemcpyAsync(d_offs, allowed_offsets, (size_t)(nq + 1) * 8, cudaMemcpyHostToDevice, c->st));
+    lists->d_allowed = d_allowed;
+    lists->d_offsets = d_offs;
+    lists->total = total;
     return YAMS_OK;
 }
 
@@ -1958,15 +2004,7 @@ yams_status_t yams_b200_search(yams_b200_corpus* c, const float* queries, uint32
         }
     }
     if (direct) {
-        const uint64_t total = allowed_offsets[nq];
-        if ((rc = c->mask.reserve((size_t)total * 8 + (size_t)(nq + 1) * 8 + 64)) != YAMS_OK) return rc;
-        int64_t* d_allowed = c->mask.as<int64_t>();
-        uint64_t* d_offs = reinterpret_cast<uint64_t*>(d_allowed + total);
-        if (total) YB_CUDA(cudaMemcpyAsync(d_allowed, allowed_rowids, (size_t)total * 8, cudaMemcpyHostToDevice, c->st));
-        YB_CUDA(cudaMemcpyAsync(d_offs, allowed_offsets, (size_t)(nq + 1) * 8, cudaMemcpyHostToDevice, c->st));
-        lists.d_allowed = d_allowed;
-        lists.d_offsets = d_offs;
-        lists.total = total;
+        if ((rc = upload_direct_lists(c, nq, allowed_rowids, allowed_offsets, &lists)) != YAMS_OK) return rc;
         plan.direct = &lists;
     } else if (allowed_offsets && c->n) {
         if ((rc = upload_mask(c, nq, allowed_rowids, allowed_offsets, &plan.d_mask, &plan.mask_ld)) != YAMS_OK) return rc;
@@ -1991,7 +2029,14 @@ yams_status_t yams_b200_search(yams_b200_corpus* c, const float* queries, uint32
     cudaEventElapsedTime(&c->last_ms[1], c->ev[1], c->ev[2]);
     cudaEventElapsedTime(&c->last_ms[2], c->ev[0], c->ev[2]);
     uint32_t resolved = 0;
-    rc = finish_scan(c, plan, d_or, d_os, d_oc, d_of, &resolved);
+    const ScanStatus* hs = c->h_pin.as<ScanStatus>();
+    if (plan.direct && hs->n_bad && hs->n_invalid == 0) {
+        // The direct path scored the listed rows without a bit mask, but the exhaustive levels score every row: they need the
+        // candidate sets as a mask.  The scan is finished (copy_out synchronised), so its lists in c->mask may be overwritten.
+        plan.direct = nullptr;
+        rc = upload_mask(c, nq, allowed_rowids, allowed_offsets, &plan.d_mask, &plan.mask_ld);
+    }
+    if (rc == YAMS_OK) rc = finish_scan(c, plan, d_or, d_os, d_oc, d_of, &resolved);
     c->last_ms[6] = (float)resolved;
     if (rc != YAMS_OK) {
         for (uint32_t q = 0; q < nq; ++q) out_counts[q] = 0;
@@ -2275,19 +2320,155 @@ yams_status_t yams_b200_debug_stage1_candidates(yams_b200_corpus* c, const float
     fill_stage1_common(c, a, nq);
     a.row_start = row_start; a.row_stride = row_stride; a.nrows = nrows;
     a.tau = c->tau.as<float>(); a.cands = c->cands.as<Cand>(); a.cap = cap; a.counts = c->counts.as<uint32_t>();
-    if (allowed_offsets && (rc = upload_mask(c, nq, allowed_rowids, allowed_offsets, &a.mask, &a.mask_ld)) != YAMS_OK) return rc;
-    if (engine == 1) {
-        rc = stage1_wgmma(c, a, true, c->st);
-    } else {
-        rc = stage1_cuda_core(a, true, c->st);
+    if (engine == 2) {
+        // the direct path's engine: every listed rowid is scored, tau and the row range do not apply
+        YB_ARG(allowed_offsets && c->metric == YAMS_B200_COSINE, "engine 2 scores cosine candidate-set lists");
+        for (uint32_t q = 0; q < nq; ++q) {
+            YB_ARG(allowed_offsets[q + 1] >= allowed_offsets[q] && allowed_offsets[q + 1] - allowed_offsets[q] <= cap,
+                   "a list is longer than cap");
+            for (uint64_t i = allowed_offsets[q] + 1; i < allowed_offsets[q + 1]; ++i)
+                YB_ARG(allowed_rowids[i - 1] <= allowed_rowids[i], "engine 2 takes ascending lists");
+        }
+        DirectLists lists;
+        if ((rc = upload_direct_lists(c, nq, allowed_rowids, allowed_offsets, &lists)) != YAMS_OK) return rc;
+        list_lengths_kernel<<<(nq + 255) / 256, 256, 0, c->st>>>(lists.d_offsets, nq, a.counts);
+        rc = gather_scores(c, lists, nq, a.q32, a.qinv, a.cands, cap, c->st);
         eps_cc_kernel<<<(nq + 255) / 256, 256, 0, c->st>>>(reinterpret_cast<double*>(c->misc.as<uint8_t>()), nq, c->dim, c->metric, c->r_max,
                                                            c->eps.as<float>(), 0);
+    } else {
+        if (allowed_offsets && (rc = upload_mask(c, nq, allowed_rowids, allowed_offsets, &a.mask, &a.mask_ld)) != YAMS_OK) return rc;
+        if (engine == 1) {
+            rc = stage1_wgmma(c, a, true, c->st);
+        } else {
+            rc = stage1_cuda_core(a, true, c->st);
+            eps_cc_kernel<<<(nq + 255) / 256, 256, 0, c->st>>>(reinterpret_cast<double*>(c->misc.as<uint8_t>()), nq, c->dim, c->metric,
+                                                               c->r_max, c->eps.as<float>(), 0);
+        }
     }
     if (rc != YAMS_OK) return rc;
     YB_CUDA(cudaMemcpyAsync(out_counts, c->counts.p, (size_t)nq * 4, cudaMemcpyDeviceToHost, c->st));
     if (cb) YB_CUDA(cudaMemcpyAsync(out_cands, c->cands.p, cb, cudaMemcpyDeviceToHost, c->st));
     YB_CUDA(cudaStreamSynchronize(c->st));
     return YAMS_OK;
+}
+
+// diagnostics: the top-K selection (topk_select_kernel) on caller-supplied scores, see include/yams_b200.h
+yams_status_t yams_b200_debug_select(yams_b200_corpus* c, uint32_t nq, const float* dense, uint64_t ld, uint64_t len, uint64_t row_start,
+                                     uint64_t row_stride, uint32_t dense_shift, const void* cands, const uint32_t* counts, uint32_t cap,
+                                     const float* tau, uint32_t K, int tau_only, float tau_margin, int fast_tau, void* out_sel,
+                                     uint32_t* out_n, float* out_bound) {
+    YB_ARG(c && nq > 0 && out_bound && (tau_only || (out_sel && out_n)), "bad argument");
+    YB_ARG(dense ? (ld >= len && dense_shift < 4) : (counts && (cands || cap == 0)), "bad input");
+    YB_ARG(tau_only || K <= SEL_MAXK, "K > 4096");
+    std::lock_guard<std::mutex> corpus_lock(c->mu);
+    YB_BIND(c);
+    c->pending.active = false;
+    yams_status_t rc;
+    cudaStream_t st = c->st;
+    SelectIn in{};
+    if (dense) {
+        const size_t nb = (size_t)nq * ld * 4;
+        if ((rc = c->dense.reserve(nb + 16)) != YAMS_OK) return rc;
+        float* d = c->dense.as<float>() + dense_shift;    // the allocation is 256-byte aligned: dense_shift sets the alignment
+        if (nb) YB_CUDA(cudaMemcpyAsync(d, dense, nb, cudaMemcpyHostToDevice, st));
+        in.dense = d; in.ld = ld; in.dense_len = len; in.row_start = row_start; in.row_stride = row_stride;
+    } else {
+        const size_t cb = (size_t)nq * cap * sizeof(Cand);
+        if ((rc = c->cands.reserve(cb + 8)) != YAMS_OK) return rc;
+        if ((rc = c->counts.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
+        if (cb) YB_CUDA(cudaMemcpyAsync(c->cands.p, cands, cb, cudaMemcpyHostToDevice, st));
+        YB_CUDA(cudaMemcpyAsync(c->counts.p, counts, (size_t)nq * 4, cudaMemcpyHostToDevice, st));
+        in.cands = c->cands.as<Cand>(); in.counts = c->counts.as<uint32_t>(); in.cap = cap;
+        if (tau) {
+            if ((rc = c->tau.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
+            YB_CUDA(cudaMemcpyAsync(c->tau.p, tau, (size_t)nq * 4, cudaMemcpyHostToDevice, st));
+            in.tau = c->tau.as<float>();
+        }
+    }
+    in.tau_margin = tau_margin;
+    in.fast_tau = fast_tau;
+    if ((rc = c->bound.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
+    float* d_bound = c->bound.as<float>();
+    if (tau_only) {
+        topk_select_kernel<<<nq, SEL_THREADS, 0, st>>>(in, K, 1, d_bound, nullptr, nullptr, nullptr);
+    } else {
+        if ((rc = c->sel.reserve((size_t)nq * K * sizeof(Cand) + (size_t)nq * 4 + 8)) != YAMS_OK) return rc;
+        Cand* d_sel = c->sel.as<Cand>();
+        uint32_t* d_n = reinterpret_cast<uint32_t*>(d_sel + (size_t)nq * K);
+        topk_select_kernel<<<nq, SEL_THREADS, 0, st>>>(in, K, 0, nullptr, d_sel, d_n, d_bound);
+        if (K) YB_CUDA(cudaMemcpyAsync(out_sel, d_sel, (size_t)nq * K * sizeof(Cand), cudaMemcpyDeviceToHost, st));
+        YB_CUDA(cudaMemcpyAsync(out_n, d_n, (size_t)nq * 4, cudaMemcpyDeviceToHost, st));
+    }
+    YB_CUDA(cudaGetLastError());
+    YB_CUDA(cudaMemcpyAsync(out_bound, d_bound, (size_t)nq * 4, cudaMemcpyDeviceToHost, st));
+    YB_CUDA(cudaStreamSynchronize(st));
+    return YAMS_OK;
+}
+
+// diagnostics: the final ordering and the exactness certificate (final_kernel) on caller-supplied exact scores, see
+// include/yams_b200.h
+yams_status_t yams_b200_debug_final(yams_b200_corpus* c, uint32_t nq, uint32_t Kp, uint32_t k, const void* exact, const uint32_t* ex_n,
+                                    const float* bound, const float* eps, const double* qnorm, float threshold, int metric, int level,
+                                    int64_t* out_rowids, float* out_scores, uint32_t* out_counts, uint64_t* out_flags,
+                                    uint32_t* out_queued, uint32_t* out_n_queued) {
+    YB_TRY
+    YB_ARG(c && nq > 0 && Kp > 0 && Kp <= SEL_MAXK && k > 0 && k <= SEL_MAXK && exact && bound && eps && qnorm, "bad argument");
+    YB_ARG(out_rowids && out_scores && out_counts && out_flags && out_queued && out_n_queued, "null output");
+    YB_ARG(metric == YAMS_B200_COSINE || metric == YAMS_B200_L2, "unknown metric");
+    std::lock_guard<std::mutex> corpus_lock(c->mu);
+    YB_BIND(c);
+    c->pending.active = false;
+    const Exact* ex = static_cast<const Exact*>(exact);
+    for (uint32_t b = 0; b < nq; ++b) {   // entries final_kernel reads must index the rowid table
+        const uint32_t m = ex_n ? std::min(ex_n[b], Kp) : Kp;
+        for (uint32_t i = 0; i < m; ++i) {
+            const Exact& e = ex[(size_t)b * Kp + i];
+            YB_ARG(e.sim != e.sim || e.row < c->n, "row out of range");
+        }
+    }
+    yams_status_t rc;
+    cudaStream_t st = c->st;
+    const size_t eb = (size_t)nq * Kp * sizeof(Exact);
+    if ((rc = c->outbuf.reserve(eb + (size_t)nq * 4 + 8)) != YAMS_OK) return rc;
+    if ((rc = c->bound.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
+    if ((rc = c->eps.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
+    if ((rc = c->misc.reserve((size_t)nq * 8)) != YAMS_OK) return rc;
+    if ((rc = c->status.reserve(sizeof(ScanStatus) + (size_t)nq * 8)) != YAMS_OK) return rc;
+    if ((rc = c->dout.reserve((size_t)nq * k * 12 + (size_t)nq * 12 + 64)) != YAMS_OK) return rc;
+    Exact* d_ex = c->outbuf.as<Exact>();
+    uint32_t* d_ex_n = reinterpret_cast<uint32_t*>(d_ex + (size_t)nq * Kp);
+    YB_CUDA(cudaMemcpyAsync(d_ex, ex, eb, cudaMemcpyHostToDevice, st));
+    if (ex_n) YB_CUDA(cudaMemcpyAsync(d_ex_n, ex_n, (size_t)nq * 4, cudaMemcpyHostToDevice, st));
+    YB_CUDA(cudaMemcpyAsync(c->bound.p, bound, (size_t)nq * 4, cudaMemcpyHostToDevice, st));
+    YB_CUDA(cudaMemcpyAsync(c->eps.p, eps, (size_t)nq * 4, cudaMemcpyHostToDevice, st));
+    YB_CUDA(cudaMemcpyAsync(c->misc.p, qnorm, (size_t)nq * 8, cudaMemcpyHostToDevice, st));
+    YB_CUDA(cudaMemsetAsync(c->status.p, 0, sizeof(ScanStatus) + (size_t)nq * 8, st));
+    int64_t* d_or = c->dout.as<int64_t>();
+    uint64_t* d_of = reinterpret_cast<uint64_t*>(d_or + (size_t)nq * k);
+    float* d_os = reinterpret_cast<float*>(d_of + nq);
+    uint32_t* d_oc = reinterpret_cast<uint32_t*>(d_os + (size_t)nq * k);
+    const bool l2 = metric == YAMS_B200_L2;
+    CertArgs cert{};
+    cert.bound = c->bound.as<float>(); cert.eps = c->eps.as<float>(); cert.qnorm = reinterpret_cast<const double*>(c->misc.p);
+    cert.threshold = threshold; cert.metric = metric; cert.l2_margin = l2_cert_margin(c->dim); cert.status = status_of(c);
+    cert.level = level; cert.nq_total = nq;
+    final_kernel<<<nq, SEL_THREADS, 0, st>>>(d_ex, ex_n ? d_ex_n : nullptr, Kp, k, c->rowids.as<int64_t>(), l2 ? 1 : 0, d_or, d_os, d_oc, d_of,
+                                             l2 ? INFINITY : -INFINITY, nullptr, cert);
+    YB_CUDA(cudaGetLastError());
+    std::vector<uint32_t> h_status(sizeof(ScanStatus) / 4 + (size_t)nq * 2);
+    YB_CUDA(cudaMemcpyAsync(out_rowids, d_or, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, st));
+    YB_CUDA(cudaMemcpyAsync(out_scores, d_os, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, st));
+    YB_CUDA(cudaMemcpyAsync(out_counts, d_oc, (size_t)nq * 4, cudaMemcpyDeviceToHost, st));
+    YB_CUDA(cudaMemcpyAsync(out_flags, d_of, (size_t)nq * 8, cudaMemcpyDeviceToHost, st));
+    YB_CUDA(cudaMemcpyAsync(h_status.data(), c->status.p, h_status.size() * 4, cudaMemcpyDeviceToHost, st));
+    YB_CUDA(cudaStreamSynchronize(st));
+    const ScanStatus* hs = reinterpret_cast<const ScanStatus*>(h_status.data());
+    const uint32_t nqd = std::min(level == 0 ? hs->n_bad : hs->n_bad2, nq);
+    const uint32_t* list = h_status.data() + sizeof(ScanStatus) / 4 + (level == 0 ? 0 : nq);
+    for (uint32_t i = 0; i < nqd; ++i) out_queued[i] = list[i];
+    *out_n_queued = nqd;
+    return YAMS_OK;
+    YB_CATCH
 }
 
 // bench / test utility: n synthetic rows of the SURVEY.md §8d generator (bit-identical to oracle yo_gen_rows_f32) as fp32
