@@ -447,6 +447,36 @@ YAMS_B200_API yams_status_t yams_b200_pq_build(yams_b200_corpus* c, uint32_t m, 
 YAMS_B200_API yams_status_t yams_b200_pq_search(yams_b200_pq* pq, const float* queries, uint32_t nq, uint32_t k,
                                                 uint32_t rerank_factor, float threshold, int64_t* out_rowids,
                                                 float* out_scores, uint32_t* out_counts, uint64_t* out_flags);
+/* simeonPqSearchUnlocked with candidateHashes, VectorTopK (sqlite_vec_backend.cpp:3910-4051): query i only scores the indexed
+ * rows of allowed_rowids[allowed_offsets[i] .. allowed_offsets[i+1]) (the format of yams_b200_search, any order; a rowid listed
+ * twice counts once; rowids unknown to the corpus or left out of the index are ignored).  candidateCount = the distinct indexed
+ * candidates (0: no results), approxK = min(candidateCount, max(k, k * rerank_factor)) <= 1024.  After the ADC scores the chain
+ * is pq_search's; with every indexed row in every list the results and flags are bit-identical to pq_search. */
+YAMS_B200_API yams_status_t yams_b200_pq_search_candidates(yams_b200_pq* pq, const float* queries, uint32_t nq, uint32_t k,
+                                                           uint32_t rerank_factor, float threshold,
+                                                           const int64_t* allowed_rowids, const uint64_t* allowed_offsets,
+                                                           int64_t* out_rowids, float* out_scores, uint32_t* out_counts,
+                                                           uint64_t* out_flags);
+/* CandidateFilterMode::DocumentTopK (vector_database.cpp:553-569): the k best DOCUMENTS of every query, each represented by its
+ * best row (retainBestRecordPerDocument, sqlite_vec_backend.cpp:86-125).  Document d is the rows
+ * doc_rowids[doc_offsets[d] .. doc_offsets[d+1]) in the caller's chunk order; query q considers documents
+ * query_docs[q] .. query_docs[q+1] (nq + 1 entries) in the caller's document order.  Callers pass documents sorted by
+ * document_hash and rows by chunk_id: the position tie-breaks below then are the reference's.
+ *   pq == NULL  the exact fallback (:1508-1518, :3882-3893): every candidate row scored like yams_b200_search_all_matching
+ *               (skip rules, threshold); a non-finite / zero query makes the call return YAMS_ERR_INVALID_ARG.
+ *   pq != NULL  the PQ engine's DocumentTopK branch (:3957-3958, :4022-4048): every candidate row IN THE INDEX re-scored like
+ *               pq_search's rerank (NaN and sim < threshold dropped); a query that cannot be normalised gets count 0.  The
+ *               index must be current and belong to c.
+ * A document's best row: (sim desc, position in the document asc); documents without a surviving row are absent; documents
+ * ordered (best sim desc, document index asc), k <= 4096 returned per query.  Outputs Q x k: out_docs = document index,
+ * out_rowids / out_scores = its best row and score; unused slots -1 / -1 / 0.  k == 0: all counts 0.  Unknown rowids are
+ * ignored.  YAMS_ERR_INVALID_ARG before any device work for non-monotone offsets, a document of 2^32 - 1 rows or more, or a
+ * rowid that appears twice among one query's documents. */
+YAMS_B200_API yams_status_t yams_b200_search_documents(yams_b200_corpus* c, yams_b200_pq* pq, const float* queries, uint32_t nq,
+                                                       uint32_t k, float threshold, const int64_t* doc_rowids,
+                                                       const uint64_t* doc_offsets, const uint64_t* query_docs,
+                                                       int64_t* out_docs, int64_t* out_rowids, float* out_scores,
+                                                       uint32_t* out_counts);
 /* the index content, for parity checks: out_codes [n_indexed][m], out_rowids [n_indexed] (both nullable), *out_n */
 YAMS_B200_API yams_status_t yams_b200_pq_codes(yams_b200_pq* pq, uint8_t* out_codes, int64_t* out_rowids,
                                                uint64_t* out_n);
@@ -536,6 +566,14 @@ typedef struct yams_vector_scan_v1 {
                                uint32_t rerank_factor, float threshold, int64_t* out_rowids, float* out_scores,
                                uint32_t* out_counts, uint64_t* out_flags);
     void (*pq_destroy)(yams_b200_pq* pq);
+    yams_status_t (*pq_search_candidates)(yams_b200_pq* pq, const float* queries, uint32_t nq, uint32_t k,
+                                          uint32_t rerank_factor, float threshold, const int64_t* allowed_rowids,
+                                          const uint64_t* allowed_offsets, int64_t* out_rowids, float* out_scores,
+                                          uint32_t* out_counts, uint64_t* out_flags);
+    yams_status_t (*search_documents)(yams_b200_corpus* c, yams_b200_pq* pq, const float* queries, uint32_t nq,
+                                      uint32_t k, float threshold, const int64_t* doc_rowids, const uint64_t* doc_offsets,
+                                      const uint64_t* query_docs, int64_t* out_docs, int64_t* out_rowids,
+                                      float* out_scores, uint32_t* out_counts);
 } yams_vector_scan_v1;
 
 /* ---- sqlite-vec-cpp C API kept bit-for-bit in signature and error behaviour ------------------

@@ -137,6 +137,10 @@ SYMBOLS = {
     "yams_b200_simeon_destroy": (None, [C.c_void_p]),
     "yams_b200_pq_build": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, f32p, u64p, C.POINTER(C.c_void_p)]),
     "yams_b200_pq_search": (C.c_int, [C.c_void_p, f32p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_float, i64p, f32p, u32p, u64p]),
+    "yams_b200_pq_search_candidates": (C.c_int, [C.c_void_p, f32p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_float, i64p, u64p, i64p, f32p,
+                                                 u32p, u64p]),
+    "yams_b200_search_documents": (C.c_int, [C.c_void_p, C.c_void_p, f32p, C.c_uint32, C.c_uint32, C.c_float, i64p, u64p, u64p, i64p, i64p,
+                                             f32p, u32p]),
     "yams_b200_pq_codes": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, u64p]),
     "yams_b200_pq_destroy": (None, [C.c_void_p]),
     "yams_b200_debug_last_eps": (C.c_int, [C.c_void_p, C.c_uint32, f32p]),
@@ -470,6 +474,48 @@ class Corpus:
         _check(lib().yams_b200_search_device_finish(self._h, C.byref(n)), "search_device_finish")
         return n.value
 
+    def search_documents(self, queries, k: int, docs, threshold: float = -1.0, pq: Optional["PqIndex"] = None):
+        """CandidateFilterMode::DocumentTopK: docs[q] is query q's list of documents, each an array of rowids in chunk order
+        (pass documents sorted by document hash: ties between documents go to the earlier one, ties inside a document to the
+        earlier row).  pq=None scores every row exactly (the exact fallback); with a PqIndex, the rows in the index are
+        re-scored like its rerank.  -> (doc i64[Q,k] = position in docs[q], rowids i64[Q,k] = the document's best row,
+        scores f32[Q,k], counts u32[Q]); unused slots -1 / -1 / 0."""
+        nq = len(docs)
+        qdocs = np.zeros(nq + 1, dtype=np.uint64)
+        qdocs[1:] = np.cumsum([len(ds) for ds in docs])
+        flat = [np.asarray(r, dtype=np.int64).reshape(-1) for ds in docs for r in ds]
+        doffs = np.zeros(len(flat) + 1, dtype=np.uint64)
+        doffs[1:] = np.cumsum([len(r) for r in flat])
+        rid = np.concatenate(flat) if int(doffs[-1]) else np.zeros(0, dtype=np.int64)
+        d, r, s, cnt = self.search_documents_csr(queries, k, rid, doffs, qdocs, threshold, pq)
+        local = np.where(d >= 0, d - qdocs[:-1, None].astype(np.int64), -1)
+        return local, r, s, cnt
+
+    def search_documents_csr(self, queries, k: int, doc_rowids, doc_offsets, query_docs, threshold: float = -1.0,
+                             pq: Optional["PqIndex"] = None):
+        """search_documents on the C ABI's layout: document d = doc_rowids[doc_offsets[d] .. doc_offsets[d+1]), query q's documents
+        query_docs[q] .. query_docs[q+1].  -> (global document index i64[Q,k], rowids, scores, counts)"""
+        q = np.ascontiguousarray(queries, dtype=np.float32)
+        if q.ndim == 1:
+            q = q[None, :]
+        nq = q.shape[0]
+        qdocs = np.ascontiguousarray(query_docs, dtype=np.uint64)
+        doffs = np.ascontiguousarray(doc_offsets, dtype=np.uint64)
+        assert len(qdocs) == nq + 1
+        rid = np.ascontiguousarray(doc_rowids, dtype=np.int64)
+        if rid.size == 0:
+            rid = np.zeros(1, dtype=np.int64)
+        kk = max(k, 1)
+        out_d = np.full((nq, kk), -1, dtype=np.int64)
+        out_r = np.full((nq, kk), -1, dtype=np.int64)
+        out_s = np.zeros((nq, kk), dtype=np.float32)
+        out_c = np.zeros(nq, dtype=np.uint32)
+        _check(lib().yams_b200_search_documents(self._h, pq.handle if pq is not None else None, q.ctypes.data_as(f32p), nq, k, threshold,
+                                                rid.ctypes.data_as(i64p), doffs.ctypes.data_as(u64p), qdocs.ctypes.data_as(u64p),
+                                                out_d.ctypes.data_as(i64p), out_r.ctypes.data_as(i64p), out_s.ctypes.data_as(f32p),
+                                                out_c.ctypes.data_as(u32p)), "search_documents")
+        return out_d[:, :k], out_r[:, :k], out_s[:, :k], out_c
+
     def search_exhaustive(self, queries: np.ndarray, k: int, threshold: float = -1.0):
         """The library's own exhaustive reference (exact score of every row + global sort); same outputs as search."""
         q = np.ascontiguousarray(queries, dtype=np.float32)
@@ -665,7 +711,13 @@ class PqIndex:
         _check(lib().yams_b200_pq_codes(self._h, codes.ctypes.data, rowids.ctypes.data, C.byref(n)), "pq_codes")
         return codes[:n.value], rowids[:n.value]
 
-    def search(self, queries, k: int, rerank_factor: int = 2, threshold: float = 0.0):
+    @property
+    def handle(self):
+        return self._h
+
+    def search(self, queries, k: int, rerank_factor: int = 2, threshold: float = 0.0, allowed=None):
+        """-> (rowids i64[Q,k], scores f32[Q,k], counts u32[Q], flags u64[Q]).  allowed: optional list (len Q) of rowid arrays
+        (any order): query i only scores the indexed rows of allowed[i] (simeonPqSearchUnlocked with candidate documents)."""
         q = np.ascontiguousarray(queries, dtype=np.float32)
         if q.ndim == 1:
             q = q[None, :]
@@ -674,8 +726,19 @@ class PqIndex:
         out_s = np.zeros((nq, max(k, 1)), dtype=np.float32)
         out_c = np.zeros(nq, dtype=np.uint32)
         out_f = np.zeros(nq, dtype=np.uint64)
-        _check(lib().yams_b200_pq_search(self._h, q.ctypes.data_as(f32p), nq, k, rerank_factor, threshold, out_r.ctypes.data_as(i64p),
-                                         out_s.ctypes.data_as(f32p), out_c.ctypes.data_as(u32p), out_f.ctypes.data_as(u64p)), "pq_search")
+        if allowed is None:
+            _check(lib().yams_b200_pq_search(self._h, q.ctypes.data_as(f32p), nq, k, rerank_factor, threshold, out_r.ctypes.data_as(i64p),
+                                             out_s.ctypes.data_as(f32p), out_c.ctypes.data_as(u32p), out_f.ctypes.data_as(u64p)), "pq_search")
+        else:
+            assert len(allowed) == nq
+            offs = np.zeros(nq + 1, dtype=np.uint64)
+            offs[1:] = np.cumsum([len(a) for a in allowed])
+            al = np.ascontiguousarray(np.concatenate([np.asarray(a, dtype=np.int64).reshape(-1) for a in allowed])
+                                      if nq and int(offs[-1]) else np.zeros(1, dtype=np.int64), dtype=np.int64)
+            _check(lib().yams_b200_pq_search_candidates(self._h, q.ctypes.data_as(f32p), nq, k, rerank_factor, threshold,
+                                                        al.ctypes.data_as(i64p), offs.ctypes.data_as(u64p), out_r.ctypes.data_as(i64p),
+                                                        out_s.ctypes.data_as(f32p), out_c.ctypes.data_as(u32p), out_f.ctypes.data_as(u64p)),
+                   "pq_search_candidates")
         return out_r[:, :k], out_s[:, :k], out_c, out_f
 
     def close(self):

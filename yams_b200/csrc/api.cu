@@ -202,6 +202,8 @@ int yams_plugin_init(const char* config_json, const void* host_context) {
     g_scan_vt.pq_build = yams_b200_pq_build;
     g_scan_vt.pq_search = yams_b200_pq_search;
     g_scan_vt.pq_destroy = yams_b200_pq_destroy;
+    g_scan_vt.pq_search_candidates = yams_b200_pq_search_candidates;
+    g_scan_vt.search_documents = yams_b200_search_documents;
     DeviceCtx* dev = nullptr;
     if (ensure_device(&dev) != YAMS_OK) return YAMS_PLUGIN_ERR_INIT_FAILED;  // no CPU fallback
     g_inited = true;

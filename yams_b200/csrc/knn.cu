@@ -22,18 +22,15 @@
 #include <new>
 #include <vector>
 
+#include "cosine.cuh"
 #include "knn.cuh"
 #include "ref_order.cuh"
 
 namespace yb {
 
 // ---------------------------------------------------------------------------------------------------
-// element helpers
+// element helpers (load_elem: cosine.cuh)
 // ---------------------------------------------------------------------------------------------------
-__device__ __forceinline__ float load_elem(const void* rows, int dtype, uint64_t idx) {
-    if (dtype == YAMS_B200_F16) return __half2float(reinterpret_cast<const __half*>(rows)[idx]);
-    return reinterpret_cast<const float*>(rows)[idx];
-}
 
 // reference truncating fp32 -> fp16 (utils/float16.hpp:20-40), restated on integer bits
 __host__ __device__ __forceinline__ uint16_t f16_from_float_trunc(float f) {
@@ -347,16 +344,7 @@ yams_status_t stage1_cuda_core(const Stage1Args& a, bool filter, cudaStream_t st
 // ---------------------------------------------------------------------------------------------------
 // top-K selection (one CTA per query): radix select on monotone keys, gather, bitonic sort
 // ---------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t fkey(float f) {
-    if (f != f) return 0u;  // NaN ranks last
-    uint32_t b = __float_as_uint(f);
-    return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-}
-__device__ __forceinline__ float fkey_inv(uint32_t k) {
-    uint32_t b = (k & 0x80000000u) ? (k & 0x7FFFFFFFu) : ~k;
-    return __uint_as_float(b);
-}
-
+// fkey / fkey_inv: cosine.cuh
 constexpr int SEL_THREADS = 256;
 constexpr int SEL_MAXK = 4096;       // survivors per query the select / final kernels can order in shared memory
 
@@ -730,61 +718,10 @@ __global__ void rescore_kernel(const void* __restrict__ rows, int dtype, uint32_
                 e.row = row;
             }
         } else {
-            double norm_sq = 0.0, dot = 0.0;
-            bool finite = true;
-            // same element order as the reference's loop; only the loads are widened (16-byte row and query chunks)
-            uint32_t c = 0;
-            if (dtype == YAMS_B200_F16 && d % 8 == 0) {
-                const uint4* rp = reinterpret_cast<const uint4*>(static_cast<const __half*>(rows) + base);
-                const float4* qp = reinterpret_cast<const float4*>(qv);
-                for (; c < d; c += 8) {
-                    const uint4 raw = __ldg(rp + (c >> 3));
-                    const float4 q0 = __ldg(qp + (c >> 2)), q1 = __ldg(qp + (c >> 2) + 1);
-                    const __half2* h2 = reinterpret_cast<const __half2*>(&raw);
-                    const float2 f0 = __half22float2(h2[0]), f1 = __half22float2(h2[1]), f2 = __half22float2(h2[2]), f3 = __half22float2(h2[3]);
-                    const float rv[8] = {f0.x, f0.y, f1.x, f1.y, f2.x, f2.y, f3.x, f3.y};
-                    const float qq[8] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w};
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) {
-                        if (!isfinite(rv[e])) finite = false;
-                        const double sv = (double)rv[e];
-                        norm_sq += sv * sv;
-                        dot += sv * (double)qq[e];
-                    }
-                }
-            } else if (dtype == YAMS_B200_F32 && d % 4 == 0) {
-                const float4* rp = reinterpret_cast<const float4*>(static_cast<const float*>(rows) + base);
-                const float4* qp = reinterpret_cast<const float4*>(qv);
-                for (; c < d; c += 4) {
-                    const float4 r4 = __ldg(rp + (c >> 2)), q4 = __ldg(qp + (c >> 2));
-                    const float rv[4] = {r4.x, r4.y, r4.z, r4.w};
-                    const float qq[4] = {q4.x, q4.y, q4.z, q4.w};
-#pragma unroll
-                    for (int e = 0; e < 4; ++e) {
-                        if (!isfinite(rv[e])) finite = false;
-                        const double sv = (double)rv[e];
-                        norm_sq += sv * sv;
-                        dot += sv * (double)qq[e];
-                    }
-                }
-            }
-            for (; c < d; ++c) {
-                float v = load_elem(rows, dtype, base + c);
-                if (!isfinite(v)) { finite = false; break; }
-                double sv = (double)v, qd = (double)qv[c];
-                norm_sq += sv * sv;
-                dot += sv * qd;
-            }
-            if (finite && norm_sq > 1e-12) {
-                double denom = sqrt(norm_sq) * qnorm[q];
-                double simd = denom > 0.0 ? dot / denom : 0.0;
-                if (isfinite(simd)) {
-                    float sim = (float)simd;
-                    if (!(sim < threshold)) {
-                        e.sim = sim;
-                        e.row = row;
-                    }
-                }
+            float sim;
+            if (exact_cosine_sim(rows, dtype, d, row, qv, qnorm[q], threshold, &sim)) {
+                e.sim = sim;
+                e.row = row;
             }
         }
     }
@@ -1548,6 +1485,16 @@ void launch_final_plain(const void* exact, uint32_t Kp, uint32_t k, uint32_t nq,
     CertArgs cert{};   // status == nullptr: no certificate (the caller's survivors are what the reference re-ranks, too)
     final_kernel<<<nq, SEL_THREADS, 0, st>>>(static_cast<const Exact*>(exact), nullptr, Kp, k, rowids, 0, out_rowids, out_scores, out_counts,
                                              out_flags, -INFINITY, nullptr, cert);
+}
+// rowids -> corpus rows (out[i].row, 0xFFFFFFFF for unknown rowids), any order
+void launch_map_rowids(const int64_t* rowids_in, uint64_t n_in, const int64_t* corpus_rowids, uint64_t n, Cand* out, cudaStream_t st) {
+    if (n_in) map_rowids_kernel<<<(unsigned)std::min<uint64_t>((n_in + 255) / 256, 65535), 256, 0, st>>>(rowids_in, n_in, corpus_rowids, n, out);
+}
+// the search's query preparation (cosine): qnorm[q] = sqrt of the sequential double sum of squares; the first uint32 of the
+// zeroed 16-byte block `status` counts the queries the reference rejects (non-finite, |q|^2 < 1e-10)
+void launch_query_prep(const float* q, uint32_t nq, uint32_t d, double* qnorm, float* qinv, void* status, cudaStream_t st) {
+    query_prep_kernel<<<(nq + QP_THREADS - 1) / QP_THREADS, QP_THREADS, 0, st>>>(q, nq, d, qnorm, qinv, YAMS_B200_COSINE,
+                                                                                static_cast<ScanStatus*>(status));
 }
 
 // Level 2: exact score of EVERY row for one query (the reference's own loop, row-parallel) + a global sort.

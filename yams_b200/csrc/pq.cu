@@ -26,6 +26,7 @@
 #include <new>
 #include <vector>
 
+#include "cosine.cuh"
 #include "knn.cuh"
 
 namespace yb {
@@ -173,7 +174,27 @@ __global__ void __launch_bounds__(256) pq_lut_kernel(const float* __restrict__ q
     }
 }
 
-// ADC scan: CTA (tile, q).  score = sequential float sum of LUT[mi][code[mi]] (inner_product_from_lut, pq.cpp:50-57);
+// inner_product_from_lut (pq.cpp:50-57): the sequential float sum of LUT[mi][code[mi]] over the row's m code bytes.  The ADC
+// scan and the candidate gather both call this one function, so their scores are the same floats.  vec: m % 16 == 0 (the
+// code row is then 16-byte aligned and read 16 bytes at a time).
+__device__ __forceinline__ float pq_adc_sum(const uint8_t* __restrict__ cd, const float* __restrict__ lut, uint32_t m, uint32_t k, bool vec) {
+    float acc = 0.f;
+    if (vec) {
+        for (uint32_t mi = 0; mi < m; mi += 16) {
+            const uint4 w = *reinterpret_cast<const uint4*>(cd + mi);
+            const uint32_t ws[4] = {w.x, w.y, w.z, w.w};
+#pragma unroll
+            for (int u = 0; u < 4; ++u)
+#pragma unroll
+                for (int b = 0; b < 4; ++b) acc = __fadd_rn(acc, lut[(mi + u * 4 + b) * k + ((ws[u] >> (8 * b)) & 0xFFu)]);
+        }
+    } else {
+        for (uint32_t mi = 0; mi < m; ++mi) acc = __fadd_rn(acc, lut[mi * k + cd[mi]]);
+    }
+    return acc;
+}
+
+// ADC scan: CTA (tile, q).  score = pq_adc_sum of the row's codes;
 // key = (score, tie rank) packed so that a descending sort is (score desc, tie-break key asc); the tile's best `approx`
 // keys are written to the query's list.
 __global__ void __launch_bounds__(PQ_THREADS) pq_adc_kernel(const uint8_t* __restrict__ codes, uint64_t n_idx, uint32_t m, uint32_t k,
@@ -193,20 +214,7 @@ __global__ void __launch_bounds__(PQ_THREADS) pq_adc_kernel(const uint8_t* __res
         const uint64_t j = r0 + t;
         uint64_t key = 0;
         if (j < n_idx) {
-            const uint8_t* cd = codes + j * m;
-            float acc = 0.f;
-            if (vec) {
-                for (uint32_t mi = 0; mi < m; mi += 16) {
-                    const uint4 w = *reinterpret_cast<const uint4*>(cd + mi);
-                    const uint32_t ws[4] = {w.x, w.y, w.z, w.w};
-#pragma unroll
-                    for (int u = 0; u < 4; ++u)
-#pragma unroll
-                        for (int b = 0; b < 4; ++b) acc = __fadd_rn(acc, lut[(mi + u * 4 + b) * k + ((ws[u] >> (8 * b)) & 0xFFu)]);
-                }
-            } else {
-                for (uint32_t mi = 0; mi < m; ++mi) acc = __fadd_rn(acc, lut[mi * k + cd[mi]]);
-            }
+            const float acc = pq_adc_sum(codes + j * m, lut, m, k, vec);
             uint32_t b = __float_as_uint(acc);
             b = (acc != acc) ? 0u : ((b & 0x80000000u) ? ~b : (b | 0x80000000u));   // monotone key, NaN last (as knn.cu fkey)
             key = ((uint64_t)b << 32) | (uint64_t)(0xFFFFFFFFu - tie_rank[j]);
@@ -366,8 +374,26 @@ struct PqExact {
     float sim;
     uint32_t row;
 };
-// VectorDatabase::computeCosineSimilarity (vector_database.cpp:1786-1810) of the ORIGINAL query against the stored row, float
-// cast, `similarity < threshold` dropped (sqlite_vec_backend.cpp:4022-4037)
+// VectorDatabase::computeCosineSimilarity (vector_database.cpp:1786-1810) of the ORIGINAL query a against corpus row `row`,
+// float cast, NaN and `similarity < threshold` dropped (sqlite_vec_backend.cpp:4022-4037).  -> true and *out = sim when kept.
+__device__ __forceinline__ bool pq_rerank_sim(const void* __restrict__ rows, int dtype, uint32_t d, uint32_t row, const float* __restrict__ a,
+                                              float threshold, float* out) {
+    double dp = 0.0, na = 0.0, nb = 0.0;
+    for (uint32_t c = 0; c < d; ++c) {
+        const double x = (double)a[c], y = (double)load_row_elem(rows, dtype, (uint64_t)row * d + c);
+        dp += x * y;
+        na += x * x;
+        nb += y * y;
+    }
+    na = sqrt(na);
+    nb = sqrt(nb);
+    const float sim = (float)((na == 0.0 || nb == 0.0) ? 0.0 : dp / (na * nb));
+    if (sim == sim && !(sim < threshold)) {
+        *out = sim;
+        return true;
+    }
+    return false;
+}
 __global__ void pq_rerank_kernel(const void* __restrict__ rows, int dtype, uint32_t d, const float* __restrict__ q32, const Cand* __restrict__ sel,
                                  const uint32_t* __restrict__ sel_n, const uint32_t* __restrict__ valid, uint32_t K, uint32_t nq,
                                  float threshold, PqExact* __restrict__ out) {
@@ -379,18 +405,8 @@ __global__ void pq_rerank_kernel(const void* __restrict__ rows, int dtype, uint3
     e.row = 0xFFFFFFFFu;
     if (valid[q] && j < sel_n[q]) {
         const uint32_t row = sel[t].row;
-        const float* a = q32 + (size_t)q * d;
-        double dp = 0.0, na = 0.0, nb = 0.0;
-        for (uint32_t c = 0; c < d; ++c) {
-            const double x = (double)a[c], y = (double)load_row_elem(rows, dtype, (uint64_t)row * d + c);
-            dp += x * y;
-            na += x * x;
-            nb += y * y;
-        }
-        na = sqrt(na);
-        nb = sqrt(nb);
-        const float sim = (float)((na == 0.0 || nb == 0.0) ? 0.0 : dp / (na * nb));
-        if (sim == sim && !(sim < threshold)) {
+        float sim;
+        if (pq_rerank_sim(rows, dtype, d, row, q32 + (size_t)q * d, threshold, &sim)) {
             e.sim = sim;
             e.row = row;
         }
@@ -398,11 +414,181 @@ __global__ void pq_rerank_kernel(const void* __restrict__ rows, int dtype, uint3
     out[t] = e;
 }
 
+// ---- candidate sets and the document pass ------------------------------------------------------------------------------
+// corpus row -> index position (0xFFFFFFFF: not in the index); the caller pre-fills the table with 0xFF bytes
+__global__ void pq_row_to_idx_kernel(const uint32_t* __restrict__ idx_rows, uint64_t n_idx, uint32_t* __restrict__ row_to_idx) {
+    for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n_idx; j += (uint64_t)gridDim.x * blockDim.x)
+        row_to_idx[idx_rows[j]] = (uint32_t)j;
+}
+
+// CTA (x, q): the mapped entries of query q's list -> index positions; an entry counts when its row is in the index and the
+// query's bit for that position was not yet set (a rowid listed twice counts once).  The distinct positions are appended to
+// cidx[offs[q] ..], their number to counts[q].
+__global__ void pq_cand_index_kernel(const Cand* __restrict__ mapped, const uint64_t* __restrict__ offs, const uint32_t* __restrict__ row_to_idx,
+                                     uint32_t* __restrict__ bits, uint64_t bits_ld, uint32_t* __restrict__ cidx, uint32_t* __restrict__ counts) {
+    const uint32_t q = blockIdx.y;
+    const uint64_t lo = offs[q], hi = offs[q + 1];
+    const unsigned lane = threadIdx.x & 31u;
+    for (uint64_t base = lo + (uint64_t)blockIdx.x * blockDim.x; base < hi; base += (uint64_t)gridDim.x * blockDim.x) {   // warp-uniform trips
+        const uint64_t i = base + threadIdx.x;
+        bool take = false;
+        uint32_t idx = 0xFFFFFFFFu;
+        if (i < hi) {
+            const uint32_t row = mapped[i].row;
+            if (row != 0xFFFFFFFFu) idx = row_to_idx[row];
+            if (idx != 0xFFFFFFFFu) {
+                const uint32_t bit = 1u << (idx & 31);
+                take = !(atomicOr(&bits[(uint64_t)q * bits_ld + (idx >> 5)], bit) & bit);
+            }
+        }
+        const unsigned mask = __ballot_sync(0xffffffffu, take);
+        if (mask) {
+            const int leader = __ffs(mask) - 1;
+            uint32_t pos = 0;
+            if ((int)lane == leader) pos = atomicAdd(&counts[q], (uint32_t)__popc(mask));
+            pos = __shfl_sync(0xffffffffu, pos, leader) + __popc(mask & ((1u << lane) - 1u));
+            if (take) cidx[lo + pos] = idx;
+        }
+    }
+}
+
+// ADC scores of the candidate positions: CTA (slice of per_cta candidates, q) with the query's LUT in shared memory;
+// lists[q * cap + j] = (pq_adc_sum, tie rank) for j < counts[q], the input of the top-approx selection
+__global__ void __launch_bounds__(PQ_THREADS) pq_adc_gather_kernel(const uint8_t* __restrict__ codes, uint32_t m, uint32_t k,
+                                                                   const float* __restrict__ lut_all, const uint32_t* __restrict__ tie_rank,
+                                                                   const uint32_t* __restrict__ cidx, const uint64_t* __restrict__ offs,
+                                                                   const uint32_t* __restrict__ counts, uint32_t per_cta,
+                                                                   Cand* __restrict__ lists, uint32_t cap) {
+    extern __shared__ float lut[];   // m * k floats
+    const uint32_t q = blockIdx.y;
+    const uint32_t cnt = counts[q];
+    const uint32_t j0 = blockIdx.x * per_cta;
+    if (j0 >= cnt) return;
+    const uint32_t j1 = min(cnt, j0 + per_cta);
+    const float* lq = lut_all + (size_t)q * m * k;
+    for (uint32_t e = threadIdx.x; e < m * k; e += PQ_THREADS) lut[e] = lq[e];
+    __syncthreads();
+    const bool vec = (m % 16) == 0;
+    const uint32_t* ci = cidx + offs[q];
+    for (uint32_t j = j0 + threadIdx.x; j < j1; j += PQ_THREADS) {
+        const uint32_t idx = ci[j];
+        Cand c;
+        c.score = pq_adc_sum(codes + (uint64_t)idx * m, lut, m, k, vec);
+        c.row = tie_rank[idx];
+        lists[(uint64_t)q * cap + j] = c;
+    }
+}
+
+// valid[q] = 1 when the query can be normalised (normalizeEmbeddingInPlace, the rule of pq_lut_kernel)
+__global__ void pq_query_valid_kernel(const float* __restrict__ q32, uint32_t nq, uint32_t d, uint32_t* __restrict__ valid) {
+    const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= nq) return;
+    double ss = 0.0;
+    for (uint32_t c = 0; c < d; ++c) ss += (double)q32[(size_t)q * d + c] * (double)q32[(size_t)q * d + c];
+    float inv;
+    valid[q] = normalize_factor(ss, &inv) ? 1u : 0u;
+}
+
+// index of the segment holding element p: the last s with starts[s] <= p (starts ascending, starts[0] <= p)
+__device__ __forceinline__ uint32_t segment_of(const uint64_t* __restrict__ starts, uint32_t nseg, uint64_t p) {
+    uint32_t a = 0, b = nseg;
+    while (b - a > 1) {
+        const uint32_t mid = (a + b) >> 1;
+        if (starts[mid] <= p) a = mid; else b = mid;
+    }
+    return a;
+}
+
+// Document pass, step 1: one thread per (query, candidate row) pair.  pairs[p].row is the corpus row (0xFFFFFFFF: unknown
+// rowid); pairs[p].score becomes its similarity, NaN when the row is no result.
+//   exact (row_to_idx == NULL): exact_cosine_sim against qnorm[q] (the exact scan's arithmetic, skip rules and threshold);
+//   PQ: rows in the index only, pq_rerank_sim (the PQ engine's rerank arithmetic and threshold), nothing for a query that
+//       cannot be normalised.
+__global__ void doc_score_kernel(const void* __restrict__ rows, int dtype, uint32_t d, const float* __restrict__ q32, const double* __restrict__ qnorm,
+                                 const uint32_t* __restrict__ valid, const uint32_t* __restrict__ row_to_idx, const uint64_t* __restrict__ qpair,
+                                 uint32_t nq, uint64_t npairs, float threshold, Cand* __restrict__ pairs) {
+    const uint64_t p = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= npairs) return;
+    const uint32_t q = segment_of(qpair, nq, p);
+    const uint32_t row = pairs[p].row;
+    float sim = __int_as_float(0x7FC00000), s;
+    if (row != 0xFFFFFFFFu) {
+        const float* qv = q32 + (size_t)q * d;
+        if (row_to_idx) {
+            if (valid[q] && row_to_idx[row] != 0xFFFFFFFFu && pq_rerank_sim(rows, dtype, d, row, qv, threshold, &s)) sim = s;
+        } else if (exact_cosine_sim(rows, dtype, d, row, qv, qnorm[q], threshold, &s)) {
+            sim = s;
+        }
+    }
+    pairs[p].score = sim;
+}
+
+// Document pass, step 2: one warp per document, the arg-max of its rows by (sim desc, position in the document asc).  A document
+// with a surviving row is appended to its query's list as (best sim, document index), the row index it came from is kept in
+// best_row[doc].
+__global__ void doc_argmax_kernel(const Cand* __restrict__ pairs, const uint64_t* __restrict__ doff, uint32_t ndocs, const uint64_t* __restrict__ qdocs,
+                                  uint32_t nq, Cand* __restrict__ lists, uint32_t cap, uint32_t* __restrict__ counts, uint32_t* __restrict__ best_row) {
+    const uint64_t doc = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const unsigned lane = threadIdx.x & 31u;
+    if (doc >= ndocs) return;
+    const uint64_t lo = doff[doc], hi = doff[doc + 1];
+    uint64_t best = 0;
+    for (uint64_t i = lo + lane; i < hi; i += 32) {
+        const float s = pairs[i].score;
+        if (s == s) best = max(best, ((uint64_t)fkey(s) << 32) | (uint64_t)(0xFFFFFFFFu - (uint32_t)(i - lo)));
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) best = max(best, (uint64_t)__shfl_xor_sync(0xffffffffu, best, o));
+    if (lane == 0 && best) {
+        const uint32_t q = segment_of(qdocs, nq, doc);
+        best_row[doc] = pairs[lo + (0xFFFFFFFFu - (uint32_t)best)].row;
+        Cand c;
+        c.score = fkey_inv((uint32_t)(best >> 32));
+        c.row = (uint32_t)doc;
+        const uint32_t pos = atomicAdd(&counts[q], 1u);
+        lists[(uint64_t)q * cap + pos] = c;
+    }
+}
+
+// Document pass, step 4: the k best documents of every query (sel, from the top-k selection) -> document index, its best row's
+// rowid and score; unused slots -1 / -1 / 0
+__global__ void doc_emit_kernel(const Cand* __restrict__ sel, const uint32_t* __restrict__ sel_n, uint32_t k, uint32_t nq, uint64_t doc_base,
+                                const uint32_t* __restrict__ best_row, const int64_t* __restrict__ rowids, int64_t* __restrict__ o_docs,
+                                int64_t* __restrict__ o_rowids, float* __restrict__ o_scores, uint32_t* __restrict__ o_counts) {
+    const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= (uint64_t)nq * k) return;
+    const uint32_t q = (uint32_t)(t / k), i = (uint32_t)(t % k);
+    if (i < sel_n[q]) {
+        const Cand c = sel[t];
+        o_docs[t] = (int64_t)(doc_base + c.row);
+        o_rowids[t] = rowids[best_row[c.row]];
+        o_scores[t] = c.score;
+    } else {
+        o_docs[t] = -1;
+        o_rowids[t] = -1;
+        o_scores[t] = 0.f;
+    }
+    if (i == 0) o_counts[q] = sel_n[q];
+}
+
 // defined in knn.cu
 void launch_topk_lists(const Cand* lists, const uint32_t* counts, uint32_t cap, uint32_t nq, uint32_t K, Cand* out_sel, uint32_t* out_n,
                        cudaStream_t st);
 void launch_final_plain(const void* exact, uint32_t Kp, uint32_t k, uint32_t nq, const int64_t* rowids, int64_t* out_rowids, float* out_scores,
                         uint32_t* out_counts, uint64_t* out_flags, cudaStream_t st);
+void launch_map_rowids(const int64_t* rowids_in, uint64_t n_in, const int64_t* corpus_rowids, uint64_t n, Cand* out, cudaStream_t st);
+void launch_query_prep(const float* q, uint32_t nq, uint32_t d, double* qnorm, float* qinv, void* status, cudaStream_t st);
+
+// Host staging of ONE host-to-device copy: the pieces of a call's input at 16-byte aligned offsets
+struct Staging {
+    std::vector<unsigned char> h;
+    size_t add(const void* src, size_t bytes) {
+        const size_t off = (h.size() + 15) & ~(size_t)15;
+        h.resize(off + bytes);
+        if (bytes) memcpy(h.data() + off, src, bytes);
+        return off;
+    }
+};
 
 }  // namespace yb
 
@@ -414,8 +600,11 @@ struct yams_b200_pq {
     uint32_t m = 0, k = 0, dim = 0;
     uint64_t n_idx = 0;
     DevBuf codebooks, codes, idx_rows, tie_rank, rank_to_idx;
+    DevBuf row_to_idx;          // corpus row -> index position, built by the first call that needs it (the index is immutable)
+    bool row_to_idx_ready = false;
     // search workspace
     DevBuf q32, lut, valid, lists, counts, sel, exact, dout, tau;
+    DevBuf cin, mapped, cidx, bits;   // candidate-set search: staged input, mapped rows, distinct positions, per-query seen bits
     std::mutex mu;
 };
 
@@ -489,8 +678,8 @@ yams_status_t yams_b200_pq_build(yams_b200_corpus* c, uint32_t m, uint32_t k, co
 
 void yams_b200_pq_destroy(yams_b200_pq* p) {
     if (!p) return;
-    for (DevBuf* b : {&p->codebooks, &p->codes, &p->idx_rows, &p->tie_rank, &p->rank_to_idx, &p->q32, &p->lut, &p->valid, &p->lists, &p->counts,
-                      &p->sel, &p->exact, &p->dout, &p->tau})
+    for (DevBuf* b : {&p->codebooks, &p->codes, &p->idx_rows, &p->tie_rank, &p->rank_to_idx, &p->row_to_idx, &p->q32, &p->lut, &p->valid, &p->lists,
+                      &p->counts, &p->sel, &p->exact, &p->dout, &p->tau, &p->cin, &p->mapped, &p->cidx, &p->bits})
         b->release();
     delete p;
 }
@@ -655,3 +844,310 @@ static yams_status_t pq_search_batch(yams_b200_pq* p, const float* queries, uint
     return YAMS_OK;
     YB_CATCH
 }
+
+// corpus row -> index position table of the handle (the caller holds both locks)
+static yams_status_t ensure_row_to_idx(yams_b200_pq* p, cudaStream_t st) {
+    if (p->row_to_idx_ready) return YAMS_OK;
+    const uint64_t n = p->corpus->n;
+    yams_status_t rc;
+    if ((rc = p->row_to_idx.reserve(std::max<uint64_t>(n, 1) * 4)) != YAMS_OK) return rc;
+    YB_CUDA(cudaMemsetAsync(p->row_to_idx.p, 0xFF, std::max<uint64_t>(n, 1) * 4, st));
+    if (p->n_idx)
+        pq_row_to_idx_kernel<<<(unsigned)std::min<uint64_t>((p->n_idx + 255) / 256, 65535), 256, 0, st>>>(p->idx_rows.as<uint32_t>(), p->n_idx,
+                                                                                                         p->row_to_idx.as<uint32_t>());
+    YB_CUDA(cudaGetLastError());
+    p->row_to_idx_ready = true;
+    return YAMS_OK;
+}
+
+// one batch of <= kPqMaxBatch queries of pq_search_candidates; offs: the batch's nq + 1 offsets into `allowed` (absolute)
+static yams_status_t pq_candidates_batch(yams_b200_pq* p, const float* queries, uint32_t nq, uint32_t k, uint32_t rerank_factor, float threshold,
+                                         const int64_t* allowed, const uint64_t* offs, int64_t* out_rowids, float* out_scores, uint32_t* out_counts,
+                                         uint64_t* out_flags) {
+    YB_TRY
+    yams_b200_corpus* c = p->corpus;
+    cudaStream_t st = c->st;
+    yams_status_t rc;
+    const uint32_t m = p->m, kc = p->k, d = p->dim;
+    if (rerank_factor == 0) rerank_factor = 1;
+    const uint64_t want = std::max<uint64_t>(k, (uint64_t)k * rerank_factor);
+    const uint64_t base = offs[0], total = offs[nq] - base;
+    uint64_t maxlen = 0;
+    for (uint32_t q = 0; q < nq; ++q) maxlen = std::max(maxlen, offs[q + 1] - offs[q]);
+    YB_ARG(maxlen < 0xFFFFFFFFull, "candidate list too long");
+    // approxK = min(candidateCount, max(k, k * rerank_factor)) (:3956-3959).  candidateCount (distinct indexed candidates) is
+    // known on the device only: list lengths bound it; when the bound allows approxK > 1024 the selection keeps one more and
+    // the limit is checked on the selected counts.
+    uint32_t K = (uint32_t)std::max<uint64_t>(1, std::min(want, maxlen));
+    const bool check_after = K > PQ_MAX_APPROX;
+    if (check_after) K = PQ_MAX_APPROX + 1;
+    const uint32_t cap = (uint32_t)std::max<uint64_t>(maxlen, 1);
+    const uint64_t bits_ld = (p->n_idx + 31) / 32;
+    if ((rc = ensure_row_to_idx(p, st)) != YAMS_OK) return rc;
+    Staging in;
+    const size_t o_q = in.add(queries, (size_t)nq * d * 4);
+    const size_t o_al = in.add(allowed ? allowed + base : nullptr, (size_t)total * 8);
+    std::vector<uint64_t> roffs(nq + 1);
+    for (uint32_t q = 0; q <= nq; ++q) roffs[q] = offs[q] - base;
+    const size_t o_of = in.add(roffs.data(), (size_t)(nq + 1) * 8);
+    if ((rc = p->cin.reserve(in.h.size())) != YAMS_OK) return rc;
+    if ((rc = p->mapped.reserve(std::max<uint64_t>(total, 1) * sizeof(Cand))) != YAMS_OK) return rc;
+    if ((rc = p->cidx.reserve(std::max<uint64_t>(total, 1) * 4)) != YAMS_OK) return rc;
+    if ((rc = p->bits.reserve((size_t)nq * bits_ld * 4 + 4)) != YAMS_OK) return rc;
+    if ((rc = p->lut.reserve((size_t)nq * m * kc * 4)) != YAMS_OK) return rc;
+    if ((rc = p->valid.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
+    if ((rc = p->lists.reserve((size_t)nq * cap * sizeof(Cand))) != YAMS_OK) return rc;
+    if ((rc = p->counts.reserve((size_t)nq * 4 + 16)) != YAMS_OK) return rc;
+    if ((rc = p->sel.reserve((size_t)nq * K * sizeof(Cand) + (size_t)nq * 4)) != YAMS_OK) return rc;
+    if ((rc = p->exact.reserve((size_t)nq * K * sizeof(PqExact))) != YAMS_OK) return rc;
+    if ((rc = p->dout.reserve((size_t)nq * k * 12 + (size_t)nq * 12 + 64)) != YAMS_OK) return rc;
+    unsigned char* din = p->cin.as<unsigned char>();
+    const float* d_q = reinterpret_cast<const float*>(din + o_q);
+    const int64_t* d_al = reinterpret_cast<const int64_t*>(din + o_al);
+    const uint64_t* d_of = reinterpret_cast<const uint64_t*>(din + o_of);
+    uint32_t* d_counts = p->counts.as<uint32_t>();
+    Cand* d_sel = p->sel.as<Cand>();
+    uint32_t* d_sel_n = reinterpret_cast<uint32_t*>(d_sel + (size_t)nq * K);
+    YB_CUDA(cudaMemcpyAsync(din, in.h.data(), in.h.size(), cudaMemcpyHostToDevice, st));
+    YB_CUDA(cudaMemsetAsync(p->bits.p, 0, (size_t)nq * bits_ld * 4 + 4, st));
+    YB_CUDA(cudaMemsetAsync(d_counts, 0, (size_t)nq * 4, st));
+    YB_CUDA(cudaFuncSetAttribute(pq_lut_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(d * 4)));
+    pq_lut_kernel<<<nq, 256, d * 4, st>>>(d_q, d, p->codebooks.as<float>(), m, kc, p->lut.as<float>(), p->valid.as<uint32_t>());
+    launch_map_rowids(d_al, total, c->rowids.as<int64_t>(), c->n, p->mapped.as<Cand>(), st);
+    if (total) {
+        const unsigned gx = (unsigned)std::min<uint64_t>((maxlen + 255) / 256, 256);
+        pq_cand_index_kernel<<<dim3(gx, nq), 256, 0, st>>>(p->mapped.as<Cand>(), d_of, p->row_to_idx.as<uint32_t>(), p->bits.as<uint32_t>(), bits_ld,
+                                                           p->cidx.as<uint32_t>(), d_counts);
+        const uint32_t per_cta = 2048;
+        const size_t lut_bytes = (size_t)m * kc * 4;
+        YB_CUDA(cudaFuncSetAttribute(pq_adc_gather_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lut_bytes));
+        pq_adc_gather_kernel<<<dim3((unsigned)((maxlen + per_cta - 1) / per_cta), nq), PQ_THREADS, lut_bytes, st>>>(
+            p->codes.as<uint8_t>(), m, kc, p->lut.as<float>(), p->tie_rank.as<uint32_t>(), p->cidx.as<uint32_t>(), d_of, d_counts, per_cta,
+            p->lists.as<Cand>(), cap);
+    }
+    // from here on the chain of pq_search: selection, rank -> row, exact rerank, final order
+    launch_topk_lists(p->lists.as<Cand>(), d_counts, cap, nq, K, d_sel, d_sel_n, st);
+    const uint32_t tot = nq * K;
+    pq_rank_to_row_kernel<<<(tot + 255) / 256, 256, 0, st>>>(d_sel, d_sel_n, K, nq, p->rank_to_idx.as<uint32_t>(), p->idx_rows.as<uint32_t>());
+    pq_rerank_kernel<<<(tot + 127) / 128, 128, 0, st>>>(c->rows.p, c->dtype, d, d_q, d_sel, d_sel_n, p->valid.as<uint32_t>(), K, nq, threshold,
+                                                        p->exact.as<PqExact>());
+    int64_t* d_or = p->dout.as<int64_t>();
+    uint64_t* d_ofl = reinterpret_cast<uint64_t*>(d_or + (size_t)nq * k);
+    float* d_os = reinterpret_cast<float*>(d_ofl + nq);
+    uint32_t* d_oc = reinterpret_cast<uint32_t*>(d_os + (size_t)nq * k);
+    launch_final_plain(p->exact.p, K, k, nq, c->rowids.as<int64_t>(), d_or, d_os, d_oc, d_ofl, st);
+    YB_CUDA(cudaGetLastError());
+    YB_CUDA(cudaMemcpyAsync(out_rowids, d_or, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, st));
+    YB_CUDA(cudaMemcpyAsync(out_scores, d_os, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, st));
+    YB_CUDA(cudaMemcpyAsync(out_counts, d_oc, (size_t)nq * 4, cudaMemcpyDeviceToHost, st));
+    if (out_flags) YB_CUDA(cudaMemcpyAsync(out_flags, d_ofl, (size_t)nq * 8, cudaMemcpyDeviceToHost, st));
+    std::vector<uint32_t> sel_n(check_after ? nq : 0);
+    if (check_after) YB_CUDA(cudaMemcpyAsync(sel_n.data(), d_sel_n, (size_t)nq * 4, cudaMemcpyDeviceToHost, st));
+    YB_CUDA(cudaStreamSynchronize(st));
+    for (uint32_t q = 0; q < (check_after ? nq : 0); ++q) {
+        if (sel_n[q] > PQ_MAX_APPROX) {
+            for (uint32_t i = 0; i < nq; ++i) out_counts[i] = 0;
+            YB_ARG(false, "k * rerank_factor > 1024 is not supported by the PQ engine (use the exact scan)");
+        }
+    }
+    return YAMS_OK;
+    YB_CATCH
+}
+
+// every rowid of one query's documents at most once: a stamp table over the rowid range when it is small, else a sort per query
+static bool rowids_unique_per_query(const int64_t* rid, const uint64_t* doc_offsets, const uint64_t* query_docs, uint32_t nq) {
+    const uint64_t p0 = doc_offsets[query_docs[0]], p1 = doc_offsets[query_docs[nq]];
+    if (p1 == p0) return true;
+    int64_t lo = INT64_MAX, hi = INT64_MIN;
+    for (uint64_t i = p0; i < p1; ++i) { lo = std::min(lo, rid[i]); hi = std::max(hi, rid[i]); }
+    const uint64_t range = (uint64_t)hi - (uint64_t)lo + 1;
+    if (range != 0 && range <= std::max<uint64_t>(16 * (p1 - p0), 1ull << 22)) {
+        std::vector<uint32_t> stamp(range, 0u);
+        for (uint32_t q = 0; q < nq; ++q)
+            for (uint64_t i = doc_offsets[query_docs[q]]; i < doc_offsets[query_docs[q + 1]]; ++i) {
+                uint32_t& s = stamp[(uint64_t)rid[i] - (uint64_t)lo];
+                if (s == q + 1) return false;
+                s = q + 1;
+            }
+        return true;
+    }
+    std::vector<int64_t> v;
+    for (uint32_t q = 0; q < nq; ++q) {
+        v.assign(rid + doc_offsets[query_docs[q]], rid + doc_offsets[query_docs[q + 1]]);
+        std::sort(v.begin(), v.end());
+        if (std::adjacent_find(v.begin(), v.end()) != v.end()) return false;
+    }
+    return true;
+}
+
+// one slice of search_documents: queries [q0, q1); the caller holds the locks, has checked the input and bound the device
+static yams_status_t documents_slice(yams_b200_corpus* c, yams_b200_pq* pq, const float* queries, uint32_t q0, uint32_t q1, uint32_t k,
+                                     float threshold, const int64_t* doc_rowids, const uint64_t* doc_offsets, const uint64_t* query_docs,
+                                     int64_t* out_docs, int64_t* out_rowids, float* out_scores, uint32_t* out_counts) {
+    YB_TRY
+    cudaStream_t st = c->st;
+    yams_status_t rc;
+    const uint32_t nq = q1 - q0, d = c->dim;
+    const uint64_t sd0 = query_docs[q0], ndocs = query_docs[q1] - sd0;
+    const uint64_t p0 = doc_offsets[sd0], np = doc_offsets[query_docs[q1]] - p0;
+    uint64_t cap = 1;
+    for (uint32_t q = q0; q < q1; ++q) cap = std::max<uint64_t>(cap, query_docs[q + 1] - query_docs[q]);
+    Staging in;
+    const size_t o_q = in.add(queries + (size_t)q0 * d, (size_t)nq * d * 4);
+    const size_t o_rid = in.add(np ? doc_rowids + p0 : nullptr, (size_t)np * 8);
+    std::vector<uint64_t> v(ndocs + 1);
+    for (uint64_t i = 0; i <= ndocs; ++i) v[i] = doc_offsets[sd0 + i] - p0;
+    const size_t o_doff = in.add(v.data(), (size_t)(ndocs + 1) * 8);
+    v.resize(nq + 1);
+    for (uint32_t q = 0; q <= nq; ++q) v[q] = query_docs[q0 + q] - sd0;
+    const size_t o_qdocs = in.add(v.data(), (size_t)(nq + 1) * 8);
+    for (uint32_t q = 0; q <= nq; ++q) v[q] = doc_offsets[query_docs[q0 + q]] - p0;
+    const size_t o_qpair = in.add(v.data(), (size_t)(nq + 1) * 8);
+    // device workspace of the corpus (its lock is held): staged input, pairs, document lists, selection, outputs
+    const size_t lists_b = (size_t)nq * cap * sizeof(Cand);
+    const size_t out_b = (size_t)nq * k * 20 + (size_t)nq * 4 + 4;
+    if ((rc = c->mask.reserve(in.h.size())) != YAMS_OK) return rc;
+    if ((rc = c->sel.reserve(std::max<uint64_t>(np, 1) * sizeof(Cand))) != YAMS_OK) return rc;
+    if ((rc = c->cands.reserve(lists_b + (size_t)nq * 4 + std::max<uint64_t>(ndocs, 1) * 4)) != YAMS_OK) return rc;
+    if ((rc = c->outbuf.reserve((size_t)nq * k * sizeof(Cand) + (size_t)nq * 4)) != YAMS_OK) return rc;
+    if ((rc = c->misc.reserve((size_t)nq * 16)) != YAMS_OK) return rc;
+    if ((rc = c->status.reserve(16)) != YAMS_OK) return rc;
+    if ((rc = c->dout.reserve(out_b)) != YAMS_OK) return rc;
+    unsigned char* din = c->mask.as<unsigned char>();
+    const float* d_q = reinterpret_cast<const float*>(din + o_q);
+    const int64_t* d_rid = reinterpret_cast<const int64_t*>(din + o_rid);
+    const uint64_t* d_doff = reinterpret_cast<const uint64_t*>(din + o_doff);
+    const uint64_t* d_qdocs = reinterpret_cast<const uint64_t*>(din + o_qdocs);
+    const uint64_t* d_qpair = reinterpret_cast<const uint64_t*>(din + o_qpair);
+    Cand* d_pairs = c->sel.as<Cand>();
+    Cand* d_lists = c->cands.as<Cand>();
+    uint32_t* d_counts = reinterpret_cast<uint32_t*>(c->cands.as<unsigned char>() + lists_b);
+    uint32_t* d_best = d_counts + nq;
+    Cand* d_sel = c->outbuf.as<Cand>();
+    uint32_t* d_sel_n = reinterpret_cast<uint32_t*>(d_sel + (size_t)nq * k);
+    double* d_qnorm = c->misc.as<double>();
+    float* d_qinv = reinterpret_cast<float*>(d_qnorm + nq);
+    uint32_t* d_valid = reinterpret_cast<uint32_t*>(d_qinv + nq);
+    int64_t* o_docs = c->dout.as<int64_t>();
+    int64_t* o_rows = o_docs + (size_t)nq * k;
+    float* o_sc = reinterpret_cast<float*>(o_rows + (size_t)nq * k);
+    uint32_t* o_cnt = reinterpret_cast<uint32_t*>(o_sc + (size_t)nq * k);
+    uint32_t* o_invalid = o_cnt + nq;
+    YB_CUDA(cudaMemcpyAsync(din, in.h.data(), in.h.size(), cudaMemcpyHostToDevice, st));
+    YB_CUDA(cudaMemsetAsync(d_counts, 0, (size_t)nq * 4, st));
+    YB_CUDA(cudaMemsetAsync(c->status.p, 0, 16, st));
+    if (pq) {
+        if ((rc = ensure_row_to_idx(pq, st)) != YAMS_OK) return rc;
+        pq_query_valid_kernel<<<(nq + 127) / 128, 128, 0, st>>>(d_q, nq, d, d_valid);
+    } else {
+        launch_query_prep(d_q, nq, d, d_qnorm, d_qinv, c->status.p, st);
+    }
+    launch_map_rowids(d_rid, np, c->rowids.as<int64_t>(), c->n, d_pairs, st);
+    if (np)
+        doc_score_kernel<<<(unsigned)((np + 127) / 128), 128, 0, st>>>(c->rows.p, c->dtype, d, d_q, d_qnorm, d_valid,
+                                                                      pq ? pq->row_to_idx.as<uint32_t>() : nullptr, d_qpair, nq, np, threshold, d_pairs);
+    if (ndocs)
+        doc_argmax_kernel<<<(unsigned)((ndocs * 32 + 255) / 256), 256, 0, st>>>(d_pairs, d_doff, (uint32_t)ndocs, d_qdocs, nq, d_lists, (uint32_t)cap,
+                                                                               d_counts, d_best);
+    launch_topk_lists(d_lists, d_counts, (uint32_t)cap, nq, k, d_sel, d_sel_n, st);
+    doc_emit_kernel<<<(unsigned)(((uint64_t)nq * k + 255) / 256), 256, 0, st>>>(d_sel, d_sel_n, k, nq, sd0, d_best, c->rowids.as<int64_t>(), o_docs,
+                                                                                o_rows, o_sc, o_cnt);
+    YB_CUDA(cudaMemcpyAsync(o_invalid, c->status.p, 4, cudaMemcpyDeviceToDevice, st));
+    YB_CUDA(cudaGetLastError());
+    std::vector<unsigned char> h(out_b);
+    YB_CUDA(cudaMemcpyAsync(h.data(), c->dout.p, out_b, cudaMemcpyDeviceToHost, st));
+    YB_CUDA(cudaStreamSynchronize(st));
+    const unsigned char* hp = h.data();
+    uint32_t n_invalid = 0;
+    memcpy(&n_invalid, hp + (size_t)nq * k * 20 + (size_t)nq * 4, 4);
+    YB_ARG(pq || n_invalid == 0, "exact vector search requires a finite, non-zero query embedding");   // :4127-4130
+    memcpy(out_docs + (size_t)q0 * k, hp, (size_t)nq * k * 8);
+    memcpy(out_rowids + (size_t)q0 * k, hp + (size_t)nq * k * 8, (size_t)nq * k * 8);
+    memcpy(out_scores + (size_t)q0 * k, hp + (size_t)nq * k * 16, (size_t)nq * k * 4);
+    memcpy(out_counts + q0, hp + (size_t)nq * k * 20, (size_t)nq * 4);
+    return YAMS_OK;
+    YB_CATCH
+}
+
+extern "C" {
+
+yams_status_t yams_b200_pq_search_candidates(yams_b200_pq* p, const float* queries, uint32_t nq, uint32_t k, uint32_t rerank_factor, float threshold,
+                                             const int64_t* allowed_rowids, const uint64_t* allowed_offsets, int64_t* out_rowids, float* out_scores,
+                                             uint32_t* out_counts, uint64_t* out_flags) {
+    YB_TRY
+    YB_ARG(p && out_counts, "null argument");
+    std::lock_guard<std::mutex> lk(p->mu);
+    yams_b200_corpus* c = p->corpus;
+    std::lock_guard<std::mutex> corpus_lock(c->mu);
+    YB_BIND(c);
+    for (uint32_t q = 0; q < nq; ++q) out_counts[q] = 0;
+    if (out_flags) for (uint32_t q = 0; q < nq; ++q) out_flags[q] = 0;
+    if (nq == 0 || k == 0 || p->n_idx == 0) return YAMS_OK;
+    YB_ARG(queries && out_rowids && out_scores && allowed_offsets, "null argument");
+    for (uint32_t q = 0; q < nq; ++q) YB_ARG(allowed_offsets[q] <= allowed_offsets[q + 1], "allowed_offsets must be non-decreasing");
+    YB_ARG(allowed_rowids || allowed_offsets[nq] == allowed_offsets[0], "allowed_rowids missing");
+    YB_ARG(c->generation == p->corpus_generation, "the corpus changed after the PQ index was built: rebuild it (the reference marks the index dirty)");
+    for (uint32_t q0 = 0; q0 < nq; q0 += kPqMaxBatch) {
+        const uint32_t nb = std::min<uint32_t>(kPqMaxBatch, nq - q0);
+        yams_status_t rc = pq_candidates_batch(p, queries + (size_t)q0 * p->dim, nb, k, rerank_factor, threshold, allowed_rowids, allowed_offsets + q0,
+                                               out_rowids + (size_t)q0 * k, out_scores + (size_t)q0 * k, out_counts + q0,
+                                               out_flags ? out_flags + q0 : nullptr);
+        if (rc != YAMS_OK) {
+            for (uint32_t q = 0; q < nq; ++q) out_counts[q] = 0;
+            return rc;
+        }
+    }
+    return YAMS_OK;
+    YB_CATCH
+}
+
+yams_status_t yams_b200_search_documents(yams_b200_corpus* c, yams_b200_pq* pq, const float* queries, uint32_t nq, uint32_t k, float threshold,
+                                         const int64_t* doc_rowids, const uint64_t* doc_offsets, const uint64_t* query_docs, int64_t* out_docs,
+                                         int64_t* out_rowids, float* out_scores, uint32_t* out_counts) {
+    YB_TRY
+    YB_ARG(c && out_counts, "null argument");
+    std::unique_lock<std::mutex> pq_lock;
+    if (pq) pq_lock = std::unique_lock<std::mutex>(pq->mu);
+    std::lock_guard<std::mutex> corpus_lock(c->mu);
+    YB_BIND(c);
+    for (uint32_t q = 0; q < nq; ++q) out_counts[q] = 0;
+    if (nq == 0) return YAMS_OK;
+    YB_ARG(queries && query_docs && out_docs && out_rowids && out_scores, "null argument");
+    YB_ARG(c->metric == YAMS_B200_COSINE, "document search is defined for the cosine scan");
+    if (pq) {
+        YB_ARG(pq->corpus == c, "the PQ index belongs to another corpus");
+        YB_ARG(c->generation == pq->corpus_generation, "the corpus changed after the PQ index was built: rebuild it (the reference marks the index dirty)");
+    }
+    YB_ARG(k <= 4096, "k > 4096 documents per query is not supported");
+    for (uint32_t q = 0; q < nq; ++q) YB_ARG(query_docs[q] <= query_docs[q + 1], "query_docs must be non-decreasing");
+    const uint64_t d0 = query_docs[0], d1 = query_docs[nq];
+    YB_ARG(d1 - d0 < 0xFFFFFFFFull, "too many documents in one call");
+    YB_ARG(doc_offsets, "null argument");
+    for (uint64_t i = d0; i < d1; ++i) {
+        YB_ARG(doc_offsets[i] <= doc_offsets[i + 1], "doc_offsets must be non-decreasing");
+        YB_ARG(doc_offsets[i + 1] - doc_offsets[i] < 0xFFFFFFFFull, "document too long");
+    }
+    const uint64_t total = doc_offsets[d1] - doc_offsets[d0];
+    YB_ARG(total == 0 || doc_rowids, "doc_rowids missing");
+    YB_ARG(total == 0 || rowids_unique_per_query(doc_rowids, doc_offsets, query_docs, nq),
+           "a rowid appears twice among one query's documents (documents are disjoint row sets)");
+    if (k == 0) return YAMS_OK;
+    c->pending.active = false;
+    // slices of <= kPqMaxBatch queries and a bounded number of (query, row) pairs; one host synchronisation each
+    const uint64_t kMaxPairs = 1ull << 26;
+    for (uint32_t q0 = 0; q0 < nq;) {
+        uint32_t q1 = q0 + 1;
+        while (q1 < nq && q1 - q0 < kPqMaxBatch && doc_offsets[query_docs[q1 + 1]] - doc_offsets[query_docs[q0]] <= kMaxPairs) ++q1;
+        yams_status_t rc = documents_slice(c, pq, queries, q0, q1, k, threshold, doc_rowids, doc_offsets, query_docs, out_docs, out_rowids, out_scores,
+                                           out_counts);
+        if (rc != YAMS_OK) {
+            for (uint32_t q = 0; q < nq; ++q) out_counts[q] = 0;
+            return rc;
+        }
+        q0 = q1;
+    }
+    return YAMS_OK;
+    YB_CATCH
+}
+
+}  // extern "C"

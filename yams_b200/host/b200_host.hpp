@@ -289,6 +289,7 @@ inline std::vector<ChunkValidationResult> validateChunks(const std::vector<std::
 struct VectorHit {
     int64_t rowid = -1;
     std::string chunk_id;
+    std::string document_hash;
     float relevance_score = 0.f;
 };
 
@@ -410,6 +411,58 @@ public:
         if (!allowed || allowed->empty()) return {};
         auto hits = allMatching(query.data(), similarity_threshold, *allowed);
         if (diagnostics) diagnostics->returnedRows = hits.size();
+        return hits;
+    }
+
+    // IDocumentCandidateVectorStore::searchDocumentCandidatesWithDiagnostics (vector_store.h:109-116), what
+    // CandidateFilterMode::DocumentTopK reaches (vector_database.cpp:553-569): the k best candidate DOCUMENTS, each represented
+    // by its best chunk (retainBestRecordPerDocument, sqlite_vec_backend.cpp:86-125).  The documents go to the device sorted by
+    // document_hash and their rows by chunk_id, so its position tie-breaks are the reference's.  pq: the PQ engine's branch
+    // (rows in the index, its rerank arithmetic); nullptr: the exact fallback.  std::invalid_argument on an empty candidate set
+    // (vector_database.cpp:554-557), a non-finite or zero query (exact mode) or a stale index (PQ mode).
+    std::vector<VectorHit> searchDocumentCandidates(const std::vector<float>& query, size_t k, float similarity_threshold,
+                                                    const std::unordered_set<std::string>& candidate_hashes, yams_b200_pq* pq = nullptr,
+                                                    VectorSearchDiagnostics* diagnostics = nullptr) {
+        if (query.size() != dim_) throw std::invalid_argument("query dimension mismatch");
+        if (candidate_hashes.empty()) throw std::invalid_argument("Document candidate search requires candidate hashes");
+        if (k > 4096) throw std::invalid_argument("k exceeds the device limit of 4096 documents per query");
+        std::vector<std::string> docs;
+        for (const auto& h : candidate_hashes)
+            if (rows_of_doc_.count(h)) docs.push_back(h);
+        std::sort(docs.begin(), docs.end());
+        std::vector<int64_t> rids;
+        std::vector<uint64_t> doffs{0};
+        for (const auto& h : docs) {
+            std::vector<int64_t> rs = rows_of_doc_.at(h);
+            std::sort(rs.begin(), rs.end(), [&](int64_t a, int64_t b) {
+                const std::string &ca = chunk_of_.at(a), &cb = chunk_of_.at(b);
+                return ca != cb ? ca < cb : a < b;
+            });
+            rids.insert(rids.end(), rs.begin(), rs.end());
+            doffs.push_back(rids.size());
+        }
+        if (diagnostics) {
+            noteScan(diagnostics);
+            diagnostics->rowsVisited += rids.size();
+        }
+        const uint64_t qdocs[2] = {0, docs.size()};
+        const size_t kk = std::max<size_t>(k, 1);
+        std::vector<int64_t> out_docs(kk), out_rid(kk);
+        std::vector<float> out_sc(kk);
+        uint32_t cnt = 0;
+        int64_t none = 0;
+        yams_status_t st = yams_b200_search_documents(c_, pq, query.data(), 1, (uint32_t)k, similarity_threshold, rids.empty() ? &none : rids.data(),
+                                                      doffs.data(), qdocs, out_docs.data(), out_rid.data(), out_sc.data(), &cnt);
+        if (st == YAMS_ERR_INVALID_ARG) throw std::invalid_argument(yams_b200_last_error());
+        if (st != YAMS_OK) throw_status("search_documents", st);
+        std::vector<VectorHit> hits(cnt);
+        for (uint32_t i = 0; i < cnt; ++i) {
+            hits[i].rowid = out_rid[i];
+            hits[i].relevance_score = out_sc[i];
+            hits[i].chunk_id = chunk_of_.at(out_rid[i]);
+            hits[i].document_hash = docs[(size_t)out_docs[i]];
+        }
+        if (diagnostics) diagnostics->returnedRows += hits.size();
         return hits;
     }
 
@@ -566,6 +619,8 @@ private:
             hits[i].relevance_score = sc[i];
             auto it = chunk_of_.find(rid[i]);
             hits[i].chunk_id = it == chunk_of_.end() ? std::string() : it->second;
+            auto dh = doc_of_.find(rid[i]);
+            if (dh != doc_of_.end()) hits[i].document_hash = dh->second;
         }
         std::stable_sort(hits.begin(), hits.end(), [](const VectorHit& a, const VectorHit& b) {
             if (a.relevance_score != b.relevance_score) return a.relevance_score > b.relevance_score;
