@@ -654,6 +654,17 @@ YAMS_B200_API yams_status_t yams_b200_debug_final(yams_b200_corpus* c, uint32_t 
 /* diagnostics: the per-query stage-1 error bound eps[q] of the last search / debug_stage1_scores call (HOST out) */
 YAMS_B200_API yams_status_t yams_b200_debug_last_eps(yams_b200_corpus* c, uint32_t nq, float* out);
 
+/* diagnostics: the PQ lookup tables of pq_search (normalised query, LUT[mi][ki] = dot(q_sub, centroid)) of nq queries (HOST
+ * in and out): out_lut[q * m * k + mi * k + ki], out_valid[q] = 0 when the query cannot be normalised (its table is then
+ * not used by a search). */
+YAMS_B200_API yams_status_t yams_b200_debug_pq_lut(yams_b200_pq* pq, const float* queries, uint32_t nq, float* out_lut,
+                                                   uint32_t* out_valid);
+/* diagnostics: the ADC pass the last yams_b200_pq_search batch took (the last slice of a call of more than 512 queries):
+ * out[0] = 1 for the filtered pass (sampled threshold, one pass over every row), 0 for the per-tile sorting pass;
+ * out[1] = queries per CTA of the filtered pass (1, 2 or 4); out[2] = the sampled tiles; out[3] = 1 when a filtered list
+ * overflowed and the selection was redone unfiltered.  All 0 after a call that did no device work. */
+YAMS_B200_API yams_status_t yams_b200_debug_pq_last_path(yams_b200_pq* pq, uint32_t* out);
+
 /* ---- misc ------------------------------------------------------------------------------------ */
 YAMS_B200_API int yams_b200_device_count(void);
 /* last error text of the calling thread (static storage) */

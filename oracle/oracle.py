@@ -356,12 +356,14 @@ def _pq_fns():
 
 def normalize_like_reference(rows: np.ndarray):
     """normalizeEmbeddingInPlace (src/vector/sqlite_vec_backend.cpp:213-226): sequential double sum of squares, rows with
-    norm_sq <= 1e-20 rejected, inv = 1.0f / sqrt(float(norm_sq)), float scale.  -> (normalised rows of the accepted, accepted mask)"""
+    norm_sq <= 1e-20 rejected (a NaN norm is not, so a row with a NaN element is accepted and normalises to NaN),
+    inv = 1.0f / sqrt(float(norm_sq)), float scale.  -> (normalised rows of the accepted, accepted mask)"""
     r = np.ascontiguousarray(rows, dtype=np.float32)
-    sq = np.cumsum(r.astype(np.float64) ** 2, axis=1)[:, -1]            # cumsum adds left to right, like the reference loop
-    ok = sq > 1e-20
-    inv = (np.float32(1.0) / np.sqrt(sq[ok].astype(np.float32))).astype(np.float32)
-    return (r[ok] * inv[:, None]).astype(np.float32), ok
+    with np.errstate(invalid="ignore", over="ignore", divide="ignore"):
+        sq = np.cumsum(r.astype(np.float64) ** 2, axis=1)[:, -1]        # cumsum adds left to right, like the reference loop
+        ok = ~(sq <= 1e-20)
+        inv = (np.float32(1.0) / np.sqrt(sq[ok].astype(np.float32))).astype(np.float32)
+        return (r[ok] * inv[:, None]).astype(np.float32), ok
 
 
 def pq_encode_ref(codebooks, dim, m, k, normalised_rows):

@@ -144,6 +144,8 @@ SYMBOLS = {
     "yams_b200_pq_codes": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, u64p]),
     "yams_b200_pq_destroy": (None, [C.c_void_p]),
     "yams_b200_debug_last_eps": (C.c_int, [C.c_void_p, C.c_uint32, f32p]),
+    "yams_b200_debug_pq_lut": (C.c_int, [C.c_void_p, f32p, C.c_uint32, f32p, u32p]),
+    "yams_b200_debug_pq_last_path": (C.c_int, [C.c_void_p, u32p]),
     "yams_b200_debug_select": (C.c_int, [C.c_void_p, C.c_uint32, f32p, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint32,
                                          C.c_void_p, u32p, C.c_uint32, f32p, C.c_uint32, C.c_int, C.c_float, C.c_int, C.c_void_p,
                                          u32p, f32p]),
@@ -740,6 +742,22 @@ class PqIndex:
                                                         out_s.ctypes.data_as(f32p), out_c.ctypes.data_as(u32p), out_f.ctypes.data_as(u64p)),
                    "pq_search_candidates")
         return out_r[:, :k], out_s[:, :k], out_c, out_f
+
+    def debug_lut(self, queries):
+        """-> (lookup tables f32[Q, m, k], valid u32[Q]) as pq_search computes them"""
+        q = np.ascontiguousarray(queries, dtype=np.float32).reshape(-1, self._corpus.dim)
+        nq = q.shape[0]
+        out = np.zeros((nq, self.m, self.k), dtype=np.float32)
+        valid = np.zeros(nq, dtype=np.uint32)
+        _check(lib().yams_b200_debug_pq_lut(self._h, q.ctypes.data_as(f32p), nq, out.ctypes.data_as(f32p), valid.ctypes.data_as(u32p)),
+               "debug_pq_lut")
+        return out, valid
+
+    def last_path(self) -> dict:
+        """the ADC pass the last search (without candidate lists) took: filtered, queries per CTA (qg), sampled tiles, rerun"""
+        out = (C.c_uint32 * 4)()
+        _check(lib().yams_b200_debug_pq_last_path(self._h, out), "debug_pq_last_path")
+        return {"filtered": bool(out[0]), "qg": int(out[1]), "sample_tiles": int(out[2]), "rerun": bool(out[3])}
 
     def close(self):
         if getattr(self, "_h", None):

@@ -47,7 +47,8 @@ __device__ __forceinline__ float load_row_elem(const void* rows, int dtype, uint
     return reinterpret_cast<const float*>(rows)[idx];
 }
 
-// one thread per corpus row: is it indexable (norm_sq > 1e-20)?  keep[row] = 1/0
+// one thread per corpus row: is it indexable (the rule of normalize_factor: not norm_sq <= 1e-20)?  keep[row] = 1/0.  A row
+// with a NaN element has a NaN norm: the reference indexes it (it encodes to code 0 everywhere and re-scores to NaN).
 __global__ void pq_keep_kernel(const void* __restrict__ rows, int dtype, uint32_t d, uint64_t n, uint32_t* __restrict__ keep) {
     uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= n) return;
@@ -56,7 +57,7 @@ __global__ void pq_keep_kernel(const void* __restrict__ rows, int dtype, uint32_
         float v = load_row_elem(rows, dtype, r * d + c);
         ss += (double)v * (double)v;
     }
-    keep[r] = ss > 1e-20 ? 1u : 0u;
+    keep[r] = ss <= 1e-20 ? 0u : 1u;
 }
 __global__ void pq_compact_kernel(const uint32_t* __restrict__ keep, const uint32_t* __restrict__ pos, uint64_t n, uint32_t* __restrict__ idx_rows) {
     uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -605,6 +606,7 @@ struct yams_b200_pq {
     // search workspace
     DevBuf q32, lut, valid, lists, counts, sel, exact, dout, tau;
     DevBuf cin, mapped, cidx, bits;   // candidate-set search: staged input, mapped rows, distinct positions, per-query seen bits
+    uint32_t last_path[4] = {0, 0, 0, 0};   // the path of the last pq_search batch (yams_b200_debug_pq_last_path)
     std::mutex mu;
 };
 
@@ -725,6 +727,7 @@ yams_status_t yams_b200_pq_search(yams_b200_pq* p, const float* queries, uint32_
     YB_BIND(c);
     for (uint32_t q = 0; q < nq; ++q) out_counts[q] = 0;
     if (out_flags) for (uint32_t q = 0; q < nq; ++q) out_flags[q] = 0;
+    for (uint32_t& v : p->last_path) v = 0;
     if (nq == 0 || k == 0 || p->n_idx == 0) return YAMS_OK;                           // :3873-3881
     YB_ARG(queries && out_rowids && out_scores, "null argument");
     YB_ARG(c->generation == p->corpus_generation, "the corpus changed after the PQ index was built: rebuild it (the reference marks the index dirty)");
@@ -792,6 +795,8 @@ static yams_status_t pq_search_batch(yams_b200_pq* p, const float* queries, uint
         launch_topk_lists(p->lists.as<Cand>(), d_counts, list_cap, nq, approx, d_sel, d_sel_n, st);
     };
     bool used_filter = false;
+    p->last_path[0] = filtered ? 1u : 0u;
+    p->last_path[1] = p->last_path[2] = p->last_path[3] = 0;
     if (filtered) {
         used_filter = true;
         const uint32_t stride = tiles / sample_tiles;
@@ -799,6 +804,8 @@ static yams_status_t pq_search_batch(yams_b200_pq* p, const float* queries, uint
         pq_tau_kernel<<<(nq + 127) / 128, 128, 0, st>>>(d_sel, d_sel_n, approx, nq, p->tau.as<uint64_t>(), d_counts);
         int qg = nq >= 4 ? 4 : (nq >= 2 ? 2 : 1);
         while (qg > 1 && (size_t)qg * lut_bytes > 200 * 1024) qg >>= 1;
+        p->last_path[1] = (uint32_t)qg;
+        p->last_path[2] = sample_tiles;
         const uint32_t groups = (nq + qg - 1) / qg;
         uint64_t chunks = std::max<uint64_t>(1, (uint64_t)c->dev->sm_count * 6 / groups);
         chunks = std::min<uint64_t>(chunks, (p->n_idx + 2047) / 2048);
@@ -819,6 +826,7 @@ static yams_status_t pq_search_batch(yams_b200_pq* p, const float* queries, uint
     for (int attempt = 0; attempt < 2; ++attempt) {
     if (attempt == 1) {
         // a filtered list overflowed: redo the selection without the filter
+        p->last_path[3] = 1;
         if ((rc = p->lists.reserve((size_t)nq * cap_unf * sizeof(Cand))) != YAMS_OK) return rc;
         unfiltered(tiles, 1, cap_unf);
     }
@@ -844,6 +852,44 @@ static yams_status_t pq_search_batch(yams_b200_pq* p, const float* queries, uint
     return YAMS_OK;
     YB_CATCH
 }
+
+extern "C" {
+
+yams_status_t yams_b200_debug_pq_lut(yams_b200_pq* p, const float* queries, uint32_t nq, float* out_lut, uint32_t* out_valid) {
+    YB_TRY
+    YB_ARG(p && (nq == 0 || (queries && out_lut && out_valid)), "null argument");
+    std::lock_guard<std::mutex> lk(p->mu);
+    yams_b200_corpus* c = p->corpus;
+    std::lock_guard<std::mutex> corpus_lock(c->mu);
+    YB_BIND(c);
+    if (nq == 0) return YAMS_OK;
+    cudaStream_t st = c->st;
+    yams_status_t rc;
+    const uint32_t m = p->m, kc = p->k, d = p->dim;
+    if ((rc = p->q32.reserve((size_t)nq * d * 4)) != YAMS_OK) return rc;
+    if ((rc = p->lut.reserve((size_t)nq * m * kc * 4)) != YAMS_OK) return rc;
+    if ((rc = p->valid.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
+    YB_CUDA(cudaMemcpyAsync(p->q32.p, queries, (size_t)nq * d * 4, cudaMemcpyHostToDevice, st));
+    YB_CUDA(cudaFuncSetAttribute(pq_lut_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(d * 4)));
+    pq_lut_kernel<<<nq, 256, d * 4, st>>>(p->q32.as<float>(), d, p->codebooks.as<float>(), m, kc, p->lut.as<float>(), p->valid.as<uint32_t>());
+    YB_CUDA(cudaGetLastError());
+    YB_CUDA(cudaMemcpyAsync(out_lut, p->lut.p, (size_t)nq * m * kc * 4, cudaMemcpyDeviceToHost, st));
+    YB_CUDA(cudaMemcpyAsync(out_valid, p->valid.p, (size_t)nq * 4, cudaMemcpyDeviceToHost, st));
+    YB_CUDA(cudaStreamSynchronize(st));
+    return YAMS_OK;
+    YB_CATCH
+}
+
+yams_status_t yams_b200_debug_pq_last_path(yams_b200_pq* p, uint32_t* out) {
+    YB_TRY
+    YB_ARG(p && out, "null argument");
+    std::lock_guard<std::mutex> lk(p->mu);
+    for (int i = 0; i < 4; ++i) out[i] = p->last_path[i];
+    return YAMS_OK;
+    YB_CATCH
+}
+
+}  // extern "C"
 
 // corpus row -> index position table of the handle (the caller holds both locks)
 static yams_status_t ensure_row_to_idx(yams_b200_pq* p, cudaStream_t st) {
