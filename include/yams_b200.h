@@ -624,6 +624,15 @@ YAMS_B200_API yams_status_t yams_b200_debug_stage1_candidates(yams_b200_corpus* 
                                                               const uint64_t* allowed_offsets, uint32_t* out_counts,
                                                               void* out_cands);
 
+/* diagnostics: one pass of the wgmma scan's profiling instantiation in filter mode over every row, as the search's corpus
+ * pass runs it (thresholds tau[q], lists of cap entries).  out_cycles[4 * b + i] for CTA b < out_info[1] (<= max_ctas):
+ * i = 0 cycles the first consumer warp waited for data (full barriers), 1 cycles the producer waited for a free stage
+ * (empty barriers), 2 the first consumer warp's epilogue cycles, 3 its total cycles.  out_info[0] = query-tile columns,
+ * out_info[1] = CTAs launched; out_ms = device time of the profiled launch (the counters slow it slightly). */
+YAMS_B200_API yams_status_t yams_b200_debug_stage1_profile(yams_b200_corpus* c, const float* queries, uint32_t nq,
+                                                           const float* tau, uint32_t cap, uint32_t max_ctas,
+                                                           uint64_t* out_cycles, uint32_t* out_info, float* out_ms);
+
 /* diagnostics: the search's top-K selection on caller-supplied scores (HOST in and out).  Input per query q, either
  *   dense (dense != NULL): dense[q * ld + i], i < len, row index row_start + i * row_stride; the device copy starts
  *                          dense_shift (0..3) floats past a 16-byte boundary, or

@@ -144,6 +144,7 @@ SYMBOLS = {
     "yams_b200_pq_codes": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, u64p]),
     "yams_b200_pq_destroy": (None, [C.c_void_p]),
     "yams_b200_debug_last_eps": (C.c_int, [C.c_void_p, C.c_uint32, f32p]),
+    "yams_b200_debug_stage1_profile": (C.c_int, [C.c_void_p, f32p, C.c_uint32, f32p, C.c_uint32, C.c_uint32, u64p, u32p, f32p]),
     "yams_b200_debug_pq_lut": (C.c_int, [C.c_void_p, f32p, C.c_uint32, f32p, u32p]),
     "yams_b200_debug_pq_last_path": (C.c_int, [C.c_void_p, u32p]),
     "yams_b200_debug_select": (C.c_int, [C.c_void_p, C.c_uint32, f32p, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint32,
@@ -622,6 +623,21 @@ class Corpus:
                                            out_s.ctypes.data_as(f32p), out_c.ctypes.data_as(u32p), out_f.ctypes.data_as(u64p),
                                            queued.ctypes.data_as(u32p), C.byref(nqd)), "debug_final")
         return out_r, out_s, out_c, out_f, queued[:nqd.value].copy()
+
+    def debug_stage1_profile(self, queries, tau, cap: int, max_ctas: int = 1024):
+        """One profiled wgmma pass in filter mode over every row -> (cycles u64[CTAs, 4] = consumer full-barrier wait,
+        producer empty-barrier wait, epilogue, total; the launch layout {n_tile, ctas}; device ms)."""
+        q = np.ascontiguousarray(queries, dtype=np.float32)
+        nq = q.shape[0]
+        t = np.ascontiguousarray(tau, dtype=np.float32).reshape(nq)
+        cyc = np.zeros((max_ctas, 4), dtype=np.uint64)
+        info = np.zeros(2, dtype=np.uint32)
+        ms = C.c_float(0.0)
+        _check(lib().yams_b200_debug_stage1_profile(self._h, q.ctypes.data_as(f32p), nq, t.ctypes.data_as(f32p), cap, max_ctas,
+                                                    cyc.ctypes.data_as(u64p), info.ctypes.data_as(u32p), C.byref(ms)),
+               "debug_stage1_profile")
+        layout = {"n_tile": int(info[0]), "ctas": int(info[1])}
+        return cyc[:layout["ctas"]].copy(), layout, float(ms.value)
 
     def debug_last_eps(self, nq: int) -> np.ndarray:
         out = np.empty(nq, dtype=np.float32)

@@ -1217,7 +1217,7 @@ __global__ void iota_rowids_kernel(int64_t* p, uint64_t n, int64_t first) {
 namespace yb {
 
 // wgmma engine (knn_umma.cu); returns YAMS_ERR_UNSUPPORTED when the shape is not covered
-yams_status_t stage1_wgmma(Corpus* c, const Stage1Args& a, bool filter, cudaStream_t st);
+yams_status_t stage1_wgmma(Corpus* c, const Stage1Args& a, bool filter, cudaStream_t st, unsigned long long* prof = nullptr);
 bool wgmma_supported(const Corpus* c, uint32_t nq);
 
 constexpr uint32_t kMaxK = 3072;          // K' = k + max(16, k/4) rounded to 32 must fit SEL_MAXK
@@ -2296,6 +2296,43 @@ yams_status_t yams_b200_debug_stage1_candidates(yams_b200_corpus* c, const float
     YB_CUDA(cudaMemcpyAsync(out_counts, c->counts.p, (size_t)nq * 4, cudaMemcpyDeviceToHost, c->st));
     if (cb) YB_CUDA(cudaMemcpyAsync(out_cands, c->cands.p, cb, cudaMemcpyDeviceToHost, c->st));
     YB_CUDA(cudaStreamSynchronize(c->st));
+    return YAMS_OK;
+}
+
+// diagnostics: one pass of the profiling instantiation of the wgmma scan in filter mode over every row (the search's corpus
+// pass) -> per-CTA cycle counters, the launch's layout and its device time (HOST out), see include/yams_b200.h
+yams_status_t yams_b200_debug_stage1_profile(yams_b200_corpus* c, const float* queries, uint32_t nq, const float* tau, uint32_t cap,
+                                             uint32_t max_ctas, uint64_t* out_cycles, uint32_t* out_info, float* out_ms) {
+    YB_ARG(c && queries && tau && out_cycles && out_info && out_ms && nq > 0, "bad argument");
+    std::lock_guard<std::mutex> corpus_lock(c->mu);
+    YB_ARG(c->n > 0, "empty corpus");
+    yams_status_t rc;
+    YB_BIND(c);
+    c->pending.active = false;
+    if ((rc = prepare_queries(c, queries, false, nq)) != YAMS_OK) return rc;
+    const size_t cb = (size_t)nq * cap * sizeof(Cand);
+    const size_t pb = (size_t)c->dev->sm_count * 4 * sizeof(unsigned long long);
+    if ((rc = c->eps.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
+    if ((rc = c->tau.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
+    if ((rc = c->cands.reserve(cb + 8)) != YAMS_OK) return rc;
+    if ((rc = c->dense.reserve(pb)) != YAMS_OK) return rc;
+    YB_CUDA(cudaMemcpyAsync(c->tau.p, tau, (size_t)nq * 4, cudaMemcpyHostToDevice, c->st));
+    YB_CUDA(cudaMemsetAsync(c->counts.p, 0, (size_t)nq * 4, c->st));
+    YB_CUDA(cudaMemsetAsync(c->dense.p, 0, pb, c->st));
+    Stage1Args a{};
+    fill_stage1_common(c, a, nq);
+    a.row_start = 0; a.row_stride = 1; a.nrows = c->n;
+    a.tau = c->tau.as<float>(); a.cands = c->cands.as<Cand>(); a.cap = cap; a.counts = c->counts.as<uint32_t>();
+    c->scan_timed = false;
+    YB_CUDA(cudaEventRecord(c->ev_scan[0], c->st));
+    if ((rc = stage1_wgmma(c, a, true, c->st, reinterpret_cast<unsigned long long*>(c->dense.p))) != YAMS_OK) return rc;
+    YB_CUDA(cudaEventRecord(c->ev_scan[1], c->st));
+    const uint32_t ctas = c->wg_launch[1];
+    YB_ARG(ctas <= max_ctas, "max_ctas is below the launch's CTA count");
+    YB_CUDA(cudaMemcpyAsync(out_cycles, c->dense.p, (size_t)ctas * 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, c->st));
+    YB_CUDA(cudaStreamSynchronize(c->st));
+    YB_CUDA(cudaEventElapsedTime(out_ms, c->ev_scan[0], c->ev_scan[1]));
+    out_info[0] = c->wg_launch[0]; out_info[1] = c->wg_launch[1];
     return YAMS_OK;
 }
 

@@ -46,6 +46,7 @@ struct Corpus {
     cudaEvent_t ev_scan[2] = {nullptr, nullptr};  // around the full-corpus filtered scan launch
     bool scan_timed = false;
     float last_ms[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    uint32_t wg_launch[2] = {0, 0};   // the last wgmma scan launch: query-tile columns, CTAs
     std::mutex mu;   // public entry points on one corpus are serialised (the workspace buffers are per corpus)
     size_t elem() const { return dtype == YAMS_B200_F16 ? 2 : 4; }
 };

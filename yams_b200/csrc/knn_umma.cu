@@ -32,6 +32,10 @@ constexpr int UM_MMAS_PER_KBLOCK = 4;    // 4 x 32 bytes of K: 4 x (K=16 fp16) o
 constexpr int UM_THREADS = 384;          // 3 warpgroups: TMA producer + 2 x (wgmma + epilogue)
 constexpr uint32_t UM_A_STAGE = UM_BLOCK_M * UM_BLOCK_K_BYTES;   // 16 KiB
 constexpr uint32_t UM_SMEM_LIMIT = 227 * 1024;                   // opt-in shared memory per block on sm_90
+// query columns per threshold group of the epilogue's pre-filter: 32 for fp16; the whole tile for tf32, whose MMAs take twice
+// as long (the finer groups measured no faster there)
+constexpr int UM_TAU_GROUP = 32;
+constexpr int UM_MAX_TAU_GROUPS = 4096 / UM_TAU_GROUP;
 constexpr long long UM_WAIT_LIMIT_CYCLES = 4000000000ll;
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -155,19 +159,22 @@ struct WgArgs {
     uint32_t nrt;         // corpus row tiles of UM_BLOCK_M rows
     uint32_t kblocks;     // ceil(dim / block_k)
     uint32_t stages;
+    unsigned long long* prof;   // PROF: per CTA {consumer full-barrier wait, producer empty-barrier wait, epilogue, total} cycles
 };
 
-template <bool FILTER, int N, bool TF32>
+template <bool FILTER, int N, bool TF32, bool PROF>
 __global__ void __launch_bounds__(UM_THREADS, 1)
 stage1_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, WgArgs u) {
+    const long long t_start = PROF ? clock64() : 0;
+    constexpr int TG = TF32 ? N : UM_TAU_GROUP;
     constexpr uint32_t B_STAGE = N * UM_BLOCK_K_BYTES;
     constexpr uint32_t STAGE = UM_A_STAGE + B_STAGE;
     extern __shared__ uint8_t smem_raw[];
     // 1024-byte alignment for the 128B-swizzled tiles
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)u.stages * STAGE);
-    float* tmin_s = reinterpret_cast<float*>(bars + 2 * u.stages);   // [32] smallest threshold of each query tile
-    float* tau_all = tmin_s + 32;                                     // [nqt * N] thresholds (+inf past nq)
+    float* tmin_s = reinterpret_cast<float*>(bars + 2 * u.stages);   // smallest threshold of each group of 32 query columns
+    float* tau_all = tmin_s + UM_MAX_TAU_GROUPS;                      // [nqt * N] thresholds (+inf past nq)
     const uint32_t tiles_u = smem_u32(smem);
     const uint32_t full_u = smem_u32(bars), empty_u = full_u + 8u * u.stages;
 
@@ -187,9 +194,9 @@ stage1_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         const uint32_t nqpad = u.nqt * N;
         for (uint32_t i = threadIdx.x; i < nqpad; i += UM_THREADS) tau_all[i] = i < u.a.nq ? __ldg(&u.a.tau[i]) : INFINITY;
         __syncthreads();
-        for (uint32_t t = threadIdx.x; t < u.nqt; t += UM_THREADS) {
+        for (uint32_t t = threadIdx.x; t < nqpad / TG; t += UM_THREADS) {
             float m = INFINITY;
-            for (uint32_t c = 0; c < N; ++c) m = fminf(m, tau_all[t * N + c]);
+            for (uint32_t c = 0; c < TG; ++c) m = fminf(m, tau_all[t * TG + c]);
             tmin_s[t] = m;
         }
     }
@@ -199,6 +206,7 @@ stage1_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         // ===================== TMA producer =====================
         asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
         if (threadIdx.x == 0) {
+            long long w_empty = 0;
             uint32_t s = 0, ph = 0;
             const int block_k = UM_BLOCK_K_BYTES / (TF32 ? 4 : 2);
             for (uint32_t rt = blockIdx.x; rt < u.nrt; rt += gridDim.x) {
@@ -210,7 +218,7 @@ stage1_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
                     const bool pf = qt == 0 && have_next;
                     int kc = 0;
                     for (uint32_t kb = 0; kb < u.kblocks; ++kb, kc += block_k) {
-                        mbar_wait_u<false>(empty_u + 8u * s, ph ^ 1u, nullptr);
+                        mbar_wait_u<PROF>(empty_u + 8u * s, ph ^ 1u, &w_empty);
                         uint8_t* sa = smem + (size_t)s * STAGE;
                         mbar_expect_tx_u(full_u + 8u * s, STAGE);
                         tma_load_2d(sa, &tmA, &bars[s], kc, a_row);
@@ -220,6 +228,7 @@ stage1_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
                     }
                 }
             }
+            if (PROF) u.prof[4 * blockIdx.x + 1] = (unsigned long long)w_empty;
         }
     } else {
         // ===================== consumers: wgmma + epilogue =====================
@@ -234,11 +243,12 @@ stage1_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         float acc[N / 2];
 #pragma unroll
         for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+        long long w_full = 0, t_epi = 0;
         uint32_t s = 0, ph = 0;
         for (uint32_t rt = blockIdx.x; rt < u.nrt; rt += gridDim.x) {
             // per-row data of this thread's two rows (row_in_tile and row_in_tile + 8)
             uint64_t li[2], grow[2];
-            float alpha[2], beta[2];
+            float alpha[2], beta[2], ialpha[2], ealpha[2];
             bool rvalid[2], rowok[2];
 #pragma unroll
             for (int r = 0; r < 2; ++r) {
@@ -251,11 +261,13 @@ stage1_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
                 alpha[r] = l2 ? 2.f : inr;
                 beta[r] = l2 ? -inr : 0.f;
                 rowok[r] = rvalid[r] && (l2 ? inr < INFINITY : inr > 0.f);
+                ialpha[r] = 1.0f / alpha[r];
+                ealpha[r] = 2e-6f / alpha[r];
             }
             for (uint32_t qt = 0; qt < u.nqt; ++qt) {
                 uint32_t prev = 0;
                 for (uint32_t kb = 0; kb < u.kblocks; ++kb) {
-                    mbar_wait_u<false>(full_u + 8u * s, ph, nullptr);
+                    mbar_wait_u<PROF>(full_u + 8u * s, ph, &w_full);
                     const uint32_t sa = tiles_u + s * STAGE;
                     const uint64_t adesc = desc_hi | (uint64_t)(((sa + cw * (UM_A_STAGE / 2)) >> 4) & 0x3FFFu);
                     const uint64_t bdesc = desc_hi | (uint64_t)(((sa + UM_A_STAGE) >> 4) & 0x3FFFu);
@@ -276,34 +288,43 @@ stage1_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
                 wgmma_wait<0>();
                 if (lane == 0) mbar_arrive_u(empty_u + 8u * prev);
 
+                const long long t_epi0 = PROF ? clock64() : 0;
                 const uint32_t q0 = qt * N;
                 if (FILTER) {
                     const float* tau_t = tau_all + q0;
+                    const float* tmin_t = tmin_s + q0 / TG;
+                    // per group of TG query columns (TG / 4 of this thread's accumulators per row) and row, a conservative bound:
+                    // acc * alpha + beta > tau_q  =>  acc > (tmin - beta) / alpha (slightly relaxed), tmin = the group's
+                    // smallest threshold.  Only groups whose maximum passes take the per-column test and the append.
 #pragma unroll
-                    for (int r = 0; r < 2; ++r) {
-                        // conservative row-level bound: acc * alpha + beta > tau_q  =>  acc > (tmin - beta) / alpha (slightly relaxed)
-                        float bound = INFINITY;
-                        if (rowok[r]) {
-                            const float b0 = (tmin_s[qt] - beta[r]) * (1.0f / alpha[r]);
-                            bound = b0 - (fabsf(tmin_s[qt]) + fabsf(beta[r])) * (2e-6f / alpha[r]) - 1e-30f;
-                        }
-                        float m = acc[2 * r];
+                    for (int h = 0; h < N / TG; ++h) {
+                        const float tmin = tmin_t[h];
 #pragma unroll
-                        for (int j = 0; j < N / 8; ++j) m = fmaxf(m, fmaxf(acc[4 * j + 2 * r], acc[4 * j + 2 * r + 1]));
-                        if (m > bound) {   // rare: some column of this row may survive
+                        for (int r = 0; r < 2; ++r) {
+                            float bound = INFINITY;
+                            if (rowok[r]) {
+                                const float b0 = (tmin - beta[r]) * ialpha[r];
+                                bound = b0 - (fabsf(tmin) + fabsf(beta[r])) * ealpha[r] - 1e-30f;
+                            }
+                            constexpr int J = TG / 8;   // accumulator column pairs per group
+                            float m = acc[4 * J * h + 2 * r];
 #pragma unroll
-                            for (int j = 0; j < N / 8; ++j) {
+                            for (int j = J * h; j < J * (h + 1); ++j) m = fmaxf(m, fmaxf(acc[4 * j + 2 * r], acc[4 * j + 2 * r + 1]));
+                            if (m > bound) {   // rare: some column of this group may survive
 #pragma unroll
-                                for (int e = 0; e < 2; ++e) {
-                                    const uint32_t c = 8 * j + col0 + e;
-                                    const float sc = fmaf(acc[4 * j + 2 * r + e], alpha[r], beta[r]);
-                                    if (sc > tau_t[c]) {
-                                        const uint32_t q = q0 + c;
-                                        if (direct) {
-                                            const uint32_t w = __ldg(&u.a.mask[(uint64_t)q * u.a.mask_ld + (grow[r] >> 5)]);
-                                            if (!((w >> (grow[r] & 31)) & 1u)) continue;
+                                for (int j = J * h; j < J * (h + 1); ++j) {
+#pragma unroll
+                                    for (int e = 0; e < 2; ++e) {
+                                        const uint32_t c = 8 * j + col0 + e;
+                                        const float sc = fmaf(acc[4 * j + 2 * r + e], alpha[r], beta[r]);
+                                        if (sc > tau_t[c]) {
+                                            const uint32_t q = q0 + c;
+                                            if (direct) {
+                                                const uint32_t w = __ldg(&u.a.mask[(uint64_t)q * u.a.mask_ld + (grow[r] >> 5)]);
+                                                if (!((w >> (grow[r] & 31)) & 1u)) continue;
+                                            }
+                                            append_candidate(u.a.counts, u.a.cands, u.a.cap, q, (uint32_t)grow[r], sc);
                                         }
-                                        append_candidate(u.a.counts, u.a.cands, u.a.cap, q, (uint32_t)grow[r], sc);
                                     }
                                 }
                             }
@@ -325,7 +346,13 @@ stage1_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
                         }
                     }
                 }
+                if (PROF) t_epi += clock64() - t_epi0;
             }
+        }
+        if (PROF && threadIdx.x == 128) {   // the first consumer warp's view
+            u.prof[4 * blockIdx.x + 0] = (unsigned long long)w_full;
+            u.prof[4 * blockIdx.x + 2] = (unsigned long long)t_epi;
+            u.prof[4 * blockIdx.x + 3] = (unsigned long long)(clock64() - t_start);
         }
     }
 }
@@ -429,11 +456,11 @@ bool wgmma_supported(const Corpus* c, uint32_t nq) {
     return c->dtype == YAMS_B200_F16 ? (c->dim % 8 == 0) : (c->dim % 4 == 0 && !getenv("YAMS_B200_DISABLE_TF32"));
 }
 
-template <bool FILTER, int N, bool TF32>
+template <bool FILTER, int N, bool TF32, bool PROF>
 static yams_status_t launch_wgmma(const CUtensorMap& tmA, const CUtensorMap& tmB, const WgArgs& u, unsigned grid, size_t smem,
                                   cudaStream_t st) {
-    YB_CUDA(cudaFuncSetAttribute(stage1_wgmma_kernel<FILTER, N, TF32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    stage1_wgmma_kernel<FILTER, N, TF32><<<grid, UM_THREADS, smem, st>>>(tmA, tmB, u);
+    YB_CUDA(cudaFuncSetAttribute(stage1_wgmma_kernel<FILTER, N, TF32, PROF>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    stage1_wgmma_kernel<FILTER, N, TF32, PROF><<<grid, UM_THREADS, smem, st>>>(tmA, tmB, u);
     YB_CUDA(cudaGetLastError());
     return YAMS_OK;
 }
@@ -441,11 +468,16 @@ static yams_status_t launch_wgmma(const CUtensorMap& tmA, const CUtensorMap& tmB
 template <int N>
 static yams_status_t launch_wgmma_n(const CUtensorMap& tmA, const CUtensorMap& tmB, const WgArgs& u, unsigned grid, size_t smem,
                                     bool filter, bool tf32, cudaStream_t st) {
-    if (filter) return tf32 ? launch_wgmma<true, N, true>(tmA, tmB, u, grid, smem, st) : launch_wgmma<true, N, false>(tmA, tmB, u, grid, smem, st);
-    return tf32 ? launch_wgmma<false, N, true>(tmA, tmB, u, grid, smem, st) : launch_wgmma<false, N, false>(tmA, tmB, u, grid, smem, st);
+    if (u.prof) {   // the profiling instantiation: filter mode, as the search's corpus pass runs it
+        if (!filter) return YAMS_ERR_UNSUPPORTED;
+        return tf32 ? launch_wgmma<true, N, true, true>(tmA, tmB, u, grid, smem, st) : launch_wgmma<true, N, false, true>(tmA, tmB, u, grid, smem, st);
+    }
+    if (filter)
+        return tf32 ? launch_wgmma<true, N, true, false>(tmA, tmB, u, grid, smem, st) : launch_wgmma<true, N, false, false>(tmA, tmB, u, grid, smem, st);
+    return tf32 ? launch_wgmma<false, N, true, false>(tmA, tmB, u, grid, smem, st) : launch_wgmma<false, N, false, false>(tmA, tmB, u, grid, smem, st);
 }
 
-yams_status_t stage1_wgmma(Corpus* c, const Stage1Args& a, bool filter, cudaStream_t st) {
+yams_status_t stage1_wgmma(Corpus* c, const Stage1Args& a, bool filter, cudaStream_t st, unsigned long long* prof) {
     const bool tf32 = a.dtype == YAMS_B200_F32;
     const uint32_t esz = tf32 ? 4 : 2;
     if ((a.dim * esz) % 16 != 0 || a.nrows == 0 || a.nq == 0) return YAMS_ERR_UNSUPPORTED;
@@ -471,13 +503,14 @@ yams_status_t stage1_wgmma(Corpus* c, const Stage1Args& a, bool filter, cudaStre
     const uint32_t n_tile = a.nq <= 64 ? 64 : 256;
     WgArgs u{};
     u.a = a;
+    u.prof = prof;
     u.nqt = (a.nq + n_tile - 1) / n_tile;
     u.nrt = (uint32_t)((a.nrows + UM_BLOCK_M - 1) / UM_BLOCK_M);
     const uint32_t block_k = UM_BLOCK_K_BYTES / esz;
     u.kblocks = (a.dim + block_k - 1) / block_k;
     if (u.nqt > 32 || (size_t)u.nqt * n_tile > 4096) return YAMS_ERR_UNSUPPORTED;   // thresholds live in shared memory
     const uint32_t stage_bytes = UM_A_STAGE + n_tile * UM_BLOCK_K_BYTES;
-    const size_t fixed = 1024 /*align slack*/ + 32 * 4 + (size_t)u.nqt * n_tile * 4;
+    const size_t fixed = 1024 /*align slack*/ + UM_MAX_TAU_GROUPS * 4 + (size_t)u.nqt * n_tile * 4;
     u.stages = std::min<uint32_t>(8, (uint32_t)((UM_SMEM_LIMIT - fixed - 16 * 8) / (stage_bytes + 16)));
     if (u.stages < 2) return YAMS_ERR_UNSUPPORTED;
     const size_t smem = (size_t)u.stages * (stage_bytes + 16) + fixed;
@@ -489,6 +522,7 @@ yams_status_t stage1_wgmma(Corpus* c, const Stage1Args& a, bool filter, cudaStre
     if (!make_map_2d(&tmB, d_q16, a.dim, a.nq, (uint64_t)a.dim * esz, block_k, n_tile, tf32)) return YAMS_ERR_UNSUPPORTED;
 
     const unsigned grid = (unsigned)std::min<uint64_t>(u.nrt, (uint64_t)c->dev->sm_count);
+    c->wg_launch[0] = n_tile; c->wg_launch[1] = grid;
     if (n_tile == 64) return launch_wgmma_n<64>(tmA, tmB, u, grid, smem, filter, tf32, st);
     return launch_wgmma_n<256>(tmA, tmB, u, grid, smem, filter, tf32, st);
 }
