@@ -32,17 +32,24 @@ def corpus_of_texts(rng, n):
     return texts
 
 
-@pytest.mark.parametrize("cfg", [
+SIMEON_CFGS = [
     dict(),                                                         # simeon-v1-384: what YAMS runs
     dict(sketch_dim=8192, output_dim=768),                          # the 768-d variant of BASELINE config C2
     dict(ngram_min=1, ngram_max=8),                                 # 8-byte grams take the whole-word hash path
     dict(ngram_min=7, ngram_max=12, sketch_dim=5000, output_dim=100),   # > 8 bytes: word + tail; non-power-of-two sketch (modulo bucket)
     dict(l2_normalize=0, output_dim=33),                            # raw projection, odd dimension (scalar tail of the normaliser unused)
     dict(output_dim=40),                                            # 40 = 2 x 16 + 8: the normaliser's fused tail
-])
+]
+
+
+def simeon_texts(cfg):
+    """the texts of test_simeon_encoder_is_bit_identical at one configuration"""
+    return corpus_of_texts(np.random.default_rng(len(cfg) + 1), 300)
+
+
+@pytest.mark.parametrize("cfg", SIMEON_CFGS)
 def test_simeon_encoder_is_bit_identical(Y, cfg):
-    rng = np.random.default_rng(len(cfg) + 1)
-    texts = corpus_of_texts(rng, 300)
+    texts = simeon_texts(cfg)
     enc = Y.SimeonEncoder(**cfg)
     got = enc.encode(texts)
     want = ref_checks.load()["simeon_encoder"][ref_checks.key(cfg)]
@@ -71,7 +78,7 @@ def test_simeon_embeddings_feed_the_scan(Y):
     enc.close()
 
 
-@pytest.mark.parametrize("cfg", [
+YAMS_PROFILE_CFGS = [
     dict(profile="yams-default"),                                                     # unconfigured YAMS: CharAndWord + Fwht, 4096 -> 1024
     dict(profile="yams-default", embedding_dim=384),
     dict(profile="yams-default", embedding_dim=768, sketch_dim=8192),
@@ -79,12 +86,25 @@ def test_simeon_embeddings_feed_the_scan(Y):
     dict(profile="yams-default", embedding_dim=4096),                                 # output_dim == pad_n: every coordinate sampled
     dict(flags=1),                                                                    # word tokens with the Achlioptas projection
     dict(flags=2, output_dim=40, l2_normalize=0),                                     # Fwht without word tokens, raw output
-])
+]
+
+
+def yams_profile_texts():
+    """the texts of test_simeon_yams_default_profile_is_bit_identical"""
+    rng = np.random.default_rng(123)
+    return corpus_of_texts(rng, 300) + [b"_", b"a_b c-d e.f 0x1F", b"word" * 3000, b"  leading and trailing  ", "Größe_42 naïve".encode()]
+
+
+# the arrays of tests/golden/simeon_golden.json and the encoder each was made with
+GOLDEN_PROFILES = (("simeon_v1_384", dict()), ("yams_default_1024", dict(profile="yams-default")),
+                   ("yams_default_384", dict(profile="yams-default", embedding_dim=384)))
+
+
+@pytest.mark.parametrize("cfg", YAMS_PROFILE_CFGS)
 def test_simeon_yams_default_profile_is_bit_identical(Y, cfg):
     """The encoder an unconfigured YAMS builds (simeon_embedding_backend.cpp:18-47,118-135): byte n-grams + word tokens, count
     sketch, FWHT projection, L2 -- against simeon's own Encoder with ngram_mode / projection set the same way."""
-    rng = np.random.default_rng(123)
-    texts = corpus_of_texts(rng, 300) + [b"_", b"a_b c-d e.f 0x1F", b"word" * 3000, b"  leading and trailing  ", "Größe_42 naïve".encode()]
+    texts = yams_profile_texts()
     enc = Y.SimeonEncoder(**cfg)
     got = enc.encode(texts)
     want = ref_checks.load()["simeon_yams_profile"][ref_checks.key(cfg)]
@@ -103,8 +123,7 @@ def test_simeon_matches_the_committed_golden_embeddings(Y):
     import os
     g = json.load(open(os.path.join(os.path.dirname(__file__), "golden", "simeon_golden.json")))
     texts = g["texts"]
-    for key, kw in (("simeon_v1_384", dict()), ("yams_default_1024", dict(profile="yams-default")),
-                    ("yams_default_384", dict(profile="yams-default", embedding_dim=384))):
+    for key, kw in GOLDEN_PROFILES:
         enc = Y.SimeonEncoder(**kw)
         got = enc.encode(texts).view(np.uint32)
         assert np.array_equal(got, np.array(g[key], dtype=np.uint32)), key

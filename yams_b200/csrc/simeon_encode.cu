@@ -19,7 +19,8 @@
 // is a hash of the pair: -1 with probability 1/6, +1 with 1/6; the reference sums the sketch values under each sign in int64 and
 // multiplies ONCE by sqrt(3)/sqrt(output_dim) in float.  Only the L2 normalisation is a float reduction; it follows the lane
 // structure of the AVX2 kernel.  The output is therefore bit-identical to the reference encoder
-// (tests/test_gpu_simeon.py pins it against simeon's own sources compiled in place).
+// (tests/test_gpu_simeon.py pins it against simeon's own sources compiled in place; tests/test_gpu_simeon_restated.py against a
+// numpy restatement of the encoder at any configuration).
 // Fwht: the sketch, zero-padded to a power of two and multiplied by a +-1 diagonal, goes through the in-place Walsh-Hadamard
 // butterflies in shared memory (same stage order and the same x + y / x - y per butterfly as fwht_inplace, so every float is the
 // reference's), output_dim sampled coordinates are scaled by 1/sqrt(output_dim).
@@ -212,6 +213,23 @@ __global__ void __launch_bounds__(ENC_THREADS) simeon_encode_kernel(EncArgs a) {
     }
 }
 
+// The dynamic shared-memory limit is an attribute of the kernel, shared by every encoder and host thread of the process.  Set
+// per call to the caller's own size, one thread could lower it between another thread's set and launch, and that launch
+// would fail.  So it is raised once per device, to the largest layout any accepted configuration needs (sketch_dim 16384,
+// output_dim 4096): the attribute permits that much, it reserves nothing -- each launch still asks for its own size.
+constexpr size_t ENC_SMEM_MAX = (size_t)16384 * 4 * 2 + (size_t)4096 * 4 + 64;
+constexpr int ENC_MAX_DEVICES = 64;
+
+cudaError_t enc_allow_max_smem(int device) {
+    static std::once_flag once[ENC_MAX_DEVICES];
+    static cudaError_t rc[ENC_MAX_DEVICES];
+    if (device < 0 || device >= ENC_MAX_DEVICES) return cudaErrorInvalidDevice;
+    std::call_once(once[device], [device] {
+        rc[device] = cudaFuncSetAttribute(simeon_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ENC_SMEM_MAX);
+    });
+    return rc[device];
+}
+
 }  // namespace yb
 
 using namespace yb;
@@ -379,7 +397,7 @@ yams_status_t yams_b200_simeon_encode(yams_b200_encoder* e, const char* const* t
     a.sample = e->sample.as<uint32_t>();
     a.fwht_scale = e->fwht_scale;
     const size_t smem = (size_t)e->cfg.sketch_dim * 4 + (size_t)std::max(e->cfg.sketch_dim, e->pad_n) * 4 + (size_t)D * 4 + 64;
-    YB_CUDA(cudaFuncSetAttribute(simeon_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    YB_CUDA(enc_allow_max_smem(e->dev->device));
     const unsigned grid = (unsigned)std::min<size_t>(n, (size_t)e->dev->sm_count * 8);
     simeon_encode_kernel<<<grid, ENC_THREADS, smem, st>>>(a);
     YB_CUDA(cudaGetLastError());
