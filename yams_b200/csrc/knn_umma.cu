@@ -50,6 +50,14 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
         ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
         : "memory");
 }
+// the same load with an L2 eviction policy (createpolicy) for the lines it reads
+__device__ __forceinline__ void tma_load_2d_hint(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1,
+                                                 uint64_t policy) {
+    asm volatile(
+        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4}], [%2], %5;"
+        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "l"(policy)
+        : "memory");
+}
 // pull a tile into L2 ahead of time (no shared-memory destination, no barrier)
 __device__ __forceinline__ void tma_prefetch_2d(const CUtensorMap* map, int c0, int c1) {
     asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];"
@@ -209,6 +217,11 @@ stage1_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
             long long w_empty = 0;
             uint32_t s = 0, ph = 0;
             const int block_k = UM_BLOCK_K_BYTES / (TF32 ? 4 : 2);
+            // A corpus tile is read from L2 once per query tile.  Its last read marks its lines evict-first: with every
+            // CTA's current and prefetched next tile (~50 MB at C2) the L2 is full, and a dead tile should leave before a
+            // live one is pushed out and fetched from HBM again.
+            uint64_t last_use;
+            asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(last_use));
             for (uint32_t rt = blockIdx.x; rt < u.nrt; rt += gridDim.x) {
                 const int a_row = (int)(rt * UM_BLOCK_M);
                 const int a_next = (int)((rt + gridDim.x) * UM_BLOCK_M);
@@ -216,12 +229,14 @@ stage1_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
                 for (uint32_t qt = 0; qt < u.nqt; ++qt) {
                     const int b_row = (int)(qt * N);
                     const bool pf = qt == 0 && have_next;
+                    const bool a_last = qt + 1 == u.nqt;
                     int kc = 0;
                     for (uint32_t kb = 0; kb < u.kblocks; ++kb, kc += block_k) {
                         mbar_wait_u<PROF>(empty_u + 8u * s, ph ^ 1u, &w_empty);
                         uint8_t* sa = smem + (size_t)s * STAGE;
                         mbar_expect_tx_u(full_u + 8u * s, STAGE);
-                        tma_load_2d(sa, &tmA, &bars[s], kc, a_row);
+                        if (a_last) tma_load_2d_hint(sa, &tmA, &bars[s], kc, a_row, last_use);
+                        else tma_load_2d(sa, &tmA, &bars[s], kc, a_row);
                         tma_load_2d(sa + UM_A_STAGE, &tmB, &bars[s], kc, b_row);
                         if (pf) tma_prefetch_2d(&tmA, kc, a_next);
                         if (++s == u.stages) { s = 0; ph ^= 1u; }
@@ -265,6 +280,9 @@ stage1_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
                 ealpha[r] = 2e-6f / alpha[r];
             }
             for (uint32_t qt = 0; qt < u.nqt; ++qt) {
+                const uint32_t q0 = qt * N;
+                constexpr int G = N / TG;   // threshold groups per tile
+                float bound[G][2];
                 uint32_t prev = 0;
                 for (uint32_t kb = 0; kb < u.kblocks; ++kb) {
                     mbar_wait_u<PROF>(full_u + 8u * s, ph, &w_full);
@@ -277,7 +295,26 @@ stage1_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
                     for (uint32_t k = 0; k < UM_MMAS_PER_KBLOCK; ++k)
                         wgmma_tile<N, TF32>(acc, adesc + 2 * k, bdesc + 2 * k, (kb != 0 || k != 0) ? 1u : 0u);
                     wgmma_commit();
-                    if (kb != 0) {
+                    if (kb == 0) {
+                        if (FILTER) {
+                            // while the first K block's MMAs run: per group of TG query columns (TG / 4 of this thread's
+                            // accumulators per row) and row, a conservative bound,
+                            //   acc * alpha + beta > tau_q  =>  acc > (tmin - beta) / alpha (slightly relaxed),
+                            // tmin = the group's smallest threshold.  Only groups whose maximum passes take the per-column test.
+#pragma unroll
+                            for (int h = 0; h < G; ++h) {
+                                const float tmin = tmin_s[q0 / TG + h];
+#pragma unroll
+                                for (int r = 0; r < 2; ++r) {
+                                    bound[h][r] = INFINITY;
+                                    if (rowok[r]) {
+                                        const float b0 = (tmin - beta[r]) * ialpha[r];
+                                        bound[h][r] = b0 - (fabsf(tmin) + fabsf(beta[r])) * ealpha[r] - 1e-30f;
+                                    }
+                                }
+                            }
+                        }
+                    } else {
                         // the previous K block's MMAs are done: its stage may be refilled
                         wgmma_wait<1>();
                         if (lane == 0) mbar_arrive_u(empty_u + 8u * prev);
@@ -289,28 +326,31 @@ stage1_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
                 if (lane == 0) mbar_arrive_u(empty_u + 8u * prev);
 
                 const long long t_epi0 = PROF ? clock64() : 0;
-                const uint32_t q0 = qt * N;
                 if (FILTER) {
-                    const float* tau_t = tau_all + q0;
-                    const float* tmin_t = tmin_s + q0 / TG;
-                    // per group of TG query columns (TG / 4 of this thread's accumulators per row) and row, a conservative bound:
-                    // acc * alpha + beta > tau_q  =>  acc > (tmin - beta) / alpha (slightly relaxed), tmin = the group's
-                    // smallest threshold.  Only groups whose maximum passes take the per-column test and the append.
+                    // common path: the maximum of each (group, row) against its bound, one branch for the whole tile
+                    constexpr int J = TG / 8;   // accumulator column pairs per group
+                    float gmax[G][2];
+                    bool any = false;
 #pragma unroll
-                    for (int h = 0; h < N / TG; ++h) {
-                        const float tmin = tmin_t[h];
+                    for (int h = 0; h < G; ++h) {
 #pragma unroll
                         for (int r = 0; r < 2; ++r) {
-                            float bound = INFINITY;
-                            if (rowok[r]) {
-                                const float b0 = (tmin - beta[r]) * ialpha[r];
-                                bound = b0 - (fabsf(tmin) + fabsf(beta[r])) * ealpha[r] - 1e-30f;
-                            }
-                            constexpr int J = TG / 8;   // accumulator column pairs per group
                             float m = acc[4 * J * h + 2 * r];
 #pragma unroll
                             for (int j = J * h; j < J * (h + 1); ++j) m = fmaxf(m, fmaxf(acc[4 * j + 2 * r], acc[4 * j + 2 * r + 1]));
-                            if (m > bound) {   // rare: some column of this group may survive
+                            gmax[h][r] = m;
+                            any |= m > bound[h][r];
+                        }
+                    }
+                    if (any) {   // rare: some column of a group of this thread may survive
+                        const float* tau_t = tau_all + q0;
+#pragma unroll
+                        for (int h = 0; h < G; ++h) {
+#pragma unroll
+                            for (int r = 0; r < 2; ++r) {
+                                // the common path's test, m > bound, in a form the compiler does not merge with it: it would
+                                // otherwise carry the 16 outcomes through the common path in a bit mask
+                                if (!(gmax[h][r] - bound[h][r] > 0.f)) continue;
 #pragma unroll
                                 for (int j = J * h; j < J * (h + 1); ++j) {
 #pragma unroll
