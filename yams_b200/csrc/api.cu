@@ -1,5 +1,5 @@
-// api.cu -- plugin envelope (abi.h:17-33 conventions), device context, error plumbing and the
-// sqlite-vec-cpp pairwise distance symbols of libyams_b200.so.
+// api.cu -- plugin envelope (abi.h:17-33 conventions), device context, error plumbing, the pooled operator workspace
+// (OpWs) and the health JSON of libyams_b200.so.
 #include <stdarg.h>
 #include <stdlib.h>
 
@@ -8,7 +8,6 @@
 #include <vector>
 
 #include "common.cuh"
-#include "ref_order.cuh"
 
 namespace yb {
 
@@ -110,35 +109,6 @@ void opws_release(OpWs* w) {
     w->h.release();
     cudaStreamDestroy(w->st);
     delete w;
-}
-
-// pairwise operators of the sqlite-vec-cpp C API: one thread evaluates the pair in the reference build's operation order
-__global__ void pair_distance_kernel(const float* __restrict__ a, const float* __restrict__ b, uint32_t d, int metric,
-                                     float* __restrict__ out) {
-    F32At fa{a}, fb{b};
-    *out = metric == YAMS_B200_L2 ? ref_l2_distance(fa, fb, d) : (metric == 2 ? ref_l1_distance(fa, fb, d) : ref_cosine_distance(fa, fb, d));
-}
-
-static int pair_distance(const void* v1, size_t size1, const void* v2, size_t size2, float* result, int metric) {
-    // sqlite_vec_c_api.cpp:57-105: SQLITE_OK 0 / SQLITE_ERROR 1
-    if (!v1 || !v2 || !result) return 1;
-    size_t d1 = size1 / sizeof(float), d2 = size2 / sizeof(float);
-    if (d1 != d2) return 1;
-    OpWsLease lease;
-    OpWs* w = lease.w;
-    if (!w) return 1;
-    const size_t bytes = (2 * d1 + 4) * sizeof(float);
-    if (w->d[0].reserve(bytes) != YAMS_OK || w->h.reserve(bytes) != YAMS_OK) return 1;
-    float* hp = w->h.as<float>();
-    memcpy(hp, v1, d1 * 4);
-    memcpy(hp + d1, v2, d1 * 4);
-    float* dp = w->d[0].as<float>();
-    if (cudaMemcpyAsync(dp, hp, 2 * d1 * 4, cudaMemcpyHostToDevice, w->st) != cudaSuccess) return 1;
-    pair_distance_kernel<<<1, 1, 0, w->st>>>(dp, dp + d1, (uint32_t)d1, metric, dp + 2 * d1);
-    if (cudaMemcpyAsync(hp + 2 * d1, dp + 2 * d1, 4, cudaMemcpyDeviceToHost, w->st) != cudaSuccess) return 1;
-    if (cudaStreamSynchronize(w->st) != cudaSuccess) return 1;
-    *result = hp[2 * d1];
-    return 0;
 }
 
 }  // namespace yb
@@ -249,16 +219,6 @@ int yams_plugin_get_health_json(char** out_json) {
              g_dev.cc_major, g_dev.cc_minor, esc);
     *out_json = strdup(buf);
     return *out_json ? YAMS_PLUGIN_OK : YAMS_PLUGIN_ERR_INVALID;
-}
-
-int sqlite3_vec_distance_l2(const void* vec1, size_t size1, const void* vec2, size_t size2, float* result) {
-    return pair_distance(vec1, size1, vec2, size2, result, YAMS_B200_L2);
-}
-int sqlite3_vec_distance_cosine(const void* vec1, size_t size1, const void* vec2, size_t size2, float* result) {
-    return pair_distance(vec1, size1, vec2, size2, result, YAMS_B200_COSINE);
-}
-int yams_b200_vec_distance_l1(const void* vec1, size_t size1, const void* vec2, size_t size2, float* result) {
-    return pair_distance(vec1, size1, vec2, size2, result, 2);
 }
 
 int yams_b200_device_count(void) {

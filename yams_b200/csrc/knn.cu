@@ -1,5 +1,6 @@
 // knn.cu -- exact brute-force vector scan: CUDA-core stage-1 engine, top-K' selection, fp64
-// rescoring, final ordering, L2 / vec0 surface, corpus mirror and the vector_scan_v1 entry points.
+// rescoring, final ordering, the device key sort, corpus mirror and the vector_scan_v1 entry points.  The stateless
+// sqlite-vec operators live in operators.cu.
 //
 // Reference semantics matched (paths under /root/reference):
 //   bruteForceSearchUnlocked fast path   src/vector/sqlite_vec_backend.cpp:4203-4331
@@ -962,57 +963,8 @@ __global__ void list_lengths_kernel(const uint64_t* __restrict__ offsets, uint32
 }
 
 // ---------------------------------------------------------------------------------------------------
-// sqlite-vec-cpp operator surface (vec0_run_exact_query, distances/batch.hpp): one thread per row evaluates the float
-// distance in the reference build's own operation order (ref_order.cuh) -> bit-identical results.  NEGATED distance out so
-// that the descending key sort used everywhere else yields ascending distances.
+// device key sort (knn.cuh), shared by the exact paths below and the sqlite-vec operators (operators.cu)
 // ---------------------------------------------------------------------------------------------------
-__global__ void batch_dist_kernel(const float* __restrict__ rows, uint32_t d, uint64_t n, const float* __restrict__ q, int metric,
-                                  float* __restrict__ out_neg) {
-    uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= n) return;
-    F32At qa{q}, ra{rows + r * d};
-    out_neg[r] = -(metric == YAMS_B200_L2 ? ref_l2_distance(qa, ra, d) : ref_cosine_distance(qa, ra, d));
-}
-// keys for the FILTERED mode: rows failing dist < threshold get key 0 (sort last)
-__global__ void make_keys_filtered_kernel(const float* __restrict__ neg_dist, uint64_t n, uint64_t np2, float threshold,
-                                          uint64_t* __restrict__ keys) {
-    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < np2; i += (uint64_t)gridDim.x * blockDim.x) {
-        uint64_t key = 0;
-        if (i < n && (-neg_dist[i]) < threshold) key = ((uint64_t)fkey(neg_dist[i]) << 32) | (uint64_t)(0xFFFFFFFFu - (uint32_t)i);
-        keys[i] = key;
-    }
-}
-__global__ void unpack_idx_keys_kernel(const uint64_t* __restrict__ keys, uint64_t m, uint64_t* __restrict__ out_idx,
-                                       float* __restrict__ out_dist) {
-    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < m; i += (uint64_t)gridDim.x * blockDim.x) {
-        uint64_t key = keys[i];
-        out_idx[i] = 0xFFFFFFFFu - (uint32_t)key;
-        out_dist[i] = -fkey_inv((uint32_t)(key >> 32));
-    }
-}
-__global__ void negate_kernel(float* p, uint64_t n) {
-    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) p[i] = -p[i];
-}
-// computeCosineSimilarity (vector_database.cpp:1786-1810): one thread, the reference's accumulation order
-__global__ void cosine_similarity_f64_kernel(const float* __restrict__ a_all, const float* __restrict__ b_all, uint64_t n, uint64_t d,
-                                             double* __restrict__ out_all) {
-    const uint64_t p = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (p >= n) return;
-    const float* a = a_all + p * d;
-    const float* b = b_all + p * d;
-    double* out = out_all + p;
-    double dp = 0.0, na = 0.0, nb = 0.0;
-    for (uint64_t i = 0; i < d; ++i) {
-        double x = (double)a[i], y = (double)b[i];
-        dp += x * y;
-        na += x * x;
-        nb += y * y;
-    }
-    na = sqrt(na);
-    nb = sqrt(nb);
-    *out = (na == 0.0 || nb == 0.0) ? 0.0 : dp / (na * nb);
-}
-
 // global-memory bitonic sort (descending) of 64-bit keys, n a power of two
 __global__ void bitonic_step_kernel(uint64_t* __restrict__ keys, uint64_t n, uint64_t size, uint64_t stride) {
     for (uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; t < n / 2; t += (uint64_t)gridDim.x * blockDim.x) {
@@ -1023,18 +975,34 @@ __global__ void bitonic_step_kernel(uint64_t* __restrict__ keys, uint64_t n, uin
         if ((x < y) == desc) { keys[lo] = y; keys[hi] = x; }
     }
 }
-__global__ void make_keys_kernel(const float* __restrict__ neg_dist, uint64_t n, uint64_t np2, uint64_t* __restrict__ keys) {
-    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < np2; i += (uint64_t)gridDim.x * blockDim.x)
-        keys[i] = i < n ? (((uint64_t)fkey(neg_dist[i]) << 32) | (uint64_t)(0xFFFFFFFFu - (uint32_t)i)) : 0ull;
+__global__ void count_nonzero_kernel(const uint64_t* __restrict__ keys, uint64_t n, unsigned long long* __restrict__ out) {
+    unsigned long long c = 0;
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) c += keys[i] != 0;
+    for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
+    if ((threadIdx.x & 31) == 0 && c) atomicAdd(out, c);
 }
-__global__ void unpack_keys_kernel(const uint64_t* __restrict__ keys, uint64_t m, const int64_t* __restrict__ rowids,
-                                   int64_t* __restrict__ out_rowids, float* __restrict__ out_dist) {
+__global__ void unpack_keys_kernel(const uint64_t* __restrict__ keys, uint64_t m, const int64_t* __restrict__ rowids, int negate,
+                                   int64_t* __restrict__ out_rowids, float* __restrict__ out_scores) {
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < m; i += (uint64_t)gridDim.x * blockDim.x) {
         uint64_t key = keys[i];
         uint32_t row = 0xFFFFFFFFu - (uint32_t)key;
+        float s = fkey_inv((uint32_t)(key >> 32));
         out_rowids[i] = rowids ? rowids[row] : (int64_t)row;
-        out_dist[i] = -fkey_inv((uint32_t)(key >> 32));
+        out_scores[i] = negate ? -s : s;
     }
+}
+
+void sort_keys_desc(uint64_t* keys, uint64_t np2, cudaStream_t st) {
+    const unsigned g = key_grid(np2);
+    for (uint64_t size = 2; size <= np2; size <<= 1)
+        for (uint64_t stride = size >> 1; stride > 0; stride >>= 1) bitonic_step_kernel<<<g, 256, 0, st>>>(keys, np2, size, stride);
+}
+void count_nonzero_keys(const uint64_t* keys, uint64_t n, unsigned long long* d_count, cudaStream_t st) {
+    count_nonzero_kernel<<<key_grid(n), 256, 0, st>>>(keys, n, d_count);
+}
+void unpack_keys(const uint64_t* keys, uint64_t m, const int64_t* rowids, bool negate, int64_t* out_rowids, float* out_scores,
+                 cudaStream_t st) {
+    unpack_keys_kernel<<<key_grid(m), 256, 0, st>>>(keys, m, rowids, negate ? 1 : 0, out_rowids, out_scores);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -1137,21 +1105,6 @@ __global__ void exact_keys_kernel(const Exact* __restrict__ ex, uint64_t n, uint
         keys[i] = key;
     }
 }
-__global__ void count_nonzero_kernel(const uint64_t* __restrict__ keys, uint64_t n, unsigned long long* __restrict__ out) {
-    unsigned long long c = 0;
-    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) c += keys[i] != 0;
-    for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
-    if ((threadIdx.x & 31) == 0 && c) atomicAdd(out, c);
-}
-__global__ void unpack_sim_keys_kernel(const uint64_t* __restrict__ keys, uint64_t m, const int64_t* __restrict__ rowids,
-                                       int64_t* __restrict__ out_rowids, float* __restrict__ out_scores) {
-    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < m; i += (uint64_t)gridDim.x * blockDim.x) {
-        uint64_t key = keys[i];
-        uint32_t row = 0xFFFFFFFFu - (uint32_t)key;
-        out_rowids[i] = rowids[row];
-        out_scores[i] = fkey_inv((uint32_t)(key >> 32));
-    }
-}
 
 // ---- corpus_remove: stable compaction ------------------------------------------------------------------
 __global__ void fill_u32_kernel(uint32_t* p, uint64_t n, uint32_t v) {
@@ -1199,9 +1152,6 @@ __global__ void scan_init_kernel(uint32_t nq, uint32_t* __restrict__ sel_n, floa
         bound[i] = -INFINITY;
         counts[i] = 0;
     }
-}
-__global__ void fill_f32_kernel(float* p, uint64_t n, float v) {
-    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) p[i] = v;
 }
 __global__ void iota_rowids_kernel(int64_t* p, uint64_t n, int64_t first) {
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x)
@@ -1334,6 +1284,12 @@ static yams_status_t gather_scores(Corpus* c, const DirectLists& L, uint32_t nq,
 
 static ScanStatus* status_of(Corpus* c) { return c->status.as<ScanStatus>(); }
 
+// the CUDA-core engine's stage-1 error bound of the nq prepared queries -> dst[nq] (keep_larger: the max with dst's values)
+static void launch_eps_cc(Corpus* c, uint32_t nq, float* dst, bool keep_larger) {
+    eps_cc_kernel<<<(nq + 255) / 256, 256, 0, c->st>>>(reinterpret_cast<const double*>(c->misc.as<uint8_t>()), nq, c->dim, c->metric,
+                                                       c->r_max, dst, keep_larger ? 1 : 0);
+}
+
 static void fill_stage1_common(Corpus* c, Stage1Args& a, uint32_t nq) {
     a.rows = c->rows.p;
     a.inv_norm = c->inv_norm.as<float>();
@@ -1455,7 +1411,7 @@ static yams_status_t scan_enqueue(Corpus* c, const ScanPlan& p, int64_t* d_out_r
     }
     // error bound of the engine(s) that produced the ranking
     if (cc_used || !tensor_used)
-        eps_cc_kernel<<<(nq + 255) / 256, 256, 0, st>>>(d_qnorm, nq, c->dim, c->metric, c->r_max, c->eps.as<float>(), tensor_used ? 1 : 0);
+        launch_eps_cc(c, nq, c->eps.as<float>(), tensor_used);
     c->last_ms[4] = tensor_used ? 1.f : 0.f;   // the engine that ran: wgmma declines shapes it does not take (nq > 4096)
     YB_CUDA(cudaEventRecord(c->ev[1], st));
     // ---- stage 2: exact re-scoring, ordering, certificate ----
@@ -1497,37 +1453,48 @@ void launch_query_prep(const float* q, uint32_t nq, uint32_t d, double* qnorm, f
                                                                                 static_cast<ScanStatus*>(status));
 }
 
-// Level 2: exact score of EVERY row for one query (the reference's own loop, row-parallel) + a global sort.
-static yams_status_t exact_all_rows(Corpus* c, const ScanPlan& p, uint32_t q, int64_t* d_out_rowids, float* d_out_scores,
-                                    uint32_t* d_out_counts, uint64_t* d_out_flags) {
+// Exact scores of m corpus rows for query q (rescore_kernel; with a mask, rows outside it are skipped) as keys sorted
+// descending into c->dense[0, np2), np2 = pow2_at_least(max(m, 1)); skipped rows and the padding are zero keys at the end.
+// The rows are those of the m rowids at d_allowed (map_rowids_kernel, unknown rowids skipped) or, without a list, rows
+// 0 .. m-1.  Workspace: c->sel (row list), c->outbuf (exact scores), c->lvl[0, 8) ({m, q}) and c->dense (keys); c->lvl past
+// its first 8 bytes is left alone.
+static yams_status_t exact_sorted_keys(Corpus* c, uint32_t q, uint64_t m, const int64_t* d_allowed, float threshold,
+                                       const uint32_t* mask, uint64_t mask_ld) {
     yams_status_t rc;
     cudaStream_t st = c->st;
-    const uint64_t m = c->n;
-    const bool l2 = c->metric == YAMS_B200_L2;
-    uint64_t np2 = 1;
-    while (np2 < std::max<uint64_t>(m, 1)) np2 <<= 1;
+    const uint64_t np2 = pow2_at_least(std::max<uint64_t>(m, 1));
     if ((rc = c->sel.reserve((size_t)m * sizeof(Cand) + 64)) != YAMS_OK) return rc;
     if ((rc = c->outbuf.reserve((size_t)m * sizeof(Exact) + 64)) != YAMS_OK) return rc;
     if ((rc = c->dense.reserve((size_t)np2 * 8 + 64)) != YAMS_OK) return rc;
     if ((rc = c->lvl.reserve(64)) != YAMS_OK) return rc;
     Cand* d_sel = c->sel.as<Cand>();
-    uint64_t* d_keys = c->dense.as<uint64_t>();
     uint32_t* d_small = c->lvl.as<uint32_t>();     // [0] = survivors (m), [1] = query index
     uint32_t h_small[2] = {(uint32_t)m, q};
     YB_CUDA(cudaMemcpyAsync(d_small, h_small, 8, cudaMemcpyHostToDevice, st));
-    unsigned g = (unsigned)std::min<uint64_t>((np2 + 255) / 256, 65535);
-    double* d_qnorm = reinterpret_cast<double*>(c->misc.as<uint8_t>());
+    const unsigned g = key_grid(np2);
     if (m) {
-        iota_sel_kernel<<<g, 256, 0, st>>>(d_sel, m);
-        rescore_kernel<<<(unsigned)((m + 127) / 128), 128, 0, st>>>(c->rows.p, c->dtype, c->dim, c->q32.as<float>(), d_qnorm, d_sel, d_small,
-                                                                   (uint32_t)m, 1, p.threshold, c->outbuf.as<Exact>(), c->metric, d_small + 1,
-                                                                   p.d_mask, p.mask_ld);
+        if (d_allowed) map_rowids_kernel<<<g, 256, 0, st>>>(d_allowed, m, c->rowids.as<int64_t>(), c->n, d_sel);
+        else iota_sel_kernel<<<g, 256, 0, st>>>(d_sel, m);
+        rescore_kernel<<<(unsigned)((m + 127) / 128), 128, 0, st>>>(c->rows.p, c->dtype, c->dim, c->q32.as<float>(),
+                                                                   reinterpret_cast<double*>(c->misc.as<uint8_t>()), d_sel, d_small,
+                                                                   (uint32_t)m, 1, threshold, c->outbuf.as<Exact>(), c->metric, d_small + 1,
+                                                                   mask, mask_ld);
     }
-    exact_keys_kernel<<<g, 256, 0, st>>>(c->outbuf.as<Exact>(), m, np2, d_keys);
-    for (uint64_t size = 2; size <= np2; size <<= 1)
-        for (uint64_t stride = size >> 1; stride > 0; stride >>= 1) bitonic_step_kernel<<<g, 256, 0, st>>>(d_keys, np2, size, stride);
-    emit_sorted_kernel<<<(p.k + 255) / 256, 256, 0, st>>>(d_keys, np2, p.k, q, c->rowids.as<int64_t>(), l2 ? 1 : 0, l2 ? INFINITY : -INFINITY,
-                                                          d_out_rowids, d_out_scores, d_out_counts, d_out_flags);
+    exact_keys_kernel<<<g, 256, 0, st>>>(c->outbuf.as<Exact>(), m, np2, c->dense.as<uint64_t>());
+    sort_keys_desc(c->dense.as<uint64_t>(), np2, st);
+    YB_CUDA(cudaGetLastError());
+    return YAMS_OK;
+}
+
+// Level 2: exact score of EVERY row for one query (the reference's own loop, row-parallel) + a global sort.
+static yams_status_t exact_all_rows(Corpus* c, const ScanPlan& p, uint32_t q, int64_t* d_out_rowids, float* d_out_scores,
+                                    uint32_t* d_out_counts, uint64_t* d_out_flags) {
+    yams_status_t rc;
+    cudaStream_t st = c->st;
+    const bool l2 = c->metric == YAMS_B200_L2;
+    if ((rc = exact_sorted_keys(c, q, c->n, nullptr, p.threshold, p.d_mask, p.mask_ld)) != YAMS_OK) return rc;
+    emit_sorted_kernel<<<(p.k + 255) / 256, 256, 0, st>>>(c->dense.as<uint64_t>(), c->n, p.k, q, c->rowids.as<int64_t>(), l2 ? 1 : 0,
+                                                          l2 ? INFINITY : -INFINITY, d_out_rowids, d_out_scores, d_out_counts, d_out_flags);
     YB_CUDA(cudaGetLastError());
     YB_CUDA(cudaStreamSynchronize(st));   // h_small / scratch reuse
     return YAMS_OK;
@@ -1558,7 +1525,7 @@ static yams_status_t resolve_uncertain(Corpus* c, const ScanPlan& p, const uint3
     uint32_t* d_sel1_n = reinterpret_cast<uint32_t*>(d_ex1 + (size_t)G * K1);
     float* d_bound1 = reinterpret_cast<float*>(d_sel1_n + G);
     double* d_qnorm = reinterpret_cast<double*>(c->misc.as<uint8_t>());
-    eps_cc_kernel<<<(p.nq + 255) / 256, 256, 0, st>>>(d_qnorm, p.nq, c->dim, c->metric, c->r_max, c->eps2.as<float>(), 0);
+    launch_eps_cc(c, p.nq, c->eps2.as<float>(), false);
     Stage1Args a{};
     fill_stage1_common(c, a, p.nq);
     for (uint32_t g0 = 0; g0 < n_bad; g0 += G) {
@@ -1899,6 +1866,44 @@ static yams_status_t enqueue_status_readback(yams_b200_corpus* c, uint32_t nq) {
     return YAMS_OK;
 }
 
+// the blocking paths: prepare the queries and reject an invalid one before any search work is enqueued
+static yams_status_t prepare_valid_queries(yams_b200_corpus* c, const float* queries, uint32_t nq) {
+    yams_status_t rc;
+    if ((rc = prepare_queries(c, queries, false, nq)) != YAMS_OK) return rc;
+    if ((rc = enqueue_status_readback(c, 0)) != YAMS_OK) return rc;
+    YB_CUDA(cudaStreamSynchronize(c->st));
+    YB_ARG(c->h_pin.as<ScanStatus>()->n_invalid == 0,
+           "exact vector search requires a finite, non-zero query embedding");   // InvalidArgument for a bad query (:4127)
+    return YAMS_OK;
+}
+
+// the padded [nq][k] results of a search on the device, in c->dout: [nq*k rowids][nq flags][nq*k scores][nq counts]
+struct DeviceResults {
+    int64_t* rowids;
+    uint64_t* flags;
+    float* scores;
+    uint32_t* counts;
+};
+static yams_status_t reserve_results(yams_b200_corpus* c, uint32_t nq, uint32_t k, DeviceResults* r) {
+    yams_status_t rc = c->dout.reserve((size_t)nq * k * 12 + (size_t)nq * 12 + 64);
+    if (rc != YAMS_OK) return rc;
+    r->rowids = c->dout.as<int64_t>();
+    r->flags = reinterpret_cast<uint64_t*>(r->rowids + (size_t)nq * k);
+    r->scores = reinterpret_cast<float*>(r->flags + nq);
+    r->counts = reinterpret_cast<uint32_t*>(r->scores + (size_t)nq * k);
+    return YAMS_OK;
+}
+// device results -> the caller's arrays (out_flags nullable), then wait for them
+static yams_status_t copy_results(yams_b200_corpus* c, const DeviceResults& r, uint32_t nq, uint32_t k, int64_t* out_rowids,
+                                  float* out_scores, uint32_t* out_counts, uint64_t* out_flags) {
+    YB_CUDA(cudaMemcpyAsync(out_rowids, r.rowids, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, c->st));
+    YB_CUDA(cudaMemcpyAsync(out_scores, r.scores, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, c->st));
+    YB_CUDA(cudaMemcpyAsync(out_counts, r.counts, (size_t)nq * 4, cudaMemcpyDeviceToHost, c->st));
+    if (out_flags) YB_CUDA(cudaMemcpyAsync(out_flags, r.flags, (size_t)nq * 8, cudaMemcpyDeviceToHost, c->st));
+    YB_CUDA(cudaStreamSynchronize(c->st));
+    return YAMS_OK;
+}
+
 yams_status_t yams_b200_search(yams_b200_corpus* c, const float* queries, uint32_t nq, uint32_t k, float threshold,
                                const int64_t* allowed_rowids, const uint64_t* allowed_offsets, int64_t* out_rowids,
                                float* out_scores, uint32_t* out_counts, uint64_t* out_flags) {
@@ -1925,14 +1930,8 @@ yams_status_t yams_b200_search(yams_b200_corpus* c, const float* queries, uint32
     c->pending.active = false;
     if ((rc = prepare_queries(c, queries, false, nq)) != YAMS_OK) return rc;
     YB_CUDA(cudaEventRecord(c->ev[0], c->st));
-    // device outputs
-    size_t ob = (size_t)nq * k * 12 + (size_t)nq * 4 + (size_t)nq * 8 + 64;
-    DevBuf& dout = c->dout;
-    if ((rc = dout.reserve(ob)) != YAMS_OK) return rc;
-    int64_t* d_or = dout.as<int64_t>();
-    uint64_t* d_of = reinterpret_cast<uint64_t*>(d_or + (size_t)nq * k);
-    float* d_os = reinterpret_cast<float*>(d_of + nq);
-    uint32_t* d_oc = reinterpret_cast<uint32_t*>(d_os + (size_t)nq * k);
+    DeviceResults r;
+    if ((rc = reserve_results(c, nq, k, &r)) != YAMS_OK) return rc;
     ScanPlan plan;
     plan.nq = nq; plan.k = k; plan.threshold = threshold;
     plan.use_tensor = wgmma_supported(c, nq);
@@ -1956,22 +1955,10 @@ yams_status_t yams_b200_search(yams_b200_corpus* c, const float* queries, uint32
     } else if (allowed_offsets && c->n) {
         if ((rc = upload_mask(c, nq, allowed_rowids, allowed_offsets, &plan.d_mask, &plan.mask_ld)) != YAMS_OK) return rc;
     }
-    if ((rc = scan_enqueue(c, plan, d_or, d_os, d_oc, d_of)) != YAMS_OK) return rc;
+    if ((rc = scan_enqueue(c, plan, r.rowids, r.scores, r.counts, r.flags)) != YAMS_OK) return rc;
     cudaEventRecord(c->ev[2], c->st);
     if ((rc = enqueue_status_readback(c, nq)) != YAMS_OK) return rc;
-    auto copy_out = [&]() -> cudaError_t {
-        cudaError_t e = cudaMemcpyAsync(out_rowids, d_or, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, c->st);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(out_scores, d_os, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, c->st);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(out_counts, d_oc, (size_t)nq * 4, cudaMemcpyDeviceToHost, c->st);
-        if (e == cudaSuccess && out_flags) e = cudaMemcpyAsync(out_flags, d_of, (size_t)nq * 8, cudaMemcpyDeviceToHost, c->st);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(c->st);
-        return e;
-    };
-    cudaError_t e = copy_out();
-    if (e != cudaSuccess) {
-        set_last_error("search failed: %s", cudaGetErrorString(e));
-        return YAMS_ERR_INTERNAL;
-    }
+    if ((rc = copy_results(c, r, nq, k, out_rowids, out_scores, out_counts, out_flags)) != YAMS_OK) return rc;
     cudaEventElapsedTime(&c->last_ms[0], c->ev[0], c->ev[1]);
     cudaEventElapsedTime(&c->last_ms[1], c->ev[1], c->ev[2]);
     cudaEventElapsedTime(&c->last_ms[2], c->ev[0], c->ev[2]);
@@ -1979,20 +1966,17 @@ yams_status_t yams_b200_search(yams_b200_corpus* c, const float* queries, uint32
     const ScanStatus* hs = c->h_pin.as<ScanStatus>();
     if (plan.direct && hs->n_bad && hs->n_invalid == 0) {
         // The direct path scored the listed rows without a bit mask, but the exhaustive levels score every row: they need the
-        // candidate sets as a mask.  The scan is finished (copy_out synchronised), so its lists in c->mask may be overwritten.
+        // candidate sets as a mask.  The scan is finished (copy_results synchronised), so its lists in c->mask may be overwritten.
         plan.direct = nullptr;
         rc = upload_mask(c, nq, allowed_rowids, allowed_offsets, &plan.d_mask, &plan.mask_ld);
     }
-    if (rc == YAMS_OK) rc = finish_scan(c, plan, d_or, d_os, d_oc, d_of, &resolved);
+    if (rc == YAMS_OK) rc = finish_scan(c, plan, r.rowids, r.scores, r.counts, r.flags, &resolved);
     c->last_ms[6] = (float)resolved;
     if (rc != YAMS_OK) {
         for (uint32_t q = 0; q < nq; ++q) out_counts[q] = 0;
         return rc;
     }
-    if (resolved && (e = copy_out()) != cudaSuccess) {
-        set_last_error("search failed: %s", cudaGetErrorString(e));
-        return YAMS_ERR_INTERNAL;
-    }
+    if (resolved) return copy_results(c, r, nq, k, out_rowids, out_scores, out_counts, out_flags);
     return YAMS_OK;
     YB_CATCH
 }
@@ -2012,26 +1996,14 @@ yams_status_t yams_b200_search_exhaustive(yams_b200_corpus* c, const float* quer
     YB_ARG(nq <= 65535, "at most 65535 queries per call");
     yams_status_t rc;
     c->pending.active = false;
-    if ((rc = prepare_queries(c, queries, false, nq)) != YAMS_OK) return rc;
-    size_t ob = (size_t)nq * k * 12 + (size_t)nq * 4 + (size_t)nq * 8 + 64;
-    if ((rc = c->dout.reserve(ob)) != YAMS_OK) return rc;
-    int64_t* d_or = c->dout.as<int64_t>();
-    uint64_t* d_of = reinterpret_cast<uint64_t*>(d_or + (size_t)nq * k);
-    float* d_os = reinterpret_cast<float*>(d_of + nq);
-    uint32_t* d_oc = reinterpret_cast<uint32_t*>(d_os + (size_t)nq * k);
-    if ((rc = enqueue_status_readback(c, 0)) != YAMS_OK) return rc;
-    YB_CUDA(cudaStreamSynchronize(c->st));
-    YB_ARG(c->h_pin.as<ScanStatus>()->n_invalid == 0, "exact vector search requires a finite, non-zero query embedding");
+    if ((rc = prepare_valid_queries(c, queries, nq)) != YAMS_OK) return rc;
+    DeviceResults r;
+    if ((rc = reserve_results(c, nq, k, &r)) != YAMS_OK) return rc;
     ScanPlan plan;
     plan.nq = nq; plan.k = k; plan.threshold = threshold;
     for (uint32_t q = 0; q < nq; ++q)
-        if ((rc = exact_all_rows(c, plan, q, d_or, d_os, d_oc, d_of)) != YAMS_OK) return rc;
-    YB_CUDA(cudaMemcpyAsync(out_rowids, d_or, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, c->st));
-    YB_CUDA(cudaMemcpyAsync(out_scores, d_os, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, c->st));
-    YB_CUDA(cudaMemcpyAsync(out_counts, d_oc, (size_t)nq * 4, cudaMemcpyDeviceToHost, c->st));
-    if (out_flags) YB_CUDA(cudaMemcpyAsync(out_flags, d_of, (size_t)nq * 8, cudaMemcpyDeviceToHost, c->st));
-    YB_CUDA(cudaStreamSynchronize(c->st));
-    return YAMS_OK;
+        if ((rc = exact_all_rows(c, plan, q, r.rowids, r.scores, r.counts, r.flags)) != YAMS_OK) return rc;
+    return copy_results(c, r, nq, k, out_rowids, out_scores, out_counts, out_flags);
     YB_CATCH
 }
 
@@ -2060,53 +2032,33 @@ yams_status_t yams_b200_search_all_matching(yams_b200_corpus* c, const float* qu
     }
     const uint64_t m = allowed_rowids ? n_allowed : c->n;
     yams_status_t rc;
-    if ((rc = prepare_queries(c, query, false, 1)) != YAMS_OK) return rc;
-    if ((rc = enqueue_status_readback(c, 0)) != YAMS_OK) return rc;
-    YB_CUDA(cudaStreamSynchronize(c->st));
-    YB_ARG(c->h_pin.as<ScanStatus>()->n_invalid == 0,
-           "exact vector search requires a finite, non-zero query embedding");   // InvalidArgument for a bad query (:4127)
+    if ((rc = prepare_valid_queries(c, query, 1)) != YAMS_OK) return rc;
     if (m == 0 || c->n == 0) return YAMS_OK;
     YB_ARG(out_rowids && out_scores, "null output");
     YB_ARG(m < (1ull << 31), "candidate set too large");
     cudaStream_t st = c->st;
-    uint64_t np2 = 1;
-    while (np2 < m) np2 <<= 1;
-    if ((rc = c->sel.reserve((size_t)m * sizeof(Cand) + 16)) != YAMS_OK) return rc;
-    if ((rc = c->outbuf.reserve((size_t)m * sizeof(Exact))) != YAMS_OK) return rc;
+    const uint64_t np2 = pow2_at_least(m);
+    // dense: the sorted keys, then the unpacked rowids and scores
     if ((rc = c->dense.reserve((size_t)np2 * 8 + (size_t)m * 12 + 64)) != YAMS_OK) return rc;
-    if ((rc = c->mask.reserve((size_t)m * 8 + 64)) != YAMS_OK) return rc;
-    Cand* d_sel = c->sel.as<Cand>();
     uint64_t* d_keys = c->dense.as<uint64_t>();
     int64_t* d_or = reinterpret_cast<int64_t*>(d_keys + np2);
     float* d_os = reinterpret_cast<float*>(d_or + m);
-    unsigned g = (unsigned)std::min<uint64_t>((np2 + 255) / 256, 65535);
+    int64_t* d_allowed = nullptr;
     if (allowed_rowids) {
-        int64_t* d_allowed = c->mask.as<int64_t>();
+        if ((rc = c->mask.reserve((size_t)m * 8 + 64)) != YAMS_OK) return rc;
+        d_allowed = c->mask.as<int64_t>();
         YB_CUDA(cudaMemcpyAsync(d_allowed, allowed_rowids, (size_t)m * 8, cudaMemcpyHostToDevice, st));
-        map_rowids_kernel<<<g, 256, 0, st>>>(d_allowed, m, c->rowids.as<int64_t>(), c->n, d_sel);
-    } else {
-        iota_sel_kernel<<<g, 256, 0, st>>>(d_sel, m);
     }
-    // one "query" with Kp = m survivors: exact re-scoring of every candidate
-    uint32_t* d_seln = c->counts.as<uint32_t>();
-    uint32_t mm = (uint32_t)m;
-    YB_CUDA(cudaMemcpyAsync(d_seln, &mm, 4, cudaMemcpyHostToDevice, st));
-    double* d_qnorm = reinterpret_cast<double*>(c->misc.as<uint8_t>());
-    rescore_kernel<<<(unsigned)((m + 127) / 128), 128, 0, st>>>(c->rows.p, c->dtype, c->dim, c->q32.as<float>(), d_qnorm, d_sel, d_seln,
-                                                               (uint32_t)m, 1, threshold, c->outbuf.as<Exact>(), YAMS_B200_COSINE, nullptr,
-                                                               nullptr, 0);
-    exact_keys_kernel<<<g, 256, 0, st>>>(c->outbuf.as<Exact>(), m, np2, d_keys);
-    for (uint64_t size = 2; size <= np2; size <<= 1)
-        for (uint64_t stride = size >> 1; stride > 0; stride >>= 1) bitonic_step_kernel<<<g, 256, 0, st>>>(d_keys, np2, size, stride);
+    if ((rc = exact_sorted_keys(c, 0, m, d_allowed, threshold, nullptr, 0)) != YAMS_OK) return rc;
     if ((rc = c->tau.reserve(8)) != YAMS_OK) return rc;
     unsigned long long* d_cnt = reinterpret_cast<unsigned long long*>(c->tau.p);
     YB_CUDA(cudaMemsetAsync(d_cnt, 0, 8, st));
-    count_nonzero_kernel<<<g, 256, 0, st>>>(d_keys, np2, d_cnt);
+    count_nonzero_keys(d_keys, np2, d_cnt, st);
     unsigned long long h_cnt = 0;
     YB_CUDA(cudaMemcpyAsync(&h_cnt, d_cnt, 8, cudaMemcpyDeviceToHost, st));
     YB_CUDA(cudaStreamSynchronize(st));
     if (h_cnt) {
-        unpack_sim_keys_kernel<<<g, 256, 0, st>>>(d_keys, h_cnt, c->rowids.as<int64_t>(), d_or, d_os);
+        unpack_keys(d_keys, h_cnt, c->rowids.as<int64_t>(), false, d_or, d_os, st);
         YB_CUDA(cudaMemcpyAsync(out_rowids, d_or, (size_t)h_cnt * 8, cudaMemcpyDeviceToHost, st));
         YB_CUDA(cudaMemcpyAsync(out_scores, d_os, (size_t)h_cnt * 4, cudaMemcpyDeviceToHost, st));
         YB_CUDA(cudaStreamSynchronize(st));
@@ -2232,8 +2184,7 @@ yams_status_t yams_b200_debug_stage1_scores(yams_b200_corpus* c, const float* qu
         rc = stage1_wgmma(c, a, false, c->st);
     } else {
         rc = stage1_cuda_core(a, false, c->st);
-        eps_cc_kernel<<<(nq + 255) / 256, 256, 0, c->st>>>(reinterpret_cast<double*>(c->misc.as<uint8_t>()), nq, c->dim, c->metric, c->r_max,
-                                                           c->eps.as<float>(), 0);
+        launch_eps_cc(c, nq, c->eps.as<float>(), false);
     }
     if (rc != YAMS_OK) return rc;
     YB_CUDA(cudaMemcpyAsync(out, c->dense.p, (size_t)nq * nrows * 4, cudaMemcpyDeviceToHost, c->st));
@@ -2280,16 +2231,14 @@ yams_status_t yams_b200_debug_stage1_candidates(yams_b200_corpus* c, const float
         if ((rc = upload_direct_lists(c, nq, allowed_rowids, allowed_offsets, &lists)) != YAMS_OK) return rc;
         list_lengths_kernel<<<(nq + 255) / 256, 256, 0, c->st>>>(lists.d_offsets, nq, a.counts);
         rc = gather_scores(c, lists, nq, a.q32, a.qinv, a.cands, cap, c->st);
-        eps_cc_kernel<<<(nq + 255) / 256, 256, 0, c->st>>>(reinterpret_cast<double*>(c->misc.as<uint8_t>()), nq, c->dim, c->metric, c->r_max,
-                                                           c->eps.as<float>(), 0);
+        launch_eps_cc(c, nq, c->eps.as<float>(), false);
     } else {
         if (allowed_offsets && (rc = upload_mask(c, nq, allowed_rowids, allowed_offsets, &a.mask, &a.mask_ld)) != YAMS_OK) return rc;
         if (engine == 1) {
             rc = stage1_wgmma(c, a, true, c->st);
         } else {
             rc = stage1_cuda_core(a, true, c->st);
-            eps_cc_kernel<<<(nq + 255) / 256, 256, 0, c->st>>>(reinterpret_cast<double*>(c->misc.as<uint8_t>()), nq, c->dim, c->metric,
-                                                               c->r_max, c->eps.as<float>(), 0);
+            launch_eps_cc(c, nq, c->eps.as<float>(), false);
         }
     }
     if (rc != YAMS_OK) return rc;
@@ -2418,7 +2367,8 @@ yams_status_t yams_b200_debug_final(yams_b200_corpus* c, uint32_t nq, uint32_t K
     if ((rc = c->eps.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
     if ((rc = c->misc.reserve((size_t)nq * 8)) != YAMS_OK) return rc;
     if ((rc = c->status.reserve(sizeof(ScanStatus) + (size_t)nq * 8)) != YAMS_OK) return rc;
-    if ((rc = c->dout.reserve((size_t)nq * k * 12 + (size_t)nq * 12 + 64)) != YAMS_OK) return rc;
+    DeviceResults r;
+    if ((rc = reserve_results(c, nq, k, &r)) != YAMS_OK) return rc;
     Exact* d_ex = c->outbuf.as<Exact>();
     uint32_t* d_ex_n = reinterpret_cast<uint32_t*>(d_ex + (size_t)nq * Kp);
     YB_CUDA(cudaMemcpyAsync(d_ex, ex, eb, cudaMemcpyHostToDevice, st));
@@ -2427,25 +2377,17 @@ yams_status_t yams_b200_debug_final(yams_b200_corpus* c, uint32_t nq, uint32_t K
     YB_CUDA(cudaMemcpyAsync(c->eps.p, eps, (size_t)nq * 4, cudaMemcpyHostToDevice, st));
     YB_CUDA(cudaMemcpyAsync(c->misc.p, qnorm, (size_t)nq * 8, cudaMemcpyHostToDevice, st));
     YB_CUDA(cudaMemsetAsync(c->status.p, 0, sizeof(ScanStatus) + (size_t)nq * 8, st));
-    int64_t* d_or = c->dout.as<int64_t>();
-    uint64_t* d_of = reinterpret_cast<uint64_t*>(d_or + (size_t)nq * k);
-    float* d_os = reinterpret_cast<float*>(d_of + nq);
-    uint32_t* d_oc = reinterpret_cast<uint32_t*>(d_os + (size_t)nq * k);
     const bool l2 = metric == YAMS_B200_L2;
     CertArgs cert{};
     cert.bound = c->bound.as<float>(); cert.eps = c->eps.as<float>(); cert.qnorm = reinterpret_cast<const double*>(c->misc.p);
     cert.threshold = threshold; cert.metric = metric; cert.l2_margin = l2_cert_margin(c->dim); cert.status = status_of(c);
     cert.level = level; cert.nq_total = nq;
-    final_kernel<<<nq, SEL_THREADS, 0, st>>>(d_ex, ex_n ? d_ex_n : nullptr, Kp, k, c->rowids.as<int64_t>(), l2 ? 1 : 0, d_or, d_os, d_oc, d_of,
-                                             l2 ? INFINITY : -INFINITY, nullptr, cert);
+    final_kernel<<<nq, SEL_THREADS, 0, st>>>(d_ex, ex_n ? d_ex_n : nullptr, Kp, k, c->rowids.as<int64_t>(), l2 ? 1 : 0, r.rowids, r.scores,
+                                             r.counts, r.flags, l2 ? INFINITY : -INFINITY, nullptr, cert);
     YB_CUDA(cudaGetLastError());
     std::vector<uint32_t> h_status(sizeof(ScanStatus) / 4 + (size_t)nq * 2);
-    YB_CUDA(cudaMemcpyAsync(out_rowids, d_or, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, st));
-    YB_CUDA(cudaMemcpyAsync(out_scores, d_os, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, st));
-    YB_CUDA(cudaMemcpyAsync(out_counts, d_oc, (size_t)nq * 4, cudaMemcpyDeviceToHost, st));
-    YB_CUDA(cudaMemcpyAsync(out_flags, d_of, (size_t)nq * 8, cudaMemcpyDeviceToHost, st));
     YB_CUDA(cudaMemcpyAsync(h_status.data(), c->status.p, h_status.size() * 4, cudaMemcpyDeviceToHost, st));
-    YB_CUDA(cudaStreamSynchronize(st));
+    if ((rc = copy_results(c, r, nq, k, out_rowids, out_scores, out_counts, out_flags)) != YAMS_OK) return rc;
     const ScanStatus* hs = reinterpret_cast<const ScanStatus*>(h_status.data());
     const uint32_t nqd = std::min(level == 0 ? hs->n_bad : hs->n_bad2, nq);
     const uint32_t* list = h_status.data() + sizeof(ScanStatus) / 4 + (level == 0 ? 0 : nq);
@@ -2488,209 +2430,6 @@ yams_status_t yams_b200_debug_last_eps(yams_b200_corpus* c, uint32_t nq, float* 
     YB_CUDA(cudaMemcpyAsync(out, c->eps.p, (size_t)nq * 4, cudaMemcpyDeviceToHost, c->st));
     YB_CUDA(cudaStreamSynchronize(c->st));
     return YAMS_OK;
-}
-
-yams_status_t yams_b200_vec0_exact(void* self, const float* query, uint32_t dim, const float* rows, const int64_t* rowids,
-                                   uint64_t n, uint64_t k, int use_range, int64_t rowid_lo, int64_t rowid_hi,
-                                   int64_t* out_rowids, float* out_dist, uint64_t* out_count) {
-    YB_TRY
-    (void)self;
-    YB_ARG(out_count, "out_count is null");
-    *out_count = 0;
-    YB_ARG(query && dim > 0, "bad query");
-    if (n == 0) return YAMS_OK;
-    YB_ARG(rows && out_rowids && out_dist, "null argument");
-    YB_ARG(n < 0xFFFFFFFFull, "too many rows");
-    yams_status_t rc = YAMS_OK;
-    // rowid range filter (vec0_module.hpp:399-401) is applied on the host side of the copy: only rows in
-    // range are uploaded (pure data movement, no arithmetic)
-    std::vector<uint32_t> keep;
-    if (use_range) {
-        keep.reserve((size_t)n);
-        for (uint64_t i = 0; i < n; ++i) {
-            int64_t rid = rowids ? rowids[i] : (int64_t)i;
-            if (rid >= rowid_lo && rid <= rowid_hi) keep.push_back((uint32_t)i);
-        }
-        if (keep.empty()) return YAMS_OK;
-    }
-    uint64_t m = use_range ? keep.size() : n;
-    OpWsLease lease;
-    if (!lease.w) return YAMS_ERR_INTERNAL;
-    cudaStream_t st = lease.w->st;
-    uint64_t np2 = 1;
-    while (np2 < m) np2 <<= 1;
-    DevBuf &d_rows = lease.w->d[0], &d_q = lease.w->d[1], &d_dist = lease.w->d[2], &d_keys = lease.w->d[3], &d_rid = lease.w->d[4],
-           &d_or = lease.w->d[5], &d_od = lease.w->d[6];
-    rc = d_rows.reserve((size_t)m * dim * 4);
-    if (rc == YAMS_OK) rc = d_q.reserve((size_t)dim * 4);
-    if (rc == YAMS_OK) rc = d_dist.reserve((size_t)m * 4);
-    if (rc == YAMS_OK) rc = d_keys.reserve((size_t)np2 * 8);
-    if (rc == YAMS_OK) rc = d_rid.reserve((size_t)m * 8);
-    if (rc == YAMS_OK) rc = d_or.reserve((size_t)m * 8);
-    if (rc == YAMS_OK) rc = d_od.reserve((size_t)m * 4);
-    if (rc == YAMS_OK) {
-        std::vector<int64_t> rid_h((size_t)m);
-        std::vector<float> packed;   // rows passing the rowid range, packed on the host: one copy instead of one per row
-        if (use_range) {
-            packed.resize((size_t)m * dim);
-            for (uint64_t j = 0; j < m; ++j) {
-                memcpy(packed.data() + (size_t)j * dim, rows + (size_t)keep[j] * dim, (size_t)dim * 4);
-                rid_h[j] = rowids ? rowids[keep[j]] : (int64_t)keep[j];
-            }
-            cudaMemcpyAsync(d_rows.p, packed.data(), (size_t)m * dim * 4, cudaMemcpyHostToDevice, st);
-        } else {
-            cudaMemcpyAsync(d_rows.p, rows, (size_t)m * dim * 4, cudaMemcpyHostToDevice, st);
-            for (uint64_t j = 0; j < m; ++j) rid_h[j] = rowids ? rowids[j] : (int64_t)j;
-        }
-        cudaMemcpyAsync(d_rid.p, rid_h.data(), (size_t)m * 8, cudaMemcpyHostToDevice, st);
-        cudaMemcpyAsync(d_q.p, query, (size_t)dim * 4, cudaMemcpyHostToDevice, st);
-        batch_dist_kernel<<<(unsigned)((m + 127) / 128), 128, 0, st>>>(d_rows.as<float>(), dim, m, d_q.as<float>(), YAMS_B200_L2, d_dist.as<float>());
-        unsigned g = (unsigned)std::min<uint64_t>((np2 + 255) / 256, 65535);
-        make_keys_kernel<<<g, 256, 0, st>>>(d_dist.as<float>(), m, np2, d_keys.as<uint64_t>());
-        for (uint64_t size = 2; size <= np2; size <<= 1)
-            for (uint64_t stride = size >> 1; stride > 0; stride >>= 1)
-                bitonic_step_kernel<<<g, 256, 0, st>>>(d_keys.as<uint64_t>(), np2, size, stride);
-        uint64_t outn = (k && k < m) ? k : m;
-        unpack_keys_kernel<<<g, 256, 0, st>>>(d_keys.as<uint64_t>(), outn, d_rid.as<int64_t>(), d_or.as<int64_t>(), d_od.as<float>());
-        cudaError_t e = cudaMemcpyAsync(out_rowids, d_or.p, (size_t)outn * 8, cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(out_dist, d_od.p, (size_t)outn * 4, cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-        if (e != cudaSuccess) {
-            set_last_error("vec0_exact failed: %s", cudaGetErrorString(e));
-            rc = YAMS_ERR_INTERNAL;
-        } else {
-            *out_count = outn;
-        }
-    }
-    return rc;
-    YB_CATCH
-}
-
-yams_status_t yams_b200_batch_distance(void* self, int metric, const float* query, uint32_t dim, const float* database,
-                                       uint64_t n, int mode, uint64_t k, float threshold, uint64_t* out_idx, float* out_dist,
-                                       uint64_t* out_count) {
-    YB_TRY
-    (void)self;
-    YB_ARG(out_count, "out_count is null");
-    *out_count = 0;
-    YB_ARG(metric == YAMS_B200_COSINE || metric == YAMS_B200_L2, "unknown metric");
-    YB_ARG(mode >= YAMS_B200_BATCH_ALL && mode <= YAMS_B200_BATCH_FILTERED, "unknown mode");
-    YB_ARG(query && dim > 0, "bad query");
-    if (n == 0 || (mode == YAMS_B200_BATCH_TOP_K && k == 0)) return YAMS_OK;
-    YB_ARG(database, "database is null");
-    YB_ARG(n < 0xFFFFFFFFull, "too many rows");
-    YB_ARG(mode == YAMS_B200_BATCH_ALL ? out_dist != nullptr : out_idx != nullptr, "null output");
-    YB_ARG(mode != YAMS_B200_BATCH_FILTERED || out_dist, "null output");
-    OpWsLease lease;
-    if (!lease.w) return YAMS_ERR_INTERNAL;
-    cudaStream_t st = lease.w->st;
-    yams_status_t rc;
-    uint64_t np2 = 1;
-    while (np2 < n) np2 <<= 1;
-    DevBuf &d_rows = lease.w->d[0], &d_q = lease.w->d[1], &d_dist = lease.w->d[2], &d_keys = lease.w->d[3], &d_oi = lease.w->d[4],
-           &d_od = lease.w->d[5], &d_cnt = lease.w->d[6];
-    rc = d_rows.reserve((size_t)n * dim * 4);
-    if (rc == YAMS_OK) rc = d_q.reserve((size_t)dim * 4);
-    if (rc == YAMS_OK) rc = d_dist.reserve((size_t)n * 4);
-    if (rc == YAMS_OK && mode != YAMS_B200_BATCH_ALL) {
-        rc = d_keys.reserve((size_t)np2 * 8);
-        if (rc == YAMS_OK) rc = d_oi.reserve((size_t)n * 8);
-        if (rc == YAMS_OK) rc = d_od.reserve((size_t)n * 4);
-        if (rc == YAMS_OK) rc = d_cnt.reserve(8);
-    }
-    if (rc == YAMS_OK) {
-        cudaError_t e = cudaMemcpyAsync(d_rows.p, database, (size_t)n * dim * 4, cudaMemcpyHostToDevice, st);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(d_q.p, query, (size_t)dim * 4, cudaMemcpyHostToDevice, st);
-        batch_dist_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(d_rows.as<float>(), dim, n, d_q.as<float>(), metric, d_dist.as<float>());
-        unsigned g = (unsigned)std::min<uint64_t>((np2 + 255) / 256, 65535);
-        uint64_t outn = n;
-        if (mode == YAMS_B200_BATCH_ALL) {
-            negate_kernel<<<g, 256, 0, st>>>(d_dist.as<float>(), n);
-            if (e == cudaSuccess) e = cudaMemcpyAsync(out_dist, d_dist.p, (size_t)n * 4, cudaMemcpyDeviceToHost, st);
-            if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-        } else {
-            if (mode == YAMS_B200_BATCH_TOP_K)
-                make_keys_kernel<<<g, 256, 0, st>>>(d_dist.as<float>(), n, np2, d_keys.as<uint64_t>());
-            else
-                make_keys_filtered_kernel<<<g, 256, 0, st>>>(d_dist.as<float>(), n, np2, threshold, d_keys.as<uint64_t>());
-            for (uint64_t size = 2; size <= np2; size <<= 1)
-                for (uint64_t stride = size >> 1; stride > 0; stride >>= 1)
-                    bitonic_step_kernel<<<g, 256, 0, st>>>(d_keys.as<uint64_t>(), np2, size, stride);
-            if (mode == YAMS_B200_BATCH_TOP_K) {
-                outn = std::min<uint64_t>(k, n);
-            } else {
-                unsigned long long h_cnt = 0;
-                if (e == cudaSuccess) e = cudaMemsetAsync(d_cnt.p, 0, 8, st);
-                count_nonzero_kernel<<<g, 256, 0, st>>>(d_keys.as<uint64_t>(), np2, d_cnt.as<unsigned long long>());
-                if (e == cudaSuccess) e = cudaMemcpyAsync(&h_cnt, d_cnt.p, 8, cudaMemcpyDeviceToHost, st);
-                if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-                outn = h_cnt;
-            }
-            if (outn && e == cudaSuccess) {
-                unpack_idx_keys_kernel<<<g, 256, 0, st>>>(d_keys.as<uint64_t>(), outn, d_oi.as<uint64_t>(), d_od.as<float>());
-                e = cudaMemcpyAsync(out_idx, d_oi.p, (size_t)outn * 8, cudaMemcpyDeviceToHost, st);
-                if (e == cudaSuccess && out_dist) e = cudaMemcpyAsync(out_dist, d_od.p, (size_t)outn * 4, cudaMemcpyDeviceToHost, st);
-                if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-            }
-        }
-        if (e == cudaSuccess) e = cudaGetLastError();
-        if (e != cudaSuccess) {
-            set_last_error("batch_distance failed: %s", cudaGetErrorString(e));
-            rc = YAMS_ERR_INTERNAL;
-        } else {
-            *out_count = outn;
-        }
-    }
-    return rc;
-    YB_CATCH
-}
-
-// n pairs (a_i, b_i) of d floats each -> n doubles; one thread per pair, the reference's accumulation order
-static yams_status_t cosine_similarity_pairs(const float* a, const float* b, size_t n, size_t d, double* out) {
-    OpWsLease lease;
-    OpWs* w = lease.w;
-    if (!w) return YAMS_ERR_INTERNAL;
-    yams_status_t rc;
-    const size_t vb = n * d * 4;
-    if ((rc = w->d[0].reserve(2 * vb + n * 8 + 64)) != YAMS_OK) return rc;
-    if ((rc = w->h.reserve(n * 8 + 64)) != YAMS_OK) return rc;
-    float* da = w->d[0].as<float>();
-    float* db = da + n * d;
-    double* dout = reinterpret_cast<double*>(w->d[0].as<uint8_t>() + ((2 * vb + 7) & ~(size_t)7));
-    YB_CUDA(cudaMemcpyAsync(da, a, vb, cudaMemcpyHostToDevice, w->st));
-    YB_CUDA(cudaMemcpyAsync(db, b, vb, cudaMemcpyHostToDevice, w->st));
-    cosine_similarity_f64_kernel<<<(unsigned)((n + 63) / 64), 64, 0, w->st>>>(da, db, n, d, dout);
-    YB_CUDA(cudaMemcpyAsync(w->h.p, dout, n * 8, cudaMemcpyDeviceToHost, w->st));
-    YB_CUDA(cudaStreamSynchronize(w->st));
-    memcpy(out, w->h.p, n * 8);
-    return YAMS_OK;
-}
-
-yams_status_t yams_b200_compute_cosine_similarity(void* self, const float* a, size_t na, const float* b, size_t nb, double* out) {
-    YB_TRY
-    (void)self;
-    YB_ARG(out, "out is null");
-    *out = 0.0;
-    if (na != nb || na == 0) return YAMS_OK;   // vector_database.cpp:1788-1790
-    YB_ARG(a && b, "null vector");
-    return cosine_similarity_pairs(a, b, 1, na, out);
-    YB_CATCH
-}
-
-// The rerank loops that call computeCosineSimilarity once per candidate (sqlite_vec_backend.cpp:4025,4374,4507) as ONE device
-// pass: n pairs, row-major a[n][dim] / b[n][dim] (pass the same query n times, or n different pairs).
-yams_status_t yams_b200_compute_cosine_similarity_many(void* self, const float* a, const float* b, size_t n, size_t dim, double* out) {
-    YB_TRY
-    (void)self;
-    YB_ARG(out || n == 0, "out is null");
-    if (n == 0) return YAMS_OK;
-    if (dim == 0) {
-        for (size_t i = 0; i < n; ++i) out[i] = 0.0;
-        return YAMS_OK;
-    }
-    YB_ARG(a && b, "null vector");
-    return cosine_similarity_pairs(a, b, n, dim, out);
-    YB_CATCH
 }
 
 }  // extern "C"

@@ -1,5 +1,6 @@
 // knn.cuh -- shared declarations of the exact vector scan (vector_scan_v1).
 #pragma once
+#include <algorithm>
 #include <mutex>
 
 #include "common.cuh"
@@ -86,6 +87,23 @@ struct Stage1Args {
 };
 
 yams_status_t stage1_cuda_core(const Stage1Args& a, bool filter, cudaStream_t st);
+
+// Device key sort of the exact paths (knn.cu) and the sqlite-vec operators (operators.cu).  A key is
+// (fkey(score) << 32) | (0xFFFFFFFF - row), so descending order is score descending, then row ascending; key 0 marks no entry.
+inline uint64_t pow2_at_least(uint64_t n) {
+    uint64_t p = 1;
+    while (p < n) p <<= 1;
+    return p;
+}
+// grid of the 256-thread grid-stride key kernels over n keys
+inline unsigned key_grid(uint64_t n) { return (unsigned)std::min<uint64_t>((n + 255) / 256, 65535); }
+// bitonic sort, descending, of np2 keys (a power of two)
+void sort_keys_desc(uint64_t* keys, uint64_t np2, cudaStream_t st);
+// *d_count += the number of non-zero keys among n
+void count_nonzero_keys(const uint64_t* keys, uint64_t n, unsigned long long* d_count, cudaStream_t st);
+// the first m keys -> out_rowids[i] = rowids ? rowids[row] : row, out_scores[i] = negate ? -score : score
+void unpack_keys(const uint64_t* keys, uint64_t m, const int64_t* rowids, bool negate, int64_t* out_rowids, float* out_scores,
+                 cudaStream_t st);
 
 }  // namespace yb
 
