@@ -679,11 +679,6 @@ __global__ void __launch_bounds__(SEL_THREADS) topk_select_kernel(SelectIn in, u
 // ---------------------------------------------------------------------------------------------------
 // stage 2: exact re-scoring + final ordering
 // ---------------------------------------------------------------------------------------------------
-struct Exact {
-    float sim;       // reference similarity (float cast of the double quotient); NaN marks "skipped"
-    uint32_t row;
-};
-
 // one thread per (query, survivor).
 // cosine: sqlite_vec_backend.cpp:4253-4279 evaluated in the same order (sequential double accumulation, skip rules, float cast)
 // L2    : distances::l2_distance<float> as the reference BUILD evaluates it (YAMS compiles sqlite-vec-cpp with AVX,
@@ -1436,11 +1431,11 @@ void launch_topk_lists(const Cand* lists, const uint32_t* counts, uint32_t cap, 
     in.cands = lists; in.counts = counts; in.cap = cap;
     topk_select_kernel<<<nq, SEL_THREADS, 0, st>>>(in, K, 0, nullptr, out_sel, out_n, nullptr);
 }
-void launch_final_plain(const void* exact, uint32_t Kp, uint32_t k, uint32_t nq, const int64_t* rowids, int64_t* out_rowids, float* out_scores,
+void launch_final_plain(const Exact* exact, uint32_t Kp, uint32_t k, uint32_t nq, const int64_t* rowids, int64_t* out_rowids, float* out_scores,
                         uint32_t* out_counts, uint64_t* out_flags, cudaStream_t st) {
     CertArgs cert{};   // status == nullptr: no certificate (the caller's survivors are what the reference re-ranks, too)
-    final_kernel<<<nq, SEL_THREADS, 0, st>>>(static_cast<const Exact*>(exact), nullptr, Kp, k, rowids, 0, out_rowids, out_scores, out_counts,
-                                             out_flags, -INFINITY, nullptr, cert);
+    final_kernel<<<nq, SEL_THREADS, 0, st>>>(exact, nullptr, Kp, k, rowids, 0, out_rowids, out_scores, out_counts, out_flags, -INFINITY, nullptr,
+                                             cert);
 }
 // rowids -> corpus rows (out[i].row, 0xFFFFFFFF for unknown rowids), any order
 void launch_map_rowids(const int64_t* rowids_in, uint64_t n_in, const int64_t* corpus_rowids, uint64_t n, Cand* out, cudaStream_t st) {
@@ -1451,6 +1446,32 @@ void launch_map_rowids(const int64_t* rowids_in, uint64_t n_in, const int64_t* c
 void launch_query_prep(const float* q, uint32_t nq, uint32_t d, double* qnorm, float* qinv, void* status, cudaStream_t st) {
     query_prep_kernel<<<(nq + QP_THREADS - 1) / QP_THREADS, QP_THREADS, 0, st>>>(q, nq, d, qnorm, qinv, YAMS_B200_COSINE,
                                                                                 static_cast<ScanStatus*>(status));
+}
+
+// DeviceResults (knn.cuh) in `buf`, the results buffer of the caller's handle
+yams_status_t reserve_results(DevBuf& buf, uint32_t nq, uint32_t k, DeviceResults* r) {
+    yams_status_t rc = buf.reserve((size_t)nq * k * 12 + (size_t)nq * 12 + 64);
+    if (rc != YAMS_OK) return rc;
+    r->rowids = buf.as<int64_t>();
+    r->flags = reinterpret_cast<uint64_t*>(r->rowids + (size_t)nq * k);
+    r->scores = reinterpret_cast<float*>(r->flags + nq);
+    r->counts = reinterpret_cast<uint32_t*>(r->scores + (size_t)nq * k);
+    return YAMS_OK;
+}
+yams_status_t enqueue_results(const DeviceResults& r, uint32_t nq, uint32_t k, int64_t* out_rowids, float* out_scores, uint32_t* out_counts,
+                              uint64_t* out_flags, cudaStream_t st) {
+    YB_CUDA(cudaMemcpyAsync(out_rowids, r.rowids, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, st));
+    YB_CUDA(cudaMemcpyAsync(out_scores, r.scores, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, st));
+    YB_CUDA(cudaMemcpyAsync(out_counts, r.counts, (size_t)nq * 4, cudaMemcpyDeviceToHost, st));
+    if (out_flags) YB_CUDA(cudaMemcpyAsync(out_flags, r.flags, (size_t)nq * 8, cudaMemcpyDeviceToHost, st));
+    return YAMS_OK;
+}
+yams_status_t copy_results(const DeviceResults& r, uint32_t nq, uint32_t k, int64_t* out_rowids, float* out_scores, uint32_t* out_counts,
+                           uint64_t* out_flags, cudaStream_t st) {
+    yams_status_t rc = enqueue_results(r, nq, k, out_rowids, out_scores, out_counts, out_flags, st);
+    if (rc != YAMS_OK) return rc;
+    YB_CUDA(cudaStreamSynchronize(st));
+    return YAMS_OK;
 }
 
 // Exact scores of m corpus rows for query q (rescore_kernel; with a mask, rows outside it are skipped) as keys sorted
@@ -1877,33 +1898,6 @@ static yams_status_t prepare_valid_queries(yams_b200_corpus* c, const float* que
     return YAMS_OK;
 }
 
-// the padded [nq][k] results of a search on the device, in c->dout: [nq*k rowids][nq flags][nq*k scores][nq counts]
-struct DeviceResults {
-    int64_t* rowids;
-    uint64_t* flags;
-    float* scores;
-    uint32_t* counts;
-};
-static yams_status_t reserve_results(yams_b200_corpus* c, uint32_t nq, uint32_t k, DeviceResults* r) {
-    yams_status_t rc = c->dout.reserve((size_t)nq * k * 12 + (size_t)nq * 12 + 64);
-    if (rc != YAMS_OK) return rc;
-    r->rowids = c->dout.as<int64_t>();
-    r->flags = reinterpret_cast<uint64_t*>(r->rowids + (size_t)nq * k);
-    r->scores = reinterpret_cast<float*>(r->flags + nq);
-    r->counts = reinterpret_cast<uint32_t*>(r->scores + (size_t)nq * k);
-    return YAMS_OK;
-}
-// device results -> the caller's arrays (out_flags nullable), then wait for them
-static yams_status_t copy_results(yams_b200_corpus* c, const DeviceResults& r, uint32_t nq, uint32_t k, int64_t* out_rowids,
-                                  float* out_scores, uint32_t* out_counts, uint64_t* out_flags) {
-    YB_CUDA(cudaMemcpyAsync(out_rowids, r.rowids, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, c->st));
-    YB_CUDA(cudaMemcpyAsync(out_scores, r.scores, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, c->st));
-    YB_CUDA(cudaMemcpyAsync(out_counts, r.counts, (size_t)nq * 4, cudaMemcpyDeviceToHost, c->st));
-    if (out_flags) YB_CUDA(cudaMemcpyAsync(out_flags, r.flags, (size_t)nq * 8, cudaMemcpyDeviceToHost, c->st));
-    YB_CUDA(cudaStreamSynchronize(c->st));
-    return YAMS_OK;
-}
-
 yams_status_t yams_b200_search(yams_b200_corpus* c, const float* queries, uint32_t nq, uint32_t k, float threshold,
                                const int64_t* allowed_rowids, const uint64_t* allowed_offsets, int64_t* out_rowids,
                                float* out_scores, uint32_t* out_counts, uint64_t* out_flags) {
@@ -1931,7 +1925,7 @@ yams_status_t yams_b200_search(yams_b200_corpus* c, const float* queries, uint32
     if ((rc = prepare_queries(c, queries, false, nq)) != YAMS_OK) return rc;
     YB_CUDA(cudaEventRecord(c->ev[0], c->st));
     DeviceResults r;
-    if ((rc = reserve_results(c, nq, k, &r)) != YAMS_OK) return rc;
+    if ((rc = reserve_results(c->dout, nq, k, &r)) != YAMS_OK) return rc;
     ScanPlan plan;
     plan.nq = nq; plan.k = k; plan.threshold = threshold;
     plan.use_tensor = wgmma_supported(c, nq);
@@ -1958,7 +1952,7 @@ yams_status_t yams_b200_search(yams_b200_corpus* c, const float* queries, uint32
     if ((rc = scan_enqueue(c, plan, r.rowids, r.scores, r.counts, r.flags)) != YAMS_OK) return rc;
     cudaEventRecord(c->ev[2], c->st);
     if ((rc = enqueue_status_readback(c, nq)) != YAMS_OK) return rc;
-    if ((rc = copy_results(c, r, nq, k, out_rowids, out_scores, out_counts, out_flags)) != YAMS_OK) return rc;
+    if ((rc = copy_results(r, nq, k, out_rowids, out_scores, out_counts, out_flags, c->st)) != YAMS_OK) return rc;
     cudaEventElapsedTime(&c->last_ms[0], c->ev[0], c->ev[1]);
     cudaEventElapsedTime(&c->last_ms[1], c->ev[1], c->ev[2]);
     cudaEventElapsedTime(&c->last_ms[2], c->ev[0], c->ev[2]);
@@ -1976,7 +1970,7 @@ yams_status_t yams_b200_search(yams_b200_corpus* c, const float* queries, uint32
         for (uint32_t q = 0; q < nq; ++q) out_counts[q] = 0;
         return rc;
     }
-    if (resolved) return copy_results(c, r, nq, k, out_rowids, out_scores, out_counts, out_flags);
+    if (resolved) return copy_results(r, nq, k, out_rowids, out_scores, out_counts, out_flags, c->st);
     return YAMS_OK;
     YB_CATCH
 }
@@ -1998,12 +1992,12 @@ yams_status_t yams_b200_search_exhaustive(yams_b200_corpus* c, const float* quer
     c->pending.active = false;
     if ((rc = prepare_valid_queries(c, queries, nq)) != YAMS_OK) return rc;
     DeviceResults r;
-    if ((rc = reserve_results(c, nq, k, &r)) != YAMS_OK) return rc;
+    if ((rc = reserve_results(c->dout, nq, k, &r)) != YAMS_OK) return rc;
     ScanPlan plan;
     plan.nq = nq; plan.k = k; plan.threshold = threshold;
     for (uint32_t q = 0; q < nq; ++q)
         if ((rc = exact_all_rows(c, plan, q, r.rowids, r.scores, r.counts, r.flags)) != YAMS_OK) return rc;
-    return copy_results(c, r, nq, k, out_rowids, out_scores, out_counts, out_flags);
+    return copy_results(r, nq, k, out_rowids, out_scores, out_counts, out_flags, c->st);
     YB_CATCH
 }
 
@@ -2368,7 +2362,7 @@ yams_status_t yams_b200_debug_final(yams_b200_corpus* c, uint32_t nq, uint32_t K
     if ((rc = c->misc.reserve((size_t)nq * 8)) != YAMS_OK) return rc;
     if ((rc = c->status.reserve(sizeof(ScanStatus) + (size_t)nq * 8)) != YAMS_OK) return rc;
     DeviceResults r;
-    if ((rc = reserve_results(c, nq, k, &r)) != YAMS_OK) return rc;
+    if ((rc = reserve_results(c->dout, nq, k, &r)) != YAMS_OK) return rc;
     Exact* d_ex = c->outbuf.as<Exact>();
     uint32_t* d_ex_n = reinterpret_cast<uint32_t*>(d_ex + (size_t)nq * Kp);
     YB_CUDA(cudaMemcpyAsync(d_ex, ex, eb, cudaMemcpyHostToDevice, st));
@@ -2387,7 +2381,7 @@ yams_status_t yams_b200_debug_final(yams_b200_corpus* c, uint32_t nq, uint32_t K
     YB_CUDA(cudaGetLastError());
     std::vector<uint32_t> h_status(sizeof(ScanStatus) / 4 + (size_t)nq * 2);
     YB_CUDA(cudaMemcpyAsync(h_status.data(), c->status.p, h_status.size() * 4, cudaMemcpyDeviceToHost, st));
-    if ((rc = copy_results(c, r, nq, k, out_rowids, out_scores, out_counts, out_flags)) != YAMS_OK) return rc;
+    if ((rc = copy_results(r, nq, k, out_rowids, out_scores, out_counts, out_flags, c->st)) != YAMS_OK) return rc;
     const ScanStatus* hs = reinterpret_cast<const ScanStatus*>(h_status.data());
     const uint32_t nqd = std::min(level == 0 ? hs->n_bad : hs->n_bad2, nq);
     const uint32_t* list = h_status.data() + sizeof(ScanStatus) / 4 + (level == 0 ? 0 : nq);

@@ -13,6 +13,12 @@ struct __align__(8) Cand {
     uint32_t row;
 };
 
+// exactly re-scored survivor of stage 2, the input of the final ordering
+struct Exact {
+    float sim;       // reference similarity (float cast of the double quotient); NaN marks "skipped"
+    uint32_t row;
+};
+
 struct Corpus {
     DeviceCtx* dev = nullptr;
     cudaStream_t st = nullptr;
@@ -87,6 +93,29 @@ struct Stage1Args {
 };
 
 yams_status_t stage1_cuda_core(const Stage1Args& a, bool filter, cudaStream_t st);
+
+// Stages of the exact scan that the other engines (pq.cu) launch on their own lists; each is described at its definition in knn.cu
+void launch_topk_lists(const Cand* lists, const uint32_t* counts, uint32_t cap, uint32_t nq, uint32_t K, Cand* out_sel, uint32_t* out_n,
+                       cudaStream_t st);
+void launch_final_plain(const Exact* exact, uint32_t Kp, uint32_t k, uint32_t nq, const int64_t* rowids, int64_t* out_rowids, float* out_scores,
+                        uint32_t* out_counts, uint64_t* out_flags, cudaStream_t st);
+void launch_map_rowids(const int64_t* rowids_in, uint64_t n_in, const int64_t* corpus_rowids, uint64_t n, Cand* out, cudaStream_t st);
+void launch_query_prep(const float* q, uint32_t nq, uint32_t d, double* qnorm, float* qinv, void* status, cudaStream_t st);
+
+// the padded [nq][k] results of a search on the device: [nq*k rowids][nq flags][nq*k scores][nq counts] carved out of one buffer
+struct DeviceResults {
+    int64_t* rowids;
+    uint64_t* flags;
+    float* scores;
+    uint32_t* counts;
+};
+yams_status_t reserve_results(DevBuf& buf, uint32_t nq, uint32_t k, DeviceResults* r);
+// device results -> the caller's arrays (out_flags nullable).  enqueue_results only enqueues the copies, for a caller with one
+// more read-back to make before it waits; copy_results also waits for them.
+yams_status_t enqueue_results(const DeviceResults& r, uint32_t nq, uint32_t k, int64_t* out_rowids, float* out_scores, uint32_t* out_counts,
+                              uint64_t* out_flags, cudaStream_t st);
+yams_status_t copy_results(const DeviceResults& r, uint32_t nq, uint32_t k, int64_t* out_rowids, float* out_scores, uint32_t* out_counts,
+                           uint64_t* out_flags, cudaStream_t st);
 
 // Device key sort of the exact paths (knn.cu) and the sqlite-vec operators (operators.cu).  A key is
 // (fkey(score) << 32) | (0xFFFFFFFF - row), so descending order is score descending, then row ascending; key 0 marks no entry.

@@ -42,11 +42,6 @@ __device__ __forceinline__ bool normalize_factor(double norm_sq, float* inv) {
     return true;
 }
 
-__device__ __forceinline__ float load_row_elem(const void* rows, int dtype, uint64_t idx) {
-    if (dtype == YAMS_B200_F16) return __half2float(reinterpret_cast<const __half*>(rows)[idx]);
-    return reinterpret_cast<const float*>(rows)[idx];
-}
-
 // one thread per corpus row: is it indexable (the rule of normalize_factor: not norm_sq <= 1e-20)?  keep[row] = 1/0.  A row
 // with a NaN element has a NaN norm: the reference indexes it (it encodes to code 0 everywhere and re-scores to NaN).
 __global__ void pq_keep_kernel(const void* __restrict__ rows, int dtype, uint32_t d, uint64_t n, uint32_t* __restrict__ keep) {
@@ -54,7 +49,7 @@ __global__ void pq_keep_kernel(const void* __restrict__ rows, int dtype, uint32_
     if (r >= n) return;
     double ss = 0.0;
     for (uint32_t c = 0; c < d; ++c) {
-        float v = load_row_elem(rows, dtype, r * d + c);
+        float v = load_elem(rows, dtype, r * d + c);
         ss += (double)v * (double)v;
     }
     keep[r] = ss <= 1e-20 ? 0u : 1u;
@@ -77,7 +72,7 @@ __global__ void __launch_bounds__(256) pq_encode_kernel(const void* __restrict__
     if (j >= n_idx) return;
     const uint64_t row = idx_rows[j];
     const uint32_t dsub = d / m;
-    for (uint32_t c = threadIdx.x; c < d; c += blockDim.x) xs[c] = load_row_elem(rows, dtype, row * d + c);
+    for (uint32_t c = threadIdx.x; c < d; c += blockDim.x) xs[c] = load_elem(rows, dtype, row * d + c);
     __syncthreads();
     if (threadIdx.x == 0) {
         double ss = 0.0;
@@ -371,17 +366,13 @@ __global__ void pq_rank_to_row_kernel(Cand* __restrict__ sel, const uint32_t* __
     }
 }
 
-struct PqExact {
-    float sim;
-    uint32_t row;
-};
 // VectorDatabase::computeCosineSimilarity (vector_database.cpp:1786-1810) of the ORIGINAL query a against corpus row `row`,
 // float cast, NaN and `similarity < threshold` dropped (sqlite_vec_backend.cpp:4022-4037).  -> true and *out = sim when kept.
 __device__ __forceinline__ bool pq_rerank_sim(const void* __restrict__ rows, int dtype, uint32_t d, uint32_t row, const float* __restrict__ a,
                                               float threshold, float* out) {
     double dp = 0.0, na = 0.0, nb = 0.0;
     for (uint32_t c = 0; c < d; ++c) {
-        const double x = (double)a[c], y = (double)load_row_elem(rows, dtype, (uint64_t)row * d + c);
+        const double x = (double)a[c], y = (double)load_elem(rows, dtype, (uint64_t)row * d + c);
         dp += x * y;
         na += x * x;
         nb += y * y;
@@ -397,11 +388,11 @@ __device__ __forceinline__ bool pq_rerank_sim(const void* __restrict__ rows, int
 }
 __global__ void pq_rerank_kernel(const void* __restrict__ rows, int dtype, uint32_t d, const float* __restrict__ q32, const Cand* __restrict__ sel,
                                  const uint32_t* __restrict__ sel_n, const uint32_t* __restrict__ valid, uint32_t K, uint32_t nq,
-                                 float threshold, PqExact* __restrict__ out) {
+                                 float threshold, Exact* __restrict__ out) {
     uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= nq * K) return;
     uint32_t q = t / K, j = t % K;
-    PqExact e;
+    Exact e;
     e.sim = __int_as_float(0x7FC00000);
     e.row = 0xFFFFFFFFu;
     if (valid[q] && j < sel_n[q]) {
@@ -572,14 +563,6 @@ __global__ void doc_emit_kernel(const Cand* __restrict__ sel, const uint32_t* __
     if (i == 0) o_counts[q] = sel_n[q];
 }
 
-// defined in knn.cu
-void launch_topk_lists(const Cand* lists, const uint32_t* counts, uint32_t cap, uint32_t nq, uint32_t K, Cand* out_sel, uint32_t* out_n,
-                       cudaStream_t st);
-void launch_final_plain(const void* exact, uint32_t Kp, uint32_t k, uint32_t nq, const int64_t* rowids, int64_t* out_rowids, float* out_scores,
-                        uint32_t* out_counts, uint64_t* out_flags, cudaStream_t st);
-void launch_map_rowids(const int64_t* rowids_in, uint64_t n_in, const int64_t* corpus_rowids, uint64_t n, Cand* out, cudaStream_t st);
-void launch_query_prep(const float* q, uint32_t nq, uint32_t d, double* qnorm, float* qinv, void* status, cudaStream_t st);
-
 // Host staging of ONE host-to-device copy: the pieces of a call's input at 16-byte aligned offsets
 struct Staging {
     std::vector<unsigned char> h;
@@ -710,47 +693,58 @@ yams_status_t yams_b200_pq_codes(yams_b200_pq* p, uint8_t* out_codes, int64_t* o
 
 }  // extern "C"
 
-// the per-query lists (32 k entries each on the filtered path) bound the batch one pass can take: larger batches are sliced
-static constexpr uint32_t kPqMaxBatch = 512;
-static yams_status_t pq_search_batch(yams_b200_pq* p, const float* queries, uint32_t nq, uint32_t k, uint32_t rerank_factor, float threshold,
-                                     int64_t* out_rowids, float* out_scores, uint32_t* out_counts, uint64_t* out_flags);
-
-extern "C" {
-
-yams_status_t yams_b200_pq_search(yams_b200_pq* p, const float* queries, uint32_t nq, uint32_t k, uint32_t rerank_factor, float threshold,
-                                  int64_t* out_rowids, float* out_scores, uint32_t* out_counts, uint64_t* out_flags) {
-    YB_TRY
-    YB_ARG(p && out_counts, "null argument");
-    std::lock_guard<std::mutex> lk(p->mu);
-    yams_b200_corpus* c = p->corpus;
-    std::lock_guard<std::mutex> corpus_lock(c->mu);
-    YB_BIND(c);
+// a public search entry reports no results until a batch has written them
+static void zero_outputs(uint32_t nq, uint32_t* out_counts, uint64_t* out_flags) {
     for (uint32_t q = 0; q < nq; ++q) out_counts[q] = 0;
     if (out_flags) for (uint32_t q = 0; q < nq; ++q) out_flags[q] = 0;
-    for (uint32_t& v : p->last_path) v = 0;
-    if (nq == 0 || k == 0 || p->n_idx == 0) return YAMS_OK;                           // :3873-3881
-    YB_ARG(queries && out_rowids && out_scores, "null argument");
-    YB_ARG(c->generation == p->corpus_generation, "the corpus changed after the PQ index was built: rebuild it (the reference marks the index dirty)");
-    for (uint32_t q0 = 0; q0 < nq; q0 += kPqMaxBatch) {
-        const uint32_t nb = std::min<uint32_t>(kPqMaxBatch, nq - q0);
-        yams_status_t rc = pq_search_batch(p, queries + (size_t)q0 * p->dim, nb, k, rerank_factor, threshold, out_rowids + (size_t)q0 * k,
-                                           out_scores + (size_t)q0 * k, out_counts + q0, out_flags ? out_flags + q0 : nullptr);
-        if (rc != YAMS_OK) return rc;
-    }
-    return YAMS_OK;
-    YB_CATCH
 }
 
-}  // extern "C"
+// rows the reference re-scores exactly, before the cut to the rows there are: max(k, k * max(1, rerank_factor)) (:3670, :3956-3959)
+static uint64_t pq_rerank_budget(uint32_t k, uint32_t rerank_factor) {
+    return std::max<uint64_t>(k, (uint64_t)k * std::max<uint32_t>(rerank_factor, 1));
+}
+
+// The query-table stage: p->lut and p->valid (pq_lut_kernel) of the nq queries at d_q, which are on the device already
+static yams_status_t pq_build_luts(yams_b200_pq* p, const float* d_q, uint32_t nq, cudaStream_t st) {
+    yams_status_t rc;
+    const uint32_t m = p->m, kc = p->k, d = p->dim;
+    if ((rc = p->lut.reserve((size_t)nq * m * kc * 4)) != YAMS_OK) return rc;
+    if ((rc = p->valid.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
+    YB_CUDA(cudaFuncSetAttribute(pq_lut_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(d * 4)));
+    pq_lut_kernel<<<nq, 256, d * 4, st>>>(d_q, d, p->codebooks.as<float>(), m, kc, p->lut.as<float>(), p->valid.as<uint32_t>());
+    YB_CUDA(cudaGetLastError());
+    return YAMS_OK;
+}
+
+// The tail of a search: the <= K selected (ADC score, tie rank) entries of every query -> corpus rows -> exact rerank against the
+// queries at d_q -> final order -> the copies to the caller's arrays, enqueued.  The caller enqueues what else it reads back
+// and waits for the stream, so a batch costs one host synchronisation.
+static yams_status_t pq_rerank_and_emit(yams_b200_pq* p, const float* d_q, Cand* d_sel, const uint32_t* d_sel_n, uint32_t K, uint32_t nq, uint32_t k,
+                                        float threshold, int64_t* out_rowids, float* out_scores, uint32_t* out_counts, uint64_t* out_flags) {
+    yams_b200_corpus* c = p->corpus;
+    cudaStream_t st = c->st;
+    yams_status_t rc;
+    DeviceResults r;
+    if ((rc = p->exact.reserve((size_t)nq * K * sizeof(Exact))) != YAMS_OK) return rc;
+    if ((rc = reserve_results(p->dout, nq, k, &r)) != YAMS_OK) return rc;
+    const uint32_t tot = nq * K;
+    pq_rank_to_row_kernel<<<(tot + 255) / 256, 256, 0, st>>>(d_sel, d_sel_n, K, nq, p->rank_to_idx.as<uint32_t>(), p->idx_rows.as<uint32_t>());
+    pq_rerank_kernel<<<(tot + 127) / 128, 128, 0, st>>>(c->rows.p, c->dtype, p->dim, d_q, d_sel, d_sel_n, p->valid.as<uint32_t>(), K, nq, threshold,
+                                                        p->exact.as<Exact>());
+    launch_final_plain(p->exact.as<Exact>(), K, k, nq, c->rowids.as<int64_t>(), r.rowids, r.scores, r.counts, r.flags, st);
+    YB_CUDA(cudaGetLastError());
+    return enqueue_results(r, nq, k, out_rowids, out_scores, out_counts, out_flags, st);
+}
+
+// the per-query lists (32 k entries each on the filtered path) bound the batch one pass can take: larger batches are sliced
+static constexpr uint32_t kPqMaxBatch = 512;
 
 // one batch of <= kPqMaxBatch queries; the caller holds both locks and has bound the device
 static yams_status_t pq_search_batch(yams_b200_pq* p, const float* queries, uint32_t nq, uint32_t k, uint32_t rerank_factor, float threshold,
                                      int64_t* out_rowids, float* out_scores, uint32_t* out_counts, uint64_t* out_flags) {
     YB_TRY
     yams_b200_corpus* c = p->corpus;
-    if (rerank_factor == 0) rerank_factor = 1;                                        // :3670 max(1, rerank_factor)
-    const uint64_t budget = (uint64_t)k * rerank_factor;
-    const uint32_t approx = (uint32_t)std::min<uint64_t>(p->n_idx, std::max<uint64_t>(k, budget));   // :3956-3959
+    const uint32_t approx = (uint32_t)std::min<uint64_t>(p->n_idx, pq_rerank_budget(k, rerank_factor));   // :3956-3959
     YB_ARG(approx <= PQ_MAX_APPROX, "k * rerank_factor > 1024 is not supported by the PQ engine (use the exact scan)");
     cudaStream_t st = c->st;
     yams_status_t rc;
@@ -770,21 +764,16 @@ static yams_status_t pq_search_batch(yams_b200_pq* p, const float* queries, uint
     const uint32_t cap_unf = tiles * approx;
     const uint32_t cap = filtered ? std::max<uint32_t>(kFilterCap, sample_tiles * approx) : cap_unf;
     if ((rc = p->q32.reserve((size_t)nq * d * 4)) != YAMS_OK) return rc;
-    if ((rc = p->lut.reserve((size_t)nq * m * kc * 4)) != YAMS_OK) return rc;
-    if ((rc = p->valid.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
     if ((rc = p->lists.reserve((size_t)nq * cap * sizeof(Cand))) != YAMS_OK) return rc;
     if ((rc = p->counts.reserve((size_t)nq * 4 + 16)) != YAMS_OK) return rc;
     if ((rc = p->sel.reserve((size_t)nq * approx * sizeof(Cand) + (size_t)nq * 4)) != YAMS_OK) return rc;
-    if ((rc = p->exact.reserve((size_t)nq * approx * sizeof(PqExact))) != YAMS_OK) return rc;
-    if ((rc = p->dout.reserve((size_t)nq * k * 12 + (size_t)nq * 12 + 64)) != YAMS_OK) return rc;
     if ((rc = p->tau.reserve((size_t)nq * 8)) != YAMS_OK) return rc;
     Cand* d_sel = p->sel.as<Cand>();
     uint32_t* d_sel_n = reinterpret_cast<uint32_t*>(d_sel + (size_t)nq * approx);
     uint32_t* d_counts = p->counts.as<uint32_t>();
     uint32_t* d_overflow = d_counts + nq;
     YB_CUDA(cudaMemcpyAsync(p->q32.p, queries, (size_t)nq * d * 4, cudaMemcpyHostToDevice, st));
-    YB_CUDA(cudaFuncSetAttribute(pq_lut_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(d * 4)));
-    pq_lut_kernel<<<nq, 256, d * 4, st>>>(p->q32.as<float>(), d, p->codebooks.as<float>(), m, kc, p->lut.as<float>(), p->valid.as<uint32_t>());
+    if ((rc = pq_build_luts(p, p->q32.as<float>(), nq, st)) != YAMS_OK) return rc;
     const size_t lut_bytes = (size_t)m * kc * 4;
     const size_t smem = ((lut_bytes + 7) & ~(size_t)7) + (size_t)PQ_TILE * 8;
     YB_CUDA(cudaFuncSetAttribute(pq_adc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -794,11 +783,9 @@ static yams_status_t pq_search_batch(yams_b200_pq* p, const float* queries, uint
                                                                   approx, p->lists.as<Cand>(), list_cap, d_counts, stride);
         launch_topk_lists(p->lists.as<Cand>(), d_counts, list_cap, nq, approx, d_sel, d_sel_n, st);
     };
-    bool used_filter = false;
     p->last_path[0] = filtered ? 1u : 0u;
     p->last_path[1] = p->last_path[2] = p->last_path[3] = 0;
     if (filtered) {
-        used_filter = true;
         const uint32_t stride = tiles / sample_tiles;
         unfiltered(sample_tiles, stride, cap);
         pq_tau_kernel<<<(nq + 127) / 128, 128, 0, st>>>(d_sel, d_sel_n, approx, nq, p->tau.as<uint64_t>(), d_counts);
@@ -823,37 +810,48 @@ static yams_status_t pq_search_batch(yams_b200_pq* p, const float* queries, uint
     } else {
         unfiltered(tiles, 1, cap);
     }
-    for (int attempt = 0; attempt < 2; ++attempt) {
-    if (attempt == 1) {
-        // a filtered list overflowed: redo the selection without the filter
-        p->last_path[3] = 1;
-        if ((rc = p->lists.reserve((size_t)nq * cap_unf * sizeof(Cand))) != YAMS_OK) return rc;
-        unfiltered(tiles, 1, cap_unf);
-    }
-    const uint32_t tot = nq * approx;
-    pq_rank_to_row_kernel<<<(tot + 255) / 256, 256, 0, st>>>(d_sel, d_sel_n, approx, nq, p->rank_to_idx.as<uint32_t>(), p->idx_rows.as<uint32_t>());
-    pq_rerank_kernel<<<(tot + 127) / 128, 128, 0, st>>>(c->rows.p, c->dtype, d, p->q32.as<float>(), d_sel, d_sel_n, p->valid.as<uint32_t>(), approx, nq,
-                                                        threshold, p->exact.as<PqExact>());
-    int64_t* d_or = p->dout.as<int64_t>();
-    uint64_t* d_of = reinterpret_cast<uint64_t*>(d_or + (size_t)nq * k);
-    float* d_os = reinterpret_cast<float*>(d_of + nq);
-    uint32_t* d_oc = reinterpret_cast<uint32_t*>(d_os + (size_t)nq * k);
-    launch_final_plain(p->exact.p, approx, k, nq, c->rowids.as<int64_t>(), d_or, d_os, d_oc, d_of, st);
-    YB_CUDA(cudaGetLastError());
-    YB_CUDA(cudaMemcpyAsync(out_rowids, d_or, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, st));
-    YB_CUDA(cudaMemcpyAsync(out_scores, d_os, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, st));
-    YB_CUDA(cudaMemcpyAsync(out_counts, d_oc, (size_t)nq * 4, cudaMemcpyDeviceToHost, st));
-    if (out_flags) YB_CUDA(cudaMemcpyAsync(out_flags, d_of, (size_t)nq * 8, cudaMemcpyDeviceToHost, st));
+    auto tail = [&] {
+        return pq_rerank_and_emit(p, p->q32.as<float>(), d_sel, d_sel_n, approx, nq, k, threshold, out_rowids, out_scores, out_counts, out_flags);
+    };
+    if ((rc = tail()) != YAMS_OK) return rc;
     uint32_t h_overflow = 0;
-    if (used_filter && attempt == 0) YB_CUDA(cudaMemcpyAsync(&h_overflow, d_overflow, 4, cudaMemcpyDeviceToHost, st));
+    if (filtered) YB_CUDA(cudaMemcpyAsync(&h_overflow, d_overflow, 4, cudaMemcpyDeviceToHost, st));
     YB_CUDA(cudaStreamSynchronize(st));
-    if (!h_overflow) break;
-    }
+    if (!h_overflow) return YAMS_OK;
+    // a filtered list overflowed: redo the selection without the filter
+    p->last_path[3] = 1;
+    if ((rc = p->lists.reserve((size_t)nq * cap_unf * sizeof(Cand))) != YAMS_OK) return rc;
+    unfiltered(tiles, 1, cap_unf);
+    if ((rc = tail()) != YAMS_OK) return rc;
+    YB_CUDA(cudaStreamSynchronize(st));
     return YAMS_OK;
     YB_CATCH
 }
 
 extern "C" {
+
+yams_status_t yams_b200_pq_search(yams_b200_pq* p, const float* queries, uint32_t nq, uint32_t k, uint32_t rerank_factor, float threshold,
+                                  int64_t* out_rowids, float* out_scores, uint32_t* out_counts, uint64_t* out_flags) {
+    YB_TRY
+    YB_ARG(p && out_counts, "null argument");
+    std::lock_guard<std::mutex> lk(p->mu);
+    yams_b200_corpus* c = p->corpus;
+    std::lock_guard<std::mutex> corpus_lock(c->mu);
+    YB_BIND(c);
+    zero_outputs(nq, out_counts, out_flags);
+    for (uint32_t& v : p->last_path) v = 0;
+    if (nq == 0 || k == 0 || p->n_idx == 0) return YAMS_OK;                           // :3873-3881
+    YB_ARG(queries && out_rowids && out_scores, "null argument");
+    YB_ARG(c->generation == p->corpus_generation, "the corpus changed after the PQ index was built: rebuild it (the reference marks the index dirty)");
+    for (uint32_t q0 = 0; q0 < nq; q0 += kPqMaxBatch) {
+        const uint32_t nb = std::min<uint32_t>(kPqMaxBatch, nq - q0);
+        yams_status_t rc = pq_search_batch(p, queries + (size_t)q0 * p->dim, nb, k, rerank_factor, threshold, out_rowids + (size_t)q0 * k,
+                                           out_scores + (size_t)q0 * k, out_counts + q0, out_flags ? out_flags + q0 : nullptr);
+        if (rc != YAMS_OK) return rc;
+    }
+    return YAMS_OK;
+    YB_CATCH
+}
 
 yams_status_t yams_b200_debug_pq_lut(yams_b200_pq* p, const float* queries, uint32_t nq, float* out_lut, uint32_t* out_valid) {
     YB_TRY
@@ -867,12 +865,8 @@ yams_status_t yams_b200_debug_pq_lut(yams_b200_pq* p, const float* queries, uint
     yams_status_t rc;
     const uint32_t m = p->m, kc = p->k, d = p->dim;
     if ((rc = p->q32.reserve((size_t)nq * d * 4)) != YAMS_OK) return rc;
-    if ((rc = p->lut.reserve((size_t)nq * m * kc * 4)) != YAMS_OK) return rc;
-    if ((rc = p->valid.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
     YB_CUDA(cudaMemcpyAsync(p->q32.p, queries, (size_t)nq * d * 4, cudaMemcpyHostToDevice, st));
-    YB_CUDA(cudaFuncSetAttribute(pq_lut_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(d * 4)));
-    pq_lut_kernel<<<nq, 256, d * 4, st>>>(p->q32.as<float>(), d, p->codebooks.as<float>(), m, kc, p->lut.as<float>(), p->valid.as<uint32_t>());
-    YB_CUDA(cudaGetLastError());
+    if ((rc = pq_build_luts(p, p->q32.as<float>(), nq, st)) != YAMS_OK) return rc;
     YB_CUDA(cudaMemcpyAsync(out_lut, p->lut.p, (size_t)nq * m * kc * 4, cudaMemcpyDeviceToHost, st));
     YB_CUDA(cudaMemcpyAsync(out_valid, p->valid.p, (size_t)nq * 4, cudaMemcpyDeviceToHost, st));
     YB_CUDA(cudaStreamSynchronize(st));
@@ -915,8 +909,7 @@ static yams_status_t pq_candidates_batch(yams_b200_pq* p, const float* queries, 
     cudaStream_t st = c->st;
     yams_status_t rc;
     const uint32_t m = p->m, kc = p->k, d = p->dim;
-    if (rerank_factor == 0) rerank_factor = 1;
-    const uint64_t want = std::max<uint64_t>(k, (uint64_t)k * rerank_factor);
+    const uint64_t want = pq_rerank_budget(k, rerank_factor);
     const uint64_t base = offs[0], total = offs[nq] - base;
     uint64_t maxlen = 0;
     for (uint32_t q = 0; q < nq; ++q) maxlen = std::max(maxlen, offs[q + 1] - offs[q]);
@@ -940,13 +933,9 @@ static yams_status_t pq_candidates_batch(yams_b200_pq* p, const float* queries, 
     if ((rc = p->mapped.reserve(std::max<uint64_t>(total, 1) * sizeof(Cand))) != YAMS_OK) return rc;
     if ((rc = p->cidx.reserve(std::max<uint64_t>(total, 1) * 4)) != YAMS_OK) return rc;
     if ((rc = p->bits.reserve((size_t)nq * bits_ld * 4 + 4)) != YAMS_OK) return rc;
-    if ((rc = p->lut.reserve((size_t)nq * m * kc * 4)) != YAMS_OK) return rc;
-    if ((rc = p->valid.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
     if ((rc = p->lists.reserve((size_t)nq * cap * sizeof(Cand))) != YAMS_OK) return rc;
     if ((rc = p->counts.reserve((size_t)nq * 4 + 16)) != YAMS_OK) return rc;
     if ((rc = p->sel.reserve((size_t)nq * K * sizeof(Cand) + (size_t)nq * 4)) != YAMS_OK) return rc;
-    if ((rc = p->exact.reserve((size_t)nq * K * sizeof(PqExact))) != YAMS_OK) return rc;
-    if ((rc = p->dout.reserve((size_t)nq * k * 12 + (size_t)nq * 12 + 64)) != YAMS_OK) return rc;
     unsigned char* din = p->cin.as<unsigned char>();
     const float* d_q = reinterpret_cast<const float*>(din + o_q);
     const int64_t* d_al = reinterpret_cast<const int64_t*>(din + o_al);
@@ -957,8 +946,7 @@ static yams_status_t pq_candidates_batch(yams_b200_pq* p, const float* queries, 
     YB_CUDA(cudaMemcpyAsync(din, in.h.data(), in.h.size(), cudaMemcpyHostToDevice, st));
     YB_CUDA(cudaMemsetAsync(p->bits.p, 0, (size_t)nq * bits_ld * 4 + 4, st));
     YB_CUDA(cudaMemsetAsync(d_counts, 0, (size_t)nq * 4, st));
-    YB_CUDA(cudaFuncSetAttribute(pq_lut_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(d * 4)));
-    pq_lut_kernel<<<nq, 256, d * 4, st>>>(d_q, d, p->codebooks.as<float>(), m, kc, p->lut.as<float>(), p->valid.as<uint32_t>());
+    if ((rc = pq_build_luts(p, d_q, nq, st)) != YAMS_OK) return rc;
     launch_map_rowids(d_al, total, c->rowids.as<int64_t>(), c->n, p->mapped.as<Cand>(), st);
     if (total) {
         const unsigned gx = (unsigned)std::min<uint64_t>((maxlen + 255) / 256, 256);
@@ -971,22 +959,8 @@ static yams_status_t pq_candidates_batch(yams_b200_pq* p, const float* queries, 
             p->codes.as<uint8_t>(), m, kc, p->lut.as<float>(), p->tie_rank.as<uint32_t>(), p->cidx.as<uint32_t>(), d_of, d_counts, per_cta,
             p->lists.as<Cand>(), cap);
     }
-    // from here on the chain of pq_search: selection, rank -> row, exact rerank, final order
     launch_topk_lists(p->lists.as<Cand>(), d_counts, cap, nq, K, d_sel, d_sel_n, st);
-    const uint32_t tot = nq * K;
-    pq_rank_to_row_kernel<<<(tot + 255) / 256, 256, 0, st>>>(d_sel, d_sel_n, K, nq, p->rank_to_idx.as<uint32_t>(), p->idx_rows.as<uint32_t>());
-    pq_rerank_kernel<<<(tot + 127) / 128, 128, 0, st>>>(c->rows.p, c->dtype, d, d_q, d_sel, d_sel_n, p->valid.as<uint32_t>(), K, nq, threshold,
-                                                        p->exact.as<PqExact>());
-    int64_t* d_or = p->dout.as<int64_t>();
-    uint64_t* d_ofl = reinterpret_cast<uint64_t*>(d_or + (size_t)nq * k);
-    float* d_os = reinterpret_cast<float*>(d_ofl + nq);
-    uint32_t* d_oc = reinterpret_cast<uint32_t*>(d_os + (size_t)nq * k);
-    launch_final_plain(p->exact.p, K, k, nq, c->rowids.as<int64_t>(), d_or, d_os, d_oc, d_ofl, st);
-    YB_CUDA(cudaGetLastError());
-    YB_CUDA(cudaMemcpyAsync(out_rowids, d_or, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, st));
-    YB_CUDA(cudaMemcpyAsync(out_scores, d_os, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, st));
-    YB_CUDA(cudaMemcpyAsync(out_counts, d_oc, (size_t)nq * 4, cudaMemcpyDeviceToHost, st));
-    if (out_flags) YB_CUDA(cudaMemcpyAsync(out_flags, d_ofl, (size_t)nq * 8, cudaMemcpyDeviceToHost, st));
+    if ((rc = pq_rerank_and_emit(p, d_q, d_sel, d_sel_n, K, nq, k, threshold, out_rowids, out_scores, out_counts, out_flags)) != YAMS_OK) return rc;
     std::vector<uint32_t> sel_n(check_after ? nq : 0);
     if (check_after) YB_CUDA(cudaMemcpyAsync(sel_n.data(), d_sel_n, (size_t)nq * 4, cudaMemcpyDeviceToHost, st));
     YB_CUDA(cudaStreamSynchronize(st));
@@ -1126,8 +1100,7 @@ yams_status_t yams_b200_pq_search_candidates(yams_b200_pq* p, const float* queri
     yams_b200_corpus* c = p->corpus;
     std::lock_guard<std::mutex> corpus_lock(c->mu);
     YB_BIND(c);
-    for (uint32_t q = 0; q < nq; ++q) out_counts[q] = 0;
-    if (out_flags) for (uint32_t q = 0; q < nq; ++q) out_flags[q] = 0;
+    zero_outputs(nq, out_counts, out_flags);
     if (nq == 0 || k == 0 || p->n_idx == 0) return YAMS_OK;
     YB_ARG(queries && out_rowids && out_scores && allowed_offsets, "null argument");
     for (uint32_t q = 0; q < nq; ++q) YB_ARG(allowed_offsets[q] <= allowed_offsets[q + 1], "allowed_offsets must be non-decreasing");
@@ -1156,7 +1129,7 @@ yams_status_t yams_b200_search_documents(yams_b200_corpus* c, yams_b200_pq* pq, 
     if (pq) pq_lock = std::unique_lock<std::mutex>(pq->mu);
     std::lock_guard<std::mutex> corpus_lock(c->mu);
     YB_BIND(c);
-    for (uint32_t q = 0; q < nq; ++q) out_counts[q] = 0;
+    zero_outputs(nq, out_counts, nullptr);
     if (nq == 0) return YAMS_OK;
     YB_ARG(queries && query_docs && out_docs && out_rowids && out_scores, "null argument");
     YB_ARG(c->metric == YAMS_B200_COSINE, "document search is defined for the cosine scan");
