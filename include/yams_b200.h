@@ -231,8 +231,11 @@ YAMS_B200_API yams_status_t yams_b200_manifest_build(void* self, const yams_chun
                                                      const uint8_t file_digest[32], uint64_t file_size,
                                                      yams_chunk_ref* out_refs, yams_manifest_summary* out);
 
-/* Per-stage device timings (ms) of the last chunk_and_hash* call on this thread's context:
- * [0] candidate scan, [1] cut selection, [2] sha256, [3] total device, [4] h2d (0 for _device) */
+/* Per-stage timings (ms) of the last chunk_and_hash* / chunk_boundaries call on this thread:
+ * device time of [0] candidate scan, [1] cut selection, [2] sha256, [3] the whole call;
+ * host wall-clock time of [4] the wait after the candidate scan, [5] the wait after the chunk-count scan,
+ * [6] descriptor-table growth, [7] cut processing as a whole.
+ * chunk_and_hash_batch sums [0..3] over its file groups and sets [4..7] to 0. */
 YAMS_B200_API yams_status_t yams_b200_ingest_last_timings(void* self, float out_ms[8]);
 
 typedef struct yams_content_ingest_v1 {

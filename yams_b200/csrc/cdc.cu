@@ -523,10 +523,9 @@ __global__ void __launch_bounds__(1024) cdc_compact_kernel(const uint64_t* __res
     }
 }
 
-yams_status_t launch_scan_single_pass(const ScanArgs& A, uint32_t ntiles, int sm_count, uint64_t* cand_tmp, uint32_t* slice_counts,
-                                      uint32_t slice_cap, uint32_t nslices, uint64_t* cand, uint64_t* scalars, cudaStream_t st,
-                                      int warps_per_cta) {
-    const int W = (warps_per_cta >= 1 && warps_per_cta <= WS_WARPS) ? warps_per_cta : WS_WARPS;
+yams_status_t launch_scan_single_pass(const ScanArgs& A, uint32_t ntiles, uint64_t* cand_tmp, uint32_t* slice_counts,
+                                      uint32_t slice_cap, uint32_t nslices, uint64_t* cand, uint64_t* scalars, cudaStream_t st) {
+    const int W = WS_WARPS;
     SinglePassArgs S{};
     S.A = A;
     S.ntiles = ntiles;
@@ -554,7 +553,6 @@ yams_status_t launch_scan_single_pass(const ScanArgs& A, uint32_t ntiles, int sm
 #undef YB_LAUNCH_SCAN
     cdc_compact_kernel<<<1, 1024, (size_t)(nslices + 1) * 8, st>>>(cand_tmp, slice_counts, nslices, slice_cap, cand, scalars);
     YB_CUDA(cudaGetLastError());
-    (void)sm_count;
     return YAMS_OK;
 }
 

@@ -64,15 +64,13 @@ constexpr uint32_t kTileBytes = kScanThreads * 16 * kScanIters;   // 16 KiB
 // single-pass candidate scan (cdc.cu); SC_TILE must divide the tile grid used by the two-pass kernels
 constexpr uint32_t kSinglePassTile = 4096;
 constexpr uint32_t kSinglePassWarpsPerCta = 16;
-yams_status_t launch_scan_single_pass(const ScanArgs& A, uint32_t ntiles, int sm_count, uint64_t* cand_tmp, uint32_t* slice_counts,
-                                      uint32_t slice_cap, uint32_t nslices, uint64_t* cand, uint64_t* scalars, cudaStream_t st,
-                                      int warps_per_cta = 0);
+yams_status_t launch_scan_single_pass(const ScanArgs& A, uint32_t ntiles, uint64_t* cand_tmp, uint32_t* slice_counts,
+                                      uint32_t slice_cap, uint32_t nslices, uint64_t* cand, uint64_t* scalars, cudaStream_t st);
 
 yams_status_t resolve_params(const yams_cdc_config* cfg, CdcParams* P, uint64_t table[256]);
 yams_status_t launch_sha256_chunks(const uint8_t* d_data, uint64_t base_pos, yams_chunk_desc* d_descs,
                                    uint32_t first, uint32_t n, unsigned int* d_counter, int sm_count,
-                                   cudaStream_t st, uint32_t* d_order_ws = nullptr, uint64_t total_bytes = 0,
-                                   int variant_per_sm = 0, int grid_per_sm = 0);
+                                   cudaStream_t st, uint32_t* d_order_ws, uint64_t total_bytes);
 // workspace of the longest-first order: 64 counters + one index per chunk
 inline size_t sha256_order_ws_bytes(uint64_t n) { return (size_t)(n + 64) * sizeof(uint32_t); }
 yams_status_t launch_dedup_stats(const yams_chunk_desc* d_descs, uint32_t n, uint32_t* d_table, uint64_t slots,

@@ -10,6 +10,7 @@
 
 #include <algorithm>
 #include <chrono>
+#include <memory>
 #include <mutex>
 #include <thread>
 #include <new>
@@ -34,10 +35,13 @@ static inline double now_ms() {
 }
 constexpr uint64_t kFeedSlice = 256ull << 20;      // host feeds are staged 256 MiB at a time
 
-// All device-side working state of one chunking stream.
-struct CdcStream {
+// All device-side resources of one ingest stream: the chunking and hashing workspace, the two staging buffers of the host
+// path and the pinned images of the upload path.  They are pooled: `yams add` calls chunk_and_hash once per file, and
+// cudaMalloc / cudaFree of the workspace would otherwise dominate small inputs.
+struct IngestRes {
     DeviceCtx* dev = nullptr;
-    cudaStream_t st = nullptr;
+    cudaStream_t st = nullptr;       // kernels
+    cudaStream_t copy_st = nullptr;  // H2D copies of the streaming session
     CdcParams P{};
     bool no_candidates = false;  // lo >= force: no candidate can ever cut
     bool two_pass_only = false;  // YAMS_B200_TWO_PASS=1: skip the single-pass scan (diagnostics)
@@ -45,10 +49,16 @@ struct CdcStream {
     DevBuf table, tile_counts, tile_offsets, cand, cand_tmp, next, forced, exit_, entry, onchain, emit_counts,
         emit_offsets, scan_scratch, descs, scalars, sha_order;
     DevBuf npos, nref, roots, fileinfo, first;   // chunk_and_hash_batch: merged node table, file layout, per-file chunk ranges
+    DevBuf stage[2];             // device copies of host input
     HostBuf h_scalars;           // pinned: [0] ncand/ntotal, [1] new chunk start
+    HostBuf pin[2];              // pinned images of two device-buffer slices (staged_upload)
     uint64_t ndescs = 0;         // chunks accumulated in `descs`
     uint64_t chunk_start = 0;    // stream position where the open chunk starts
-    cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
+    cudaEvent_t ev[4] = {};      // stage marks of one process(), one batch group or one session hash
+    cudaEvent_t call[3] = {};    // whole-call marks: start, chunking done, hashing done
+    cudaEvent_t copied[2] = {};  // session: H2D copy into stage[b] finished
+    cudaEvent_t freed[2] = {};   // session: stage[b] no longer read
+    cudaEvent_t pin_done[2] = {};  // H2D copy out of pin[b] finished
     float ms_scan = 0, ms_select = 0;
     double host_sync1 = 0, host_sync2 = 0, host_alloc = 0, host_total = 0;  // wall-clock ms (diagnostics)
 
@@ -58,7 +68,10 @@ struct CdcStream {
         yams_status_t rc = ensure_device(&dev);
         if (rc != YAMS_OK) return rc;
         YB_CUDA(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-        for (auto& e : ev) YB_CUDA(cudaEventCreate(&e));
+        YB_CUDA(cudaStreamCreateWithFlags(&copy_st, cudaStreamNonBlocking));
+        for (cudaEvent_t* e : {&ev[0], &ev[1], &ev[2], &ev[3], &call[0], &call[1], &call[2]}) YB_CUDA(cudaEventCreate(e));
+        for (cudaEvent_t* e : {&copied[0], &copied[1], &freed[0], &freed[1], &pin_done[0], &pin_done[1]})
+            YB_CUDA(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
         if ((rc = table.reserve(256 * 8)) != YAMS_OK) return rc;
         if ((rc = scalars.reserve(64)) != YAMS_OK) return rc;
         if ((rc = h_scalars.reserve(64 + 256 * 8)) != YAMS_OK) return rc;
@@ -67,11 +80,9 @@ struct CdcStream {
     }
     // (re)configure for a new stream: parameters, table, counters. Buffers are kept.
     yams_status_t init(const yams_cdc_config* cfg) {
-        yams_status_t rc = create();
-        if (rc != YAMS_OK) return rc;
         uint64_t* tbl = h_scalars.as<uint64_t>() + 8;   // pinned staging for the table
         YB_CUDA(cudaStreamSynchronize(st));
-        rc = resolve_params(cfg, &P, tbl);
+        yams_status_t rc = resolve_params(cfg, &P, tbl);
         if (rc != YAMS_OK) return rc;
         no_candidates = P.lo >= P.force;
         two_pass_only = getenv("YAMS_B200_TWO_PASS") != nullptr;
@@ -84,15 +95,26 @@ struct CdcStream {
         return YAMS_OK;
     }
     void destroy() {
+        if (st) cudaStreamSynchronize(st);
+        if (copy_st) cudaStreamSynchronize(copy_st);
         for (DevBuf* b : {&table, &tile_counts, &tile_offsets, &cand, &cand_tmp, &next, &forced, &exit_, &entry, &onchain,
-                          &emit_counts, &emit_offsets, &scan_scratch, &descs, &scalars, &sha_order, &npos, &nref, &roots, &fileinfo, &first})
+                          &emit_counts, &emit_offsets, &scan_scratch, &descs, &scalars, &sha_order, &npos, &nref, &roots, &fileinfo,
+                          &first, &stage[0], &stage[1]})
             b->release();
-        h_scalars.release();
-        for (auto& e : ev)
+        for (HostBuf* b : {&h_scalars, &pin[0], &pin[1]}) b->release();
+        for (cudaEvent_t e : {ev[0], ev[1], ev[2], ev[3], call[0], call[1], call[2], copied[0], copied[1], freed[0], freed[1],
+                              pin_done[0], pin_done[1]})
             if (e) cudaEventDestroy(e);
-        if (st) cudaStreamDestroy(st);
-        st = nullptr;
-        created = false;
+        for (cudaStream_t s : {st, copy_st})
+            if (s) cudaStreamDestroy(s);
+    }
+
+    // Waits for the kernel stream; the host time spent waiting is added to *acc.
+    yams_status_t wait(double* acc) {
+        const double t0 = now_ms();
+        YB_CUDA(cudaStreamSynchronize(st));
+        *acc += now_ms() - t0;
+        return YAMS_OK;
     }
 
     // Candidate scan of stream positions [scan_lo, scan_hi): the ascending candidate positions land in `cand`,
@@ -127,11 +149,11 @@ struct CdcStream {
                 if ((rc = cand_tmp.reserve(total_cap * 8)) != YAMS_OK) return rc;
                 if ((rc = cand.reserve(total_cap * 8)) != YAMS_OK) return rc;
                 if ((rc = tile_counts.reserve((size_t)std::max<uint32_t>(ntiles, nslices) * 4)) != YAMS_OK) return rc;
-                if ((rc = launch_scan_single_pass(A, ntiles4, dev->sm_count, cand_tmp.as<uint64_t>(), tile_counts.as<uint32_t>(),
-                                                  slice_cap, nslices, cand.as<uint64_t>(), d_sc, st)) != YAMS_OK)
+                if ((rc = launch_scan_single_pass(A, ntiles4, cand_tmp.as<uint64_t>(), tile_counts.as<uint32_t>(), slice_cap,
+                                                  nslices, cand.as<uint64_t>(), d_sc, st)) != YAMS_OK)
                     return rc;
                 YB_CUDA(cudaMemcpyAsync((void*)h_sc, d_sc, 24, cudaMemcpyDeviceToHost, st));
-                { const double t0 = now_ms(); YB_CUDA(cudaStreamSynchronize(st)); host_sync1 += now_ms() - t0; }
+                if ((rc = wait(&host_sync1)) != YAMS_OK) return rc;
                 if (h_sc[2] != 0) {
                     need_two_pass = true;   // dense candidates: exact two-pass kernels take over
                     ++two_pass_fallbacks;
@@ -149,7 +171,7 @@ struct CdcStream {
                                              d_sc + 0, scan_scratch, st)) != YAMS_OK)
                     return rc;
                 YB_CUDA(cudaMemcpyAsync((void*)h_sc, d_sc, 8, cudaMemcpyDeviceToHost, st));
-                { const double t0 = now_ms(); YB_CUDA(cudaStreamSynchronize(st)); host_sync1 += now_ms() - t0; }
+                if ((rc = wait(&host_sync1)) != YAMS_OK) return rc;
                 uint64_t nc = h_sc[0];
                 YB_ARG(nc < 0xFFFFFFF0ull, "too many boundary candidates in one segment");
                 ncand = (uint32_t)nc;
@@ -161,6 +183,41 @@ struct CdcStream {
             }
         }
         *ncand_out = ncand;
+        return YAMS_OK;
+    }
+
+    // ---- cut selection over a node table: the stream's root and candidates, or a batch group's merged roots and candidates ----
+    // The caller fills next[] / forced[] before mark_chain and emit_counts[] between mark_chain and count_offsets.
+    yams_status_t reserve_nodes(uint32_t nnodes) {
+        const uint32_t nblocks = (nnodes + kNodeBlock - 1) / kNodeBlock;
+        yams_status_t rc;
+        for (DevBuf* b : {&next, &forced, &exit_})
+            if ((rc = b->reserve((size_t)nnodes * 4)) != YAMS_OK) return rc;
+        if ((rc = entry.reserve((size_t)nblocks * 4)) != YAMS_OK) return rc;
+        if ((rc = onchain.reserve((size_t)nnodes)) != YAMS_OK) return rc;
+        for (DevBuf* b : {&emit_counts, &emit_offsets})
+            if ((rc = b->reserve((size_t)nnodes * 4)) != YAMS_OK) return rc;
+        if (!cand.p && (rc = cand.reserve(8)) != YAMS_OK) return rc;
+        return YAMS_OK;
+    }
+    // onchain[i] = 1 for the nodes on the chain of cuts that starts at node 0; every byte of onchain[0, nnodes) is written
+    yams_status_t mark_chain(uint32_t nnodes) {
+        const uint32_t nblocks = (nnodes + kNodeBlock - 1) / kNodeBlock;
+        cdc_exit_kernel<<<nblocks, 32, 0, st>>>(next.as<uint32_t>(), nnodes, exit_.as<uint32_t>());
+        YB_CUDA(cudaMemsetAsync(entry.p, 0xFF, (size_t)nblocks * 4, st));
+        cdc_walk_kernel<<<1, 32, 0, st>>>(exit_.as<uint32_t>(), nnodes, entry.as<uint32_t>());
+        cdc_mark_kernel<<<nblocks, 32, 0, st>>>(next.as<uint32_t>(), nnodes, entry.as<uint32_t>(), onchain.as<uint8_t>());
+        return YAMS_OK;
+    }
+    // emit_offsets = exclusive scan of emit_counts; *total (their sum) is read back to the host
+    yams_status_t count_offsets(uint32_t nnodes, uint64_t* total) {
+        uint64_t* d_sc = scalars.as<uint64_t>();
+        yams_status_t rc = exclusive_scan_u32(emit_counts.as<uint32_t>(), emit_offsets.as<uint32_t>(), nnodes, d_sc + 0,
+                                              scan_scratch, st);
+        if (rc != YAMS_OK) return rc;
+        YB_CUDA(cudaMemcpyAsync(h_scalars.p, d_sc, 8, cudaMemcpyDeviceToHost, st));
+        if ((rc = wait(&host_sync2)) != YAMS_OK) return rc;
+        *total = h_scalars.as<volatile uint64_t>()[0];
         return YAMS_OK;
     }
 
@@ -177,33 +234,16 @@ struct CdcStream {
         YB_CUDA(cudaEventRecord(ev[0], st));
         if ((rc = scan(data, base_pos, lowest, scan_lo, scan_hi, &ncand)) != YAMS_OK) return rc;
         YB_CUDA(cudaEventRecord(ev[1], st));
-        // ---- selection ------------------------------------------------------------------------
-        uint32_t nnodes = ncand + 1;
-        uint32_t nblocks = (nnodes + kNodeBlock - 1) / kNodeBlock;
-        if ((rc = next.reserve((size_t)nnodes * 4)) != YAMS_OK) return rc;
-        if ((rc = forced.reserve((size_t)nnodes * 4)) != YAMS_OK) return rc;
-        if ((rc = exit_.reserve((size_t)nnodes * 4)) != YAMS_OK) return rc;
-        if ((rc = entry.reserve((size_t)nblocks * 4)) != YAMS_OK) return rc;
-        if ((rc = onchain.reserve((size_t)nnodes)) != YAMS_OK) return rc;
-        if ((rc = emit_counts.reserve((size_t)nnodes * 4)) != YAMS_OK) return rc;
-        if ((rc = emit_offsets.reserve((size_t)nnodes * 4)) != YAMS_OK) return rc;
-        if (!cand.p && (rc = cand.reserve(8)) != YAMS_OK) return rc;
+        const uint32_t nnodes = ncand + 1;
+        if ((rc = reserve_nodes(nnodes)) != YAMS_OK) return rc;
         SelectArgs S{cand.as<uint64_t>(), ncand, chunk_start, scan_hi, final ? 1 : 0, P};
-        uint32_t tgrid = (nnodes + 255) / 256;
+        const uint32_t tgrid = (nnodes + 255) / 256;
         cdc_next_kernel<<<tgrid, 256, 0, st>>>(S, next.as<uint32_t>(), forced.as<uint32_t>());
-        cdc_exit_kernel<<<nblocks, 32, 0, st>>>(next.as<uint32_t>(), nnodes, exit_.as<uint32_t>());
-        YB_CUDA(cudaMemsetAsync(entry.p, 0xFF, (size_t)nblocks * 4, st));
-        cdc_walk_kernel<<<1, 32, 0, st>>>(exit_.as<uint32_t>(), nnodes, entry.as<uint32_t>());
-        cdc_mark_kernel<<<nblocks, 32, 0, st>>>(next.as<uint32_t>(), nnodes, entry.as<uint32_t>(),
-                                                onchain.as<uint8_t>());
+        if ((rc = mark_chain(nnodes)) != YAMS_OK) return rc;
         cdc_emit_count_kernel<<<tgrid, 256, 0, st>>>(S, next.as<uint32_t>(), forced.as<uint32_t>(),
                                                      onchain.as<uint8_t>(), emit_counts.as<uint32_t>());
-        if ((rc = exclusive_scan_u32(emit_counts.as<uint32_t>(), emit_offsets.as<uint32_t>(), nnodes, d_sc + 0,
-                                     scan_scratch, st)) != YAMS_OK)
-            return rc;
-        YB_CUDA(cudaMemcpyAsync((void*)h_sc, d_sc, 8, cudaMemcpyDeviceToHost, st));
-        { const double t0 = now_ms(); YB_CUDA(cudaStreamSynchronize(st)); host_sync2 += now_ms() - t0; }
-        uint64_t nnew = h_sc[0];
+        uint64_t nnew = 0;
+        if ((rc = count_offsets(nnodes, &nnew)) != YAMS_OK) return rc;
         { const double t0 = now_ms();
           if ((rc = descs.reserve((size_t)(ndescs + nnew + 1) * sizeof(yams_chunk_desc), true, st)) != YAMS_OK)
             return rc;
@@ -225,54 +265,52 @@ struct CdcStream {
         host_total += now_ms() - t_begin;
         return YAMS_OK;
     }
+
+    // SHA-256 of descs[first, first + n) over `data` (data[0] is stream position base_pos); total_bytes / n is the mean
+    // chunk size the longest-first order buckets by.
+    yams_status_t hash(const uint8_t* data, uint64_t base_pos, uint64_t first, uint64_t n, uint64_t total_bytes) {
+        if (n == 0) return YAMS_OK;
+        if (n >= 0xFFFFFFFFull) {
+            set_last_error("too many chunks");
+            return YAMS_ERR_INVALID_ARG;
+        }
+        yams_status_t rc = sha_order.reserve(sha256_order_ws_bytes(n));
+        if (rc != YAMS_OK) return rc;
+        return launch_sha256_chunks(data, base_pos, descs.as<yams_chunk_desc>(), (uint32_t)first, (uint32_t)n,
+                                    reinterpret_cast<unsigned int*>(scalars.as<uint64_t>() + 4), dev->sm_count, st,
+                                    sha_order.as<uint32_t>(), total_bytes);
+    }
+    // Digests of the host table h (offset / size into d_data) into digests[32 * i], through descs.
+    yams_status_t hash_table(const uint8_t* d_data, std::vector<yams_chunk_desc>& h, uint64_t total_bytes, uint8_t* digests) {
+        const size_t n = h.size();
+        yams_status_t rc = descs.reserve(n * sizeof(yams_chunk_desc));
+        if (rc != YAMS_OK) return rc;
+        YB_CUDA(cudaMemcpyAsync(descs.p, h.data(), n * sizeof(yams_chunk_desc), cudaMemcpyHostToDevice, st));
+        if ((rc = hash(d_data, 0, 0, n, total_bytes)) != YAMS_OK) return rc;
+        YB_CUDA(cudaMemcpyAsync(h.data(), descs.p, n * sizeof(yams_chunk_desc), cudaMemcpyDeviceToHost, st));
+        YB_CUDA(cudaStreamSynchronize(st));
+        for (size_t i = 0; i < n; ++i) memcpy(digests + 32 * i, h[i].digest, 32);
+        return YAMS_OK;
+    }
+
+    // size the descriptor table of a len-byte stream once: every chunk but the last is at least max(min_chunk,1) bytes long
+    yams_status_t presize_descs(uint64_t len) {
+        const uint64_t per = std::max<uint64_t>(P.lo + 1, 4096);
+        return descs.reserve((size_t)(len / per + 16) * sizeof(yams_chunk_desc));
+    }
 };
 
 static thread_local float g_last_ms[8] = {0};
 
-// Device-side resources of one ingest stream (kernel workspace + the two staging buffers of the host
-// path). They are pooled: `yams add` calls chunk_and_hash once per file, and cudaMalloc / cudaFree of the
-// workspace would otherwise dominate small inputs.
-struct IngestRes {
-    CdcStream cs;
-    cudaStream_t copy_st = nullptr;
-    DevBuf stage[2];
-    cudaEvent_t copied[2] = {nullptr, nullptr};
-    cudaEvent_t freed[2] = {nullptr, nullptr};
-    cudaEvent_t t0 = nullptr, t1 = nullptr, e0 = nullptr, e1 = nullptr, e2 = nullptr;
-    HostBuf pin[2];                                   // batch path: pinned images of two device-buffer slices
-    cudaEvent_t pin_done[2] = {nullptr, nullptr};     // H2D copy out of pin[b] finished
-    bool created = false;
-    yams_status_t create() {
-        if (created) return YAMS_OK;
-        yams_status_t rc = cs.create();
-        if (rc != YAMS_OK) return rc;
-        YB_CUDA(cudaStreamCreateWithFlags(&copy_st, cudaStreamNonBlocking));
-        for (int b = 0; b < 2; ++b) {
-            YB_CUDA(cudaEventCreateWithFlags(&copied[b], cudaEventDisableTiming));
-            YB_CUDA(cudaEventCreateWithFlags(&freed[b], cudaEventDisableTiming));
-        }
-        for (cudaEvent_t* e : {&t0, &t1, &e0, &e1, &e2}) YB_CUDA(cudaEventCreate(e));
-        for (int b = 0; b < 2; ++b) YB_CUDA(cudaEventCreateWithFlags(&pin_done[b], cudaEventDisableTiming));
-        created = true;
-        return YAMS_OK;
-    }
-    void destroy() {
-        if (cs.st) cudaStreamSynchronize(cs.st);
-        if (copy_st) cudaStreamSynchronize(copy_st);
-        for (int b = 0; b < 2; ++b) {
-            stage[b].release();
-            if (copied[b]) cudaEventDestroy(copied[b]);
-            if (freed[b]) cudaEventDestroy(freed[b]);
-        }
-        for (cudaEvent_t e : {t0, t1, e0, e1, e2, pin_done[0], pin_done[1]})
-            if (e) cudaEventDestroy(e);
-        pin[0].release();
-        pin[1].release();
-        if (copy_st) cudaStreamDestroy(copy_st);
-        cs.destroy();
-        created = false;
-    }
-};
+// The one writer of the ingest_last_timings slots: [0..3] device ms of the candidate scan, the cut selection, SHA-256 and
+// the whole call; [4..7] the host ms that r spent in its two waits, in descriptor-table growth and in process() (0 without r).
+static void report_timings(const float (&dev_ms)[4], const IngestRes* r) {
+    for (int i = 0; i < 4; ++i) g_last_ms[i] = dev_ms[i];
+    g_last_ms[4] = r ? (float)r->host_sync1 : 0.f;
+    g_last_ms[5] = r ? (float)r->host_sync2 : 0.f;
+    g_last_ms[6] = r ? (float)r->host_alloc : 0.f;
+    g_last_ms[7] = r ? (float)r->host_total : 0.f;
+}
 
 static std::mutex g_pool_mu;
 static std::vector<IngestRes*> g_pool;
@@ -283,6 +321,7 @@ static size_t pool_max() {
     return v;
 }
 
+// cfg == nullptr: the caller only hashes, so no chunking parameters are loaded
 static yams_status_t acquire_res(const yams_cdc_config* cfg, IngestRes** out) {
     IngestRes* r = nullptr;
     {
@@ -301,7 +340,7 @@ static yams_status_t acquire_res(const yams_cdc_config* cfg, IngestRes** out) {
     if (!r) r = new (std::nothrow) IngestRes();
     if (!r) return YAMS_ERR_INTERNAL;
     yams_status_t rc = r->create();
-    if (rc == YAMS_OK) rc = r->cs.init(cfg);
+    if (rc == YAMS_OK) rc = cfg ? r->init(cfg) : YAMS_OK;
     if (rc != YAMS_OK) {
         r->destroy();
         delete r;
@@ -313,11 +352,11 @@ static yams_status_t acquire_res(const yams_cdc_config* cfg, IngestRes** out) {
 
 static void release_res(IngestRes* r) {
     if (!r) return;
-    if (r->cs.st) cudaStreamSynchronize(r->cs.st);
+    if (r->st) cudaStreamSynchronize(r->st);
     if (r->copy_st) cudaStreamSynchronize(r->copy_st);
     // drop very large buffers instead of parking them in the pool
     const size_t kKeep = 1ull << 30;
-    for (DevBuf* b : {&r->stage[0], &r->stage[1], &r->cs.descs, &r->cs.cand, &r->cs.cand_tmp})
+    for (DevBuf* b : {&r->stage[0], &r->stage[1], &r->descs, &r->cand, &r->cand_tmp})
         if (b->cap > kKeep) b->release();
     {
         std::lock_guard<std::mutex> lk(g_pool_mu);
@@ -330,7 +369,17 @@ static void release_res(IngestRes* r) {
     delete r;
 }
 
-static yams_status_t copy_out(CdcStream& cs, uint64_t first, uint64_t n, yams_chunk_desc** out, size_t* out_n) {
+// A pooled workspace held for the lifetime of the lease; rc says whether one could be had (r is null otherwise).
+struct IngestLease {
+    IngestRes* r = nullptr;
+    yams_status_t rc;
+    explicit IngestLease(const yams_cdc_config* cfg) : rc(acquire_res(cfg, &r)) {}
+    ~IngestLease() { release_res(r); }
+    IngestLease(const IngestLease&) = delete;
+    IngestLease& operator=(const IngestLease&) = delete;
+};
+
+static yams_status_t copy_out(IngestRes& r, uint64_t first, uint64_t n, yams_chunk_desc** out, size_t* out_n) {
     *out = nullptr;
     *out_n = 0;
     if (n == 0) return YAMS_OK;
@@ -339,9 +388,9 @@ static yams_status_t copy_out(CdcStream& cs, uint64_t first, uint64_t n, yams_ch
         set_last_error("out of host memory for %llu chunk descriptors", (unsigned long long)n);
         return YAMS_ERR_INTERNAL;
     }
-    cudaError_t e = cudaMemcpyAsync(h, cs.descs.as<yams_chunk_desc>() + first, (size_t)n * sizeof(yams_chunk_desc),
-                                    cudaMemcpyDeviceToHost, cs.st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(cs.st);
+    cudaError_t e = cudaMemcpyAsync(h, r.descs.as<yams_chunk_desc>() + first, (size_t)n * sizeof(yams_chunk_desc),
+                                    cudaMemcpyDeviceToHost, r.st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(r.st);
     if (e != cudaSuccess) {
         free(h);
         set_last_error("D2H of chunk descriptors failed: %s", cudaGetErrorString(e));
@@ -353,53 +402,60 @@ static yams_status_t copy_out(CdcStream& cs, uint64_t first, uint64_t n, yams_ch
 }
 
 // One-shot over device-resident data.
-static yams_status_t run_device(const uint8_t* d_data, size_t len, const yams_cdc_config* cfg, bool hash,
-                                yams_chunk_desc** out, size_t* out_n) {
-    IngestRes* r = nullptr;
-    yams_status_t rc = acquire_res(cfg, &r);
+static yams_status_t run_device(const uint8_t* d_data, size_t len, const yams_cdc_config* cfg, yams_chunk_desc** out,
+                                size_t* out_n) {
+    IngestLease ws(cfg);
+    if (ws.rc != YAMS_OK) return ws.rc;
+    IngestRes& r = *ws.r;
+    yams_status_t rc = r.presize_descs(len);
     if (rc != YAMS_OK) return rc;
-    CdcStream& cs = r->cs;
-    // size the descriptor table once: every chunk but the last is at least max(min_chunk,1) bytes long
-    {
-        uint64_t per = std::max<uint64_t>(cs.P.lo + 1, 4096);
-        rc = cs.descs.reserve((size_t)(len / per + 16) * sizeof(yams_chunk_desc));
-    }
-    cudaEventRecord(r->e0, cs.st);
+    YB_CUDA(cudaEventRecord(r.call[0], r.st));
     const uint64_t seg = segment_bytes();
-    for (uint64_t lo = 0; lo < len && rc == YAMS_OK; lo += seg) {
+    for (uint64_t lo = 0; lo < len; lo += seg) {
         uint64_t hi = std::min<uint64_t>(len, lo + seg);
-        rc = cs.process(d_data, 0, 0, lo, hi, hi == len);
+        if ((rc = r.process(d_data, 0, 0, lo, hi, hi == len)) != YAMS_OK) return rc;
     }
-    cudaEventRecord(r->e1, cs.st);
-    if (rc == YAMS_OK && hash && cs.ndescs) {
-        if (cs.ndescs >= 0xFFFFFFFFull) {
-            set_last_error("too many chunks");
-            rc = YAMS_ERR_INVALID_ARG;
-        } else {
-            rc = cs.sha_order.reserve(sha256_order_ws_bytes(cs.ndescs));
-            if (rc == YAMS_OK)
-                rc = launch_sha256_chunks(d_data, 0, cs.descs.as<yams_chunk_desc>(), 0, (uint32_t)cs.ndescs,
-                                          reinterpret_cast<unsigned int*>(cs.scalars.as<uint64_t>() + 4), cs.dev->sm_count, cs.st,
-                                          cs.sha_order.as<uint32_t>(), len);
-        }
-    }
-    cudaEventRecord(r->e2, cs.st);
-    if (rc == YAMS_OK) rc = copy_out(cs, 0, cs.ndescs, out, out_n);
-    if (rc == YAMS_OK) {
-        float t_sha = 0, t_all = 0;
-        cudaEventElapsedTime(&t_sha, r->e1, r->e2);
-        cudaEventElapsedTime(&t_all, r->e0, r->e2);
-        g_last_ms[0] = cs.ms_scan; g_last_ms[1] = cs.ms_select; g_last_ms[2] = t_sha; g_last_ms[3] = t_all;
-        g_last_ms[4] = (float)cs.host_sync1; g_last_ms[5] = (float)cs.host_sync2; g_last_ms[6] = (float)cs.host_alloc;
-        g_last_ms[7] = (float)cs.host_total;
-    }
-    release_res(r);
-    return rc;
+    YB_CUDA(cudaEventRecord(r.call[1], r.st));
+    if ((rc = r.hash(d_data, 0, 0, r.ndescs, len)) != YAMS_OK) return rc;
+    YB_CUDA(cudaEventRecord(r.call[2], r.st));
+    if ((rc = copy_out(r, 0, r.ndescs, out, out_n)) != YAMS_OK) return rc;
+    float t_sha = 0, t_all = 0;
+    cudaEventElapsedTime(&t_sha, r.call[1], r.call[2]);
+    cudaEventElapsedTime(&t_all, r.call[0], r.call[2]);
+    report_timings({r.ms_scan, r.ms_select, t_sha, t_all}, &r);
+    return YAMS_OK;
 }
 
-// Upload from ordinary (pageable) host memory.  A plain cudaMemcpy moves pageable memory at ~10 GB/s through the
-// driver's single staging thread; here host threads assemble each slice of the destination in one of two pinned buffers
-// (fill(dst, lo, hi) writes the image of destination bytes [lo, hi)) while the previous slice is on the wire.
+// One piece of a packed layout: `len` bytes from host memory `src` at layout position `pos`.
+struct LayoutPiece {
+    uint64_t pos, len;
+    const uint8_t* src;
+};
+// Writes the image of layout positions [lo, hi) to dst: the bytes of the pieces (ascending, disjoint), zeros elsewhere.
+static void layout_image(const std::vector<LayoutPiece>& pieces, uint8_t* dst, uint64_t lo, uint64_t hi) {
+    // first piece that ends beyond lo
+    size_t j = std::partition_point(pieces.begin(), pieces.end(), [lo](const LayoutPiece& x) { return x.pos + x.len <= lo; }) -
+               pieces.begin();
+    uint64_t p = lo;
+    for (; j < pieces.size() && p < hi; ++j) {
+        const LayoutPiece& x = pieces[j];
+        if (x.pos > p) {   // gap before the piece
+            const uint64_t e = std::min<uint64_t>(hi, x.pos);
+            memset(dst + (p - lo), 0, (size_t)(e - p));
+            p = e;
+        }
+        const uint64_t e = std::min<uint64_t>(hi, x.pos + x.len);
+        if (e > p) {
+            memcpy(dst + (p - lo), x.src + (p - x.pos), (size_t)(e - p));
+            p = e;
+        }
+    }
+    if (p < hi) memset(dst + (p - lo), 0, (size_t)(hi - p));
+}
+
+// Upload of a packed layout (layout_image) whose pieces sit in ordinary (pageable) host memory.  A plain cudaMemcpy moves
+// pageable memory at ~10 GB/s through the driver's single staging thread; here host threads assemble each slice of the
+// destination in one of two pinned buffers while the previous slice is on the wire.
 static uint64_t stage_slice_bytes() {
     static const uint64_t v = [] { const char* e = getenv("YAMS_B200_STAGE_MIB"); long x = e ? atol(e) : 64; return (uint64_t)(x < 1 ? 1 : x) << 20; }();
     return v;
@@ -412,32 +468,32 @@ static unsigned stage_threads() {
     }();
     return v;
 }
-template <typename Fill>
-static yams_status_t staged_upload(IngestRes* r, uint8_t* d_dst, uint64_t total, const Fill& fill, cudaStream_t st) {
+static yams_status_t staged_upload(IngestRes& r, uint8_t* d_dst, uint64_t total, const std::vector<LayoutPiece>& pieces,
+                                   cudaStream_t st) {
     if (total == 0) return YAMS_OK;
     yams_status_t rc;
     const uint64_t S = std::min<uint64_t>(stage_slice_bytes(), (total + 255) & ~255ull);
     for (int b = 0; b < 2; ++b)
-        if ((rc = r->pin[b].reserve((size_t)S)) != YAMS_OK) return rc;
+        if ((rc = r.pin[b].reserve((size_t)S)) != YAMS_OK) return rc;
     const unsigned T = total < (4u << 20) ? 1u : stage_threads();
     int b = 0;
     for (uint64_t lo = 0; lo < total; lo += S, b ^= 1) {
         const uint64_t hi = std::min<uint64_t>(total, lo + S);
-        YB_CUDA(cudaEventSynchronize(r->pin_done[b]));   // the copy that last used this pinned buffer has finished
-        uint8_t* img = r->pin[b].as<uint8_t>();
+        YB_CUDA(cudaEventSynchronize(r.pin_done[b]));   // the copy that last used this pinned buffer has finished
+        uint8_t* img = r.pin[b].as<uint8_t>();
         if (T == 1) {
-            fill(img, lo, hi);
+            layout_image(pieces, img, lo, hi);
         } else {
             std::vector<std::thread> th;
             const uint64_t part = (((hi - lo) + T - 1) / T + 4095) & ~4095ull;
             for (unsigned t = 0; t < T; ++t) {
                 uint64_t a = lo + (uint64_t)t * part, e = std::min<uint64_t>(hi, a + part);
-                if (a < e) th.emplace_back([&fill, img, lo, a, e] { fill(img + (a - lo), a, e); });
+                if (a < e) th.emplace_back([&pieces, img, lo, a, e] { layout_image(pieces, img + (a - lo), a, e); });
             }
             for (auto& x : th) x.join();
         }
         YB_CUDA(cudaMemcpyAsync(d_dst + lo, img, (size_t)(hi - lo), cudaMemcpyHostToDevice, st));
-        YB_CUDA(cudaEventRecord(r->pin_done[b], st));
+        YB_CUDA(cudaEventRecord(r.pin_done[b], st));
     }
     return YAMS_OK;
 }
@@ -452,8 +508,8 @@ static bool is_pageable(const void* p) {
 
 // ---- many files per call ----------------------------------------------------------------------------------------
 // One group = consecutive files whose padded total fits the staging budget.  Layout: every file starts at a
-// 256-byte-aligned buffer position preceded by >= 64 zero bytes (the whole buffer is zeroed first), so ONE candidate
-// scan, ONE selection pass and ONE SHA-256 launch serve every file of the group.
+// 256-byte-aligned buffer position preceded by >= 64 zero bytes, so ONE candidate scan, ONE selection pass and ONE
+// SHA-256 launch serve every file of the group.
 constexpr uint64_t kBatchGap = 64;
 static uint64_t batch_group_bytes() {
     static const uint64_t v = [] { const char* e = getenv("YAMS_B200_BATCH_MIB"); long x = e ? atol(e) : 1024; return (uint64_t)(x < 1 ? 1 : x) << 20; }();
@@ -461,122 +517,103 @@ static uint64_t batch_group_bytes() {
 }
 static inline uint64_t batch_padded(uint64_t len) { return (len + kBatchGap + 255) & ~255ull; }
 
-static yams_status_t run_batch_group(IngestRes* r, const uint8_t* const* files, const size_t* lens, size_t f0, size_t f1, bool hash,
+static yams_status_t run_batch_group(IngestRes& r, const uint8_t* const* files, const size_t* lens, size_t f0, size_t f1,
                                      std::vector<yams_chunk_desc>& out, uint64_t* out_first, float* ms_acc) {
-    CdcStream& cs = r->cs;
-    cudaStream_t st = cs.st;
+    cudaStream_t st = r.st;
     yams_status_t rc;
     const uint32_t nf = (uint32_t)(f1 - f0);
     std::vector<uint64_t> lay(2 * (size_t)nf);   // starts | ends
+    std::vector<LayoutPiece> pieces(nf);
     uint64_t pos = 256;
     for (uint32_t f = 0; f < nf; ++f) {
         lay[f] = pos;
         lay[nf + f] = pos + lens[f0 + f];
+        pieces[f] = {pos, lens[f0 + f], files[f0 + f]};
         pos += batch_padded(lens[f0 + f]);
     }
     const uint64_t L = pos;
-    if ((rc = r->stage[0].reserve((size_t)L + 256)) != YAMS_OK) return rc;
-    uint8_t* d_buf = r->stage[0].as<uint8_t>();
-    if ((rc = cs.fileinfo.reserve((size_t)nf * 16)) != YAMS_OK) return rc;
-    if ((rc = cs.roots.reserve((size_t)nf * 4)) != YAMS_OK) return rc;
-    if ((rc = cs.first.reserve(((size_t)nf + 1) * 8)) != YAMS_OK) return rc;
-    YB_CUDA(cudaEventRecord(r->e0, st));
-    // Upload: the files sit in ordinary (pageable) host memory, which a plain cudaMemcpy moves at ~10 GB/s through
-    // the driver's single staging thread.  Instead, host threads assemble an exact image of each 32 MiB slice of the
-    // device buffer (file bytes + zero gaps) in one of two pinned buffers while the previous slice is on the wire.
-    {
-        auto fill = [&](uint8_t* dst, uint64_t lo, uint64_t hi) {   // image of buffer positions [lo, hi)
-            // first file whose end lies beyond lo
-            uint32_t f = (uint32_t)(std::upper_bound(lay.begin() + nf, lay.begin() + 2 * (size_t)nf, lo) - (lay.begin() + nf));
-            uint64_t p = lo;
-            while (p < hi) {
-                if (f < nf && lay[f] <= p) {   // inside file f
-                    uint64_t e = std::min<uint64_t>(hi, lay[nf + f]);
-                    if (e > p) memcpy(dst + (p - lo), files[f0 + f] + (p - lay[f]), (size_t)(e - p));
-                    p = std::max(p, e);
-                    if (p >= lay[nf + f]) ++f;
-                } else {                       // gap up to the next file start (or the end of the buffer)
-                    uint64_t e = std::min<uint64_t>(hi, f < nf ? lay[f] : hi);
-                    memset(dst + (p - lo), 0, (size_t)(e - p));
-                    p = e;
-                }
-            }
-        };
-        if ((rc = staged_upload(r, d_buf, L + 256, fill, st)) != YAMS_OK) return rc;
-    }
-    YB_CUDA(cudaMemcpyAsync(cs.fileinfo.p, lay.data(), (size_t)nf * 16, cudaMemcpyHostToDevice, st));
-    YB_CUDA(cudaEventRecord(cs.ev[0], st));
+    if ((rc = r.stage[0].reserve((size_t)L + 256)) != YAMS_OK) return rc;
+    uint8_t* d_buf = r.stage[0].as<uint8_t>();
+    if ((rc = r.fileinfo.reserve((size_t)nf * 16)) != YAMS_OK) return rc;
+    if ((rc = r.roots.reserve((size_t)nf * 4)) != YAMS_OK) return rc;
+    if ((rc = r.first.reserve(((size_t)nf + 1) * 8)) != YAMS_OK) return rc;
+    YB_CUDA(cudaEventRecord(r.call[0], st));
+    // the whole buffer is uploaded, file bytes and zero gaps alike
+    if ((rc = staged_upload(r, d_buf, L + 256, pieces, st)) != YAMS_OK) return rc;
+    YB_CUDA(cudaMemcpyAsync(r.fileinfo.p, lay.data(), (size_t)nf * 16, cudaMemcpyHostToDevice, st));
+    YB_CUDA(cudaEventRecord(r.ev[0], st));
     uint32_t ncand = 0;
-    if ((rc = cs.scan(d_buf, 0, 0, 0, L, &ncand)) != YAMS_OK) return rc;
-    YB_CUDA(cudaEventRecord(cs.ev[1], st));
+    if ((rc = r.scan(d_buf, 0, 0, 0, L, &ncand)) != YAMS_OK) return rc;
+    YB_CUDA(cudaEventRecord(r.ev[1], st));
     // ---- selection over the merged node table ----
     YB_ARG((uint64_t)ncand + nf < 0xFFFFFFF0ull, "too many nodes in one batch group");
     const uint32_t nnodes = ncand + nf;
-    const uint32_t nblocks = (nnodes + kNodeBlock - 1) / kNodeBlock;
-    if ((rc = cs.npos.reserve((size_t)nnodes * 8)) != YAMS_OK) return rc;
-    if ((rc = cs.nref.reserve((size_t)nnodes * 4)) != YAMS_OK) return rc;
-    if ((rc = cs.next.reserve((size_t)nnodes * 4)) != YAMS_OK) return rc;
-    if ((rc = cs.forced.reserve((size_t)nnodes * 4)) != YAMS_OK) return rc;
-    if ((rc = cs.exit_.reserve((size_t)nnodes * 4)) != YAMS_OK) return rc;
-    if ((rc = cs.entry.reserve((size_t)nblocks * 4)) != YAMS_OK) return rc;
-    if ((rc = cs.onchain.reserve((size_t)nnodes)) != YAMS_OK) return rc;
-    if ((rc = cs.emit_counts.reserve((size_t)nnodes * 4)) != YAMS_OK) return rc;
-    if ((rc = cs.emit_offsets.reserve((size_t)nnodes * 4)) != YAMS_OK) return rc;
-    if (!cs.cand.p && (rc = cs.cand.reserve(8)) != YAMS_OK) return rc;
-    uint64_t* d_sc = cs.scalars.as<uint64_t>();
-    volatile uint64_t* h_sc = cs.h_scalars.as<uint64_t>();
-    BatchArgs B{BatchLayout{cs.cand.as<uint64_t>(), ncand, cs.fileinfo.as<uint64_t>(), cs.fileinfo.as<uint64_t>() + nf, nf}, cs.P};
+    if ((rc = r.npos.reserve((size_t)nnodes * 8)) != YAMS_OK) return rc;
+    if ((rc = r.nref.reserve((size_t)nnodes * 4)) != YAMS_OK) return rc;
+    if ((rc = r.reserve_nodes(nnodes)) != YAMS_OK) return rc;
+    uint64_t* d_sc = r.scalars.as<uint64_t>();
+    BatchArgs B{BatchLayout{r.cand.as<uint64_t>(), ncand, r.fileinfo.as<uint64_t>(), r.fileinfo.as<uint64_t>() + nf, nf}, r.P};
     const uint32_t tgrid = (nnodes + 255) / 256;
-    batch_nodes_kernel<<<tgrid, 256, 0, st>>>(B, cs.npos.as<uint64_t>(), cs.nref.as<uint32_t>(), cs.roots.as<uint32_t>());
-    batch_next_kernel<<<tgrid, 256, 0, st>>>(B, cs.npos.as<uint64_t>(), cs.nref.as<uint32_t>(), cs.roots.as<uint32_t>(), nnodes,
-                                             cs.next.as<uint32_t>(), cs.forced.as<uint32_t>(), cs.emit_counts.as<uint32_t>());
-    cdc_exit_kernel<<<nblocks, 32, 0, st>>>(cs.next.as<uint32_t>(), nnodes, cs.exit_.as<uint32_t>());
-    YB_CUDA(cudaMemsetAsync(cs.entry.p, 0xFF, (size_t)nblocks * 4, st));
-    YB_CUDA(cudaMemsetAsync(cs.onchain.p, 0, (size_t)nnodes, st));
-    cdc_walk_kernel<<<1, 32, 0, st>>>(cs.exit_.as<uint32_t>(), nnodes, cs.entry.as<uint32_t>());
-    cdc_mark_kernel<<<nblocks, 32, 0, st>>>(cs.next.as<uint32_t>(), nnodes, cs.entry.as<uint32_t>(), cs.onchain.as<uint8_t>());
-    batch_mask_counts_kernel<<<tgrid, 256, 0, st>>>(cs.onchain.as<uint8_t>(), cs.emit_counts.as<uint32_t>(), nnodes);
-    if ((rc = exclusive_scan_u32(cs.emit_counts.as<uint32_t>(), cs.emit_offsets.as<uint32_t>(), nnodes, d_sc + 0, cs.scan_scratch,
-                                 st)) != YAMS_OK)
-        return rc;
-    YB_CUDA(cudaMemcpyAsync((void*)h_sc, d_sc, 8, cudaMemcpyDeviceToHost, st));
-    YB_CUDA(cudaStreamSynchronize(st));
-    const uint64_t nnew = h_sc[0];
+    batch_nodes_kernel<<<tgrid, 256, 0, st>>>(B, r.npos.as<uint64_t>(), r.nref.as<uint32_t>(), r.roots.as<uint32_t>());
+    batch_next_kernel<<<tgrid, 256, 0, st>>>(B, r.npos.as<uint64_t>(), r.nref.as<uint32_t>(), r.roots.as<uint32_t>(), nnodes,
+                                             r.next.as<uint32_t>(), r.forced.as<uint32_t>(), r.emit_counts.as<uint32_t>());
+    if ((rc = r.mark_chain(nnodes)) != YAMS_OK) return rc;
+    batch_mask_counts_kernel<<<tgrid, 256, 0, st>>>(r.onchain.as<uint8_t>(), r.emit_counts.as<uint32_t>(), nnodes);
+    uint64_t nnew = 0;
+    if ((rc = r.count_offsets(nnodes, &nnew)) != YAMS_OK) return rc;
     YB_ARG(nnew < 0xFFFFFFFFull, "too many chunks in one batch group");
-    if ((rc = cs.descs.reserve((size_t)(nnew + 1) * sizeof(yams_chunk_desc))) != YAMS_OK) return rc;
-    batch_emit_kernel<<<tgrid, 256, 0, st>>>(B, cs.npos.as<uint64_t>(), cs.next.as<uint32_t>(), cs.forced.as<uint32_t>(),
-                                             cs.onchain.as<uint8_t>(), cs.emit_offsets.as<uint32_t>(), nnodes,
-                                             cs.descs.as<yams_chunk_desc>());
-    batch_first_kernel<<<(nf + 1 + 255) / 256, 256, 0, st>>>(cs.roots.as<uint32_t>(), cs.emit_offsets.as<uint32_t>(), nf, d_sc + 0,
-                                                             cs.first.as<uint64_t>());
-    YB_CUDA(cudaEventRecord(cs.ev[2], st));
-    if (hash && nnew) {
-        if ((rc = cs.sha_order.reserve(sha256_order_ws_bytes(nnew))) != YAMS_OK) return rc;
-        if ((rc = launch_sha256_chunks(d_buf, 0, cs.descs.as<yams_chunk_desc>(), 0, (uint32_t)nnew,
-                                       reinterpret_cast<unsigned int*>(d_sc + 4), cs.dev->sm_count, st, cs.sha_order.as<uint32_t>(),
-                                       L)) != YAMS_OK)
-            return rc;
-    }
-    YB_CUDA(cudaEventRecord(cs.ev[3], st));
-    if (nnew) batch_rebase_kernel<<<(unsigned)((nnew + 255) / 256), 256, 0, st>>>(cs.descs.as<yams_chunk_desc>(), nnew,
-                                                                               cs.fileinfo.as<uint64_t>(), nf);
+    if ((rc = r.descs.reserve((size_t)(nnew + 1) * sizeof(yams_chunk_desc))) != YAMS_OK) return rc;
+    batch_emit_kernel<<<tgrid, 256, 0, st>>>(B, r.npos.as<uint64_t>(), r.next.as<uint32_t>(), r.forced.as<uint32_t>(),
+                                             r.onchain.as<uint8_t>(), r.emit_offsets.as<uint32_t>(), nnodes,
+                                             r.descs.as<yams_chunk_desc>());
+    batch_first_kernel<<<(nf + 1 + 255) / 256, 256, 0, st>>>(r.roots.as<uint32_t>(), r.emit_offsets.as<uint32_t>(), nf, d_sc + 0,
+                                                             r.first.as<uint64_t>());
+    YB_CUDA(cudaEventRecord(r.ev[2], st));
+    if ((rc = r.hash(d_buf, 0, 0, nnew, L)) != YAMS_OK) return rc;
+    YB_CUDA(cudaEventRecord(r.ev[3], st));
+    if (nnew) batch_rebase_kernel<<<(unsigned)((nnew + 255) / 256), 256, 0, st>>>(r.descs.as<yams_chunk_desc>(), nnew,
+                                                                               r.fileinfo.as<uint64_t>(), nf);
     YB_CUDA(cudaGetLastError());
     const size_t base = out.size();
     out.resize(base + (size_t)nnew);
     std::vector<uint64_t> first((size_t)nf + 1);
-    if (nnew) YB_CUDA(cudaMemcpyAsync(out.data() + base, cs.descs.p, (size_t)nnew * sizeof(yams_chunk_desc), cudaMemcpyDeviceToHost, st));
-    YB_CUDA(cudaMemcpyAsync(first.data(), cs.first.p, ((size_t)nf + 1) * 8, cudaMemcpyDeviceToHost, st));
-    YB_CUDA(cudaEventRecord(r->e1, st));
+    if (nnew) YB_CUDA(cudaMemcpyAsync(out.data() + base, r.descs.p, (size_t)nnew * sizeof(yams_chunk_desc), cudaMemcpyDeviceToHost, st));
+    YB_CUDA(cudaMemcpyAsync(first.data(), r.first.p, ((size_t)nf + 1) * 8, cudaMemcpyDeviceToHost, st));
+    YB_CUDA(cudaEventRecord(r.call[1], st));
     YB_CUDA(cudaStreamSynchronize(st));
     if (out_first)
         for (uint32_t f = 0; f <= nf; ++f) out_first[f0 + f] = base + first[f];
     float a = 0, b = 0, c = 0, d = 0;
-    cudaEventElapsedTime(&a, cs.ev[0], cs.ev[1]);
-    cudaEventElapsedTime(&b, cs.ev[1], cs.ev[2]);
-    cudaEventElapsedTime(&c, cs.ev[2], cs.ev[3]);
-    cudaEventElapsedTime(&d, r->e0, r->e1);
+    cudaEventElapsedTime(&a, r.ev[0], r.ev[1]);
+    cudaEventElapsedTime(&b, r.ev[1], r.ev[2]);
+    cudaEventElapsedTime(&c, r.ev[2], r.ev[3]);
+    cudaEventElapsedTime(&d, r.call[0], r.call[1]);
     ms_acc[0] += a; ms_acc[1] += b; ms_acc[2] += c; ms_acc[3] += d;
     return YAMS_OK;
+}
+
+// SHA-256 of the spans [offsets[i], offsets[i] + sizes[i]) of one buffer; a host buffer is first copied into stage[0].
+static yams_status_t hash_spans(const uint8_t* base, bool on_host, size_t base_len, const uint64_t* offsets,
+                                const uint64_t* sizes, size_t n, uint8_t* digests) {
+    IngestLease ws(nullptr);
+    if (ws.rc != YAMS_OK) return ws.rc;
+    IngestRes& r = *ws.r;
+    if (on_host) {
+        yams_status_t rc = r.stage[0].reserve(base_len + 64);
+        if (rc != YAMS_OK) return rc;
+        if (base_len) YB_CUDA(cudaMemcpyAsync(r.stage[0].p, base, base_len, cudaMemcpyHostToDevice, r.st));
+        base = r.stage[0].as<uint8_t>();
+    }
+    YB_ARG(n < 0xFFFFFFFFull, "too many spans");
+    std::vector<yams_chunk_desc> h(n);
+    uint64_t total = 0;
+    for (size_t i = 0; i < n; ++i) {
+        YB_ARG(offsets[i] <= base_len && sizes[i] <= base_len - offsets[i], "span outside the base buffer");
+        h[i].offset = offsets[i];
+        h[i].size = sizes[i];
+        total += sizes[i];
+    }
+    return r.hash_table(base, h, total, digests);
 }
 
 }  // namespace yb
@@ -586,74 +623,59 @@ using namespace yb;
 // Streaming session: host bytes are staged [carry | slice] into one of two device buffers; the H2D copy
 // of slice i+1 overlaps the kernels of slice i (when the host memory is pinned).
 struct yams_b200_ingest {
-    IngestRes* r = nullptr;
+    IngestLease ws;               // held until the session is closed
+    bool hash;
     uint64_t head = 0;            // bytes reserved in front of a slice for the carry
     uint64_t stream_pos = 0;      // bytes fed so far
     uint64_t keep_from = 0;       // lowest stream position still resident on the device
     const uint8_t* res_ptr = nullptr;  // device address of stream position keep_from
     int cur = -1;                 // stage buffer holding the resident bytes (-1: none yet)
-    bool hash = true;
     bool finished = false;
     float ms_sha = 0;
     uint64_t sha_pos = 0;         // stream position up to which chunks have been hashed (mean chunk size of a slice)
+    yams_b200_ingest(const yams_cdc_config* cfg, bool hash_chunks) : ws(cfg), hash(hash_chunks) {}
 };
 
-static yams_status_t session_open(const yams_cdc_config* cfg, bool hash, yams_b200_ingest** out) {
-    yams_b200_ingest* s = new (std::nothrow) yams_b200_ingest();
+static yams_status_t session_open(const yams_cdc_config* cfg, bool hash, std::unique_ptr<yams_b200_ingest>* out) {
+    std::unique_ptr<yams_b200_ingest> s(new (std::nothrow) yams_b200_ingest(cfg, hash));
     if (!s) return YAMS_ERR_INTERNAL;
-    s->hash = hash;
-    yams_status_t rc = acquire_res(cfg, &s->r);
-    if (rc != YAMS_OK) {
-        delete s;
-        return rc;
-    }
+    if (s->ws.rc != YAMS_OK) return s->ws.rc;
     // the open chunk is always shorter than `force`, and a position needs <= kHistory bytes behind it
-    uint64_t need = std::max<uint64_t>(s->r->cs.P.force, (uint64_t)kHistory) + 16;
+    uint64_t need = std::max<uint64_t>(s->ws.r->P.force, (uint64_t)kHistory) + 16;
     s->head = (need + 255) & ~255ull;
-    *out = s;
+    *out = std::move(s);
     return YAMS_OK;
 }
 
-static void session_close(yams_b200_ingest* s) {
-    if (!s) return;
-    release_res(s->r);
-    delete s;
-}
-
 static yams_status_t session_sha(yams_b200_ingest* s, const uint8_t* data, uint64_t base_pos, uint64_t first) {
-    CdcStream& cs = s->r->cs;
-    if (!s->hash || cs.ndescs <= first) return YAMS_OK;
-    YB_ARG(cs.ndescs - first < 0xFFFFFFFFull, "too many chunks in one slice");
-    YB_CUDA(cudaEventRecord(s->r->t0, cs.st));
-    yams_status_t rc = cs.sha_order.reserve(sha256_order_ws_bytes(cs.ndescs - first));
-    if (rc != YAMS_OK) return rc;
+    IngestRes& r = *s->ws.r;
+    if (!s->hash || r.ndescs <= first) return YAMS_OK;
+    YB_ARG(r.ndescs - first < 0xFFFFFFFFull, "too many chunks in one slice");
+    YB_CUDA(cudaEventRecord(r.ev[0], r.st));
     // mean chunk size of the slice: the new chunks end at the open chunk's start
-    const uint64_t slice_bytes = cs.chunk_start > s->sha_pos ? cs.chunk_start - s->sha_pos : 0;
-    s->sha_pos = cs.chunk_start;
-    rc = launch_sha256_chunks(data, base_pos, cs.descs.as<yams_chunk_desc>(), (uint32_t)first, (uint32_t)(cs.ndescs - first),
-                              reinterpret_cast<unsigned int*>(cs.scalars.as<uint64_t>() + 4), cs.dev->sm_count, cs.st,
-                              cs.sha_order.as<uint32_t>(), slice_bytes);
+    const uint64_t slice_bytes = r.chunk_start > s->sha_pos ? r.chunk_start - s->sha_pos : 0;
+    s->sha_pos = r.chunk_start;
+    yams_status_t rc = r.hash(data, base_pos, first, r.ndescs - first, slice_bytes);
     if (rc != YAMS_OK) return rc;
-    YB_CUDA(cudaEventRecord(s->r->t1, cs.st));
-    YB_CUDA(cudaEventSynchronize(s->r->t1));
+    YB_CUDA(cudaEventRecord(r.ev[1], r.st));
+    YB_CUDA(cudaEventSynchronize(r.ev[1]));
     float ms = 0;
-    cudaEventElapsedTime(&ms, s->r->t0, s->r->t1);
+    cudaEventElapsedTime(&ms, r.ev[0], r.ev[1]);
     s->ms_sha += ms;
     return YAMS_OK;
 }
 
 // Feed `len` host bytes; when `final`, also close the stream.  Newly completed chunks are appended to
-// cs.descs (digests included when hashing is on).
+// the workspace's descs (digests included when hashing is on).
 static yams_status_t session_feed(yams_b200_ingest* s, const uint8_t* data, size_t len, bool final) {
-    IngestRes* r = s->r;
-    CdcStream& cs = r->cs;
+    IngestRes& r = *s->ws.r;
     yams_status_t rc;
     YB_ARG(!s->finished, "ingest session already finished");
     const size_t nslices = (size_t)((len + kFeedSlice - 1) / kFeedSlice);
     if (nslices == 0) {
         if (final) {
-            uint64_t first = cs.ndescs;
-            rc = cs.process(s->res_ptr, s->keep_from, s->keep_from, s->stream_pos, s->stream_pos, true);
+            uint64_t first = r.ndescs;
+            rc = r.process(s->res_ptr, s->keep_from, s->keep_from, s->stream_pos, s->stream_pos, true);
             if (rc != YAMS_OK) return rc;
             if ((rc = session_sha(s, s->res_ptr, s->keep_from, first)) != YAMS_OK) return rc;
             s->finished = true;
@@ -664,19 +686,18 @@ static yams_status_t session_feed(yams_b200_ingest* s, const uint8_t* data, size
     const bool pageable = len >= (4u << 20) && is_pageable(data);
     auto issue_copy = [&](size_t i, int b) -> yams_status_t {
         size_t sl = slice_len(i);
-        yams_status_t rr = r->stage[b].reserve((size_t)s->head + sl + 64);
+        yams_status_t rr = r.stage[b].reserve((size_t)s->head + sl + 64);
         if (rr != YAMS_OK) return rr;
-        YB_CUDA(cudaStreamWaitEvent(r->copy_st, r->freed[b], 0));
+        YB_CUDA(cudaStreamWaitEvent(r.copy_st, r.freed[b], 0));
         const uint8_t* src = data + i * kFeedSlice;
         if (pageable && sl >= (4u << 20)) {
             // ordinary host memory: pinned double-buffered upload filled by host threads (see staged_upload)
-            auto fill = [src](uint8_t* dst, uint64_t lo, uint64_t hi) { memcpy(dst, src + lo, (size_t)(hi - lo)); };
-            yams_status_t ur = staged_upload(r, r->stage[b].as<uint8_t>() + s->head, sl, fill, r->copy_st);
+            yams_status_t ur = staged_upload(r, r.stage[b].as<uint8_t>() + s->head, sl, {{0, (uint64_t)sl, src}}, r.copy_st);
             if (ur != YAMS_OK) return ur;
         } else {
-            YB_CUDA(cudaMemcpyAsync(r->stage[b].as<uint8_t>() + s->head, src, sl, cudaMemcpyHostToDevice, r->copy_st));
+            YB_CUDA(cudaMemcpyAsync(r.stage[b].as<uint8_t>() + s->head, src, sl, cudaMemcpyHostToDevice, r.copy_st));
         }
-        YB_CUDA(cudaEventRecord(r->copied[b], r->copy_st));
+        YB_CUDA(cudaEventRecord(r.copied[b], r.copy_st));
         return YAMS_OK;
     };
     int b = s->cur < 0 ? 0 : (s->cur ^ 1);
@@ -684,24 +705,24 @@ static yams_status_t session_feed(yams_b200_ingest* s, const uint8_t* data, size
     for (size_t i = 0; i < nslices; ++i) {
         const size_t sl = slice_len(i);
         const uint64_t carry = s->stream_pos - s->keep_from;
-        uint8_t* dst0 = r->stage[b].as<uint8_t>() + s->head;  // device address of stream position stream_pos
+        uint8_t* dst0 = r.stage[b].as<uint8_t>() + s->head;  // device address of stream position stream_pos
         if (carry) {
-            YB_CUDA(cudaMemcpyAsync(dst0 - carry, s->res_ptr, (size_t)carry, cudaMemcpyDeviceToDevice, cs.st));
+            YB_CUDA(cudaMemcpyAsync(dst0 - carry, s->res_ptr, (size_t)carry, cudaMemcpyDeviceToDevice, r.st));
         }
-        if (s->cur >= 0) YB_CUDA(cudaEventRecord(r->freed[s->cur], cs.st));
+        if (s->cur >= 0) YB_CUDA(cudaEventRecord(r.freed[s->cur], r.st));
         if (i + 1 < nslices) {
             if ((rc = issue_copy(i + 1, b ^ 1)) != YAMS_OK) return rc;
         }
-        YB_CUDA(cudaStreamWaitEvent(cs.st, r->copied[b], 0));
+        YB_CUDA(cudaStreamWaitEvent(r.st, r.copied[b], 0));
         const uint64_t new_pos = s->stream_pos + sl;
-        const uint64_t first = cs.ndescs;
+        const uint64_t first = r.ndescs;
         const uint8_t* view = dst0 - carry;  // stream position keep_from
         const bool last = final && (i + 1 == nslices);
-        rc = cs.process(view, s->keep_from, s->keep_from, s->stream_pos, new_pos, last);
+        rc = r.process(view, s->keep_from, s->keep_from, s->stream_pos, new_pos, last);
         if (rc != YAMS_OK) return rc;
         if ((rc = session_sha(s, view, s->keep_from, first)) != YAMS_OK) return rc;
         s->stream_pos = new_pos;
-        uint64_t nk = std::min<uint64_t>(cs.chunk_start, new_pos > (uint64_t)kHistory ? new_pos - kHistory : 0);
+        uint64_t nk = std::min<uint64_t>(r.chunk_start, new_pos > (uint64_t)kHistory ? new_pos - kHistory : 0);
         if (nk < s->keep_from) nk = s->keep_from;
         s->res_ptr = view + (nk - s->keep_from);
         s->keep_from = nk;
@@ -713,33 +734,28 @@ static yams_status_t session_feed(yams_b200_ingest* s, const uint8_t* data, size
 }
 
 static yams_status_t session_take(yams_b200_ingest* s, yams_chunk_desc** out, size_t* out_n) {
-    yams_status_t rc = copy_out(s->r->cs, 0, s->r->cs.ndescs, out, out_n);
-    if (rc == YAMS_OK) s->r->cs.ndescs = 0;  // descriptors handed over; reuse the device table
+    IngestRes& r = *s->ws.r;
+    yams_status_t rc = copy_out(r, 0, r.ndescs, out, out_n);
+    if (rc == YAMS_OK) r.ndescs = 0;  // descriptors handed over; reuse the device table
     return rc;
 }
 
 static yams_status_t run_host(const uint8_t* data, size_t len, const yams_cdc_config* cfg, bool hash,
                               yams_chunk_desc** out, size_t* out_n) {
-    yams_b200_ingest* s = nullptr;
+    std::unique_ptr<yams_b200_ingest> s;
     yams_status_t rc = session_open(cfg, hash, &s);
     if (rc != YAMS_OK) return rc;
-    CdcStream& cs = s->r->cs;
-    {
-        uint64_t per = std::max<uint64_t>(cs.P.lo + 1, 4096);
-        rc = cs.descs.reserve((size_t)(len / per + 16) * sizeof(yams_chunk_desc));
-    }
-    cudaEventRecord(s->r->e0, cs.st);
-    if (rc == YAMS_OK) rc = session_feed(s, data, len, true);
-    if (rc == YAMS_OK) rc = session_take(s, out, out_n);
-    cudaEventRecord(s->r->e1, cs.st);
-    cudaEventSynchronize(s->r->e1);
+    IngestRes& r = *s->ws.r;
+    if ((rc = r.presize_descs(len)) != YAMS_OK) return rc;
+    YB_CUDA(cudaEventRecord(r.call[0], r.st));
+    if ((rc = session_feed(s.get(), data, len, true)) != YAMS_OK) return rc;
+    if ((rc = session_take(s.get(), out, out_n)) != YAMS_OK) return rc;
+    YB_CUDA(cudaEventRecord(r.call[1], r.st));
+    YB_CUDA(cudaEventSynchronize(r.call[1]));
     float t = 0;
-    cudaEventElapsedTime(&t, s->r->e0, s->r->e1);
-    g_last_ms[0] = cs.ms_scan; g_last_ms[1] = cs.ms_select; g_last_ms[2] = s->ms_sha; g_last_ms[3] = t;
-    g_last_ms[4] = (float)cs.host_sync1; g_last_ms[5] = (float)cs.host_sync2; g_last_ms[6] = (float)cs.host_alloc;
-    g_last_ms[7] = (float)cs.host_total;
-    session_close(s);
-    return rc;
+    cudaEventElapsedTime(&t, r.call[0], r.call[1]);
+    report_timings({r.ms_scan, r.ms_select, s->ms_sha, t}, &r);
+    return YAMS_OK;
 }
 
 extern "C" {
@@ -795,7 +811,7 @@ yams_status_t yams_b200_chunk_and_hash_device(void* self, const uint8_t* d_data,
     *out_n = 0;
     YB_ARG(d_data || len == 0, "d_data is null");
     YB_ARG(cfg, "cfg is null");
-    return run_device(d_data, len, cfg, true, out, out_n);
+    return run_device(d_data, len, cfg, out, out_n);
     YB_CATCH
 }
 
@@ -811,39 +827,34 @@ yams_status_t yams_b200_chunk_and_hash_batch(void* self, const uint8_t* const* f
     if (n_files == 0) return YAMS_OK;
     YB_ARG(files && lens && out_first, "null argument");
     for (size_t f = 0; f < n_files; ++f) YB_ARG(files[f] || lens[f] == 0, "a file pointer is null");
-    IngestRes* r = nullptr;
-    yams_status_t rc = acquire_res(cfg, &r);
-    if (rc != YAMS_OK) return rc;
+    IngestLease ws(cfg);
+    if (ws.rc != YAMS_OK) return ws.rc;
+    yams_status_t rc;
     std::vector<yams_chunk_desc> all;
     float ms[4] = {0, 0, 0, 0};
     const uint64_t budget = batch_group_bytes();
     size_t f = 0;
-    while (f < n_files && rc == YAMS_OK) {
+    while (f < n_files) {
         if (batch_padded(lens[f]) + 256 > budget) {
             // a file larger than a whole group goes through the streaming path on its own
             yams_chunk_desc* d = nullptr;
             size_t n = 0;
-            rc = run_host(files[f], lens[f], cfg, true, &d, &n);
-            if (rc == YAMS_OK) {
-                out_first[f] = all.size();
-                all.insert(all.end(), d, d + n);
-                out_first[f + 1] = all.size();
-                free(d);
-                for (int i = 0; i < 4; ++i) ms[i] += g_last_ms[i];
-            }
+            if ((rc = run_host(files[f], lens[f], cfg, true, &d, &n)) != YAMS_OK) return rc;
+            out_first[f] = all.size();
+            all.insert(all.end(), d, d + n);
+            out_first[f + 1] = all.size();
+            free(d);
+            for (int i = 0; i < 4; ++i) ms[i] += g_last_ms[i];
             ++f;
             continue;
         }
         size_t g = f;
         uint64_t tot = 256;
         while (g < n_files && tot + batch_padded(lens[g]) <= budget) tot += batch_padded(lens[g++]);
-        rc = run_batch_group(r, files, lens, f, g, true, all, out_first, ms);
+        if ((rc = run_batch_group(*ws.r, files, lens, f, g, all, out_first, ms)) != YAMS_OK) return rc;
         f = g;
     }
-    release_res(r);
-    if (rc != YAMS_OK) return rc;
-    for (int i = 0; i < 4; ++i) g_last_ms[i] = ms[i];
-    g_last_ms[4] = g_last_ms[5] = g_last_ms[6] = g_last_ms[7] = 0;
+    report_timings(ms, nullptr);
     if (!all.empty()) {
         yams_chunk_desc* h = static_cast<yams_chunk_desc*>(malloc(all.size() * sizeof(yams_chunk_desc)));
         if (!h) {
@@ -870,7 +881,10 @@ yams_status_t yams_b200_ingest_open(void* self, const yams_cdc_config* cfg, yams
     YB_ARG(out, "out is null");
     *out = nullptr;
     YB_ARG(cfg, "cfg is null");
-    return session_open(cfg, true, out);
+    std::unique_ptr<yams_b200_ingest> s;
+    yams_status_t rc = session_open(cfg, true, &s);
+    if (rc == YAMS_OK) *out = s.release();
+    return rc;
     YB_CATCH
 }
 
@@ -878,7 +892,7 @@ yams_status_t yams_b200_ingest_feed(yams_b200_ingest* s, const uint8_t* data, si
                                     size_t* out_n) {
     YB_TRY
     YB_ARG(s && out && out_n, "null argument");
-    if (s->r && s->r->cs.dev) cudaSetDevice(s->r->cs.dev->device);   // a session may be fed from another thread than the one that opened it
+    cudaSetDevice(s->ws.r->dev->device);   // a session may be fed from another thread than the one that opened it
     *out = nullptr;
     *out_n = 0;
     YB_ARG(data || len == 0, "data is null");
@@ -891,7 +905,7 @@ yams_status_t yams_b200_ingest_feed(yams_b200_ingest* s, const uint8_t* data, si
 yams_status_t yams_b200_ingest_finish(yams_b200_ingest* s, yams_chunk_desc** out, size_t* out_n) {
     YB_TRY
     YB_ARG(s && out && out_n, "null argument");
-    if (s->r && s->r->cs.dev) cudaSetDevice(s->r->cs.dev->device);   // a session may be fed from another thread than the one that opened it
+    cudaSetDevice(s->ws.r->dev->device);   // a session may be fed from another thread than the one that opened it
     *out = nullptr;
     *out_n = 0;
     yams_status_t rc = session_feed(s, nullptr, 0, true);
@@ -900,39 +914,7 @@ yams_status_t yams_b200_ingest_finish(yams_b200_ingest* s, yams_chunk_desc** out
     YB_CATCH
 }
 
-void yams_b200_ingest_close(yams_b200_ingest* s) { session_close(s); }
-
-static yams_status_t sha_batch_impl(const uint8_t* d_base, size_t base_len, const uint64_t* offsets,
-                                    const uint64_t* sizes, size_t n, uint8_t* digests, DeviceCtx* dev,
-                                    cudaStream_t st) {
-    YB_ARG(n < 0xFFFFFFFFull, "too many spans");
-    std::vector<yams_chunk_desc> h(n);
-    for (size_t i = 0; i < n; ++i) {
-        YB_ARG(offsets[i] <= base_len && sizes[i] <= base_len - offsets[i], "span outside the base buffer");
-        h[i].offset = offsets[i];
-        h[i].size = sizes[i];
-    }
-    DevBuf d_descs, d_cnt;
-    yams_status_t rc = d_descs.reserve(n * sizeof(yams_chunk_desc));
-    if (rc == YAMS_OK) rc = d_cnt.reserve(16);
-    if (rc == YAMS_OK) {
-        cudaError_t e = cudaMemcpyAsync(d_descs.p, h.data(), n * sizeof(yams_chunk_desc), cudaMemcpyHostToDevice, st);
-        if (e != cudaSuccess) { set_last_error("H2D failed: %s", cudaGetErrorString(e)); rc = YAMS_ERR_INTERNAL; }
-    }
-    if (rc == YAMS_OK)
-        rc = launch_sha256_chunks(d_base, 0, d_descs.as<yams_chunk_desc>(), 0, (uint32_t)n,
-                                  d_cnt.as<unsigned int>(), dev->sm_count, st);
-    if (rc == YAMS_OK) {
-        cudaError_t e = cudaMemcpyAsync(h.data(), d_descs.p, n * sizeof(yams_chunk_desc), cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-        if (e != cudaSuccess) { set_last_error("sha256 batch failed: %s", cudaGetErrorString(e)); rc = YAMS_ERR_INTERNAL; }
-    }
-    if (rc == YAMS_OK)
-        for (size_t i = 0; i < n; ++i) memcpy(digests + 32 * i, h[i].digest, 32);
-    d_descs.release();
-    d_cnt.release();
-    return rc;
-}
+void yams_b200_ingest_close(yams_b200_ingest* s) { delete s; }
 
 yams_status_t yams_b200_sha256_batch_device(void* self, const uint8_t* d_base, size_t base_len,
                                             const uint64_t* offsets, const uint64_t* sizes, size_t n,
@@ -942,14 +924,7 @@ yams_status_t yams_b200_sha256_batch_device(void* self, const uint8_t* d_base, s
     if (n == 0) return YAMS_OK;
     YB_ARG(offsets && sizes && digests, "null argument");
     YB_ARG(d_base || base_len == 0, "d_base is null");
-    DeviceCtx* dev = nullptr;
-    yams_status_t rc = ensure_device(&dev);
-    if (rc != YAMS_OK) return rc;
-    cudaStream_t st;
-    YB_CUDA(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-    rc = sha_batch_impl(d_base, base_len, offsets, sizes, n, digests, dev, st);
-    cudaStreamDestroy(st);
-    return rc;
+    return hash_spans(d_base, false, base_len, offsets, sizes, n, digests);
     YB_CATCH
 }
 
@@ -960,21 +935,7 @@ yams_status_t yams_b200_sha256_batch(void* self, const uint8_t* base, size_t bas
     if (n == 0) return YAMS_OK;
     YB_ARG(offsets && sizes && digests, "null argument");
     YB_ARG(base || base_len == 0, "base is null");
-    DeviceCtx* dev = nullptr;
-    yams_status_t rc = ensure_device(&dev);
-    if (rc != YAMS_OK) return rc;
-    cudaStream_t st;
-    YB_CUDA(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-    DevBuf d_base;
-    rc = d_base.reserve(base_len + 64);
-    if (rc == YAMS_OK && base_len) {
-        cudaError_t e = cudaMemcpyAsync(d_base.p, base, base_len, cudaMemcpyHostToDevice, st);
-        if (e != cudaSuccess) { set_last_error("H2D failed: %s", cudaGetErrorString(e)); rc = YAMS_ERR_INTERNAL; }
-    }
-    if (rc == YAMS_OK) rc = sha_batch_impl(d_base.as<uint8_t>(), base_len, offsets, sizes, n, digests, dev, st);
-    d_base.release();
-    cudaStreamDestroy(st);
-    return rc;
+    return hash_spans(base, true, base_len, offsets, sizes, n, digests);
     YB_CATCH
 }
 
@@ -988,73 +949,31 @@ yams_status_t yams_b200_sha256_many(void* self, const uint8_t* const* msgs, cons
     for (size_t i = 0; i < n; ++i) YB_ARG(msgs[i] || lens[i] == 0, "a message pointer is null");
     yams_cdc_config cfg;
     yams_b200_cdc_default_config(&cfg);
-    IngestRes* r = nullptr;
-    yams_status_t rc = acquire_res(&cfg, &r);
-    if (rc != YAMS_OK) return rc;
-    CdcStream& cs = r->cs;
-    cudaStream_t st = cs.st;
+    IngestLease ws(&cfg);
+    if (ws.rc != YAMS_OK) return ws.rc;
+    IngestRes& r = *ws.r;
+    yams_status_t rc;
     const uint64_t budget = batch_group_bytes();
-    size_t i0 = 0;
-    while (i0 < n && rc == YAMS_OK) {
+    for (size_t i0 = 0, i1; i0 < n; i0 = i1) {
         // group [i0, i1): packed size within the budget (a single larger message forms its own group)
-        size_t i1 = i0;
+        i1 = i0;
         uint64_t tot = 0;
         std::vector<yams_chunk_desc> h;
+        std::vector<LayoutPiece> pieces;
         while (i1 < n && (i1 == i0 || tot + lens[i1] + 16 <= budget) && h.size() < 0xFFFFFFF0ull) {
             yams_chunk_desc d{};
             d.offset = tot;
             d.size = lens[i1];
             h.push_back(d);
+            pieces.push_back({tot, lens[i1], msgs[i1]});
             tot = (tot + lens[i1] + 15) & ~15ull;
             ++i1;
         }
-        const size_t m = i1 - i0;
-        rc = r->stage[0].reserve((size_t)tot + 256);
-        if (rc == YAMS_OK) rc = cs.descs.reserve(m * sizeof(yams_chunk_desc));
-        if (rc != YAMS_OK) break;
-        uint8_t* d_buf = r->stage[0].as<uint8_t>();
-        auto fill = [&](uint8_t* dst, uint64_t lo, uint64_t hi) {
-            // first message whose packed range ends beyond lo
-            size_t a = 0, b = m;
-            while (a < b) {
-                size_t mid = a + ((b - a) >> 1);
-                if (h[mid].offset + h[mid].size <= lo) a = mid + 1; else b = mid;
-            }
-            uint64_t p = lo;
-            for (size_t j = a; j < m && p < hi; ++j) {
-                if (h[j].offset > p) {   // alignment padding
-                    uint64_t e = std::min<uint64_t>(hi, h[j].offset);
-                    memset(dst + (p - lo), 0, (size_t)(e - p));
-                    p = e;
-                }
-                uint64_t e = std::min<uint64_t>(hi, h[j].offset + h[j].size);
-                if (e > p) {
-                    memcpy(dst + (p - lo), msgs[i0 + j] + (p - h[j].offset), (size_t)(e - p));
-                    p = e;
-                }
-            }
-            if (p < hi) memset(dst + (p - lo), 0, (size_t)(hi - p));
-        };
-        rc = staged_upload(r, d_buf, tot, fill, st);
-        if (rc != YAMS_OK) break;
-        cudaError_t e = cudaMemcpyAsync(cs.descs.p, h.data(), m * sizeof(yams_chunk_desc), cudaMemcpyHostToDevice, st);
-        if (e == cudaSuccess) rc = cs.sha_order.reserve(sha256_order_ws_bytes(m));
-        if (e == cudaSuccess && rc == YAMS_OK)
-            rc = launch_sha256_chunks(d_buf, 0, cs.descs.as<yams_chunk_desc>(), 0, (uint32_t)m,
-                                      reinterpret_cast<unsigned int*>(cs.scalars.as<uint64_t>() + 4), cs.dev->sm_count, st,
-                                      cs.sha_order.as<uint32_t>(), tot);
-        if (rc == YAMS_OK && e == cudaSuccess) e = cudaMemcpyAsync(h.data(), cs.descs.p, m * sizeof(yams_chunk_desc), cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-        if (e != cudaSuccess) {
-            set_last_error("sha256_many failed: %s", cudaGetErrorString(e));
-            rc = YAMS_ERR_INTERNAL;
-        }
-        if (rc == YAMS_OK)
-            for (size_t j = 0; j < m; ++j) memcpy(digests + 32 * (i0 + j), h[j].digest, 32);
-        i0 = i1;
+        if ((rc = r.stage[0].reserve((size_t)tot + 256)) != YAMS_OK) return rc;
+        if ((rc = staged_upload(r, r.stage[0].as<uint8_t>(), tot, pieces, r.st)) != YAMS_OK) return rc;
+        if ((rc = r.hash_table(r.stage[0].as<uint8_t>(), h, tot, digests + 32 * i0)) != YAMS_OK) return rc;
     }
-    release_res(r);
-    return rc;
+    return YAMS_OK;
     YB_CATCH
 }
 

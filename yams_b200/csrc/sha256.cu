@@ -258,13 +258,13 @@ __global__ void sha_order_scatter_kernel(const yams_chunk_desc* __restrict__ des
 // Launch helper: hashes descs[first .. first+n). d_counter must point at a zeroed uint32.
 yams_status_t launch_sha256_chunks(const uint8_t* d_data, uint64_t base_pos, yams_chunk_desc* d_descs,
                                    uint32_t first, uint32_t n, unsigned int* d_counter, int sm_count,
-                                   cudaStream_t st, uint32_t* d_order_ws, uint64_t total_bytes, int variant_per_sm, int grid_per_sm) {
+                                   cudaStream_t st, uint32_t* d_order_ws, uint64_t total_bytes) {
     if (n == 0) return YAMS_OK;
     YB_CUDA(cudaMemsetAsync(d_counter, 0, sizeof(unsigned int), st));
     // d_order_ws: 64 counters + n indices (sha256_order_ws_bytes); tables that leave every lane under ~2 chunks are not worth it
     static const int lpt = [] { const char* e = getenv("YAMS_B200_SHA_ORDER"); return e ? atoi(e) : 1; }();
     const uint32_t* d_order = nullptr;
-    if (d_order_ws && lpt && n >= 4096) {
+    if (lpt && n >= 4096) {
         const uint64_t mean = std::max<uint64_t>(1, total_bytes / n);
         YB_CUDA(cudaMemsetAsync(d_order_ws, 0, 64 * sizeof(uint32_t), st));
         const unsigned g = (unsigned)std::min<uint32_t>((n + 255) / 256, (uint32_t)sm_count * 8u);
@@ -273,13 +273,12 @@ yams_status_t launch_sha256_chunks(const uint8_t* d_data, uint64_t base_pos, yam
         d_order = d_order_ws + 64;
     }
     static const int madd = [] { const char* e = getenv("YAMS_B200_SHA_MADD"); return e ? atoi(e) : 1; }();
-    static const int env_per_sm = [] { const char* e = getenv("YAMS_B200_SHA_CTAS"); int v = e ? atoi(e) : 4; return v < 3 ? 3 : (v > 6 ? 6 : v); }();
-    // experiment knob: grid CTAs per SM independent of the occupancy variant (co-residency with the candidate scan)
+    // per_sm picks the register budget the kernel was compiled for (launch bounds 128 x per_sm)
+    static const int per_sm = [] { const char* e = getenv("YAMS_B200_SHA_CTAS"); int v = e ? atoi(e) : 4; return v < 3 ? 3 : (v > 6 ? 6 : v); }();
+    // experiment knob: grid CTAs per SM independent of the occupancy variant (co-residency with the candidate scan); fewer
+    // than the variant allows leaves registers for a co-resident kernel
     static const int env_grid = [] { const char* e = getenv("YAMS_B200_SHA_GRID"); return e ? atoi(e) : 0; }();
-    // variant_per_sm picks the register budget the kernel was compiled for (launch bounds 128 x per_sm); grid_per_sm how many
-    // CTAs per SM are launched - fewer than the variant allows leaves registers for a co-resident kernel
-    const int per_sm = variant_per_sm > 0 ? (variant_per_sm < 3 ? 3 : (variant_per_sm > 6 ? 6 : variant_per_sm)) : env_per_sm;
-    const int grid = grid_per_sm > 0 ? grid_per_sm : (env_grid > 0 ? env_grid : per_sm);
+    const int grid = env_grid > 0 ? env_grid : per_sm;
     uint32_t warps_needed = (n + 31) / 32;
     uint32_t ctas = (warps_needed + kShaWarpsPerCta - 1) / kShaWarpsPerCta;
     uint32_t max_ctas = (uint32_t)sm_count * (uint32_t)grid;
