@@ -1,5 +1,6 @@
-// cosine.cuh -- the exact scan's per-row similarity, shared by its re-scoring kernel (knn.cu) and the document pass (pq.cu),
-// and the score keys both order by.
+// cosine.cuh -- device building blocks shared by the exact scan (knn.cu), the PQ engine (pq.cu) and the sqlite-vec operators
+// (operators.cu): the exact per-row similarity, the score keys every ordered path ranks by, the in-block key sort and the
+// rowid -> row lookup.
 #pragma once
 #include <cuda_fp16.h>
 #include <math.h>
@@ -22,6 +23,40 @@ __device__ __forceinline__ uint32_t fkey(float f) {
 __device__ __forceinline__ float fkey_inv(uint32_t k) {
     uint32_t b = (k & 0x80000000u) ? (k & 0x7FFFFFFFu) : ~k;
     return __uint_as_float(b);
+}
+
+// The sort key of an entry: (fkey(score) << 32) | (0xFFFFFFFF - row).  Descending key order is score descending, then row
+// ascending; key 0 marks "no entry".  word_key takes the score word fkey(score) of a caller that has already tested it.
+// knn.cu's sel_key writes this format out on purpose, to keep topk_select_kernel's machine code (see there).
+__device__ __forceinline__ uint64_t word_key(uint32_t w, uint32_t row) { return ((uint64_t)w << 32) | (uint64_t)(0xFFFFFFFFu - row); }
+__device__ __forceinline__ uint64_t score_key(float s, uint32_t row) { return word_key(fkey(s), row); }
+__device__ __forceinline__ float key_score(uint64_t key) { return fkey_inv((uint32_t)(key >> 32)); }
+__device__ __forceinline__ uint32_t key_row(uint64_t key) { return 0xFFFFFFFFu - (uint32_t)key; }
+
+// bitonic sort, descending, of buf[0, n) in shared memory (n a power of two) by the block's NT threads; ends with a barrier
+template <int NT, typename T>
+__device__ __forceinline__ void block_sort_desc(T* buf, uint32_t n) {
+    for (uint32_t size = 2; size <= n; size <<= 1) {
+        for (uint32_t stride = size >> 1; stride > 0; stride >>= 1) {
+            for (uint32_t t = threadIdx.x; t < n / 2; t += NT) {
+                const uint32_t lo = (t / stride) * (stride * 2) + (t % stride), hi = lo + stride;
+                const bool desc = ((lo & size) == 0);
+                const T x = buf[lo], y = buf[hi];
+                if ((x < y) == desc) { buf[lo] = y; buf[hi] = x; }
+            }
+            __syncthreads();
+        }
+    }
+}
+
+// index of `want` in the ascending rowid table rowids[0, n), or n when it is not there
+__device__ __forceinline__ uint64_t find_row(const int64_t* __restrict__ rowids, uint64_t n, int64_t want) {
+    uint64_t a = 0, b = n;
+    while (a < b) {
+        const uint64_t m = a + ((b - a) >> 1);
+        if (rowids[m] < want) a = m + 1; else b = m;
+    }
+    return (a < n && rowids[a] == want) ? a : n;
 }
 
 // bruteForceSearchUnlocked's cosine (sqlite_vec_backend.cpp:4253-4279) of corpus row `row` against the query qv (fp32, 16-byte

@@ -117,10 +117,11 @@ yams_status_t enqueue_results(const DeviceResults& r, uint32_t nq, uint32_t k, i
 yams_status_t copy_results(const DeviceResults& r, uint32_t nq, uint32_t k, int64_t* out_rowids, float* out_scores, uint32_t* out_counts,
                            uint64_t* out_flags, cudaStream_t st);
 
-// Device key sort of the exact paths (knn.cu) and the sqlite-vec operators (operators.cu).  A key is
-// (fkey(score) << 32) | (0xFFFFFFFF - row), so descending order is score descending, then row ascending; key 0 marks no entry.
-inline uint64_t pow2_at_least(uint64_t n) {
-    uint64_t p = 1;
+// Device key sort of the exact paths (knn.cu) and the sqlite-vec operators (operators.cu); the keys are score_key (cosine.cuh).
+// pow2_at_least computes in the type of n: the kernels size their shared-memory sorts in 32 bits.
+template <typename T>
+__host__ __device__ inline T pow2_at_least(T n) {
+    T p = 1;
     while (p < n) p <<= 1;
     return p;
 }

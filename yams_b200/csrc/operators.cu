@@ -56,14 +56,14 @@ __global__ void batch_dist_kernel(const float* __restrict__ rows, uint32_t d, ui
     F32At qa{q}, ra{rows + r * d};
     out_neg[r] = -(metric == YAMS_B200_L2 ? ref_l2_distance(qa, ra, d) : ref_cosine_distance(qa, ra, d));
 }
-// sort keys of np2 entries: row i < n gets (fkey(-dist) << 32) | (0xFFFFFFFF - i), so a NaN distance (fkey 0) still ranks
-// after every finite one but above the zero padding.  filtered: only rows with dist < threshold get a key (NaN rows do not).
+// sort keys of np2 entries: row i < n gets score_key(-dist, i), so a NaN distance (fkey 0) still ranks after every finite one
+// but above the zero padding.  filtered: only rows with dist < threshold get a key (NaN rows do not).
 __global__ void dist_keys_kernel(const float* __restrict__ neg_dist, uint64_t n, uint64_t np2, int filtered, float threshold,
                                  uint64_t* __restrict__ keys) {
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < np2; i += (uint64_t)gridDim.x * blockDim.x) {
         uint64_t key = 0;
         if (i < n && (!filtered || (-neg_dist[i]) < threshold))
-            key = ((uint64_t)fkey(neg_dist[i]) << 32) | (uint64_t)(0xFFFFFFFFu - (uint32_t)i);
+            key = score_key(neg_dist[i], (uint32_t)i);
         keys[i] = key;
     }
 }

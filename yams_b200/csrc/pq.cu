@@ -211,26 +211,13 @@ __global__ void __launch_bounds__(PQ_THREADS) pq_adc_kernel(const uint8_t* __res
         uint64_t key = 0;
         if (j < n_idx) {
             const float acc = pq_adc_sum(codes + j * m, lut, m, k, vec);
-            uint32_t b = __float_as_uint(acc);
-            b = (acc != acc) ? 0u : ((b & 0x80000000u) ? ~b : (b | 0x80000000u));   // monotone key, NaN last (as knn.cu fkey)
-            key = ((uint64_t)b << 32) | (uint64_t)(0xFFFFFFFFu - tie_rank[j]);
+            key = score_key(acc, tie_rank[j]);
             if (key == 0) key = 1;
         }
         keys[t] = key;
     }
     __syncthreads();
-    // bitonic sort, descending
-    for (uint32_t size = 2; size <= PQ_TILE; size <<= 1) {
-        for (uint32_t stride = size >> 1; stride > 0; stride >>= 1) {
-            for (uint32_t t = threadIdx.x; t < PQ_TILE / 2; t += PQ_THREADS) {
-                const uint32_t lo = (t / stride) * (stride * 2) + (t % stride), hi = lo + stride;
-                const bool desc = ((lo & size) == 0);
-                const uint64_t x = keys[lo], y = keys[hi];
-                if ((x < y) == desc) { keys[lo] = y; keys[hi] = x; }
-            }
-            __syncthreads();
-        }
-    }
+    block_sort_desc<PQ_THREADS>(keys, PQ_TILE);
     const uint64_t in_tile = n_idx > r0 ? min((uint64_t)PQ_TILE, n_idx - r0) : 0;
     const uint32_t nout = (uint32_t)min((uint64_t)approx, in_tile);
     __shared__ uint32_t s_base;
@@ -238,11 +225,9 @@ __global__ void __launch_bounds__(PQ_THREADS) pq_adc_kernel(const uint8_t* __res
     __syncthreads();
     for (uint32_t i = threadIdx.x; i < nout; i += PQ_THREADS) {
         const uint64_t key = keys[i];
-        uint32_t b = (uint32_t)(key >> 32);
-        b = (b & 0x80000000u) ? (b & 0x7FFFFFFFu) : ~b;
         Cand c;
-        c.score = __uint_as_float(b);
-        c.row = 0xFFFFFFFFu - (uint32_t)key;     // tie rank: topk_select orders equal scores by ascending `row`
+        c.score = key_score(key);
+        c.row = key_row(key);     // tie rank: topk_select orders equal scores by ascending `row`
         if (s_base + i < list_cap) lists[(size_t)q * list_cap + s_base + i] = c;
     }
 }
@@ -256,9 +241,7 @@ __global__ void pq_tau_kernel(const Cand* __restrict__ sel, const uint32_t* __re
     uint64_t t = 0;
     if (sel_n[q] >= approx) {
         const Cand c = sel[(size_t)q * approx + approx - 1];
-        uint32_t b = __float_as_uint(c.score);
-        b = (c.score != c.score) ? 0u : ((b & 0x80000000u) ? ~b : (b | 0x80000000u));
-        t = ((uint64_t)b << 32) | (uint64_t)(0xFFFFFFFFu - c.row);
+        t = score_key(c.score, c.row);
     }
     tau[q] = t;
     counts[q] = 0;
@@ -319,14 +302,13 @@ __global__ void __launch_bounds__(PQ_THREADS) pq_adc_filter_kernel(const uint8_t
         }
 #pragma unroll
         for (int g = 0; g < QG; ++g) {
-            uint32_t b = __float_as_uint(acc[g]);
-            b = (acc[g] != acc[g]) ? 0u : ((b & 0x80000000u) ? ~b : (b | 0x80000000u));
+            const uint32_t b = fkey(acc[g]);
             const uint32_t th = (uint32_t)(tq[g] >> 32);
             bool pass = valid && b >= th;           // tq = ~0 for the padding queries of the last group: never passes
             uint32_t rank = 0;
             if (pass) {
                 rank = tie_rank[j];
-                uint64_t key = ((uint64_t)b << 32) | (uint64_t)(0xFFFFFFFFu - rank);
+                uint64_t key = word_key(b, rank);
                 if (key == 0) key = 1;
                 pass = key >= tq[g] && tq[g] != ~0ull;
             }
@@ -527,15 +509,15 @@ __global__ void doc_argmax_kernel(const Cand* __restrict__ pairs, const uint64_t
     uint64_t best = 0;
     for (uint64_t i = lo + lane; i < hi; i += 32) {
         const float s = pairs[i].score;
-        if (s == s) best = max(best, ((uint64_t)fkey(s) << 32) | (uint64_t)(0xFFFFFFFFu - (uint32_t)(i - lo)));
+        if (s == s) best = max(best, score_key(s, (uint32_t)(i - lo)));
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) best = max(best, (uint64_t)__shfl_xor_sync(0xffffffffu, best, o));
     if (lane == 0 && best) {
         const uint32_t q = segment_of(qdocs, nq, doc);
-        best_row[doc] = pairs[lo + (0xFFFFFFFFu - (uint32_t)best)].row;
+        best_row[doc] = pairs[lo + key_row(best)].row;
         Cand c;
-        c.score = fkey_inv((uint32_t)(best >> 32));
+        c.score = key_score(best);
         c.row = (uint32_t)doc;
         const uint32_t pos = atomicAdd(&counts[q], 1u);
         lists[(uint64_t)q * cap + pos] = c;
