@@ -11,7 +11,7 @@ Y.synth_bytes_device(12345, 0, n, buf.data_ptr())
 for i in range(4):
     t0 = time.perf_counter(); ch = Y.chunk_and_hash_device(buf.data_ptr(), n, Y.default_config()); dt = time.perf_counter() - t0
 t = Y.ingest_last_timings()
-print(f"env MADD={os.environ.get('YAMS_B200_SHA_MADD')} TWO_PASS={os.environ.get('YAMS_B200_TWO_PASS')} gib={gib} wall {dt*1e3:.1f} ms  "
+print(f"gib={gib} wall {dt*1e3:.1f} ms  "
       f"dev GB/s {n/t['total_ms']/1e6:.1f} sha GB/s {n/t['sha256_ms']/1e6:.1f} scan GB/s {n/max(t['scan_ms'],1e-6)/1e6:.1f}", json.dumps(t))
 # host path e2e (pinned)
 hb = torch.empty(min(n, 4 << 30), dtype=torch.uint8).pin_memory()

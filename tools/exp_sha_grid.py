@@ -1,4 +1,4 @@
-"""SHA-256 throughput: longest-first chunk order on/off, resident CTAs per SM.  EXP_GIB sets the stream size."""
+"""Ingest throughput and stage times at several segment sizes.  EXP_GIB sets the stream size."""
 import os
 import subprocess
 import sys
@@ -29,7 +29,6 @@ CASES = [
     {"YAMS_B200_SEGMENT_MIB": "8192"},
     {"YAMS_B200_SEGMENT_MIB": "16384"},
     {"YAMS_B200_SEGMENT_MIB": "2048"},
-    {"YAMS_B200_SHA_ORDER": "0"},
 ]
 for extra in CASES:
     env = dict(os.environ)

@@ -8,7 +8,7 @@
 //                          closed-form masked rolling value (cdc_logic.h is_candidate); a SIMD
 //                          low-byte prefilter keeps the common case at ~1 instr/byte;
 //   2. ordered compaction of candidate positions (count -> scan -> write);
-//   3. next-cut per candidate (parallel), block-wise chain resolution, chunk emission.
+//   3. next-cut per candidate and file root (parallel), block-wise chain resolution, chunk emission.
 // All results are bit-identical to the sequential reference; the logic lives in cdc_logic.h so the
 // same lines are unit-tested on the CPU against the oracle.
 #include "cdc_kernels.cuh"
@@ -558,15 +558,6 @@ yams_status_t launch_scan_single_pass(const ScanArgs& A, uint32_t ntiles, uint64
 
 // ---- cut selection ----------------------------------------------------------------------------
 
-__global__ void cdc_next_kernel(SelectArgs S, uint32_t* __restrict__ next, uint32_t* __restrict__ forced) {
-    uint32_t node = blockIdx.x * blockDim.x + threadIdx.x;
-    if (node > S.ncand) return;
-    uint64_t s = node_start(S.cand, node, S.root_start);
-    NextCut r = next_cut(S.cand, S.ncand, node, s, S.P);
-    next[node] = r.j + 1;  // node index; END = ncand + 1
-    forced[node] = (uint32_t)r.forced;
-}
-
 // one warp per block of kNodeBlock nodes; lanes load coalesced, lane 0 does the backward pass
 __global__ void __launch_bounds__(32) cdc_exit_kernel(const uint32_t* __restrict__ next, uint32_t nnodes,
                                                       uint32_t* __restrict__ exit_out) {
@@ -610,77 +601,17 @@ __global__ void __launch_bounds__(32) cdc_mark_kernel(const uint32_t* __restrict
     for (uint32_t i = threadIdx.x; i < blk_end - blk_start; i += 32) onchain[blk_start + i] = oc[i];
 }
 
-__global__ void cdc_emit_count_kernel(SelectArgs S, const uint32_t* __restrict__ next,
-                                      const uint32_t* __restrict__ forced,
-                                      const uint8_t* __restrict__ onchain, uint32_t* __restrict__ counts) {
-    uint32_t node = blockIdx.x * blockDim.x + threadIdx.x;
-    if (node > S.ncand) return;
-    uint32_t c = 0;
-    if (onchain[node]) {
-        uint64_t s = node_start(S.cand, node, S.root_start);
-        c = (uint32_t)node_emit_count(next[node], forced[node], S.ncand + 1, s, S.end_pos, S.final != 0, S.P);
-    }
-    counts[node] = c;
-}
-
-// scalars[0] = new open-chunk start (written by the END node)
-__global__ void cdc_emit_kernel(SelectArgs S, const uint32_t* __restrict__ next,
-                                const uint32_t* __restrict__ forced, const uint8_t* __restrict__ onchain,
-                                const uint32_t* __restrict__ offsets, yams_chunk_desc* __restrict__ out,
-                                uint64_t out_base, uint64_t* __restrict__ scalars) {
-    uint32_t node = blockIdx.x * blockDim.x + threadIdx.x;
-    if (node > S.ncand || !onchain[node]) return;
-    const uint32_t END = S.ncand + 1;
-    uint64_t s = node_start(S.cand, node, S.root_start);
-    uint32_t nx = next[node];
-    uint64_t cnt = node_emit_count(nx, forced[node], END, s, S.end_pos, S.final != 0, S.P);
-    yams_chunk_desc* o = out + out_base + offsets[node];
-    if (nx != END) {
-        uint64_t F = forced[node];
-        for (uint64_t t = 0; t < F; ++t) {
-            o[t].offset = s + t * S.P.force;
-            o[t].size = S.P.force;
-        }
-        uint64_t ls = s + F * S.P.force;
-        o[F].offset = ls;
-        o[F].size = S.cand[nx - 1] + 1 - ls;
-    } else {
-        for (uint64_t t = 0; t < cnt; ++t) {
-            uint64_t cs = s + t * S.P.force;
-            uint64_t sz = S.end_pos - cs < S.P.force ? S.end_pos - cs : S.P.force;
-            o[t].offset = cs;
-            o[t].size = sz;
-        }
-        uint64_t ns = s + cnt * S.P.force;
-        scalars[0] = ns < S.end_pos ? ns : (S.final ? S.end_pos : ns);
-    }
-}
-
-// ---- cut selection over a batch of files (chunk_and_hash_batch): thin wrappers over cdc_logic.h ---------------------
-__global__ void batch_nodes_kernel(BatchArgs B, uint64_t* __restrict__ npos, uint32_t* __restrict__ nref, uint32_t* __restrict__ root_node) {
-    uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-    if (t < B.L.ncand) {
-        uint32_t node = batch_node_of_cand(B.L, t);
-        npos[node] = B.L.cand[t] + 1;   // a cut after byte cand[t] starts the next chunk at cand[t] + 1
-        nref[node] = t;
-    } else if (t < B.L.ncand + B.L.nfiles) {
-        uint32_t f = t - B.L.ncand;
-        uint32_t node = batch_node_of_root(B.L, f);
-        npos[node] = B.L.starts[f];
-        nref[node] = kBatchRootFlag | f;
-        root_node[f] = node;
-    }
-}
-
-__global__ void batch_next_kernel(BatchArgs B, const uint64_t* __restrict__ npos, const uint32_t* __restrict__ nref,
-                                  const uint32_t* __restrict__ root_node, uint32_t nnodes, uint32_t* __restrict__ next,
-                                  uint32_t* __restrict__ forced, uint32_t* __restrict__ cnt) {
+// ---- cut selection over a layout of files (a streaming feed or chunk_and_hash_batch): thin wrappers over cdc_logic.h ----
+// one thread per item (a candidate or a file root); it fills the entries of the item's node
+__global__ void batch_next_kernel(BatchArgs B, uint64_t* __restrict__ npos, uint32_t* __restrict__ next, uint32_t* __restrict__ forced,
+                                  uint32_t* __restrict__ cnt) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= nnodes) return;
-    BatchNext r = batch_next(B.L, B.P, i, npos[i], nref[i], root_node, nnodes);
-    next[i] = r.next;
-    forced[i] = r.forced;
-    cnt[i] = r.count;
+    if (i >= B.L.ncand + B.L.nfiles) return;
+    BatchNext r = batch_next(B.L, B.P, i);
+    npos[r.node] = r.pos;
+    next[r.node] = r.next;
+    forced[r.node] = r.forced;
+    cnt[r.node] = r.count;
 }
 
 __global__ void batch_mask_counts_kernel(const uint8_t* __restrict__ onchain, uint32_t* __restrict__ cnt, uint32_t nnodes) {
@@ -688,32 +619,33 @@ __global__ void batch_mask_counts_kernel(const uint8_t* __restrict__ onchain, ui
     if (i < nnodes && !onchain[i]) cnt[i] = 0;
 }
 
+// *open_start = where the chunk after the last node of the chain starts
 __global__ void batch_emit_kernel(BatchArgs B, const uint64_t* __restrict__ npos, const uint32_t* __restrict__ next,
                                   const uint32_t* __restrict__ forced, const uint8_t* __restrict__ onchain,
-                                  const uint32_t* __restrict__ offsets, uint32_t nnodes, yams_chunk_desc* __restrict__ out) {
+                                  const uint32_t* __restrict__ offsets, yams_chunk_desc* __restrict__ out,
+                                  uint64_t* __restrict__ open_start) {
+    const uint32_t nnodes = B.L.ncand + B.L.nfiles;
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= nnodes || !onchain[i]) return;
     yams_chunk_desc* o = out + offsets[i];
     const uint32_t nx = next[i];
-    batch_emit(B.L, B.P, npos[i], forced[i], nx < nnodes ? npos[nx] : 0ull, [o](uint64_t k, uint64_t off, uint64_t size) {
+    const uint64_t end = batch_emit(B.L, B.P, npos[i], forced[i], nx < nnodes ? npos[nx] : 0ull, [o](uint64_t k, uint64_t off, uint64_t size) {
         o[k].offset = off;
         o[k].size = size;
     });
+    if (nx == nnodes) *open_start = end;
 }
 
-__global__ void batch_first_kernel(const uint32_t* __restrict__ root_node, const uint32_t* __restrict__ offsets, uint32_t nfiles,
-                                   const uint64_t* __restrict__ total, uint64_t* __restrict__ first) {
+__global__ void batch_first_kernel(BatchArgs B, const uint32_t* __restrict__ offsets, const uint64_t* __restrict__ total,
+                                   uint64_t* __restrict__ first) {
     uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
-    if (f < nfiles) first[f] = offsets[root_node[f]];
-    if (f == nfiles) first[f] = *total;
+    if (f < B.L.nfiles) first[f] = offsets[batch_node_of_root(B.L, f)];
+    if (f == B.L.nfiles) first[f] = *total;
 }
 
-__global__ void batch_rebase_kernel(yams_chunk_desc* __restrict__ descs, uint64_t n, const uint64_t* __restrict__ starts, uint32_t nfiles) {
+__global__ void batch_rebase_kernel(BatchArgs B, yams_chunk_desc* __restrict__ descs, uint64_t n) {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    uint64_t off = descs[i].offset;
-    uint32_t fup = upper_bound_u64(starts, nfiles, off);
-    descs[i].offset = off - starts[fup - 1];
+    if (i < n) descs[i].offset = batch_file_offset(B.L, descs[i].offset);
 }
 
 // ---- generic exclusive scan (u32) ----------------------------------------------------------------

@@ -16,46 +16,27 @@ struct ScanArgs {
     CdcParams P;
 };
 
-struct SelectArgs {
-    const uint64_t* cand;
-    uint32_t ncand;
-    uint64_t root_start;   // start of the open chunk
-    uint64_t end_pos;      // one past the last available stream byte
-    int final;             // stream ends at end_pos
-    CdcParams P;
-};
-
-
-// Many independent streams ("files") laid out in ONE device buffer: file f occupies buffer positions
-// [starts[f], ends[f]); every file start is preceded by >= 64 zero bytes, so the rolling hash of the buffer equals the
+// Cut selection over a layout of files (cdc_logic.h): one streaming feed, or many independent streams ("files") in ONE
+// device buffer, where every file start is preceded by >= 64 zero bytes, so the rolling hash of the buffer equals the
 // hash of the file alone (the reference's ring buffer starts zeroed, chunker.h:150-154).
 struct BatchArgs {
     BatchLayout L;            // candidates + file layout (cdc_logic.h)
     CdcParams P;
 };
 
-__global__ void batch_nodes_kernel(BatchArgs B, uint64_t* npos, uint32_t* nref, uint32_t* root_node);
-__global__ void batch_next_kernel(BatchArgs B, const uint64_t* npos, const uint32_t* nref, const uint32_t* root_node, uint32_t nnodes,
-                                  uint32_t* next, uint32_t* forced, uint32_t* cnt);
+__global__ void batch_next_kernel(BatchArgs B, uint64_t* npos, uint32_t* next, uint32_t* forced, uint32_t* cnt);
 __global__ void batch_mask_counts_kernel(const uint8_t* onchain, uint32_t* cnt, uint32_t nnodes);
 __global__ void batch_emit_kernel(BatchArgs B, const uint64_t* npos, const uint32_t* next, const uint32_t* forced,
-                                  const uint8_t* onchain, const uint32_t* offsets, uint32_t nnodes, yams_chunk_desc* out);
-__global__ void batch_first_kernel(const uint32_t* root_node, const uint32_t* offsets, uint32_t nfiles, const uint64_t* total,
-                                   uint64_t* first);
-__global__ void batch_rebase_kernel(yams_chunk_desc* descs, uint64_t n, const uint64_t* starts, uint32_t nfiles);
+                                  const uint8_t* onchain, const uint32_t* offsets, yams_chunk_desc* out, uint64_t* open_start);
+__global__ void batch_first_kernel(BatchArgs B, const uint32_t* offsets, const uint64_t* total, uint64_t* first);
+__global__ void batch_rebase_kernel(BatchArgs B, yams_chunk_desc* descs, uint64_t n);
 
 __global__ void cdc_count_kernel(ScanArgs A, uint32_t ntiles, uint32_t* tile_counts);
 __global__ void cdc_write_kernel(ScanArgs A, uint32_t ntiles, const uint32_t* tile_counts,
                                  const uint32_t* tile_offsets, uint64_t* cand);
-__global__ void cdc_next_kernel(SelectArgs S, uint32_t* next, uint32_t* forced);
 __global__ void cdc_exit_kernel(const uint32_t* next, uint32_t nnodes, uint32_t* exit_out);
 __global__ void cdc_walk_kernel(const uint32_t* exit_in, uint32_t nnodes, uint32_t* entry);
 __global__ void cdc_mark_kernel(const uint32_t* next, uint32_t nnodes, const uint32_t* entry, uint8_t* onchain);
-__global__ void cdc_emit_count_kernel(SelectArgs S, const uint32_t* next, const uint32_t* forced,
-                                      const uint8_t* onchain, uint32_t* counts);
-__global__ void cdc_emit_kernel(SelectArgs S, const uint32_t* next, const uint32_t* forced,
-                                const uint8_t* onchain, const uint32_t* offsets, yams_chunk_desc* out,
-                                uint64_t out_base, uint64_t* scalars);
 
 constexpr int kScanThreads = 256;
 constexpr int kScanIters = 4;                                     // 16-byte loads per thread per tile

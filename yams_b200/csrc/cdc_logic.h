@@ -1,6 +1,8 @@
 // cdc_logic.h -- integer logic of the content-defined chunker, shared by the CUDA kernels
-// (cdc.cu) and by a host-side unit-test shim (tests/_sim) so the exact same source lines are
-// checked against the oracle on machines without a GPU.  No reference code is reproduced here:
+// (cdc.cu) and by a host-side emulation (tests/sim/cdc_sim.cpp) that calls the same functions in
+// the same order, so the exact source lines the GPU runs -- candidates, cut selection, chain
+// resolution and every chunk's offset and size -- are checked against the oracle on machines
+// without a GPU.  No reference code is reproduced here:
 // this is the closed-form / data-parallel re-derivation described in DESIGN.md §ingest.
 //
 // Reference behaviour being matched (paths under /root/reference):
@@ -132,16 +134,10 @@ YB_HD NextCut next_cut(const uint64_t* cand, uint32_t ncand, uint32_t hint, uint
 
 
 // ---- chain resolution over "nodes" ------------------------------------------------------------
-// Node 0 is the root (a chunk starting at the session's open-chunk start); node i+1 is candidate
-// i (a chunk starting at cand[i]+1).  next[node] is the node of the next candidate cut, or
-// END = ncand+1.  next[node] > node always, so a block of consecutive nodes can be resolved by a
-// single backward pass.
+// The nodes of a layout (below) are the chunk starts it can have, numbered by position.  next[node] is the node of the next
+// cut, or END = nnodes.  next[node] > node always, so a block of consecutive nodes can be resolved by a single backward pass.
 constexpr uint32_t kNodeBlock = 1024;
 constexpr uint32_t kNoEntry = 0xFFFFFFFFu;
-
-YB_HD uint64_t node_start(const uint64_t* cand, uint32_t node, uint64_t root_start) {
-    return node == 0 ? root_start : cand[node - 1] + 1;
-}
 
 // exit_out[i] = first node >= blk_end reached from node blk_start+i by following next[]
 YB_HD void block_exit_seq(const uint32_t* next_blk, uint32_t blk_start, uint32_t blk_end,
@@ -162,21 +158,11 @@ YB_HD void block_mark_seq(const uint32_t* next_blk, uint32_t blk_start, uint32_t
     }
 }
 
-// number of chunks a chain node emits.  `end_pos` is the stream position one past the last byte
-// available; `final` says whether the stream ends there (then the trailing partial chunk is
-// emitted, streaming_chunker.h:115-118 / rabin_chunker.cpp:66-67 min(start+max, size)).
-YB_HD uint64_t node_emit_count(uint32_t next_node, uint64_t forced, uint32_t end_node, uint64_t s,
-                               uint64_t end_pos, bool final, const CdcParams& P) {
-    if (next_node != end_node) return forced + 1;
-    if (s >= end_pos) return 0;
-    uint64_t rem = end_pos - s;
-    return final ? (rem + P.force - 1) / P.force : rem / P.force;
-}
-
-// ---- many files in one buffer (chunk_and_hash_batch) --------------------------------------------------------------
-// File f occupies buffer positions [starts[f], ends[f]) (ascending, zero gaps of >= 64 bytes in front of every file).
-// Nodes = file roots + candidate cuts merged by position (a root sorts before a candidate at the same position).
-// next[] keeps the single-stream shape (strictly increasing), so block_exit_seq / block_mark_seq are reused: the chain
+// ---- cut selection over a layout of files ----------------------------------------------------------------------------
+// File f occupies positions [starts[f], ends[f]).  chunk_and_hash_batch lays many files out in one buffer (ascending, zero
+// gaps of >= 64 bytes in front of every file); a streaming feed is a layout of one file that starts at the open chunk and
+// ends at the last fed byte, final when the stream ends there.
+// Nodes = file roots + candidate cuts merged by position (a root sorts before a candidate at the same position).  The chain
 // runs root(0) -> cuts of file 0 -> root(1) -> ...; nodes lying in a gap or at a file's end are dead links.
 struct BatchLayout {
     const uint64_t* cand;     // ascending candidate positions of the whole buffer
@@ -184,8 +170,8 @@ struct BatchLayout {
     const uint64_t* starts;
     const uint64_t* ends;
     uint32_t nfiles;
+    bool final;               // the last file is complete; otherwise the stream goes on past ends[nfiles - 1]
 };
-constexpr uint32_t kBatchRootFlag = 0x80000000u;   // nref[]: node is the root of file (nref & 0x7FFFFFFF)
 constexpr uint32_t kBatchTail = 0x80000000u;       // forced[]: the node's chunks run to the end of its file
 
 YB_HD uint32_t upper_bound_u64(const uint64_t* a, uint32_t n, uint64_t key) {   // first idx with a[idx] > key
@@ -203,52 +189,73 @@ YB_HD uint32_t batch_node_of_root(const BatchLayout& B, uint32_t f) {
     uint64_t s = B.starts[f];
     return f + (s == 0 ? 0u : lower_bound_u64(B.cand, 0, B.ncand, s - 1));   // candidates with cand + 1 < s
 }
+// offset of layout position pos inside the file that holds it
+YB_HD uint64_t batch_file_offset(const BatchLayout& B, uint64_t pos) { return pos - B.starts[upper_bound_u64(B.starts, B.nfiles, pos) - 1]; }
+// Chunks of the tail [s, ends[f]) of file f: all of it, the remainder included (streaming_chunker.h:115-118,
+// rabin_chunker.cpp:66-67 min(start+max, size)), unless the stream goes on past the file: then the remainder stays open.
+YB_HD uint64_t batch_tail_count(const BatchLayout& B, uint32_t f, uint64_t s, uint64_t force) {
+    const uint64_t rem = B.ends[f] - s;
+    return (B.final || f + 1 < B.nfiles) ? (rem + force - 1) / force : rem / force;
+}
 struct BatchNext {
+    uint32_t node;     // node index of the item
+    uint64_t pos;      // start position of the node
     uint32_t next;     // node index, nnodes = END
     uint32_t forced;   // forced chunks before the candidate cut, or kBatchTail
     uint32_t count;    // chunks this node emits when it is on the chain
 };
-// s = start position of the node, ref = nref[] of the node, root_node[] = node index of every file root
-YB_HD BatchNext batch_next(const BatchLayout& B, const CdcParams& P, uint32_t node, uint64_t s, uint32_t ref, const uint32_t* root_node,
-                           uint32_t nnodes) {
+// Selection step of item i: candidate i (i < ncand) or the root of file i - ncand.
+YB_HD BatchNext batch_next(const BatchLayout& B, const CdcParams& P, uint32_t i) {
     BatchNext r;
-    r.next = node + 1;
+    uint32_t hint;
+    if (i < B.ncand) {
+        r.pos = B.cand[i] + 1;   // a cut after byte cand[i] starts the next chunk at cand[i] + 1
+        r.node = batch_node_of_cand(B, i);
+        hint = i + 1;
+    } else {
+        const uint32_t f = i - B.ncand;
+        r.pos = B.starts[f];
+        r.node = batch_node_of_root(B, f);
+        hint = lower_bound_u64(B.cand, 0, B.ncand, r.pos);
+    }
+    r.next = r.node + 1;
     r.forced = 0;
     r.count = 0;
-    const uint32_t fup = upper_bound_u64(B.starts, B.nfiles, s);   // files starting at or before s
-    if (fup == 0 || s >= B.ends[fup - 1]) return r;                // gap / file end: dead link
+    const uint32_t fup = upper_bound_u64(B.starts, B.nfiles, r.pos);   // files starting at or before pos
+    if (fup == 0 || r.pos >= B.ends[fup - 1]) return r;                // gap / file end: dead link
     const uint32_t f = fup - 1;
-    const uint64_t e = B.ends[f];
-    const uint32_t hint = (ref & kBatchRootFlag) ? lower_bound_u64(B.cand, 0, B.ncand, s) : ref + 1;
-    NextCut c = next_cut(B.cand, B.ncand, hint, s, P);
-    if (c.j < B.ncand && B.cand[c.j] < e) {
+    NextCut c = next_cut(B.cand, B.ncand, hint, r.pos, P);
+    if (c.j < B.ncand && B.cand[c.j] < B.ends[f]) {
         r.next = batch_node_of_cand(B, c.j);
         r.forced = (uint32_t)c.forced;
         r.count = r.forced + 1;
     } else {
-        r.next = f + 1 < B.nfiles ? root_node[f + 1] : nnodes;
+        r.next = f + 1 < B.nfiles ? batch_node_of_root(B, f + 1) : B.ncand + B.nfiles;
         r.forced = kBatchTail;
-        r.count = (uint32_t)((e - s + P.force - 1) / P.force);   // streaming_chunker.h:115-118: the remainder is emitted too
+        r.count = (uint32_t)batch_tail_count(B, f, r.pos, P.force);
     }
     return r;
 }
-// Chunks of an on-chain node: emit(k, offset, size) for k = 0 .. count-1.  next_pos = start position of next[node].
+// Chunks of an on-chain node that starts at s: emit(k, offset, size) for k = 0 .. count-1.  next_pos = start position of
+// next[node].  Returns the position after the node's chunks, which for the last node of the chain is the new open-chunk start.
 template <typename EmitT>
-YB_HD void batch_emit(const BatchLayout& B, const CdcParams& P, uint64_t s, uint32_t forced, uint64_t next_pos, EmitT emit) {
+YB_HD uint64_t batch_emit(const BatchLayout& B, const CdcParams& P, uint64_t s, uint32_t forced, uint64_t next_pos, EmitT emit) {
     const uint32_t fup = upper_bound_u64(B.starts, B.nfiles, s);
-    if (fup == 0 || s >= B.ends[fup - 1]) return;   // dead link
+    if (fup == 0 || s >= B.ends[fup - 1]) return s;   // dead link
     if (forced & kBatchTail) {
         const uint64_t e = B.ends[fup - 1];
-        const uint64_t n = (e - s + P.force - 1) / P.force;
+        const uint64_t n = batch_tail_count(B, fup - 1, s, P.force);
         for (uint64_t t = 0; t < n; ++t) {
             uint64_t cs = s + t * P.force;
             emit(t, cs, e - cs < P.force ? e - cs : P.force);
         }
-    } else {
-        for (uint32_t t = 0; t < forced; ++t) emit((uint64_t)t, s + (uint64_t)t * P.force, P.force);
-        const uint64_t ls = s + (uint64_t)forced * P.force;
-        emit((uint64_t)forced, ls, next_pos - ls);
+        const uint64_t ns = s + n * P.force;
+        return ns < e ? ns : e;
     }
+    for (uint32_t t = 0; t < forced; ++t) emit((uint64_t)t, s + (uint64_t)t * P.force, P.force);
+    const uint64_t ls = s + (uint64_t)forced * P.force;
+    emit((uint64_t)forced, ls, next_pos - ls);
+    return next_pos;
 }
 
 }  // namespace yb

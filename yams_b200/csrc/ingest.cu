@@ -44,13 +44,11 @@ struct IngestRes {
     cudaStream_t copy_st = nullptr;  // H2D copies of the streaming session
     CdcParams P{};
     bool no_candidates = false;  // lo >= force: no candidate can ever cut
-    bool two_pass_only = false;  // YAMS_B200_TWO_PASS=1: skip the single-pass scan (diagnostics)
-    uint32_t two_pass_fallbacks = 0;
     DevBuf table, tile_counts, tile_offsets, cand, cand_tmp, next, forced, exit_, entry, onchain, emit_counts,
         emit_offsets, scan_scratch, descs, scalars, sha_order;
-    DevBuf npos, nref, roots, fileinfo, first;   // chunk_and_hash_batch: merged node table, file layout, per-file chunk ranges
+    DevBuf npos, fileinfo, first;   // node start positions, file layout [starts | ends], per-file chunk ranges (batch)
     DevBuf stage[2];             // device copies of host input
-    HostBuf h_scalars;           // pinned: [0] ncand/ntotal, [1] new chunk start
+    HostBuf h_scalars;           // pinned: [0] ncand/ntotal, [1] new chunk start, [6..7] layout of a feed
     HostBuf pin[2];              // pinned images of two device-buffer slices (staged_upload)
     uint64_t ndescs = 0;         // chunks accumulated in `descs`
     uint64_t chunk_start = 0;    // stream position where the open chunk starts
@@ -85,12 +83,10 @@ struct IngestRes {
         yams_status_t rc = resolve_params(cfg, &P, tbl);
         if (rc != YAMS_OK) return rc;
         no_candidates = P.lo >= P.force;
-        two_pass_only = getenv("YAMS_B200_TWO_PASS") != nullptr;
         ndescs = 0;
         chunk_start = 0;
         ms_scan = ms_select = 0;
         host_sync1 = host_sync2 = host_alloc = host_total = 0;
-        two_pass_fallbacks = 0;
         YB_CUDA(cudaMemcpyAsync(table.p, tbl, 256 * 8, cudaMemcpyHostToDevice, st));
         return YAMS_OK;
     }
@@ -98,8 +94,8 @@ struct IngestRes {
         if (st) cudaStreamSynchronize(st);
         if (copy_st) cudaStreamSynchronize(copy_st);
         for (DevBuf* b : {&table, &tile_counts, &tile_offsets, &cand, &cand_tmp, &next, &forced, &exit_, &entry, &onchain,
-                          &emit_counts, &emit_offsets, &scan_scratch, &descs, &scalars, &sha_order, &npos, &nref, &roots, &fileinfo,
-                          &first, &stage[0], &stage[1]})
+                          &emit_counts, &emit_offsets, &scan_scratch, &descs, &scalars, &sha_order, &npos, &fileinfo, &first,
+                          &stage[0], &stage[1]})
             b->release();
         for (HostBuf* b : {&h_scalars, &pin[0], &pin[1]}) b->release();
         for (cudaEvent_t e : {ev[0], ev[1], ev[2], ev[3], call[0], call[1], call[2], copied[0], copied[1], freed[0], freed[1],
@@ -125,6 +121,7 @@ struct IngestRes {
         uint64_t* d_sc = scalars.as<uint64_t>();
         volatile uint64_t* h_sc = h_scalars.as<uint64_t>();
         uint32_t ncand = 0;
+        if (!cand.p && (rc = cand.reserve(8)) != YAMS_OK) return rc;   // a valid pointer even when there is no candidate
         if (!no_candidates && scan_hi > scan_lo) {
             // tiles start at a 16-byte-aligned ADDRESS: normally at or below scan_lo (the positions in
             // [origin, scan_lo) are masked and never dereferenced); when that would fall before stream position
@@ -138,31 +135,25 @@ struct IngestRes {
             YB_ARG(ntiles64 < (1ull << 31), "segment too large");
             uint32_t ntiles = (uint32_t)ntiles64;
             ScanArgs A{data, base_pos, lowest, origin, scan_lo, scan_hi, table.as<uint64_t>(), P};
-            bool need_two_pass = two_pass_only;
-            if (!two_pass_only) {
-                // single pass: every warp scans a contiguous range (4 KiB tiles) and appends to its own slice
-                uint32_t ntiles4 = (uint32_t)((span + kSinglePassTile - 1) / kSinglePassTile);
-                uint32_t nslices = std::min<uint32_t>(ntiles4, (uint32_t)dev->sm_count * kSinglePassWarpsPerCta);
-                uint32_t tpw = (ntiles4 + nslices - 1) / nslices;
-                uint32_t slice_cap = std::max<uint32_t>(64u, tpw * 16u);   // 32x the 1/8192 density of random data
-                size_t total_cap = (size_t)nslices * slice_cap;
-                if ((rc = cand_tmp.reserve(total_cap * 8)) != YAMS_OK) return rc;
-                if ((rc = cand.reserve(total_cap * 8)) != YAMS_OK) return rc;
-                if ((rc = tile_counts.reserve((size_t)std::max<uint32_t>(ntiles, nslices) * 4)) != YAMS_OK) return rc;
-                if ((rc = launch_scan_single_pass(A, ntiles4, cand_tmp.as<uint64_t>(), tile_counts.as<uint32_t>(), slice_cap,
-                                                  nslices, cand.as<uint64_t>(), d_sc, st)) != YAMS_OK)
-                    return rc;
-                YB_CUDA(cudaMemcpyAsync((void*)h_sc, d_sc, 24, cudaMemcpyDeviceToHost, st));
-                if ((rc = wait(&host_sync1)) != YAMS_OK) return rc;
-                if (h_sc[2] != 0) {
-                    need_two_pass = true;   // dense candidates: exact two-pass kernels take over
-                    ++two_pass_fallbacks;
-                } else {
-                    YB_ARG(h_sc[0] < 0xFFFFFFF0ull, "too many boundary candidates in one segment");
-                    ncand = (uint32_t)h_sc[0];
-                }
-            }
-            if (need_two_pass) {
+            // single pass: every warp scans a contiguous range (4 KiB tiles) and appends to its own slice
+            uint32_t ntiles4 = (uint32_t)((span + kSinglePassTile - 1) / kSinglePassTile);
+            uint32_t nslices = std::min<uint32_t>(ntiles4, (uint32_t)dev->sm_count * kSinglePassWarpsPerCta);
+            uint32_t tpw = (ntiles4 + nslices - 1) / nslices;
+            uint32_t slice_cap = std::max<uint32_t>(64u, tpw * 16u);   // 32x the 1/8192 density of random data
+            size_t total_cap = (size_t)nslices * slice_cap;
+            if ((rc = cand_tmp.reserve(total_cap * 8)) != YAMS_OK) return rc;
+            if ((rc = cand.reserve(total_cap * 8)) != YAMS_OK) return rc;
+            if ((rc = tile_counts.reserve((size_t)std::max<uint32_t>(ntiles, nslices) * 4)) != YAMS_OK) return rc;
+            if ((rc = launch_scan_single_pass(A, ntiles4, cand_tmp.as<uint64_t>(), tile_counts.as<uint32_t>(), slice_cap,
+                                              nslices, cand.as<uint64_t>(), d_sc, st)) != YAMS_OK)
+                return rc;
+            YB_CUDA(cudaMemcpyAsync((void*)h_sc, d_sc, 24, cudaMemcpyDeviceToHost, st));
+            if ((rc = wait(&host_sync1)) != YAMS_OK) return rc;
+            if (h_sc[2] == 0) {
+                YB_ARG(h_sc[0] < 0xFFFFFFF0ull, "too many boundary candidates in one segment");
+                ncand = (uint32_t)h_sc[0];
+            } else {
+                // dense candidates overflowed a slice: the exact two-pass kernels take over
                 if ((rc = tile_counts.reserve((size_t)ntiles * 4)) != YAMS_OK) return rc;
                 if ((rc = tile_offsets.reserve((size_t)ntiles * 4)) != YAMS_OK) return rc;
                 uint32_t grid = std::min<uint32_t>(ntiles, (uint32_t)dev->sm_count * 8u);
@@ -186,18 +177,17 @@ struct IngestRes {
         return YAMS_OK;
     }
 
-    // ---- cut selection over a node table: the stream's root and candidates, or a batch group's merged roots and candidates ----
-    // The caller fills next[] / forced[] before mark_chain and emit_counts[] between mark_chain and count_offsets.
+    // ---- cut selection over a layout (cdc_logic.h): one streaming feed, or the files of a batch group ----
     yams_status_t reserve_nodes(uint32_t nnodes) {
         const uint32_t nblocks = (nnodes + kNodeBlock - 1) / kNodeBlock;
         yams_status_t rc;
+        if ((rc = npos.reserve((size_t)nnodes * 8)) != YAMS_OK) return rc;
         for (DevBuf* b : {&next, &forced, &exit_})
             if ((rc = b->reserve((size_t)nnodes * 4)) != YAMS_OK) return rc;
         if ((rc = entry.reserve((size_t)nblocks * 4)) != YAMS_OK) return rc;
         if ((rc = onchain.reserve((size_t)nnodes)) != YAMS_OK) return rc;
         for (DevBuf* b : {&emit_counts, &emit_offsets})
             if ((rc = b->reserve((size_t)nnodes * 4)) != YAMS_OK) return rc;
-        if (!cand.p && (rc = cand.reserve(8)) != YAMS_OK) return rc;
         return YAMS_OK;
     }
     // onchain[i] = 1 for the nodes on the chain of cuts that starts at node 0; every byte of onchain[0, nnodes) is written
@@ -220,6 +210,28 @@ struct IngestRes {
         *total = h_scalars.as<volatile uint64_t>()[0];
         return YAMS_OK;
     }
+    // The next cut from every node, the chain from node 0, the chunk counts of its nodes and their offsets; *total is the
+    // number of chunks emit_cuts writes.
+    yams_status_t select_cuts(const BatchArgs& B, uint64_t* total) {
+        const uint32_t nnodes = B.L.ncand + B.L.nfiles;
+        yams_status_t rc = reserve_nodes(nnodes);
+        if (rc != YAMS_OK) return rc;
+        const uint32_t tgrid = (nnodes + 255) / 256;
+        batch_next_kernel<<<tgrid, 256, 0, st>>>(B, npos.as<uint64_t>(), next.as<uint32_t>(), forced.as<uint32_t>(),
+                                                 emit_counts.as<uint32_t>());
+        if ((rc = mark_chain(nnodes)) != YAMS_OK) return rc;
+        batch_mask_counts_kernel<<<tgrid, 256, 0, st>>>(onchain.as<uint8_t>(), emit_counts.as<uint32_t>(), nnodes);
+        return count_offsets(nnodes, total);
+    }
+    // The selected chunks to out[0, total), the open-chunk start to scalars[1].
+    yams_status_t emit_cuts(const BatchArgs& B, yams_chunk_desc* out) {
+        const uint32_t nnodes = B.L.ncand + B.L.nfiles;
+        batch_emit_kernel<<<(nnodes + 255) / 256, 256, 0, st>>>(B, npos.as<uint64_t>(), next.as<uint32_t>(), forced.as<uint32_t>(),
+                                                                onchain.as<uint8_t>(), emit_offsets.as<uint32_t>(), out,
+                                                                scalars.as<uint64_t>() + 1);
+        YB_CUDA(cudaGetLastError());
+        return YAMS_OK;
+    }
 
     // Scan stream positions [scan_lo, scan_hi) (bytes readable from `lowest`), select cuts from the
     // open chunk at chunk_start, append the completed chunks to descs. `data[0]` is stream position
@@ -232,26 +244,23 @@ struct IngestRes {
         volatile uint64_t* h_sc = h_scalars.as<uint64_t>();
         uint32_t ncand = 0;
         YB_CUDA(cudaEventRecord(ev[0], st));
+        // The feed is a layout of one file, from the open chunk's start to scan_hi.  Its upload is queued ahead of the scan,
+        // so that it is not on the path from the host's wait for the scan to the selection kernels.
+        uint64_t* lay = h_scalars.as<uint64_t>() + 6;   // pinned; the copy out of it ended with the previous process()
+        lay[0] = chunk_start;
+        lay[1] = scan_hi;
+        if ((rc = fileinfo.reserve(16)) != YAMS_OK) return rc;
+        YB_CUDA(cudaMemcpyAsync(fileinfo.p, lay, 16, cudaMemcpyHostToDevice, st));
         if ((rc = scan(data, base_pos, lowest, scan_lo, scan_hi, &ncand)) != YAMS_OK) return rc;
         YB_CUDA(cudaEventRecord(ev[1], st));
-        const uint32_t nnodes = ncand + 1;
-        if ((rc = reserve_nodes(nnodes)) != YAMS_OK) return rc;
-        SelectArgs S{cand.as<uint64_t>(), ncand, chunk_start, scan_hi, final ? 1 : 0, P};
-        const uint32_t tgrid = (nnodes + 255) / 256;
-        cdc_next_kernel<<<tgrid, 256, 0, st>>>(S, next.as<uint32_t>(), forced.as<uint32_t>());
-        if ((rc = mark_chain(nnodes)) != YAMS_OK) return rc;
-        cdc_emit_count_kernel<<<tgrid, 256, 0, st>>>(S, next.as<uint32_t>(), forced.as<uint32_t>(),
-                                                     onchain.as<uint8_t>(), emit_counts.as<uint32_t>());
+        const BatchArgs B{BatchLayout{cand.as<uint64_t>(), ncand, fileinfo.as<uint64_t>(), fileinfo.as<uint64_t>() + 1, 1, final}, P};
         uint64_t nnew = 0;
-        if ((rc = count_offsets(nnodes, &nnew)) != YAMS_OK) return rc;
+        if ((rc = select_cuts(B, &nnew)) != YAMS_OK) return rc;
         { const double t0 = now_ms();
           if ((rc = descs.reserve((size_t)(ndescs + nnew + 1) * sizeof(yams_chunk_desc), true, st)) != YAMS_OK)
             return rc;
           host_alloc += now_ms() - t0; }
-        cdc_emit_kernel<<<tgrid, 256, 0, st>>>(S, next.as<uint32_t>(), forced.as<uint32_t>(),
-                                               onchain.as<uint8_t>(), emit_offsets.as<uint32_t>(),
-                                               descs.as<yams_chunk_desc>(), ndescs, d_sc + 1);
-        YB_CUDA(cudaGetLastError());
+        if ((rc = emit_cuts(B, descs.as<yams_chunk_desc>() + ndescs)) != YAMS_OK) return rc;
         YB_CUDA(cudaMemcpyAsync((void*)(h_sc + 1), d_sc + 1, 8, cudaMemcpyDeviceToHost, st));
         YB_CUDA(cudaEventRecord(ev[2], st));
         YB_CUDA(cudaStreamSynchronize(st));
@@ -535,7 +544,6 @@ static yams_status_t run_batch_group(IngestRes& r, const uint8_t* const* files, 
     if ((rc = r.stage[0].reserve((size_t)L + 256)) != YAMS_OK) return rc;
     uint8_t* d_buf = r.stage[0].as<uint8_t>();
     if ((rc = r.fileinfo.reserve((size_t)nf * 16)) != YAMS_OK) return rc;
-    if ((rc = r.roots.reserve((size_t)nf * 4)) != YAMS_OK) return rc;
     if ((rc = r.first.reserve(((size_t)nf + 1) * 8)) != YAMS_OK) return rc;
     YB_CUDA(cudaEventRecord(r.call[0], st));
     // the whole buffer is uploaded, file bytes and zero gaps alike
@@ -547,32 +555,18 @@ static yams_status_t run_batch_group(IngestRes& r, const uint8_t* const* files, 
     YB_CUDA(cudaEventRecord(r.ev[1], st));
     // ---- selection over the merged node table ----
     YB_ARG((uint64_t)ncand + nf < 0xFFFFFFF0ull, "too many nodes in one batch group");
-    const uint32_t nnodes = ncand + nf;
-    if ((rc = r.npos.reserve((size_t)nnodes * 8)) != YAMS_OK) return rc;
-    if ((rc = r.nref.reserve((size_t)nnodes * 4)) != YAMS_OK) return rc;
-    if ((rc = r.reserve_nodes(nnodes)) != YAMS_OK) return rc;
-    uint64_t* d_sc = r.scalars.as<uint64_t>();
-    BatchArgs B{BatchLayout{r.cand.as<uint64_t>(), ncand, r.fileinfo.as<uint64_t>(), r.fileinfo.as<uint64_t>() + nf, nf}, r.P};
-    const uint32_t tgrid = (nnodes + 255) / 256;
-    batch_nodes_kernel<<<tgrid, 256, 0, st>>>(B, r.npos.as<uint64_t>(), r.nref.as<uint32_t>(), r.roots.as<uint32_t>());
-    batch_next_kernel<<<tgrid, 256, 0, st>>>(B, r.npos.as<uint64_t>(), r.nref.as<uint32_t>(), r.roots.as<uint32_t>(), nnodes,
-                                             r.next.as<uint32_t>(), r.forced.as<uint32_t>(), r.emit_counts.as<uint32_t>());
-    if ((rc = r.mark_chain(nnodes)) != YAMS_OK) return rc;
-    batch_mask_counts_kernel<<<tgrid, 256, 0, st>>>(r.onchain.as<uint8_t>(), r.emit_counts.as<uint32_t>(), nnodes);
+    const BatchArgs B{BatchLayout{r.cand.as<uint64_t>(), ncand, r.fileinfo.as<uint64_t>(), r.fileinfo.as<uint64_t>() + nf, nf, true}, r.P};
     uint64_t nnew = 0;
-    if ((rc = r.count_offsets(nnodes, &nnew)) != YAMS_OK) return rc;
+    if ((rc = r.select_cuts(B, &nnew)) != YAMS_OK) return rc;
     YB_ARG(nnew < 0xFFFFFFFFull, "too many chunks in one batch group");
     if ((rc = r.descs.reserve((size_t)(nnew + 1) * sizeof(yams_chunk_desc))) != YAMS_OK) return rc;
-    batch_emit_kernel<<<tgrid, 256, 0, st>>>(B, r.npos.as<uint64_t>(), r.next.as<uint32_t>(), r.forced.as<uint32_t>(),
-                                             r.onchain.as<uint8_t>(), r.emit_offsets.as<uint32_t>(), nnodes,
-                                             r.descs.as<yams_chunk_desc>());
-    batch_first_kernel<<<(nf + 1 + 255) / 256, 256, 0, st>>>(r.roots.as<uint32_t>(), r.emit_offsets.as<uint32_t>(), nf, d_sc + 0,
+    if ((rc = r.emit_cuts(B, r.descs.as<yams_chunk_desc>())) != YAMS_OK) return rc;
+    batch_first_kernel<<<(nf + 1 + 255) / 256, 256, 0, st>>>(B, r.emit_offsets.as<uint32_t>(), r.scalars.as<uint64_t>(),
                                                              r.first.as<uint64_t>());
     YB_CUDA(cudaEventRecord(r.ev[2], st));
     if ((rc = r.hash(d_buf, 0, 0, nnew, L)) != YAMS_OK) return rc;
     YB_CUDA(cudaEventRecord(r.ev[3], st));
-    if (nnew) batch_rebase_kernel<<<(unsigned)((nnew + 255) / 256), 256, 0, st>>>(r.descs.as<yams_chunk_desc>(), nnew,
-                                                                               r.fileinfo.as<uint64_t>(), nf);
+    if (nnew) batch_rebase_kernel<<<(unsigned)((nnew + 255) / 256), 256, 0, st>>>(B, r.descs.as<yams_chunk_desc>(), nnew);
     YB_CUDA(cudaGetLastError());
     const size_t base = out.size();
     out.resize(base + (size_t)nnew);

@@ -16,7 +16,6 @@
 // big-endian word order are both absorbed by ONE prmt per message word.
 // The kernel is INT32-ALU bound (~22 instr/byte), not HBM bound (SURVEY.md §8d).
 #include <algorithm>
-#include <stdlib.h>
 
 #include "common.cuh"
 
@@ -39,15 +38,13 @@ __device__ __constant__ uint32_t kSha256K[64] = {
 
 __device__ __forceinline__ uint32_t rotr(uint32_t x, int n) { return __funnelshift_r(x, x, n); }
 
-// MADD: with `one` an opaque runtime 1, x * one + y compiles to IMAD, which runs on the FMA pipe and takes
+// With `one` an opaque runtime 1, x * one + y compiles to IMAD, which runs on the FMA pipe and takes
 // the additions off the INT32 ALU pipe where the SHF/LOP3 of the round function already saturate issue
 // (DESIGN.md §sha256: ALU-pipe instructions per block drop from ~1330 to ~1030).
-template <bool MADD>
 __device__ __forceinline__ uint32_t add2(uint32_t x, uint32_t y, uint32_t one) {
-    return MADD ? x * one + y : x + y;
+    return x * one + y;
 }
 
-template <bool MADD>
 __device__ __forceinline__ void sha256_compress(uint32_t (&st)[8], uint32_t (&w)[16], uint32_t one) {
     uint32_t a = st[0], b = st[1], c = st[2], d = st[3], e = st[4], f = st[5], g = st[6], h = st[7];
 #pragma unroll
@@ -56,23 +53,24 @@ __device__ __forceinline__ void sha256_compress(uint32_t (&st)[8], uint32_t (&w)
             uint32_t w15 = w[(i - 15) & 15], w2 = w[(i - 2) & 15];
             uint32_t s0 = rotr(w15, 7) ^ rotr(w15, 18) ^ (w15 >> 3);
             uint32_t s1 = rotr(w2, 17) ^ rotr(w2, 19) ^ (w2 >> 10);
-            w[i & 15] = add2<MADD>(add2<MADD>(add2<MADD>(w[i & 15], s0, one), w[(i - 7) & 15], one), s1, one);
+            w[i & 15] = add2(add2(add2(w[i & 15], s0, one), w[(i - 7) & 15], one), s1, one);
         }
         uint32_t S1 = rotr(e, 6) ^ rotr(e, 11) ^ rotr(e, 25);
         uint32_t ch = (e & f) ^ (~e & g);
-        uint32_t kw = add2<MADD>(w[i & 15], kSha256K[i], one);
-        uint32_t t1 = add2<MADD>(add2<MADD>(add2<MADD>(h, S1, one), ch, one), kw, one);
+        uint32_t kw = add2(w[i & 15], kSha256K[i], one);
+        uint32_t t1 = add2(add2(add2(h, S1, one), ch, one), kw, one);
         uint32_t S0 = rotr(a, 2) ^ rotr(a, 13) ^ rotr(a, 22);
         uint32_t mj = (a & b) ^ (a & c) ^ (b & c);
-        uint32_t t2 = add2<MADD>(S0, mj, one);
-        h = g; g = f; f = e; e = add2<MADD>(d, t1, one); d = c; c = b; b = a; a = add2<MADD>(t1, t2, one);
+        uint32_t t2 = add2(S0, mj, one);
+        h = g; g = f; f = e; e = add2(d, t1, one); d = c; c = b; b = a; a = add2(t1, t2, one);
     }
     st[0] += a; st[1] += b; st[2] += c; st[3] += d; st[4] += e; st[5] += f; st[6] += g; st[7] += h;
 }
 
+constexpr int kShaCtasPerSm = 4;   // resident CTAs per SM: the register budget of the launch bounds and the grid's cap
+
 // data[0] is stream position base_pos; desc.offset is a stream position.
-template <bool MADD, int MINB>
-__global__ void __launch_bounds__(kShaWarpsPerCta * 32, MINB)
+__global__ void __launch_bounds__(kShaWarpsPerCta * 32, kShaCtasPerSm)
 sha256_chunks_kernel(const uint8_t* __restrict__ data, uint64_t base_pos,
                      yams_chunk_desc* __restrict__ descs, uint32_t first, uint32_t n,
                      unsigned int* __restrict__ counter, uint32_t one, const uint32_t* __restrict__ order) {
@@ -184,7 +182,7 @@ sha256_chunks_kernel(const uint8_t* __restrict__ data, uint64_t base_pos,
                         }
                     }
                 }
-                sha256_compress<MADD>(st, w, one);
+                sha256_compress(st, w, one);
                 if (done) {
                     uint4 lo, hi;
                     lo.x = __byte_perm(st[0], 0, 0x0123); lo.y = __byte_perm(st[1], 0, 0x0123);
@@ -262,9 +260,8 @@ yams_status_t launch_sha256_chunks(const uint8_t* d_data, uint64_t base_pos, yam
     if (n == 0) return YAMS_OK;
     YB_CUDA(cudaMemsetAsync(d_counter, 0, sizeof(unsigned int), st));
     // d_order_ws: 64 counters + n indices (sha256_order_ws_bytes); tables that leave every lane under ~2 chunks are not worth it
-    static const int lpt = [] { const char* e = getenv("YAMS_B200_SHA_ORDER"); return e ? atoi(e) : 1; }();
     const uint32_t* d_order = nullptr;
-    if (lpt && n >= 4096) {
+    if (n >= 4096) {
         const uint64_t mean = std::max<uint64_t>(1, total_bytes / n);
         YB_CUDA(cudaMemsetAsync(d_order_ws, 0, 64 * sizeof(uint32_t), st));
         const unsigned g = (unsigned)std::min<uint32_t>((n + 255) / 256, (uint32_t)sm_count * 8u);
@@ -272,24 +269,11 @@ yams_status_t launch_sha256_chunks(const uint8_t* d_data, uint64_t base_pos, yam
         sha_order_scatter_kernel<<<g, 256, 0, st>>>(d_descs, first, n, mean, d_order_ws, d_order_ws + 32, d_order_ws + 64);
         d_order = d_order_ws + 64;
     }
-    static const int madd = [] { const char* e = getenv("YAMS_B200_SHA_MADD"); return e ? atoi(e) : 1; }();
-    // per_sm picks the register budget the kernel was compiled for (launch bounds 128 x per_sm)
-    static const int per_sm = [] { const char* e = getenv("YAMS_B200_SHA_CTAS"); int v = e ? atoi(e) : 4; return v < 3 ? 3 : (v > 6 ? 6 : v); }();
-    // experiment knob: grid CTAs per SM independent of the occupancy variant (co-residency with the candidate scan); fewer
-    // than the variant allows leaves registers for a co-resident kernel
-    static const int env_grid = [] { const char* e = getenv("YAMS_B200_SHA_GRID"); return e ? atoi(e) : 0; }();
-    const int grid = env_grid > 0 ? env_grid : per_sm;
     uint32_t warps_needed = (n + 31) / 32;
     uint32_t ctas = (warps_needed + kShaWarpsPerCta - 1) / kShaWarpsPerCta;
-    uint32_t max_ctas = (uint32_t)sm_count * (uint32_t)grid;
+    uint32_t max_ctas = (uint32_t)sm_count * (uint32_t)kShaCtasPerSm;
     if (ctas > max_ctas) ctas = max_ctas;
-#define YB_SHA(M, B) sha256_chunks_kernel<M, B><<<ctas, kShaWarpsPerCta * 32, 0, st>>>(d_data, base_pos, d_descs, first, n, d_counter, 1u, d_order)
-    if (madd) {
-        switch (per_sm) { case 3: YB_SHA(true, 3); break; case 4: YB_SHA(true, 4); break; case 5: YB_SHA(true, 5); break; default: YB_SHA(true, 6); break; }
-    } else {
-        YB_SHA(false, 4);
-    }
-#undef YB_SHA
+    sha256_chunks_kernel<<<ctas, kShaWarpsPerCta * 32, 0, st>>>(d_data, base_pos, d_descs, first, n, d_counter, 1u, d_order);
     YB_CUDA(cudaGetLastError());
     return YAMS_OK;
 }
