@@ -335,7 +335,7 @@ YAMS_B200_API void yams_b200_corpus_destroy(yams_b200_corpus* c);
  * allowed_rowids[allowed_offsets[i] .. allowed_offsets[i+1]) (ascending) -- CandidateFilterMode::
  * Exact (src/vector/vector_database.cpp:570-597). allowed_offsets has Q+1 entries.
  * Outputs (caller-owned HOST): out_rowids/out_scores Q x k (unused slots: rowid -1, score 0),
- * out_counts Q, out_flags Q (nullable). * k <= 3072 (cosine) / 4096 (L2). */
+ * out_counts Q, out_flags Q (nullable). * k <= 3072. */
 YAMS_B200_API yams_status_t yams_b200_search(yams_b200_corpus* c, const float* queries, uint32_t nq,
                                              uint32_t k, float threshold,
                                              const int64_t* allowed_rowids,
@@ -355,7 +355,7 @@ YAMS_B200_API yams_status_t yams_b200_search_all_matching(yams_b200_corpus* c, c
 /* Device-pointer form for multi-GPU sharding: queries and outputs are DEVICE pointers, the whole pipeline is enqueued on
  * the corpus stream and the call returns WITHOUT synchronising (query validity, list overflow and the exactness
  * certificate are evaluated on the device and parked in a status block).  Outputs are the rank-local partial top-k in
- * the padded Q x k layout (unused: score -inf / +inf(l2), rowid -1).
+ * the padded Q x k layout (unused: score -inf / +inf(l2), rowid -1).  k <= 768.
  * yams_b200_search_device_finish waits for the stream, returns YAMS_ERR_INVALID_ARG if a query was non-finite / zero,
  * and re-runs the queries the certificate rejected through the exhaustive levels, patching the device outputs in place
  * (*out_resolved = how many; 0 for ordinary data).  A caller that pipelines batches calls it before it consumes the
@@ -522,11 +522,12 @@ YAMS_B200_API yams_status_t yams_b200_simeon_encode(yams_b200_encoder* e, const 
                                                     size_t n, float* out);
 YAMS_B200_API void yams_b200_simeon_destroy(yams_b200_encoder* e);
 
-/* [0] stage-1 scan ms, [1] rescoring+select ms, [2] total device ms, [3] h2d+d2h ms of the last
- * yams_b200_search on this corpus; [4] = which stage-1 kernel ran (0 cuda-core, 1 wgmma);
+/* [0] stage-1 scan ms, [1] rescoring+select ms, [2] total device ms of the last yams_b200_search or
+ * yams_b200_search_device on this corpus (the latter's once its work is done); [3] unused (0);
+ * [4] = which stage-1 kernel ran (0 cuda-core, 1 wgmma);
  * [5] = duration of the full-corpus filtered scan launch alone (the dominant kernel);
  * [6] = queries of that call the certificate sent to the exhaustive levels, [7] = of those, the queries level 1 could not
- * certify either, answered by the full exact pass */
+ * certify either, answered by the full exact pass ([6] and [7] of a search_device: set by yams_b200_search_device_finish) */
 YAMS_B200_API yams_status_t yams_b200_search_last_timings(yams_b200_corpus* c, float out_ms[8]);
 
 typedef struct yams_vector_scan_v1 {

@@ -1188,24 +1188,6 @@ static yams_status_t corpus_finish_append(Corpus* c, uint64_t n_new, const int64
     return YAMS_OK;
 }
 
-// Small candidate sets (CandidateFilterMode::Exact): device lists (ascending rowids, d_offsets[nq+1]) short enough that
-// scoring the listed rows one by one is cheaper than a corpus pass -> gather_score_kernel
-struct DirectLists {
-    const int64_t* d_allowed = nullptr;
-    const uint64_t* d_offsets = nullptr;
-    uint64_t total = 0;
-    uint32_t max_len = 0;
-};
-
-struct ScanPlan {
-    uint32_t nq = 0, k = 0;
-    float threshold = -1.f;
-    const uint32_t* d_mask = nullptr;   // bit matrix [nq][mask_ld*32] of allowed rows -> masked corpus pass
-    uint64_t mask_ld = 0;
-    const DirectLists* direct = nullptr;
-    bool use_tensor = false;
-};
-
 // stage 1 of the direct path: cands[q * cap + j] = (score, row) of list entry j (cap >= the longest list)
 static yams_status_t gather_scores(Corpus* c, const DirectLists& L, uint32_t nq, const float* q32, const float* qinv, Cand* cands,
                                    uint32_t cap, cudaStream_t st) {
@@ -1226,8 +1208,64 @@ static ScanStatus* status_of(Corpus* c) { return c->status.as<ScanStatus>(); }
 
 // the CUDA-core engine's stage-1 error bound of the nq prepared queries -> dst[nq] (keep_larger: the max with dst's values)
 static void launch_eps_cc(Corpus* c, uint32_t nq, float* dst, bool keep_larger) {
-    eps_cc_kernel<<<(nq + 255) / 256, 256, 0, c->st>>>(reinterpret_cast<const double*>(c->misc.as<uint8_t>()), nq, c->dim, c->metric,
-                                                       c->r_max, dst, keep_larger ? 1 : 0);
+    eps_cc_kernel<<<(nq + 255) / 256, 256, 0, c->st>>>(c->qnorm.as<double>(), nq, c->dim, c->metric, c->r_max, dst, keep_larger ? 1 : 0);
+}
+
+// The stage-1 engine of a search (tensor = wgmma_supported, fall_back) or of a diagnostic call (one engine forced).  The
+// wgmma engine prepares its operand-typed queries on its first run of the call; with fall_back, a shape it declines goes to
+// the CUDA-core engine.
+struct Stage1Engine {
+    Corpus* c;
+    bool tensor, fall_back;
+    bool qprep_done = false, tensor_used = false, cc_used = false;
+    yams_status_t run(Stage1Args a, bool filter, unsigned long long* prof = nullptr) {
+        if (tensor) {
+            a.skip_qprep = qprep_done;
+            yams_status_t r = stage1_wgmma(c, a, filter, c->st, prof);
+            if (r == YAMS_OK) qprep_done = tensor_used = true;
+            if (r != YAMS_ERR_UNSUPPORTED || !fall_back) return r;
+        }
+        cc_used = true;
+        return stage1_cuda_core(a, filter, c->st);
+    }
+    // eps[] of the engine(s) that ran: the CUDA-core bound (also that of the direct path's gathered fp32 dot products),
+    // max-combined with the wgmma engine's when both ran
+    void launch_eps(uint32_t nq) {
+        if (cc_used || !tensor_used) launch_eps_cc(c, nq, c->eps.as<float>(), tensor_used);
+    }
+};
+
+// the certificate of stage 2 (final_kernel) in the corpus's metric; failures are queued in the status block (level 0: bad[],
+// level 1: bad2[])
+static CertArgs cert_args(Corpus* c, const float* bound, const float* eps, float threshold, int level, uint32_t nq_total) {
+    CertArgs cert{};
+    cert.bound = bound; cert.eps = eps; cert.qnorm = c->qnorm.as<double>(); cert.threshold = threshold;
+    cert.metric = c->metric; cert.l2_margin = l2_cert_margin(c->dim); cert.status = status_of(c); cert.level = level;
+    cert.nq_total = nq_total;
+    return cert;
+}
+
+// final_kernel over `grid` CTAs in the result convention of cert.metric (L2: distances = negated scores, padding +inf)
+static void launch_final(const Exact* ex, const uint32_t* ex_n, uint32_t Kp, uint32_t k, const int64_t* rowids, const DeviceResults& out,
+                         uint32_t grid, const uint32_t* qmap, const CertArgs& cert, cudaStream_t st) {
+    const bool l2 = cert.metric == YAMS_B200_L2;
+    final_kernel<<<grid, SEL_THREADS, 0, st>>>(ex, ex_n, Kp, k, rowids, l2 ? 1 : 0, out.rowids, out.scores, out.counts, out.flags,
+                                               l2 ? INFINITY : -INFINITY, qmap, cert);
+}
+
+// Stage 2 of `grid` queries (CTA b serves query qmap[b], or b): exact re-scoring of the Kp survivors of each (sel, sel_n) into
+// ex, ordering, the k results into p.out and the certificate of `level` against bound[b] and eps[query].  Level 1 hands its
+// survivor counts to final_kernel; level 0 orders all Kp entries (rescore_kernel marks the missing ones skipped).
+static yams_status_t rescore_and_certify(Corpus* c, const ScanPlan& p, const Cand* sel, const uint32_t* sel_n, uint32_t Kp, uint32_t grid,
+                                         const uint32_t* qmap, Exact* ex, const float* bound, const float* eps, int level) {
+    const uint64_t tot = (uint64_t)grid * Kp;
+    rescore_kernel<<<(unsigned)((tot + 127) / 128), 128, 0, c->st>>>(c->rows.p, c->dtype, c->dim, c->q32.as<float>(), c->qnorm.as<double>(),
+                                                                     sel, sel_n, Kp, grid, p.threshold, ex, c->metric, qmap, p.d_mask,
+                                                                     p.mask_ld);
+    launch_final(ex, level ? sel_n : nullptr, Kp, p.k, c->rowids.as<int64_t>(), p.out, grid, qmap,
+                 cert_args(c, bound, eps, p.threshold, level, p.nq), c->st);
+    YB_CUDA(cudaGetLastError());
+    return YAMS_OK;
 }
 
 static void fill_stage1_common(Corpus* c, Stage1Args& a, uint32_t nq) {
@@ -1247,36 +1285,23 @@ static void fill_stage1_common(Corpus* c, Stage1Args& a, uint32_t nq) {
 }
 
 // Enqueues the whole pipeline for the nq queries already prepared on the device (prepare_queries) and writes the padded
-// [nq][k] result into device buffers.  NO host synchronisation: list overflow, short lists and stage-1 rounding are all
-// caught by the certificate in final_kernel, which queues such queries in the ScanStatus block for resolve_uncertain().
-static yams_status_t scan_enqueue(Corpus* c, const ScanPlan& p, int64_t* d_out_rowids, float* d_out_scores, uint32_t* d_out_counts,
-                                  uint64_t* d_out_flags) {
+// [nq][k] result into p.out.  NO host synchronisation: list overflow, short lists and stage-1 rounding are all caught by
+// the certificate in final_kernel, which queues such queries in the ScanStatus block for resolve_uncertain().
+static yams_status_t scan_enqueue(Corpus* c, const ScanPlan& p) {
     yams_status_t rc;
     cudaStream_t st = c->st;
-    const uint32_t nq = p.nq, k = p.k;
-    const uint32_t Kp = survivors_for(k);
+    const uint32_t nq = p.nq;
+    const uint32_t Kp = survivors_for(p.k);
     const uint64_t n = c->n;
     const bool l2 = c->metric == YAMS_B200_L2;
     c->scan_timed = false;
-    double* d_qnorm = reinterpret_cast<double*>(c->misc.as<uint8_t>());           // nq doubles
     uint32_t* d_counts = c->counts.as<uint32_t>();
-    Stage1Args a{};
-    fill_stage1_common(c, a, nq);
-    bool qprep_done = false, tensor_used = false, cc_used = false;
-    auto run_stage1 = [&](Stage1Args args, bool filter) -> yams_status_t {
-        if (p.use_tensor) {
-            args.skip_qprep = qprep_done;
-            yams_status_t r = stage1_wgmma(c, args, filter, st);
-            if (r == YAMS_OK) { qprep_done = true; tensor_used = true; }
-            if (r != YAMS_ERR_UNSUPPORTED) return r;
-        }
-        cc_used = true;
-        return stage1_cuda_core(args, filter, st);
-    };
     if ((rc = c->sel.reserve((size_t)nq * Kp * sizeof(Cand) + (size_t)nq * 4)) != YAMS_OK) return rc;
     if ((rc = c->bound.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
     if ((rc = c->eps.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
-    a.eps = c->eps.as<float>();
+    Stage1Args a{};
+    fill_stage1_common(c, a, nq);
+    Stage1Engine s1{c, wgmma_supported(c, nq), true};
     Cand* d_sel = c->sel.as<Cand>();
     uint32_t* d_sel_n = reinterpret_cast<uint32_t*>(d_sel + (size_t)nq * Kp);
     float* d_bound = c->bound.as<float>();
@@ -1286,17 +1311,15 @@ static yams_status_t scan_enqueue(Corpus* c, const ScanPlan& p, int64_t* d_out_r
         // nothing to score: every list is empty, bound = -inf
     } else if (p.direct) {
         // ---- small candidate sets: score the listed rows only ----
-        const DirectLists* direct = p.direct;
-        const uint32_t cap = std::max<uint32_t>(direct->max_len, 1);
+        const uint32_t cap = std::max<uint32_t>(p.lists.max_len, 1);
         if ((rc = c->cands.reserve((size_t)nq * cap * sizeof(Cand))) != YAMS_OK) return rc;
-        list_lengths_kernel<<<(nq + 255) / 256, 256, 0, st>>>(direct->d_offsets, nq, d_counts);
-        if (direct->total) YB_CUDA(cudaEventRecord(c->ev_scan[0], st));
-        if ((rc = gather_scores(c, *direct, nq, a.q32, a.qinv, c->cands.as<Cand>(), cap, st)) != YAMS_OK) return rc;
-        if (direct->total) {
+        list_lengths_kernel<<<(nq + 255) / 256, 256, 0, st>>>(p.lists.d_offsets, nq, d_counts);
+        if (p.lists.total) YB_CUDA(cudaEventRecord(c->ev_scan[0], st));
+        if ((rc = gather_scores(c, p.lists, nq, a.q32, a.qinv, c->cands.as<Cand>(), cap, st)) != YAMS_OK) return rc;
+        if (p.lists.total) {
             YB_CUDA(cudaEventRecord(c->ev_scan[1], st));
             c->scan_timed = true;
         }
-        cc_used = true;   // fp32 CUDA-core dot products: same error bound as the CUDA-core engine
         SelectIn in{};
         in.cands = c->cands.as<Cand>(); in.counts = d_counts; in.cap = cap;
         topk_select_kernel<<<nq, SEL_THREADS, 0, st>>>(in, Kp, 0, nullptr, d_sel, d_sel_n, d_bound);
@@ -1305,7 +1328,7 @@ static yams_status_t scan_enqueue(Corpus* c, const ScanPlan& p, int64_t* d_out_r
         if ((rc = c->dense.reserve((size_t)nq * n * 4)) != YAMS_OK) return rc;
         a.row_start = 0; a.row_stride = 1; a.nrows = n;
         a.out_scores = c->dense.as<float>(); a.ld = n;
-        if ((rc = run_stage1(a, false)) != YAMS_OK) return rc;
+        if ((rc = s1.run(a, false)) != YAMS_OK) return rc;
         SelectIn in{};
         in.dense = c->dense.as<float>(); in.ld = n; in.row_start = 0; in.row_stride = 1; in.dense_len = n;
         topk_select_kernel<<<nq, SEL_THREADS, 0, st>>>(in, Kp, 0, nullptr, d_sel, d_sel_n, d_bound);
@@ -1323,10 +1346,10 @@ static yams_status_t scan_enqueue(Corpus* c, const ScanPlan& p, int64_t* d_out_r
             uint64_t expected = (uint64_t)m * stride;
             cap = (uint32_t)std::max<uint64_t>(kCandCap, ((3 * expected + 1023) / 1024) * 1024);
             if ((rc = c->sample_scores.reserve((size_t)nq * S * 4)) != YAMS_OK) return rc;
-            Stage1Args s1 = a;
-            s1.row_start = 0; s1.row_stride = stride; s1.nrows = S;
-            s1.out_scores = c->sample_scores.as<float>(); s1.ld = S;
-            if ((rc = run_stage1(s1, false)) != YAMS_OK) return rc;
+            Stage1Args s = a;
+            s.row_start = 0; s.row_stride = stride; s.nrows = S;
+            s.out_scores = c->sample_scores.as<float>(); s.ld = S;
+            if ((rc = s1.run(s, false)) != YAMS_OK) return rc;
             if (p.d_mask)
                 mask_scores_kernel<<<dim3((unsigned)((S + 255) / 256), nq), 256, 0, st>>>(c->sample_scores.as<float>(), S, S, stride,
                                                                                          p.d_mask, p.mask_ld, nullptr);
@@ -1342,31 +1365,19 @@ static yams_status_t scan_enqueue(Corpus* c, const ScanPlan& p, int64_t* d_out_r
         f.tau = d_tau; f.cands = c->cands.as<Cand>(); f.cap = cap; f.counts = d_counts;
         f.mask = p.d_mask; f.mask_ld = p.mask_ld;
         YB_CUDA(cudaEventRecord(c->ev_scan[0], st));
-        if ((rc = run_stage1(f, true)) != YAMS_OK) return rc;
+        if ((rc = s1.run(f, true)) != YAMS_OK) return rc;
         YB_CUDA(cudaEventRecord(c->ev_scan[1], st));
         c->scan_timed = true;
         SelectIn in{};
         in.cands = c->cands.as<Cand>(); in.counts = d_counts; in.cap = cap; in.tau = d_tau;
         topk_select_kernel<<<nq, SEL_THREADS, 0, st>>>(in, Kp, 0, nullptr, d_sel, d_sel_n, d_bound);
     }
-    // error bound of the engine(s) that produced the ranking
-    if (cc_used || !tensor_used)
-        launch_eps_cc(c, nq, c->eps.as<float>(), tensor_used);
-    c->last_ms[4] = tensor_used ? 1.f : 0.f;   // the engine that ran: wgmma declines shapes it does not take (nq > 4096)
+    s1.launch_eps(nq);
+    c->last_ms[4] = s1.tensor_used ? 1.f : 0.f;   // the engine that ran: wgmma declines shapes it does not take (nq > 4096)
     YB_CUDA(cudaEventRecord(c->ev[1], st));
     // ---- stage 2: exact re-scoring, ordering, certificate ----
     if ((rc = c->outbuf.reserve((size_t)nq * Kp * sizeof(Exact))) != YAMS_OK) return rc;
-    Exact* d_ex = c->outbuf.as<Exact>();
-    uint64_t tot = (uint64_t)nq * Kp;
-    rescore_kernel<<<(unsigned)((tot + 127) / 128), 128, 0, st>>>(c->rows.p, c->dtype, c->dim, a.q32, d_qnorm, d_sel, d_sel_n, Kp, nq,
-                                                                  p.threshold, d_ex, c->metric, nullptr, p.d_mask, p.mask_ld);
-    CertArgs cert{};
-    cert.bound = d_bound; cert.eps = c->eps.as<float>(); cert.qnorm = d_qnorm; cert.threshold = p.threshold;
-    cert.metric = c->metric; cert.l2_margin = l2_cert_margin(c->dim); cert.status = status_of(c); cert.level = 0; cert.nq_total = nq;
-    final_kernel<<<nq, SEL_THREADS, 0, st>>>(d_ex, nullptr, Kp, k, c->rowids.as<int64_t>(), l2 ? 1 : 0, d_out_rowids, d_out_scores,
-                                             d_out_counts, d_out_flags, l2 ? INFINITY : -INFINITY, nullptr, cert);
-    YB_CUDA(cudaGetLastError());
-    return YAMS_OK;
+    return rescore_and_certify(c, p, d_sel, d_sel_n, Kp, nq, nullptr, c->outbuf.as<Exact>(), d_bound, c->eps.as<float>(), 0);
 }
 
 // entry points for the other engines (pq.cu): exact top-K of per-query candidate lists, and the plain final ordering
@@ -1376,11 +1387,10 @@ void launch_topk_lists(const Cand* lists, const uint32_t* counts, uint32_t cap, 
     in.cands = lists; in.counts = counts; in.cap = cap;
     topk_select_kernel<<<nq, SEL_THREADS, 0, st>>>(in, K, 0, nullptr, out_sel, out_n, nullptr);
 }
-void launch_final_plain(const Exact* exact, uint32_t Kp, uint32_t k, uint32_t nq, const int64_t* rowids, int64_t* out_rowids, float* out_scores,
-                        uint32_t* out_counts, uint64_t* out_flags, cudaStream_t st) {
-    CertArgs cert{};   // status == nullptr: no certificate (the caller's survivors are what the reference re-ranks, too)
-    final_kernel<<<nq, SEL_THREADS, 0, st>>>(exact, nullptr, Kp, k, rowids, 0, out_rowids, out_scores, out_counts, out_flags, -INFINITY, nullptr,
-                                             cert);
+void launch_final_plain(const Exact* exact, uint32_t Kp, uint32_t k, uint32_t nq, const int64_t* rowids, const DeviceResults& out,
+                        cudaStream_t st) {
+    // status == nullptr: no certificate (the caller's survivors are what the reference re-ranks, too); cosine results
+    launch_final(exact, nullptr, Kp, k, rowids, out, nq, nullptr, CertArgs{}, st);
 }
 // rowids -> corpus rows (out[i].row, 0xFFFFFFFF for unknown rowids), any order
 void launch_map_rowids(const int64_t* rowids_in, uint64_t n_in, const int64_t* corpus_rowids, uint64_t n, Cand* out, cudaStream_t st) {
@@ -1441,8 +1451,7 @@ static yams_status_t exact_sorted_keys(Corpus* c, uint32_t q, uint64_t m, const 
     if (m) {
         if (d_allowed) map_rowids_kernel<<<g, 256, 0, st>>>(d_allowed, m, c->rowids.as<int64_t>(), c->n, d_sel);
         else iota_sel_kernel<<<g, 256, 0, st>>>(d_sel, m);
-        rescore_kernel<<<(unsigned)((m + 127) / 128), 128, 0, st>>>(c->rows.p, c->dtype, c->dim, c->q32.as<float>(),
-                                                                   reinterpret_cast<double*>(c->misc.as<uint8_t>()), d_sel, d_small,
+        rescore_kernel<<<(unsigned)((m + 127) / 128), 128, 0, st>>>(c->rows.p, c->dtype, c->dim, c->q32.as<float>(), c->qnorm.as<double>(), d_sel, d_small,
                                                                    (uint32_t)m, 1, threshold, c->outbuf.as<Exact>(), c->metric, d_small + 1,
                                                                    mask, mask_ld);
     }
@@ -1453,14 +1462,13 @@ static yams_status_t exact_sorted_keys(Corpus* c, uint32_t q, uint64_t m, const 
 }
 
 // Level 2: exact score of EVERY row for one query (the reference's own loop, row-parallel) + a global sort.
-static yams_status_t exact_all_rows(Corpus* c, const ScanPlan& p, uint32_t q, int64_t* d_out_rowids, float* d_out_scores,
-                                    uint32_t* d_out_counts, uint64_t* d_out_flags) {
+static yams_status_t exact_all_rows(Corpus* c, const ScanPlan& p, uint32_t q) {
     yams_status_t rc;
     cudaStream_t st = c->st;
     const bool l2 = c->metric == YAMS_B200_L2;
     if ((rc = exact_sorted_keys(c, q, c->n, nullptr, p.threshold, p.d_mask, p.mask_ld)) != YAMS_OK) return rc;
     emit_sorted_kernel<<<(p.k + 255) / 256, 256, 0, st>>>(c->dense.as<uint64_t>(), c->n, p.k, q, c->rowids.as<int64_t>(), l2 ? 1 : 0,
-                                                          l2 ? INFINITY : -INFINITY, d_out_rowids, d_out_scores, d_out_counts, d_out_flags);
+                                                          l2 ? INFINITY : -INFINITY, p.out.rowids, p.out.scores, p.out.counts, p.out.flags);
     YB_CUDA(cudaGetLastError());
     YB_CUDA(cudaStreamSynchronize(st));   // h_small / scratch reuse
     return YAMS_OK;
@@ -1471,14 +1479,11 @@ static yams_status_t exact_all_rows(Corpus* c, const ScanPlan& p, uint32_t q, in
 //            best kLevel1K (4096) rows instead of K', same certificate;
 //   level 2: whatever level 1 cannot certify either (more than ~4000 rows within eps of the k-th score: a corpus of
 //            duplicates) is answered by the exact score of every row.
-static yams_status_t resolve_uncertain(Corpus* c, const ScanPlan& p, const uint32_t* bad, uint32_t n_bad, int64_t* d_out_rowids,
-                                       float* d_out_scores, uint32_t* d_out_counts, uint64_t* d_out_flags, uint32_t* out_full) {
+static yams_status_t resolve_uncertain(Corpus* c, const ScanPlan& p, const uint32_t* bad, uint32_t n_bad, uint32_t* out_full) {
     yams_status_t rc;
     cudaStream_t st = c->st;
     const uint64_t n = c->n;
-    const uint32_t k = p.k, G = kLevel1Group, K1 = kLevel1K;
-    const bool l2 = c->metric == YAMS_B200_L2;
-    if (n_bad == 0) return YAMS_OK;
+    const uint32_t G = kLevel1Group, K1 = kLevel1K;
     if ((rc = c->dense.reserve((size_t)G * n * 4 + (size_t)G * c->dim * 4 + (size_t)G * 8 + 64)) != YAMS_OK) return rc;
     if ((rc = c->lvl.reserve((size_t)G * K1 * (sizeof(Cand) + sizeof(Exact)) + (size_t)G * 16 + 64)) != YAMS_OK) return rc;
     if ((rc = c->eps2.reserve((size_t)p.nq * 4)) != YAMS_OK) return rc;
@@ -1490,7 +1495,6 @@ static yams_status_t resolve_uncertain(Corpus* c, const ScanPlan& p, const uint3
     Exact* d_ex1 = reinterpret_cast<Exact*>(d_sel1 + (size_t)G * K1);
     uint32_t* d_sel1_n = reinterpret_cast<uint32_t*>(d_ex1 + (size_t)G * K1);
     float* d_bound1 = reinterpret_cast<float*>(d_sel1_n + G);
-    double* d_qnorm = reinterpret_cast<double*>(c->misc.as<uint8_t>());
     launch_eps_cc(c, p.nq, c->eps2.as<float>(), false);
     Stage1Args a{};
     fill_stage1_common(c, a, p.nq);
@@ -1512,16 +1516,7 @@ static yams_status_t resolve_uncertain(Corpus* c, const ScanPlan& p, const uint3
         SelectIn in{};
         in.dense = d_scores; in.ld = n; in.row_start = 0; in.row_stride = 1; in.dense_len = n;
         topk_select_kernel<<<g, SEL_THREADS, 0, st>>>(in, K1, 0, nullptr, d_sel1, d_sel1_n, d_bound1);
-        uint64_t tot = (uint64_t)g * K1;
-        rescore_kernel<<<(unsigned)((tot + 127) / 128), 128, 0, st>>>(c->rows.p, c->dtype, c->dim, a.q32, d_qnorm, d_sel1, d_sel1_n, K1, g,
-                                                                      p.threshold, d_ex1, c->metric, d_qmap, p.d_mask, p.mask_ld);
-        CertArgs cert{};
-        cert.bound = d_bound1; cert.eps = c->eps2.as<float>(); cert.qnorm = d_qnorm; cert.threshold = p.threshold;
-        cert.metric = c->metric; cert.l2_margin = l2_cert_margin(c->dim); cert.status = status_of(c); cert.level = 1;
-        cert.nq_total = p.nq;
-        final_kernel<<<g, SEL_THREADS, 0, st>>>(d_ex1, d_sel1_n, K1, k, c->rowids.as<int64_t>(), l2 ? 1 : 0, d_out_rowids, d_out_scores,
-                                                d_out_counts, d_out_flags, l2 ? INFINITY : -INFINITY, d_qmap, cert);
-        YB_CUDA(cudaGetLastError());
+        if ((rc = rescore_and_certify(c, p, d_sel1, d_sel1_n, K1, g, d_qmap, d_ex1, d_bound1, c->eps2.as<float>(), 1)) != YAMS_OK) return rc;
         YB_CUDA(cudaStreamSynchronize(st));  // d_qmap / bad reuse
     }
     // level 2 for what is left
@@ -1536,7 +1531,7 @@ static yams_status_t resolve_uncertain(Corpus* c, const ScanPlan& p, const uint3
         YB_CUDA(cudaMemcpyAsync(bad2.data(), d_list2, (size_t)n_bad2 * 4, cudaMemcpyDeviceToHost, st));
         YB_CUDA(cudaStreamSynchronize(st));
         for (uint32_t q : bad2)
-            if ((rc = exact_all_rows(c, p, q, d_out_rowids, d_out_scores, d_out_counts, d_out_flags)) != YAMS_OK) return rc;
+            if ((rc = exact_all_rows(c, p, q)) != YAMS_OK) return rc;
     }
     return YAMS_OK;
 }
@@ -1607,7 +1602,7 @@ void yams_b200_corpus_destroy(yams_b200_corpus* c) {
     if (!c) return;
     if (c->st) cudaStreamSynchronize(c->st);
     for (DevBuf* b : {&c->rows, &c->rowids, &c->inv_norm, &c->q32, &c->q16, &c->qinv, &c->tau, &c->counts, &c->cands,
-                      &c->sample_scores, &c->sel, &c->outbuf, &c->dense, &c->mask, &c->misc, &c->dout, &c->stats, &c->status,
+                      &c->sample_scores, &c->sel, &c->outbuf, &c->dense, &c->mask, &c->misc, &c->qnorm, &c->dout, &c->stats, &c->status,
                       &c->bound, &c->eps, &c->eps2, &c->lvl})
         b->release();
     c->h_pin.release();
@@ -1752,43 +1747,32 @@ yams_status_t yams_b200_corpus_sync(yams_b200_corpus* c) {
 
 void* yams_b200_corpus_stream(yams_b200_corpus* c) { return c ? (void*)c->st : nullptr; }
 
-// uploads the queries and enqueues their preparation: q32, qinv, qnorm (misc) on the device, status block zeroed,
+// uploads the queries and enqueues their preparation: q32, qinv, qnorm on the device, status block zeroed,
 // invalid queries counted in status->n_invalid (read by the host together with the results -- no synchronisation here)
 static yams_status_t prepare_queries(yams_b200_corpus* c, const float* q_src, bool src_is_device, uint32_t nq) {
     yams_status_t rc;
     size_t qb = (size_t)nq * c->dim * 4;
     if ((rc = c->q32.reserve(qb)) != YAMS_OK) return rc;
     if ((rc = c->qinv.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
-    if ((rc = c->misc.reserve((size_t)nq * 8 + (size_t)nq * 4)) != YAMS_OK) return rc;
+    if ((rc = c->qnorm.reserve((size_t)nq * 8)) != YAMS_OK) return rc;
     if ((rc = c->counts.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
     if ((rc = c->status.reserve(sizeof(ScanStatus) + (size_t)nq * 8)) != YAMS_OK) return rc;
     if ((rc = c->h_pin.reserve(sizeof(ScanStatus) + (size_t)nq * 8 + 64)) != YAMS_OK) return rc;
     YB_CUDA(cudaMemsetAsync(c->status.p, 0, sizeof(ScanStatus), c->st));
     YB_CUDA(cudaMemcpyAsync(c->q32.p, q_src, qb, src_is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, c->st));
-    double* d_qnorm = reinterpret_cast<double*>(c->misc.as<uint8_t>());
-    query_prep_kernel<<<(nq + QP_THREADS - 1) / QP_THREADS, QP_THREADS, 0, c->st>>>(c->q32.as<float>(), nq, c->dim, d_qnorm, c->qinv.as<float>(), c->metric,
-                                                        status_of(c));
+    query_prep_kernel<<<(nq + QP_THREADS - 1) / QP_THREADS, QP_THREADS, 0, c->st>>>(c->q32.as<float>(), nq, c->dim, c->qnorm.as<double>(),
+                                                                                  c->qinv.as<float>(), c->metric, status_of(c));
     YB_CUDA(cudaGetLastError());
     return YAMS_OK;
 }
 
-// After the stream has been synchronised: the status block of the call (pinned copy) -> invalid queries are an error,
-// uncertain queries are resolved by the exhaustive levels (results patched in the device output buffers).
-static yams_status_t finish_scan(yams_b200_corpus* c, const ScanPlan& p, int64_t* d_or, float* d_os, uint32_t* d_oc, uint64_t* d_of,
-                                 uint32_t* out_resolved) {
-    const ScanStatus* hs = c->h_pin.as<ScanStatus>();
-    if (out_resolved) *out_resolved = 0;
-    c->last_ms[7] = 0.f;
-    YB_ARG(hs->n_invalid == 0, "exact vector search requires a finite, non-zero query embedding");
-    uint32_t n_bad = std::min(hs->n_bad, p.nq);
-    if (n_bad == 0) return YAMS_OK;
-    std::vector<uint32_t> bad(reinterpret_cast<const uint32_t*>(hs + 1), reinterpret_cast<const uint32_t*>(hs + 1) + n_bad);
-    std::sort(bad.begin(), bad.end());
-    if (out_resolved) *out_resolved = n_bad;
-    uint32_t full = 0;
-    yams_status_t rc = resolve_uncertain(c, p, bad.data(), n_bad, d_or, d_os, d_oc, d_of, &full);
-    c->last_ms[7] = (float)full;   // queries answered by the full exact pass (level 2)
-    return rc;
+// [0..2] and [5] of search_last_timings from the events of the last scan; the caller has seen them complete
+static void time_scan_events(yams_b200_corpus* c) {
+    cudaEventElapsedTime(&c->last_ms[0], c->ev[0], c->ev[1]);
+    cudaEventElapsedTime(&c->last_ms[1], c->ev[1], c->ev[2]);
+    cudaEventElapsedTime(&c->last_ms[2], c->ev[0], c->ev[2]);
+    c->last_ms[5] = 0.f;
+    if (c->scan_timed) cudaEventElapsedTime(&c->last_ms[5], c->ev_scan[0], c->ev_scan[1]);
 }
 // candidate sets as a bit matrix [nq][mask_ld * 32] of allowed corpus rows (allowed_offsets[nq + 1] into allowed_rowids)
 static yams_status_t upload_mask(yams_b200_corpus* c, uint32_t nq, const int64_t* allowed_rowids, const uint64_t* allowed_offsets,
@@ -1832,6 +1816,50 @@ static yams_status_t enqueue_status_readback(yams_b200_corpus* c, uint32_t nq) {
     return YAMS_OK;
 }
 
+// Enqueues search p on the queries at q_src: their preparation, the candidate sets (host allowed_rowids / allowed_offsets,
+// nullable) as p's device lists or mask, the scan and the read-back of its status block.  No host synchronisation.
+static yams_status_t enqueue_search(yams_b200_corpus* c, ScanPlan& p, const float* q_src, bool src_is_device, const int64_t* allowed_rowids,
+                                    const uint64_t* allowed_offsets) {
+    yams_status_t rc;
+    if ((rc = prepare_queries(c, q_src, src_is_device, p.nq)) != YAMS_OK) return rc;
+    YB_CUDA(cudaEventRecord(c->ev[0], c->st));
+    if (p.direct) rc = upload_direct_lists(c, p.nq, allowed_rowids, allowed_offsets, &p.lists);
+    else if (allowed_offsets && c->n) rc = upload_mask(c, p.nq, allowed_rowids, allowed_offsets, &p.d_mask, &p.mask_ld);
+    if (rc != YAMS_OK) return rc;
+    if ((rc = scan_enqueue(c, p)) != YAMS_OK) return rc;
+    YB_CUDA(cudaEventRecord(c->ev[2], c->st));
+    return enqueue_status_readback(c, p.nq);
+}
+
+// After the stream of search p has been synchronised: its status block (pinned copy) -> an invalid query is an error, the
+// queries the certificate rejected (*out_resolved of them) are answered by the exhaustive levels, patching p.out in place.
+// allowed_rowids / allowed_offsets: the host candidate sets of a direct-path search.
+static yams_status_t finish_search(yams_b200_corpus* c, ScanPlan& p, const int64_t* allowed_rowids, const uint64_t* allowed_offsets,
+                                   uint32_t* out_resolved) {
+    const ScanStatus* hs = c->h_pin.as<ScanStatus>();
+    const uint32_t n_bad = std::min(hs->n_bad, p.nq);
+    time_scan_events(c);
+    c->last_ms[6] = c->last_ms[7] = 0.f;
+    *out_resolved = 0;
+    YB_ARG(hs->n_invalid == 0, "exact vector search requires a finite, non-zero query embedding");
+    if (n_bad == 0) return YAMS_OK;
+    std::vector<uint32_t> bad(reinterpret_cast<const uint32_t*>(hs + 1), reinterpret_cast<const uint32_t*>(hs + 1) + n_bad);
+    std::sort(bad.begin(), bad.end());
+    yams_status_t rc;
+    if (p.direct) {
+        // The direct path scored the listed rows without a bit mask, but the exhaustive levels score every row: they need the
+        // candidate sets as a mask.  The scan is finished, so its lists in c->mask may be overwritten.
+        p.direct = false;
+        if ((rc = upload_mask(c, p.nq, allowed_rowids, allowed_offsets, &p.d_mask, &p.mask_ld)) != YAMS_OK) return rc;
+    }
+    *out_resolved = n_bad;
+    c->last_ms[6] = (float)n_bad;
+    uint32_t full = 0;
+    rc = resolve_uncertain(c, p, bad.data(), n_bad, &full);
+    c->last_ms[7] = (float)full;   // queries answered by the full exact pass (level 2)
+    return rc;
+}
+
 // the blocking paths: prepare the queries and reject an invalid one before any search work is enqueued
 static yams_status_t prepare_valid_queries(yams_b200_corpus* c, const float* queries, uint32_t nq) {
     yams_status_t rc;
@@ -1856,9 +1884,6 @@ yams_status_t yams_b200_search(yams_b200_corpus* c, const float* queries, uint32
     YB_ARG(!allowed_offsets || allowed_rowids || allowed_offsets[nq] == 0, "allowed_rowids missing");
     for (uint32_t q = 0; q < nq; ++q) out_counts[q] = 0;
     if (out_flags) for (uint32_t q = 0; q < nq; ++q) out_flags[q] = 0;
-    yams_status_t rc;
-    cudaEvent_t w0 = c->ev[3];
-    YB_CUDA(cudaEventRecord(w0, c->st));
     // the reference looks at k before it validates the query (sqlite_vec_backend.cpp:4123-4130: k == 0 returns
     // empty first): mirror that order
     if (k == 0) return YAMS_OK;
@@ -1867,51 +1892,27 @@ yams_status_t yams_b200_search(yams_b200_corpus* c, const float* queries, uint32
     YB_ARG(nq <= 65535, "at most 65535 queries per call (split larger batches)");   // per-query grid dimensions
     YB_ARG(!allowed_offsets || c->metric == YAMS_B200_COSINE, "candidate sets are only supported for the cosine metric");
     c->pending.active = false;
-    if ((rc = prepare_queries(c, queries, false, nq)) != YAMS_OK) return rc;
-    YB_CUDA(cudaEventRecord(c->ev[0], c->st));
-    DeviceResults r;
-    if ((rc = reserve_results(c->dout, nq, k, &r)) != YAMS_OK) return rc;
+    yams_status_t rc;
     ScanPlan plan;
     plan.nq = nq; plan.k = k; plan.threshold = threshold;
-    plan.use_tensor = wgmma_supported(c, nq);
-    DirectLists lists;
-    bool direct = false;
+    if ((rc = reserve_results(c->dout, nq, k, &plan.out)) != YAMS_OK) return rc;
     if (allowed_offsets && c->n) {
         // small ascending lists: score the listed rows directly instead of passing over the corpus.  Break-even
         // (DESIGN.md §4.4): a corpus pass costs ~max(1, nq/400) row reads per row, a gathered row about two.
         const uint64_t total = allowed_offsets[nq];
-        direct = total <= std::max<uint64_t>(c->n / 2, c->n / 400 * nq) && total < (1ull << 31);
-        for (uint32_t q = 0; q < nq && direct; ++q) {
+        plan.direct = total <= std::max<uint64_t>(c->n / 2, c->n / 400 * nq) && total < (1ull << 31);
+        for (uint32_t q = 0; q < nq && plan.direct; ++q) {
             uint64_t lo = allowed_offsets[q], hi = allowed_offsets[q + 1];
-            direct = hi >= lo && hi - lo < 0xFFFFFFFFull;
-            for (uint64_t i = lo + 1; i < hi && direct; ++i) direct = allowed_rowids[i - 1] <= allowed_rowids[i];
-            if (direct) lists.max_len = std::max<uint32_t>(lists.max_len, (uint32_t)(hi - lo));
+            plan.direct = hi >= lo && hi - lo < 0xFFFFFFFFull;
+            for (uint64_t i = lo + 1; i < hi && plan.direct; ++i) plan.direct = allowed_rowids[i - 1] <= allowed_rowids[i];
+            if (plan.direct) plan.lists.max_len = std::max<uint32_t>(plan.lists.max_len, (uint32_t)(hi - lo));
         }
     }
-    if (direct) {
-        if ((rc = upload_direct_lists(c, nq, allowed_rowids, allowed_offsets, &lists)) != YAMS_OK) return rc;
-        plan.direct = &lists;
-    } else if (allowed_offsets && c->n) {
-        if ((rc = upload_mask(c, nq, allowed_rowids, allowed_offsets, &plan.d_mask, &plan.mask_ld)) != YAMS_OK) return rc;
-    }
-    if ((rc = scan_enqueue(c, plan, r.rowids, r.scores, r.counts, r.flags)) != YAMS_OK) return rc;
-    cudaEventRecord(c->ev[2], c->st);
-    if ((rc = enqueue_status_readback(c, nq)) != YAMS_OK) return rc;
+    if ((rc = enqueue_search(c, plan, queries, false, allowed_rowids, allowed_offsets)) != YAMS_OK) return rc;
+    const DeviceResults& r = plan.out;
     if ((rc = copy_results(r, nq, k, out_rowids, out_scores, out_counts, out_flags, c->st)) != YAMS_OK) return rc;
-    cudaEventElapsedTime(&c->last_ms[0], c->ev[0], c->ev[1]);
-    cudaEventElapsedTime(&c->last_ms[1], c->ev[1], c->ev[2]);
-    cudaEventElapsedTime(&c->last_ms[2], c->ev[0], c->ev[2]);
     uint32_t resolved = 0;
-    const ScanStatus* hs = c->h_pin.as<ScanStatus>();
-    if (plan.direct && hs->n_bad && hs->n_invalid == 0) {
-        // The direct path scored the listed rows without a bit mask, but the exhaustive levels score every row: they need the
-        // candidate sets as a mask.  The scan is finished (copy_results synchronised), so its lists in c->mask may be overwritten.
-        plan.direct = nullptr;
-        rc = upload_mask(c, nq, allowed_rowids, allowed_offsets, &plan.d_mask, &plan.mask_ld);
-    }
-    if (rc == YAMS_OK) rc = finish_scan(c, plan, r.rowids, r.scores, r.counts, r.flags, &resolved);
-    c->last_ms[6] = (float)resolved;
-    if (rc != YAMS_OK) {
+    if ((rc = finish_search(c, plan, allowed_rowids, allowed_offsets, &resolved)) != YAMS_OK) {
         for (uint32_t q = 0; q < nq; ++q) out_counts[q] = 0;
         return rc;
     }
@@ -1936,13 +1937,12 @@ yams_status_t yams_b200_search_exhaustive(yams_b200_corpus* c, const float* quer
     yams_status_t rc;
     c->pending.active = false;
     if ((rc = prepare_valid_queries(c, queries, nq)) != YAMS_OK) return rc;
-    DeviceResults r;
-    if ((rc = reserve_results(c->dout, nq, k, &r)) != YAMS_OK) return rc;
     ScanPlan plan;
     plan.nq = nq; plan.k = k; plan.threshold = threshold;
+    if ((rc = reserve_results(c->dout, nq, k, &plan.out)) != YAMS_OK) return rc;
     for (uint32_t q = 0; q < nq; ++q)
-        if ((rc = exact_all_rows(c, plan, q, r.rowids, r.scores, r.counts, r.flags)) != YAMS_OK) return rc;
-    return copy_results(r, nq, k, out_rowids, out_scores, out_counts, out_flags, c->st);
+        if ((rc = exact_all_rows(c, plan, q)) != YAMS_OK) return rc;
+    return copy_results(plan.out, nq, k, out_rowids, out_scores, out_counts, out_flags, c->st);
     YB_CATCH
 }
 
@@ -2016,22 +2016,14 @@ yams_status_t yams_b200_search_device(yams_b200_corpus* c, const float* d_querie
     YB_ARG(k > 0 && k <= 768, "k must be in 1..768");
     YB_ARG(nq <= 65535, "at most 65535 queries per call (split larger batches)");
     if (nq == 0) return YAMS_OK;
-    yams_status_t rc;
     c->pending.active = false;
-    if ((rc = prepare_queries(c, d_queries, true, nq)) != YAMS_OK) return rc;
-    YB_CUDA(cudaEventRecord(c->ev[0], c->st));
     ScanPlan plan;
     plan.nq = nq; plan.k = k; plan.threshold = threshold;
-    plan.use_tensor = wgmma_supported(c, nq);
-    if ((rc = scan_enqueue(c, plan, d_out_rowids, d_out_scores, nullptr, nullptr)) != YAMS_OK) return rc;
-    YB_CUDA(cudaEventRecord(c->ev[2], c->st));
-    if ((rc = enqueue_status_readback(c, nq)) != YAMS_OK) return rc;
+    plan.out.rowids = d_out_rowids; plan.out.scores = d_out_scores;
+    yams_status_t rc = enqueue_search(c, plan, d_queries, true, nullptr, nullptr);
+    if (rc != YAMS_OK) return rc;
+    c->pending.plan = plan;
     c->pending.active = true;
-    c->pending.nq = nq;
-    c->pending.k = k;
-    c->pending.threshold = threshold;
-    c->pending.d_out_rowids = d_out_rowids;
-    c->pending.d_out_scores = d_out_scores;
     return YAMS_OK;
     YB_CATCH
 }
@@ -2045,9 +2037,10 @@ yams_status_t yams_b200_search_device_finish(yams_b200_corpus* c, uint32_t* out_
     if (!c->pending.active) return YAMS_OK;
     YB_CUDA(cudaStreamSynchronize(c->st));
     c->pending.active = false;
-    ScanPlan plan;
-    plan.nq = c->pending.nq; plan.k = c->pending.k; plan.threshold = c->pending.threshold;
-    return finish_scan(c, plan, c->pending.d_out_rowids, c->pending.d_out_scores, nullptr, nullptr, out_resolved);
+    uint32_t resolved = 0;
+    yams_status_t rc = finish_search(c, c->pending.plan, nullptr, nullptr, &resolved);
+    if (out_resolved) *out_resolved = resolved;
+    return rc;
     YB_CATCH
 }
 
@@ -2089,13 +2082,8 @@ yams_status_t yams_b200_merge_packed_device(yams_b200_corpus* c, const void* d_p
 
 yams_status_t yams_b200_search_last_timings(yams_b200_corpus* c, float out_ms[8]) {
     YB_ARG(c && out_ms, "null argument");
-    if (cudaEventQuery(c->ev[2]) == cudaSuccess) {
-        cudaEventElapsedTime(&c->last_ms[0], c->ev[0], c->ev[1]);
-        cudaEventElapsedTime(&c->last_ms[1], c->ev[1], c->ev[2]);
-        cudaEventElapsedTime(&c->last_ms[2], c->ev[0], c->ev[2]);
-        c->last_ms[5] = 0.f;
-        if (c->scan_timed) cudaEventElapsedTime(&c->last_ms[5], c->ev_scan[0], c->ev_scan[1]);
-    }
+    // a search_device whose work is done reports its device times before (or without) its finish
+    if (c->pending.active && cudaEventQuery(c->ev[2]) == cudaSuccess) time_scan_events(c);
     for (int i = 0; i < 8; ++i) out_ms[i] = c->last_ms[i];
     return YAMS_OK;
 }
@@ -2118,15 +2106,28 @@ yams_status_t yams_b200_debug_stage1_scores(yams_b200_corpus* c, const float* qu
     fill_stage1_common(c, a, nq);
     a.row_start = row_start; a.row_stride = row_stride; a.nrows = nrows;
     a.out_scores = c->dense.as<float>(); a.ld = nrows;
-    if (engine == 1) {
-        rc = stage1_wgmma(c, a, false, c->st);
-    } else {
-        rc = stage1_cuda_core(a, false, c->st);
-        launch_eps_cc(c, nq, c->eps.as<float>(), false);
-    }
-    if (rc != YAMS_OK) return rc;
+    Stage1Engine s1{c, engine == 1, false};
+    if ((rc = s1.run(a, false)) != YAMS_OK) return rc;
+    s1.launch_eps(nq);
     YB_CUDA(cudaMemcpyAsync(out, c->dense.p, (size_t)nq * nrows * 4, cudaMemcpyDeviceToHost, c->st));
     YB_CUDA(cudaStreamSynchronize(c->st));
+    return YAMS_OK;
+}
+
+// the filter-mode set-up of the stage-1 diagnostics: the queries prepared, tau[nq] uploaded, the list counters zeroed and `a`
+// filled for lists of cap entries (the caller sets the rows)
+static yams_status_t debug_filter_setup(yams_b200_corpus* c, const float* queries, uint32_t nq, const float* tau, uint32_t cap,
+                                        Stage1Args& a) {
+    yams_status_t rc;
+    c->pending.active = false;
+    if ((rc = prepare_queries(c, queries, false, nq)) != YAMS_OK) return rc;
+    if ((rc = c->eps.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
+    if ((rc = c->tau.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
+    if ((rc = c->cands.reserve((size_t)nq * cap * sizeof(Cand) + 8)) != YAMS_OK) return rc;
+    YB_CUDA(cudaMemcpyAsync(c->tau.p, tau, (size_t)nq * 4, cudaMemcpyHostToDevice, c->st));
+    YB_CUDA(cudaMemsetAsync(c->counts.p, 0, (size_t)nq * 4, c->st));
+    fill_stage1_common(c, a, nq);
+    a.tau = c->tau.as<float>(); a.cands = c->cands.as<Cand>(); a.cap = cap; a.counts = c->counts.as<uint32_t>();
     return YAMS_OK;
 }
 
@@ -2143,19 +2144,12 @@ yams_status_t yams_b200_debug_stage1_candidates(yams_b200_corpus* c, const float
     YB_ARG(row_start + (nrows - 1) * row_stride < c->n, "rows out of range");
     yams_status_t rc;
     YB_BIND(c);
-    c->pending.active = false;
-    if ((rc = prepare_queries(c, queries, false, nq)) != YAMS_OK) return rc;
-    const size_t cb = (size_t)nq * cap * sizeof(Cand);
-    if ((rc = c->eps.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
-    if ((rc = c->tau.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
-    if ((rc = c->cands.reserve(cb + 8)) != YAMS_OK) return rc;
-    YB_CUDA(cudaMemcpyAsync(c->tau.p, tau, (size_t)nq * 4, cudaMemcpyHostToDevice, c->st));
-    YB_CUDA(cudaMemsetAsync(c->counts.p, 0, (size_t)nq * 4, c->st));
-    YB_CUDA(cudaMemsetAsync(c->cands.p, 0xFF, cb, c->st));
     Stage1Args a{};
-    fill_stage1_common(c, a, nq);
+    if ((rc = debug_filter_setup(c, queries, nq, tau, cap, a)) != YAMS_OK) return rc;
+    const size_t cb = (size_t)nq * cap * sizeof(Cand);
+    YB_CUDA(cudaMemsetAsync(c->cands.p, 0xFF, cb, c->st));
     a.row_start = row_start; a.row_stride = row_stride; a.nrows = nrows;
-    a.tau = c->tau.as<float>(); a.cands = c->cands.as<Cand>(); a.cap = cap; a.counts = c->counts.as<uint32_t>();
+    Stage1Engine s1{c, engine == 1, false};
     if (engine == 2) {
         // the direct path's engine: every listed rowid is scored, tau and the row range do not apply
         YB_ARG(allowed_offsets && c->metric == YAMS_B200_COSINE, "engine 2 scores cosine candidate-set lists");
@@ -2169,17 +2163,12 @@ yams_status_t yams_b200_debug_stage1_candidates(yams_b200_corpus* c, const float
         if ((rc = upload_direct_lists(c, nq, allowed_rowids, allowed_offsets, &lists)) != YAMS_OK) return rc;
         list_lengths_kernel<<<(nq + 255) / 256, 256, 0, c->st>>>(lists.d_offsets, nq, a.counts);
         rc = gather_scores(c, lists, nq, a.q32, a.qinv, a.cands, cap, c->st);
-        launch_eps_cc(c, nq, c->eps.as<float>(), false);
     } else {
         if (allowed_offsets && (rc = upload_mask(c, nq, allowed_rowids, allowed_offsets, &a.mask, &a.mask_ld)) != YAMS_OK) return rc;
-        if (engine == 1) {
-            rc = stage1_wgmma(c, a, true, c->st);
-        } else {
-            rc = stage1_cuda_core(a, true, c->st);
-            launch_eps_cc(c, nq, c->eps.as<float>(), false);
-        }
+        rc = s1.run(a, true);
     }
     if (rc != YAMS_OK) return rc;
+    s1.launch_eps(nq);
     YB_CUDA(cudaMemcpyAsync(out_counts, c->counts.p, (size_t)nq * 4, cudaMemcpyDeviceToHost, c->st));
     if (cb) YB_CUDA(cudaMemcpyAsync(out_cands, c->cands.p, cb, cudaMemcpyDeviceToHost, c->st));
     YB_CUDA(cudaStreamSynchronize(c->st));
@@ -2195,24 +2184,15 @@ yams_status_t yams_b200_debug_stage1_profile(yams_b200_corpus* c, const float* q
     YB_ARG(c->n > 0, "empty corpus");
     yams_status_t rc;
     YB_BIND(c);
-    c->pending.active = false;
-    if ((rc = prepare_queries(c, queries, false, nq)) != YAMS_OK) return rc;
-    const size_t cb = (size_t)nq * cap * sizeof(Cand);
-    const size_t pb = (size_t)c->dev->sm_count * 4 * sizeof(unsigned long long);
-    if ((rc = c->eps.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
-    if ((rc = c->tau.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
-    if ((rc = c->cands.reserve(cb + 8)) != YAMS_OK) return rc;
-    if ((rc = c->dense.reserve(pb)) != YAMS_OK) return rc;
-    YB_CUDA(cudaMemcpyAsync(c->tau.p, tau, (size_t)nq * 4, cudaMemcpyHostToDevice, c->st));
-    YB_CUDA(cudaMemsetAsync(c->counts.p, 0, (size_t)nq * 4, c->st));
-    YB_CUDA(cudaMemsetAsync(c->dense.p, 0, pb, c->st));
     Stage1Args a{};
-    fill_stage1_common(c, a, nq);
+    if ((rc = debug_filter_setup(c, queries, nq, tau, cap, a)) != YAMS_OK) return rc;
+    const size_t pb = (size_t)c->dev->sm_count * 4 * sizeof(unsigned long long);
+    if ((rc = c->dense.reserve(pb)) != YAMS_OK) return rc;
+    YB_CUDA(cudaMemsetAsync(c->dense.p, 0, pb, c->st));
     a.row_start = 0; a.row_stride = 1; a.nrows = c->n;
-    a.tau = c->tau.as<float>(); a.cands = c->cands.as<Cand>(); a.cap = cap; a.counts = c->counts.as<uint32_t>();
-    c->scan_timed = false;
+    Stage1Engine s1{c, true, false};
     YB_CUDA(cudaEventRecord(c->ev_scan[0], c->st));
-    if ((rc = stage1_wgmma(c, a, true, c->st, reinterpret_cast<unsigned long long*>(c->dense.p))) != YAMS_OK) return rc;
+    if ((rc = s1.run(a, true, reinterpret_cast<unsigned long long*>(c->dense.p))) != YAMS_OK) return rc;
     YB_CUDA(cudaEventRecord(c->ev_scan[1], c->st));
     const uint32_t ctas = c->wg_launch[1];
     YB_ARG(ctas <= max_ctas, "max_ctas is below the launch's CTA count");
@@ -2303,7 +2283,7 @@ yams_status_t yams_b200_debug_final(yams_b200_corpus* c, uint32_t nq, uint32_t K
     if ((rc = c->outbuf.reserve(eb + (size_t)nq * 4 + 8)) != YAMS_OK) return rc;
     if ((rc = c->bound.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
     if ((rc = c->eps.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
-    if ((rc = c->misc.reserve((size_t)nq * 8)) != YAMS_OK) return rc;
+    if ((rc = c->qnorm.reserve((size_t)nq * 8)) != YAMS_OK) return rc;
     if ((rc = c->status.reserve(sizeof(ScanStatus) + (size_t)nq * 8)) != YAMS_OK) return rc;
     DeviceResults r;
     if ((rc = reserve_results(c->dout, nq, k, &r)) != YAMS_OK) return rc;
@@ -2313,15 +2293,11 @@ yams_status_t yams_b200_debug_final(yams_b200_corpus* c, uint32_t nq, uint32_t K
     if (ex_n) YB_CUDA(cudaMemcpyAsync(d_ex_n, ex_n, (size_t)nq * 4, cudaMemcpyHostToDevice, st));
     YB_CUDA(cudaMemcpyAsync(c->bound.p, bound, (size_t)nq * 4, cudaMemcpyHostToDevice, st));
     YB_CUDA(cudaMemcpyAsync(c->eps.p, eps, (size_t)nq * 4, cudaMemcpyHostToDevice, st));
-    YB_CUDA(cudaMemcpyAsync(c->misc.p, qnorm, (size_t)nq * 8, cudaMemcpyHostToDevice, st));
+    YB_CUDA(cudaMemcpyAsync(c->qnorm.p, qnorm, (size_t)nq * 8, cudaMemcpyHostToDevice, st));
     YB_CUDA(cudaMemsetAsync(c->status.p, 0, sizeof(ScanStatus) + (size_t)nq * 8, st));
-    const bool l2 = metric == YAMS_B200_L2;
-    CertArgs cert{};
-    cert.bound = c->bound.as<float>(); cert.eps = c->eps.as<float>(); cert.qnorm = reinterpret_cast<const double*>(c->misc.p);
-    cert.threshold = threshold; cert.metric = metric; cert.l2_margin = l2_cert_margin(c->dim); cert.status = status_of(c);
-    cert.level = level; cert.nq_total = nq;
-    final_kernel<<<nq, SEL_THREADS, 0, st>>>(d_ex, ex_n ? d_ex_n : nullptr, Kp, k, c->rowids.as<int64_t>(), l2 ? 1 : 0, r.rowids, r.scores,
-                                             r.counts, r.flags, l2 ? INFINITY : -INFINITY, nullptr, cert);
+    CertArgs cert = cert_args(c, c->bound.as<float>(), c->eps.as<float>(), threshold, level, nq);
+    cert.metric = metric;   // either result convention on any corpus
+    launch_final(d_ex, ex_n ? d_ex_n : nullptr, Kp, k, c->rowids.as<int64_t>(), r, nq, nullptr, cert, st);
     YB_CUDA(cudaGetLastError());
     std::vector<uint32_t> h_status(sizeof(ScanStatus) / 4 + (size_t)nq * 2);
     YB_CUDA(cudaMemcpyAsync(h_status.data(), c->status.p, h_status.size() * 4, cudaMemcpyDeviceToHost, st));

@@ -19,6 +19,35 @@ struct Exact {
     uint32_t row;
 };
 
+// the padded [nq][k] results of a search on the device: [nq*k rowids][nq flags][nq*k scores][nq counts] carved out of one buffer
+// (reserve_results); search_device writes only rowids and scores, into the caller's buffers (counts, flags null)
+struct DeviceResults {
+    int64_t* rowids = nullptr;
+    uint64_t* flags = nullptr;
+    float* scores = nullptr;
+    uint32_t* counts = nullptr;
+};
+
+// Small candidate sets (CandidateFilterMode::Exact): device lists (ascending rowids, d_offsets[nq+1]) short enough that
+// scoring the listed rows one by one is cheaper than a corpus pass -> gather_score_kernel
+struct DirectLists {
+    const int64_t* d_allowed = nullptr;
+    const uint64_t* d_offsets = nullptr;
+    uint64_t total = 0;
+    uint32_t max_len = 0;
+};
+
+// one exact search (knn.cu): the candidate-set form it scans and the device results it writes, from the enqueue to the finish
+struct ScanPlan {
+    uint32_t nq = 0, k = 0;
+    float threshold = -1.f;
+    bool direct = false;                // candidate sets as the lists below
+    DirectLists lists;
+    const uint32_t* d_mask = nullptr;   // else nullable: bit matrix [nq][mask_ld*32] of allowed rows -> masked corpus pass
+    uint64_t mask_ld = 0;
+    DeviceResults out;
+};
+
 struct Corpus {
     DeviceCtx* dev = nullptr;
     cudaStream_t st = nullptr;
@@ -37,19 +66,18 @@ struct Corpus {
     float r_max = 0.f, dr_abs_max = 0.f, dr_rel_max = 0.f, inv_max = 0.f;   // host copies of stats (upper bounds; removals keep them)
     // search workspace
     DevBuf q32, q16, qinv, tau, counts, cands, sample_scores, sel, outbuf, dense, mask, misc, dout;
+    DevBuf qnorm;      // nq doubles: |q| of the search's queries, written by its query preparation only (misc is scratch that
+                       // mutators overwrite while a search_device is still pending)
     DevBuf status;     // ScanStatus + bad[nq] + bad2[nq] of the call in flight
     DevBuf bound, eps, eps2;   // per query: certificate inputs (knn.cu final_kernel)
     DevBuf lvl;        // exhaustive level 1 workspace
     HostBuf h_pin;
     // the call enqueued by search_device and not yet finished (search_device_finish)
     struct Pending {
+        ScanPlan plan;
         bool active = false;
-        uint32_t nq = 0, k = 0;
-        float threshold = 0.f;
-        int64_t* d_out_rowids = nullptr;
-        float* d_out_scores = nullptr;
     } pending;
-    cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
+    cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};
     cudaEvent_t ev_scan[2] = {nullptr, nullptr};  // around the full-corpus filtered scan launch
     bool scan_timed = false;
     float last_ms[8] = {0, 0, 0, 0, 0, 0, 0, 0};
@@ -97,18 +125,11 @@ yams_status_t stage1_cuda_core(const Stage1Args& a, bool filter, cudaStream_t st
 // Stages of the exact scan that the other engines (pq.cu) launch on their own lists; each is described at its definition in knn.cu
 void launch_topk_lists(const Cand* lists, const uint32_t* counts, uint32_t cap, uint32_t nq, uint32_t K, Cand* out_sel, uint32_t* out_n,
                        cudaStream_t st);
-void launch_final_plain(const Exact* exact, uint32_t Kp, uint32_t k, uint32_t nq, const int64_t* rowids, int64_t* out_rowids, float* out_scores,
-                        uint32_t* out_counts, uint64_t* out_flags, cudaStream_t st);
+void launch_final_plain(const Exact* exact, uint32_t Kp, uint32_t k, uint32_t nq, const int64_t* rowids, const DeviceResults& out,
+                        cudaStream_t st);
 void launch_map_rowids(const int64_t* rowids_in, uint64_t n_in, const int64_t* corpus_rowids, uint64_t n, Cand* out, cudaStream_t st);
 void launch_query_prep(const float* q, uint32_t nq, uint32_t d, double* qnorm, float* qinv, void* status, cudaStream_t st);
 
-// the padded [nq][k] results of a search on the device: [nq*k rowids][nq flags][nq*k scores][nq counts] carved out of one buffer
-struct DeviceResults {
-    int64_t* rowids;
-    uint64_t* flags;
-    float* scores;
-    uint32_t* counts;
-};
 yams_status_t reserve_results(DevBuf& buf, uint32_t nq, uint32_t k, DeviceResults* r);
 // device results -> the caller's arrays (out_flags nullable).  enqueue_results only enqueues the copies, for a caller with one
 // more read-back to make before it waits; copy_results also waits for them.

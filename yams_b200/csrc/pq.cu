@@ -713,7 +713,7 @@ static yams_status_t pq_rerank_and_emit(yams_b200_pq* p, const float* d_q, Cand*
     pq_rank_to_row_kernel<<<(tot + 255) / 256, 256, 0, st>>>(d_sel, d_sel_n, K, nq, p->rank_to_idx.as<uint32_t>(), p->idx_rows.as<uint32_t>());
     pq_rerank_kernel<<<(tot + 127) / 128, 128, 0, st>>>(c->rows.p, c->dtype, p->dim, d_q, d_sel, d_sel_n, p->valid.as<uint32_t>(), K, nq, threshold,
                                                         p->exact.as<Exact>());
-    launch_final_plain(p->exact.as<Exact>(), K, k, nq, c->rowids.as<int64_t>(), r.rowids, r.scores, r.counts, r.flags, st);
+    launch_final_plain(p->exact.as<Exact>(), K, k, nq, c->rowids.as<int64_t>(), r, st);
     YB_CUDA(cudaGetLastError());
     return enqueue_results(r, nq, k, out_rowids, out_scores, out_counts, out_flags, st);
 }
