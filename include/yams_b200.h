@@ -316,6 +316,8 @@ YAMS_B200_API void yams_b200_corpus_destroy(yams_b200_corpus* c);
                                            /* adapter must re-break by chunk_id (:4218-4223)   */
 #define YAMS_B200_FLAG_FALLBACK_PATH 2ull  /* the fast path could not PROVE its answer exact;   */
                                            /* the query was answered by an exhaustive level     */
+#define YAMS_B200_FLAG_NOT_A_SOURCE 4ull   /* yams_b200_semantic_neighbors: the rowid is unknown */
+                                           /* or its row is not in the graph (count 0)          */
 
 /* Exact top-k of every query against the corpus (bruteForceSearchUnlocked fast path semantics,
  * sqlite_vec_backend.cpp:4203-4331):
@@ -351,6 +353,36 @@ YAMS_B200_API yams_status_t yams_b200_search_all_matching(yams_b200_corpus* c, c
                                                           const int64_t* allowed_rowids, uint64_t n_allowed,
                                                           int64_t* out_rowids, float* out_scores,
                                                           uint64_t* out_count);
+
+/* The semantic-neighbour graph over document-level embeddings (EmbeddingService::updateSemanticNeighborGraphUnlocked,
+ * src/daemon/components/EmbeddingService.cpp:405-431, 856-1030): the exact top-k neighbour DOCUMENTS of every source document.
+ * c is a cosine corpus (fp32 or fp16; L2 -> YAMS_ERR_INVALID_ARG) of one document per row, appended in document_hash order,
+ * so that rowid ascending is the reference's hash ascending.
+ *   row taken  every element finite and inv = float(1 / sqrt(sum (double)r^2)) > 0 (:405-415, :875-877).  Unlike
+ *              yams_b200_search, rows with 0 < |r|^2 <= 1e-12 ARE neighbours, and so are rows whose inv overflows to +inf
+ *              (|r|^2 < 2^-256; their similarities are +-inf, and every source then goes to the exhaustive levels).
+ *   NaN        the one case without a reference answer: a NaN similarity (a row with a NaN element, whose inv is NaN, or
+ *              0 * inf from a row with an infinite inv) enters the reference's candidate lists, where its replace-worst
+ *              and sort have no defined result.  Here it is never a neighbour; a row with a NaN element is not a source.
+ *   score      sim = float((dot * (double)inv_s) * (double)inv_n), dot the sequential double sum of s[i] * n[i], s the source
+ *              (cosineSimilarity, :417-431).  The source's own row is never its neighbour.  sim < threshold is dropped.
+ *              The reference's adaptive mode (no explicit threshold: sim > 0) is threshold = FLT_TRUE_MIN; its explicit
+ *              YAMS_GRAPH_SEMANTIC_THRESHOLD is that value clamped to [0, 1].
+ *   order      (sim desc, rowid asc), -0.0 and +0.0 one score; the best k kept (:949-1017).
+ * source_rowids: NULL = every row is a source (n_sources must equal the corpus size), else strictly ascending rowids; an unknown
+ * rowid or a row that is not taken gets count 0 and YAMS_B200_FLAG_NOT_A_SOURCE.  k == 0 -> all counts and flags 0;
+ * k <= 3072.
+ * Outputs (caller-owned HOST) n_sources x k: out_rowids (unused slots -1), out_sims (unused slots 0), out_counts, out_flags
+ * (nullable; YAMS_B200_FLAG_TIE_AT_K and YAMS_B200_FLAG_FALLBACK_PATH as for yams_b200_search, NOT_A_SOURCE above).  The sources run in batches of
+ * 1024 through the exact scan of yams_b200_search, with the same certificate and exhaustive levels. */
+YAMS_B200_API yams_status_t yams_b200_semantic_neighbors(yams_b200_corpus* c, const int64_t* source_rowids, uint64_t n_sources,
+                                                         uint32_t k, float threshold, int64_t* out_rowids, float* out_sims,
+                                                         uint32_t* out_counts, uint64_t* out_flags);
+/* diagnostics: dense stage-1 scores of the graph (the graph's own 1/|r| scales) of every corpus row against the n_sources
+ * (<= 1024, all taken) sources with the chosen engine (0 cuda-core, 1 wgmma) -> out_scores[s * corpus_size + row] (HOST), and
+ * the certificate's per-source error bound (stage 1 plus the score's float cast) -> out_eps[s] */
+YAMS_B200_API yams_status_t yams_b200_debug_semantic_stage1(yams_b200_corpus* c, const int64_t* source_rowids, uint32_t n_sources,
+                                                            int engine, float* out_scores, float* out_eps);
 
 /* Device-pointer form for multi-GPU sharding: queries and outputs are DEVICE pointers, the whole pipeline is enqueued on
  * the corpus stream and the call returns WITHOUT synchronising (query validity, list overflow and the exactness
@@ -578,6 +610,9 @@ typedef struct yams_vector_scan_v1 {
                                       uint32_t k, float threshold, const int64_t* doc_rowids, const uint64_t* doc_offsets,
                                       const uint64_t* query_docs, int64_t* out_docs, int64_t* out_rowids,
                                       float* out_scores, uint32_t* out_counts);
+    yams_status_t (*semantic_neighbors)(yams_b200_corpus* c, const int64_t* source_rowids, uint64_t n_sources, uint32_t k,
+                                        float threshold, int64_t* out_rowids, float* out_sims, uint32_t* out_counts,
+                                        uint64_t* out_flags);
 } yams_vector_scan_v1;
 
 /* ---- sqlite-vec-cpp C API kept bit-for-bit in signature and error behaviour ------------------

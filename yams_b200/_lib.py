@@ -14,7 +14,8 @@ _SO = os.path.join(HERE, "libyams_b200.so")
 STREAMING, RABIN = 0, 1
 F32, F16 = 0, 1
 COSINE, L2 = 0, 1
-FLAG_TIE_AT_K, FLAG_FALLBACK_PATH = 1, 2
+FLAG_TIE_AT_K, FLAG_FALLBACK_PATH, FLAG_NOT_A_SOURCE = 1, 2, 4
+FLT_TRUE_MIN = float(np.float32(1.4e-45))   # the smallest positive float: semantic_neighbors' adaptive mode (sim > 0)
 
 u8p = C.POINTER(C.c_uint8)
 u32p = C.POINTER(C.c_uint32)
@@ -110,6 +111,8 @@ SYMBOLS = {
     "yams_b200_corpus_destroy": (None, [C.c_void_p]),
     "yams_b200_search": (C.c_int, [C.c_void_p, f32p, C.c_uint32, C.c_uint32, C.c_float, i64p, u64p, i64p, f32p, u32p, u64p]),
     "yams_b200_search_all_matching": (C.c_int, [C.c_void_p, f32p, C.c_float, i64p, C.c_uint64, i64p, f32p, u64p]),
+    "yams_b200_semantic_neighbors": (C.c_int, [C.c_void_p, i64p, C.c_uint64, C.c_uint32, C.c_float, i64p, f32p, u32p, u64p]),
+    "yams_b200_debug_semantic_stage1": (C.c_int, [C.c_void_p, i64p, C.c_uint32, C.c_int, f32p, f32p]),
     "yams_b200_search_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_float, C.c_void_p, C.c_void_p]),
     "yams_b200_search_device_finish": (C.c_int, [C.c_void_p, u32p]),
     "yams_b200_search_exhaustive": (C.c_int, [C.c_void_p, f32p, C.c_uint32, C.c_uint32, C.c_float, i64p, f32p, u32p, u64p]),
@@ -467,6 +470,32 @@ class Corpus:
                                                  out_s.ctypes.data_as(f32p), C.byref(cnt))
         _check(rc, "search_all_matching")
         return out_r[:cnt.value].copy(), out_s[:cnt.value].copy()
+
+    def semantic_neighbors(self, k: int, threshold: float = FLT_TRUE_MIN, sources=None):
+        """The semantic-neighbour graph (EmbeddingService's semantic_neighbor edges): the k best other rows of every source row by
+        float((dot inv_s) inv_n), ordered (sim desc, rowid asc), sim >= threshold (FLT_TRUE_MIN: the reference's adaptive
+        mode).  sources: None = every row, else strictly ascending rowids.
+        -> (rowids i64[S,k] (-1 unused), sims f32[S,k] (0 unused), counts u32[S], flags u64[S])."""
+        src = None if sources is None else np.ascontiguousarray(sources, dtype=np.int64).reshape(-1)
+        ns = len(self) if src is None else len(src)
+        out_r = np.full((max(ns, 1), max(k, 1)), -1, dtype=np.int64)
+        out_s = np.zeros((max(ns, 1), max(k, 1)), dtype=np.float32)
+        out_c = np.zeros(max(ns, 1), dtype=np.uint32)
+        out_f = np.zeros(max(ns, 1), dtype=np.uint64)
+        rc = lib().yams_b200_semantic_neighbors(self._h, src.ctypes.data_as(i64p) if src is not None else None, ns, k, threshold,
+                                                out_r.ctypes.data_as(i64p), out_s.ctypes.data_as(f32p), out_c.ctypes.data_as(u32p),
+                                                out_f.ctypes.data_as(u64p))
+        _check(rc, "semantic_neighbors")
+        return out_r[:ns, :k], out_s[:ns, :k], out_c[:ns], out_f[:ns]
+
+    def debug_semantic_stage1(self, sources, engine: int):
+        """-> (stage-1 scores f32[S, n] of the graph's scales, certificate error bound f32[S]) of the sources (rowids)"""
+        src = np.ascontiguousarray(sources, dtype=np.int64).reshape(-1)
+        out = np.empty((len(src), len(self)), dtype=np.float32)
+        eps = np.empty(len(src), dtype=np.float32)
+        _check(lib().yams_b200_debug_semantic_stage1(self._h, src.ctypes.data_as(i64p), len(src), engine, out.ctypes.data_as(f32p),
+                                                     eps.ctypes.data_as(f32p)), "debug_semantic_stage1")
+        return out, eps
 
     def search_device(self, d_queries: int, nq: int, k: int, threshold: float, d_out_rowids: int, d_out_scores: int):
         _check(lib().yams_b200_search_device(self._h, d_queries, nq, k, threshold, d_out_rowids, d_out_scores), "search_device")

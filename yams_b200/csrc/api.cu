@@ -174,6 +174,7 @@ int yams_plugin_init(const char* config_json, const void* host_context) {
     g_scan_vt.pq_destroy = yams_b200_pq_destroy;
     g_scan_vt.pq_search_candidates = yams_b200_pq_search_candidates;
     g_scan_vt.search_documents = yams_b200_search_documents;
+    g_scan_vt.semantic_neighbors = yams_b200_semantic_neighbors;
     DeviceCtx* dev = nullptr;
     if (ensure_device(&dev) != YAMS_OK) return YAMS_PLUGIN_ERR_INIT_FAILED;  // no CPU fallback
     g_inited = true;

@@ -59,11 +59,10 @@ __device__ __forceinline__ uint64_t find_row(const int64_t* __restrict__ rowids,
     return (a < n && rowids[a] == want) ? a : n;
 }
 
-// bruteForceSearchUnlocked's cosine (sqlite_vec_backend.cpp:4253-4279) of corpus row `row` against the query qv (fp32, 16-byte
-// aligned) of double norm qnorm: sequential double accumulation, skip rules (a non-finite element or |row|^2 <= 1e-12), float
-// cast of dot / (|row| * |q|), `sim < threshold` dropped.  -> true and *out = sim when the row is a result.
-__device__ __forceinline__ bool exact_cosine_sim(const void* __restrict__ rows, int dtype, uint32_t d, uint32_t row, const float* __restrict__ qv,
-                                                 double qnorm, float threshold, float* out) {
+// Sequential double sums of corpus row `row` against qv (fp32, 16-byte aligned): *norm_sq = sum r^2, *dot = sum r q, in the
+// reference's element order; -> false when the row holds a non-finite element (the sums are then partial).
+__device__ __forceinline__ bool row_dot(const void* __restrict__ rows, int dtype, uint32_t d, uint32_t row, const float* __restrict__ qv,
+                                        double* norm_sq_out, double* dot_out) {
     const uint64_t base = (uint64_t)row * d;
     double norm_sq = 0.0, dot = 0.0;
     bool finite = true;
@@ -110,6 +109,18 @@ __device__ __forceinline__ bool exact_cosine_sim(const void* __restrict__ rows, 
         norm_sq += sv * sv;
         dot += sv * qd;
     }
+    *norm_sq_out = norm_sq;
+    *dot_out = dot;
+    return finite;
+}
+
+// bruteForceSearchUnlocked's cosine (sqlite_vec_backend.cpp:4253-4279) of corpus row `row` against the query qv (fp32, 16-byte
+// aligned) of double norm qnorm: sequential double accumulation, skip rules (a non-finite element or |row|^2 <= 1e-12), float
+// cast of dot / (|row| * |q|), `sim < threshold` dropped.  -> true and *out = sim when the row is a result.
+__device__ __forceinline__ bool exact_cosine_sim(const void* __restrict__ rows, int dtype, uint32_t d, uint32_t row, const float* __restrict__ qv,
+                                                 double qnorm, float threshold, float* out) {
+    double norm_sq, dot;
+    const bool finite = row_dot(rows, dtype, d, row, qv, &norm_sq, &dot);
     if (finite && norm_sq > 1e-12) {
         double denom = sqrt(norm_sq) * qnorm;
         double simd = denom > 0.0 ? dot / denom : 0.0;
@@ -122,6 +133,19 @@ __device__ __forceinline__ bool exact_cosine_sim(const void* __restrict__ rows, 
         }
     }
     return false;
+}
+
+// the semantic-neighbour graph's cosineSimilarity (EmbeddingService.cpp:417-431) of corpus row `row` (graph scale inv_n > 0)
+// against the source qv (graph scale inv_s > 0): float((dot * (double)inv_s) * (double)inv_n), the loads and element order of
+// exact_cosine_sim; `sim < threshold` dropped.  -> true and *out = sim when the row is a result.
+__device__ __forceinline__ bool semantic_sim(const void* __restrict__ rows, int dtype, uint32_t d, uint32_t row, const float* __restrict__ qv,
+                                             float inv_s, float inv_n, float threshold, float* out) {
+    double norm_sq, dot;
+    row_dot(rows, dtype, d, row, qv, &norm_sq, &dot);
+    const float sim = (float)((dot * (double)inv_s) * (double)inv_n);
+    if (sim < threshold) return false;
+    *out = sim;
+    return true;
 }
 
 }  // namespace yb

@@ -94,13 +94,14 @@ __device__ __forceinline__ void atomic_max_nonneg(float* addr, float v) {
 }
 
 // per-row validity + 1/|row| exactly as the reference evaluates it (sqlite_vec_backend.cpp:4253-4269):
-// sequential double accumulation; rows with a non-finite element or |row|^2 <= 1e-12 get 0.
+// sequential double accumulation; rows with a non-finite element or |row|^2 <= min_sq get 0 -- min_sq = 1e-12 for the search,
+// 0 for the semantic graph (EmbeddingService.cpp:405-415), whose 1/|row| overflows to +inf below |row|^2 = 2^-256.
 // L2 corpora (vec0 surface, no skip rules) keep |row|^2 in the same slot instead: stage 1 ranks by 2 q.r - |row|^2.
 // stats[0] = max |row|, stats[1] = max |row - tf32(row)| (fp32 corpora read by the tf32 tensor-core engine),
 // stats[2] = max of that residual relative to |row|, stats[3] = max 1/|row| of the rows cosine scores: the inputs of the
 // stage-1 error bound (DESIGN.md §4.2)
 __global__ void row_stats_kernel(const void* __restrict__ rows, int dtype, uint32_t d, uint64_t first, uint64_t n,
-                                 float* __restrict__ inv_norm, int metric, float* __restrict__ stats) {
+                                 float* __restrict__ inv_norm, int metric, float* __restrict__ stats, double min_sq) {
     uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= n) return;
     uint64_t base = (first + r) * (uint64_t)d;
@@ -116,12 +117,12 @@ __global__ void row_stats_kernel(const void* __restrict__ rows, int dtype, uint3
         }
     }
     if (metric == YAMS_B200_L2) inv_norm[first + r] = finite ? (float)ss : INFINITY;
-    else inv_norm[first + r] = (finite && ss > 1e-12) ? (float)(1.0 / sqrt(ss)) : 0.0f;
+    else inv_norm[first + r] = (finite && ss > min_sq) ? (float)(1.0 / sqrt(ss)) : 0.0f;
     if (finite && ss > 0.0) {
         float nrm = (float)sqrt(ss), rs = (float)sqrt(res);
         atomic_max_nonneg(&stats[0], nrm * 1.0000002f);
         atomic_max_nonneg(&stats[1], rs * 1.0000002f);
-        if (ss > 1e-12) {
+        if (ss > min_sq) {
             atomic_max_nonneg(&stats[2], (rs / nrm) * 1.0000002f);
             atomic_max_nonneg(&stats[3], (float)(1.0 / sqrt(ss)) * 1.0000002f);
         }
@@ -664,10 +665,12 @@ __global__ void __launch_bounds__(SEL_THREADS) topk_select_kernel(SelectIn in, u
 //         src/vector/meson.build:79-87): dim >= 16 && dim % 16 == 0 -> simd/avx.hpp:20-66 (eight lane-strided float partial
 //         sums, separate multiply and add, lanes summed left to right), else the scalar loop l2.hpp:108-118; sim = -dist.
 // Entry b of sel/out belongs to query qmap[b] (or b).
+// Semantic graph (graph.inv non-null): the graph's score (semantic_sim) of the rows it takes, the source's own row skipped, and
+// -0.0 stored as +0.0 so that the two zeros order as one score (restore_zero_signs_kernel gives the results their sign back).
 __global__ void rescore_kernel(const void* __restrict__ rows, int dtype, uint32_t d, const float* __restrict__ q32,
                                const double* __restrict__ qnorm, const Cand* __restrict__ sel, const uint32_t* __restrict__ sel_n,
                                uint32_t Kp, uint32_t nq, float threshold, Exact* __restrict__ out, int metric,
-                               const uint32_t* __restrict__ qmap, const uint32_t* __restrict__ mask, uint64_t mask_ld) {
+                               const uint32_t* __restrict__ qmap, const uint32_t* __restrict__ mask, uint64_t mask_ld, GraphRows graph) {
     uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= (uint64_t)nq * Kp) return;
     uint32_t b = (uint32_t)(t / Kp), j = (uint32_t)(t % Kp);
@@ -684,7 +687,15 @@ __global__ void rescore_kernel(const void* __restrict__ rows, int dtype, uint32_
         uint32_t row = sel[(uint64_t)b * Kp + j].row;
         uint64_t base = (uint64_t)row * d;
         const float* qv = q32 + (uint64_t)q * d;
-        if (metric == YAMS_B200_L2) {
+        if (graph.inv) {
+            const float inv_n = graph.inv[row];
+            float sim;
+            if (inv_n > 0.f && row != graph.src_row[q] &&
+                semantic_sim(rows, dtype, d, row, qv, graph.inv[graph.src_row[q]], inv_n, threshold, &sim)) {
+                e.sim = sim == 0.f ? 0.f : sim;
+                e.row = row;
+            }
+        } else if (metric == YAMS_B200_L2) {
             auto row_at = [&](uint32_t c) { return load_elem(rows, dtype, base + c); };
             auto q_at = [&](uint32_t c) { return qv[c]; };
             float dist = ref_l2_distance(q_at, row_at, d);
@@ -703,6 +714,46 @@ __global__ void rescore_kernel(const void* __restrict__ rows, int dtype, uint32_
     out[(uint64_t)b * Kp + j] = e;
 }
 
+// semantic graph: a batch's sources as the queries of the scan.  q32[q] = corpus row src_row[q] (fp16 widened exactly),
+// qinv[q] = its graph scale; the search's query preparation (norms, validity) does not run.
+__global__ void gather_sources_kernel(const void* __restrict__ rows, int dtype, uint32_t d, GraphRows graph, uint32_t nq,
+                                      float* __restrict__ q32, float* __restrict__ qinv) {
+    const uint64_t total = (uint64_t)nq * d;
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (uint64_t)gridDim.x * blockDim.x) {
+        const uint32_t q = (uint32_t)(i / d), c = (uint32_t)(i - (uint64_t)q * d);
+        const uint32_t row = graph.src_row[q];
+        q32[i] = load_elem(rows, dtype, (uint64_t)row * d + c);
+        if (c == 0) qinv[q] = graph.inv[row];
+    }
+}
+
+// semantic graph: the results of a batch with similarity 0 are re-scored to give them their sign (rescore_kernel orders -0.0 as
+// +0.0).  Only a call with threshold <= 0 can return a zero.
+__global__ void restore_zero_signs_kernel(const void* __restrict__ rows, int dtype, uint32_t d, const float* __restrict__ q32,
+                                          GraphRows graph, const int64_t* __restrict__ rowids, uint64_t n, DeviceResults out,
+                                          uint32_t nq, uint32_t k) {
+    const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= (uint64_t)nq * k || out.rowids[t] < 0 || out.scores[t] != 0.f) return;
+    const uint32_t q = (uint32_t)(t / k);
+    const uint32_t row = (uint32_t)find_row(rowids, n, out.rowids[t]);
+    float sim;
+    if (semantic_sim(rows, dtype, d, row, q32 + (uint64_t)q * d, graph.inv[graph.src_row[q]], graph.inv[row], -INFINITY, &sim))
+        out.scores[t] = sim;
+}
+
+// The semantic graph's certificate adds to eps[q] (DESIGN.md §4.9)
+//   * the exact score's own rounding: it is float((dot inv_s) inv_n) with the same float scales stage 1 multiplies by, so
+//     only the float cast (2^-24 |v|, |v| <= (1 + 2^-23)^2), the double products and the double sum (below 2^-32 for
+//     d < 2^20) remain -- at most 2^-23;
+//   * underflow: an fp32 product or partial sum below 2^-126 may be flushed or rounded to the subnormal grid, an absolute error
+//     eps's relative terms do not cover.  Each of the d + 4 steps loses at most 2^-126 of the dot product of the engine's
+//     operands (the raw source on the CUDA-core engine, the source scaled by 1/|s| on the wgmma engine), which the scales then
+//     multiply by at most max(1/|s|, 1) * max 1/|r|: uf = (d + 4) 2^-126 max 1/|r| per unit of max(inv_s, 1).  It is negligible
+//     unless rows or sources have norms below ~1e-30, and +inf (nothing certified, the exhaustive levels answer) when a
+//     scale overflowed.
+constexpr float kGraphEps = 1.1920929e-07f;
+__host__ __device__ inline float graph_eps(float inv_s, float uf) { return kGraphEps + uf * fmaxf(inv_s, 1.f); }
+
 // The exactness certificate (DESIGN.md §4.2).  Stage 1 ranks rows by an approximate score s~ with |s~ - s| <= eps[q];
 // only the top-K' by s~ are re-scored exactly.  Every row that was NOT re-scored has s~ <= bound (topk_select_kernel), hence
 // a true score <= bound + eps.  The emitted top-k is provably the reference's top-k iff no such row can reach the k-th exact
@@ -720,6 +771,8 @@ struct CertArgs {
     ScanStatus* status;       // nullable: no certificate (results already exhaustive)
     int level;                // 0: failures go to bad[], 1: to bad2[]
     uint32_t nq_total;        // capacity of each list
+    const float* graph_qinv;  // semantic graph: its sources' scales -> eps[q] + graph_eps(graph_qinv[q], graph_uf); null: search
+    float graph_uf;
 };
 
 // one CTA per query: order survivors by (sim desc, row asc), emit k, certify.  CTA b serves query qmap[b] (or b).
@@ -770,7 +823,9 @@ __global__ void __launch_bounds__(SEL_THREADS) final_kernel(const Exact* __restr
         if (valid > k && k > 0 && (buf[k - 1] >> 32) == (buf[k] >> 32)) f |= YAMS_B200_FLAG_TIE_AT_K;
         if (cert.status && k > 0) {
             const float bd = cert.bound[b];
-            bool certified = true;
+            const float extra = cert.graph_qinv ? graph_eps(cert.graph_qinv[q], cert.graph_uf) : 0.f;
+            // a graph bound of 1 or more certifies nothing: its scales may have made stage-1 scores NaN, which no bound sees
+            bool certified = extra < 1.f;
             if (bd > -INFINITY) {
                 const float e = cert.eps[q];
                 if (cert.metric == YAMS_B200_L2) {
@@ -784,7 +839,7 @@ __global__ void __launch_bounds__(SEL_THREADS) final_kernel(const Exact* __restr
                     }
                 } else {
                     const float lvl = valid >= k ? key_score(buf[k - 1]) : cert.threshold;
-                    certified = bd + e < lvl;
+                    certified = bd + e + extra < lvl;
                 }
             }
             if (!certified) {
@@ -1119,6 +1174,7 @@ constexpr uint32_t kCandCap = 8192;       // candidate list capacity per query
 constexpr uint32_t kDenseLimit = 65536;   // corpora up to this many rows are scored densely
 constexpr uint32_t kLevel1K = SEL_MAXK;   // survivors re-scored per query by exhaustive level 1
 constexpr uint32_t kLevel1Group = 8;      // queries per level-1 group: group * n floats of scratch
+constexpr uint32_t kGraphBatch = 1024;    // semantic-graph sources per scan (the C2 shape the wgmma engine is tuned for)
 
 static uint32_t survivors_for(uint32_t k) {
     uint32_t slack = std::max<uint32_t>(16, k / 4);
@@ -1172,7 +1228,7 @@ static yams_status_t corpus_finish_append(Corpus* c, uint64_t n_new, const int64
         last = first + (int64_t)n_new - 1;
     }
     row_stats_kernel<<<(unsigned)((n_new + 127) / 128), 128, 0, c->st>>>(c->rows.p, c->dtype, c->dim, c->n, n_new,
-                                                                       c->inv_norm.as<float>(), c->metric, c->stats.as<float>());
+                                                                       c->inv_norm.as<float>(), c->metric, c->stats.as<float>(), 1e-12);
     YB_CUDA(cudaGetLastError());
     float h_stats[4] = {0, 0, 0, 0};
     YB_CUDA(cudaMemcpyAsync(h_stats, c->stats.p, 16, cudaMemcpyDeviceToHost, c->st));
@@ -1237,11 +1293,13 @@ struct Stage1Engine {
 
 // the certificate of stage 2 (final_kernel) in the corpus's metric; failures are queued in the status block (level 0: bad[],
 // level 1: bad2[])
-static CertArgs cert_args(Corpus* c, const float* bound, const float* eps, float threshold, int level, uint32_t nq_total) {
+static CertArgs cert_args(Corpus* c, const ScanPlan& p, const float* bound, const float* eps, int level) {
     CertArgs cert{};
-    cert.bound = bound; cert.eps = eps; cert.qnorm = c->qnorm.as<double>(); cert.threshold = threshold;
+    cert.bound = bound; cert.eps = eps; cert.qnorm = c->qnorm.as<double>(); cert.threshold = p.threshold;
     cert.metric = c->metric; cert.l2_margin = l2_cert_margin(c->dim); cert.status = status_of(c); cert.level = level;
-    cert.nq_total = nq_total;
+    cert.nq_total = p.nq;
+    cert.graph_qinv = p.graph ? c->qinv.as<float>() : nullptr;
+    cert.graph_uf = p.graph ? p.graph->uf : 0.f;
     return cert;
 }
 
@@ -1261,16 +1319,17 @@ static yams_status_t rescore_and_certify(Corpus* c, const ScanPlan& p, const Can
     const uint64_t tot = (uint64_t)grid * Kp;
     rescore_kernel<<<(unsigned)((tot + 127) / 128), 128, 0, c->st>>>(c->rows.p, c->dtype, c->dim, c->q32.as<float>(), c->qnorm.as<double>(),
                                                                      sel, sel_n, Kp, grid, p.threshold, ex, c->metric, qmap, p.d_mask,
-                                                                     p.mask_ld);
-    launch_final(ex, level ? sel_n : nullptr, Kp, p.k, c->rowids.as<int64_t>(), p.out, grid, qmap,
-                 cert_args(c, bound, eps, p.threshold, level, p.nq), c->st);
+                                                                     p.mask_ld, p.graph ? *p.graph : GraphRows{});
+    launch_final(ex, level ? sel_n : nullptr, Kp, p.k, c->rowids.as<int64_t>(), p.out, grid, qmap, cert_args(c, p, bound, eps, level), c->st);
     YB_CUDA(cudaGetLastError());
     return YAMS_OK;
 }
 
-static void fill_stage1_common(Corpus* c, Stage1Args& a, uint32_t nq) {
+// the stage-1 inputs shared by every call: the corpus, the prepared queries and the row scales with their statistics (the
+// cached ones of the search, or those of the semantic graph g)
+static void fill_stage1_common(Corpus* c, Stage1Args& a, uint32_t nq, const GraphRows* g = nullptr) {
     a.rows = c->rows.p;
-    a.inv_norm = c->inv_norm.as<float>();
+    a.inv_norm = g ? g->inv : c->inv_norm.as<float>();
     a.dim = c->dim;
     a.dtype = c->dtype;
     a.q32 = c->q32.as<float>();
@@ -1278,10 +1337,10 @@ static void fill_stage1_common(Corpus* c, Stage1Args& a, uint32_t nq) {
     a.nq = nq;
     a.metric = c->metric;
     a.eps = c->eps.as<float>();
-    a.r_max = c->r_max;
-    a.dr_abs_max = c->dr_abs_max;
-    a.dr_rel_max = c->dr_rel_max;
-    a.inv_max = c->inv_max;
+    a.r_max = g ? g->r_max : c->r_max;
+    a.dr_abs_max = g ? g->dr_abs_max : c->dr_abs_max;
+    a.dr_rel_max = g ? g->dr_rel_max : c->dr_rel_max;
+    a.inv_max = g ? g->inv_max : c->inv_max;
 }
 
 // Enqueues the whole pipeline for the nq queries already prepared on the device (prepare_queries) and writes the padded
@@ -1300,7 +1359,7 @@ static yams_status_t scan_enqueue(Corpus* c, const ScanPlan& p) {
     if ((rc = c->bound.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
     if ((rc = c->eps.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
     Stage1Args a{};
-    fill_stage1_common(c, a, nq);
+    fill_stage1_common(c, a, nq, p.graph);
     Stage1Engine s1{c, wgmma_supported(c, nq), true};
     Cand* d_sel = c->sel.as<Cand>();
     uint32_t* d_sel_n = reinterpret_cast<uint32_t*>(d_sel + (size_t)nq * Kp);
@@ -1435,7 +1494,7 @@ yams_status_t copy_results(const DeviceResults& r, uint32_t nq, uint32_t k, int6
 // 0 .. m-1.  Workspace: c->sel (row list), c->outbuf (exact scores), c->lvl[0, 8) ({m, q}) and c->dense (keys); c->lvl past
 // its first 8 bytes is left alone.
 static yams_status_t exact_sorted_keys(Corpus* c, uint32_t q, uint64_t m, const int64_t* d_allowed, float threshold,
-                                       const uint32_t* mask, uint64_t mask_ld) {
+                                       const uint32_t* mask, uint64_t mask_ld, const GraphRows* graph = nullptr) {
     yams_status_t rc;
     cudaStream_t st = c->st;
     const uint64_t np2 = pow2_at_least(std::max<uint64_t>(m, 1));
@@ -1453,7 +1512,7 @@ static yams_status_t exact_sorted_keys(Corpus* c, uint32_t q, uint64_t m, const 
         else iota_sel_kernel<<<g, 256, 0, st>>>(d_sel, m);
         rescore_kernel<<<(unsigned)((m + 127) / 128), 128, 0, st>>>(c->rows.p, c->dtype, c->dim, c->q32.as<float>(), c->qnorm.as<double>(), d_sel, d_small,
                                                                    (uint32_t)m, 1, threshold, c->outbuf.as<Exact>(), c->metric, d_small + 1,
-                                                                   mask, mask_ld);
+                                                                   mask, mask_ld, graph ? *graph : GraphRows{});
     }
     exact_keys_kernel<<<g, 256, 0, st>>>(c->outbuf.as<Exact>(), m, np2, c->dense.as<uint64_t>());
     sort_keys_desc(c->dense.as<uint64_t>(), np2, st);
@@ -1466,7 +1525,7 @@ static yams_status_t exact_all_rows(Corpus* c, const ScanPlan& p, uint32_t q) {
     yams_status_t rc;
     cudaStream_t st = c->st;
     const bool l2 = c->metric == YAMS_B200_L2;
-    if ((rc = exact_sorted_keys(c, q, c->n, nullptr, p.threshold, p.d_mask, p.mask_ld)) != YAMS_OK) return rc;
+    if ((rc = exact_sorted_keys(c, q, c->n, nullptr, p.threshold, p.d_mask, p.mask_ld, p.graph)) != YAMS_OK) return rc;
     emit_sorted_kernel<<<(p.k + 255) / 256, 256, 0, st>>>(c->dense.as<uint64_t>(), c->n, p.k, q, c->rowids.as<int64_t>(), l2 ? 1 : 0,
                                                           l2 ? INFINITY : -INFINITY, p.out.rowids, p.out.scores, p.out.counts, p.out.flags);
     YB_CUDA(cudaGetLastError());
@@ -1497,7 +1556,7 @@ static yams_status_t resolve_uncertain(Corpus* c, const ScanPlan& p, const uint3
     float* d_bound1 = reinterpret_cast<float*>(d_sel1_n + G);
     launch_eps_cc(c, p.nq, c->eps2.as<float>(), false);
     Stage1Args a{};
-    fill_stage1_common(c, a, p.nq);
+    fill_stage1_common(c, a, p.nq, p.graph);
     for (uint32_t g0 = 0; g0 < n_bad; g0 += G) {
         uint32_t g = std::min<uint32_t>(G, n_bad - g0);
         for (uint32_t i = 0; i < g; ++i) {
@@ -1603,7 +1662,7 @@ void yams_b200_corpus_destroy(yams_b200_corpus* c) {
     if (c->st) cudaStreamSynchronize(c->st);
     for (DevBuf* b : {&c->rows, &c->rowids, &c->inv_norm, &c->q32, &c->q16, &c->qinv, &c->tau, &c->counts, &c->cands,
                       &c->sample_scores, &c->sel, &c->outbuf, &c->dense, &c->mask, &c->misc, &c->qnorm, &c->dout, &c->stats, &c->status,
-                      &c->bound, &c->eps, &c->eps2, &c->lvl})
+                      &c->bound, &c->eps, &c->eps2, &c->lvl, &c->graph})
         b->release();
     c->h_pin.release();
     for (auto& e : c->ev)
@@ -1749,19 +1808,33 @@ void* yams_b200_corpus_stream(yams_b200_corpus* c) { return c ? (void*)c->st : n
 
 // uploads the queries and enqueues their preparation: q32, qinv, qnorm on the device, status block zeroed,
 // invalid queries counted in status->n_invalid (read by the host together with the results -- no synchronisation here)
-static yams_status_t prepare_queries(yams_b200_corpus* c, const float* q_src, bool src_is_device, uint32_t nq) {
+static yams_status_t reserve_queries(yams_b200_corpus* c, uint32_t nq) {
     yams_status_t rc;
-    size_t qb = (size_t)nq * c->dim * 4;
-    if ((rc = c->q32.reserve(qb)) != YAMS_OK) return rc;
+    if ((rc = c->q32.reserve((size_t)nq * c->dim * 4)) != YAMS_OK) return rc;
     if ((rc = c->qinv.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
     if ((rc = c->qnorm.reserve((size_t)nq * 8)) != YAMS_OK) return rc;
     if ((rc = c->counts.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
     if ((rc = c->status.reserve(sizeof(ScanStatus) + (size_t)nq * 8)) != YAMS_OK) return rc;
     if ((rc = c->h_pin.reserve(sizeof(ScanStatus) + (size_t)nq * 8 + 64)) != YAMS_OK) return rc;
     YB_CUDA(cudaMemsetAsync(c->status.p, 0, sizeof(ScanStatus), c->st));
+    return YAMS_OK;
+}
+static yams_status_t prepare_queries(yams_b200_corpus* c, const float* q_src, bool src_is_device, uint32_t nq) {
+    yams_status_t rc;
+    size_t qb = (size_t)nq * c->dim * 4;
+    if ((rc = reserve_queries(c, nq)) != YAMS_OK) return rc;
     YB_CUDA(cudaMemcpyAsync(c->q32.p, q_src, qb, src_is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, c->st));
     query_prep_kernel<<<(nq + QP_THREADS - 1) / QP_THREADS, QP_THREADS, 0, c->st>>>(c->q32.as<float>(), nq, c->dim, c->qnorm.as<double>(),
                                                                                   c->qinv.as<float>(), c->metric, status_of(c));
+    YB_CUDA(cudaGetLastError());
+    return YAMS_OK;
+}
+// the semantic-graph form: the sources of batch p (all of them taken) as queries; the status block zeroed
+static yams_status_t prepare_sources(yams_b200_corpus* c, const ScanPlan& p) {
+    yams_status_t rc;
+    if ((rc = reserve_queries(c, p.nq)) != YAMS_OK) return rc;
+    gather_sources_kernel<<<key_grid((uint64_t)p.nq * c->dim), 256, 0, c->st>>>(c->rows.p, c->dtype, c->dim, *p.graph, p.nq,
+                                                                               c->q32.as<float>(), c->qinv.as<float>());
     YB_CUDA(cudaGetLastError());
     return YAMS_OK;
 }
@@ -1816,12 +1889,13 @@ static yams_status_t enqueue_status_readback(yams_b200_corpus* c, uint32_t nq) {
     return YAMS_OK;
 }
 
-// Enqueues search p on the queries at q_src: their preparation, the candidate sets (host allowed_rowids / allowed_offsets,
-// nullable) as p's device lists or mask, the scan and the read-back of its status block.  No host synchronisation.
+// Enqueues search p on the queries at q_src (a semantic-graph batch: on its sources): their preparation, the candidate sets
+// (host allowed_rowids / allowed_offsets, nullable) as p's device lists or mask, the scan and the read-back of its status
+// block.  No host synchronisation.
 static yams_status_t enqueue_search(yams_b200_corpus* c, ScanPlan& p, const float* q_src, bool src_is_device, const int64_t* allowed_rowids,
                                     const uint64_t* allowed_offsets) {
     yams_status_t rc;
-    if ((rc = prepare_queries(c, q_src, src_is_device, p.nq)) != YAMS_OK) return rc;
+    if ((rc = p.graph ? prepare_sources(c, p) : prepare_queries(c, q_src, src_is_device, p.nq)) != YAMS_OK) return rc;
     YB_CUDA(cudaEventRecord(c->ev[0], c->st));
     if (p.direct) rc = upload_direct_lists(c, p.nq, allowed_rowids, allowed_offsets, &p.lists);
     else if (allowed_offsets && c->n) rc = upload_mask(c, p.nq, allowed_rowids, allowed_offsets, &p.d_mask, &p.mask_ld);
@@ -2005,6 +2079,147 @@ yams_status_t yams_b200_search_all_matching(yams_b200_corpus* c, const float* qu
     *out_count = h_cnt;
     return YAMS_OK;
     YB_CATCH
+}
+
+// The semantic graph's rows (GraphRows): its scales and statistics over its own row set, one row_stats_kernel pass with the
+// reference's inv > 0 rule, in c->graph; *h_inv = the scales on the host (the valid sources), *h_rowids = the corpus rowids.
+// g->src_row has room for kGraphBatch sources.
+static yams_status_t graph_rows(yams_b200_corpus* c, GraphRows* g, std::vector<float>* h_inv, std::vector<int64_t>* h_rowids) {
+    yams_status_t rc;
+    const uint64_t n = c->n;
+    if ((rc = c->graph.reserve((size_t)n * 4 + 16 + (size_t)kGraphBatch * 4 + 64)) != YAMS_OK) return rc;
+    float* inv = c->graph.as<float>();
+    float* stats = inv + n;
+    YB_CUDA(cudaMemsetAsync(stats, 0, 16, c->st));
+    if (n) row_stats_kernel<<<(unsigned)((n + 127) / 128), 128, 0, c->st>>>(c->rows.p, c->dtype, c->dim, 0, n, inv, YAMS_B200_COSINE, stats, 0.0);
+    YB_CUDA(cudaGetLastError());
+    float h_stats[4];
+    h_inv->resize(n);
+    h_rowids->resize(n);
+    YB_CUDA(cudaMemcpyAsync(h_stats, stats, 16, cudaMemcpyDeviceToHost, c->st));
+    YB_CUDA(cudaMemcpyAsync(h_inv->data(), inv, (size_t)n * 4, cudaMemcpyDeviceToHost, c->st));
+    YB_CUDA(cudaMemcpyAsync(h_rowids->data(), c->rowids.p, (size_t)n * 8, cudaMemcpyDeviceToHost, c->st));
+    YB_CUDA(cudaStreamSynchronize(c->st));
+    g->inv = inv;
+    g->r_max = h_stats[0]; g->dr_abs_max = h_stats[1]; g->dr_rel_max = h_stats[2]; g->inv_max = h_stats[3];
+    g->uf = (float)((c->dim + 4.0) * 0x1p-126 * (double)g->inv_max);   // +inf with a row whose scale is +inf
+    g->src_row = reinterpret_cast<const uint32_t*>(stats + 4);
+    return YAMS_OK;
+}
+
+yams_status_t yams_b200_semantic_neighbors(yams_b200_corpus* c, const int64_t* source_rowids, uint64_t n_sources, uint32_t k,
+                                           float threshold, int64_t* out_rowids, float* out_sims, uint32_t* out_counts,
+                                           uint64_t* out_flags) {
+    YB_TRY
+    YB_ARG(c, "corpus is null");
+    std::lock_guard<std::mutex> corpus_lock(c->mu);
+    YB_BIND(c);
+    YB_ARG(c->metric == YAMS_B200_COSINE, "the semantic graph needs a cosine corpus");
+    YB_ARG(source_rowids || n_sources == c->n, "without source_rowids, n_sources must equal the corpus size");
+    YB_ARG(k <= kMaxK, "k > 3072 is not supported by the fused top-k path");
+    YB_ARG(threshold == threshold, "threshold is NaN");
+    if (n_sources == 0) return YAMS_OK;
+    YB_ARG(out_counts, "null argument");
+    if (source_rowids)
+        for (uint64_t i = 1; i < n_sources; ++i) YB_ARG(source_rowids[i - 1] < source_rowids[i], "source_rowids must be strictly ascending");
+    for (uint64_t i = 0; i < n_sources; ++i) out_counts[i] = 0;
+    if (out_flags) for (uint64_t i = 0; i < n_sources; ++i) out_flags[i] = 0;
+    if (k == 0) return YAMS_OK;
+    YB_ARG(out_rowids && out_sims, "null output");
+    if (out_flags) for (uint64_t i = 0; i < n_sources; ++i) out_flags[i] = YAMS_B200_FLAG_NOT_A_SOURCE;   // until answered
+    for (uint64_t i = 0; i < n_sources * k; ++i) { out_rowids[i] = -1; out_sims[i] = 0.f; }
+    c->pending.active = false;
+    yams_status_t rc;
+    GraphRows g;
+    std::vector<float> h_inv;
+    std::vector<int64_t> h_rowids;
+    if ((rc = graph_rows(c, &g, &h_inv, &h_rowids)) != YAMS_OK) return rc;
+    // the valid sources: their corpus rows and output slots (unknown rowids and rows the graph does not take keep count 0)
+    std::vector<uint32_t> src_row;
+    std::vector<uint64_t> slot;
+    for (uint64_t i = 0, r = 0; i < n_sources; ++i) {
+        if (source_rowids) {
+            while (r < c->n && h_rowids[r] < source_rowids[i]) ++r;
+            if (r == c->n || h_rowids[r] != source_rowids[i]) continue;
+        } else {
+            r = i;
+        }
+        if (h_inv[r] > 0.f) { src_row.push_back((uint32_t)r); slot.push_back(i); }
+    }
+    const uint64_t nv = src_row.size();
+    if (nv == 0) return YAMS_OK;
+    DeviceResults all;
+    if ((rc = reserve_results(c->dout, (uint32_t)nv, k, &all)) != YAMS_OK) return rc;   // nv <= rows < 2^32
+    for (uint64_t b0 = 0; b0 < nv; b0 += kGraphBatch) {
+        const uint32_t nb = (uint32_t)std::min<uint64_t>(kGraphBatch, nv - b0);
+        YB_CUDA(cudaMemcpyAsync(const_cast<uint32_t*>(g.src_row), src_row.data() + b0, (size_t)nb * 4, cudaMemcpyHostToDevice, c->st));
+        ScanPlan p;
+        p.nq = nb; p.k = k; p.threshold = threshold; p.graph = &g;
+        p.out.rowids = all.rowids + b0 * k; p.out.flags = all.flags + b0;
+        p.out.scores = all.scores + b0 * k; p.out.counts = all.counts + b0;
+        if ((rc = enqueue_search(c, p, nullptr, false, nullptr, nullptr)) != YAMS_OK) return rc;
+        YB_CUDA(cudaStreamSynchronize(c->st));
+        uint32_t resolved = 0;
+        if ((rc = finish_search(c, p, nullptr, nullptr, &resolved)) != YAMS_OK) return rc;
+        if (threshold <= 0.f)
+            restore_zero_signs_kernel<<<(unsigned)(((uint64_t)nb * k + 255) / 256), 256, 0, c->st>>>(
+                c->rows.p, c->dtype, c->dim, c->q32.as<float>(), g, c->rowids.as<int64_t>(), c->n, p.out, nb, k);
+        YB_CUDA(cudaGetLastError());
+    }
+    std::vector<int64_t> rid(nv * k);
+    std::vector<float> sim(nv * k);
+    std::vector<uint32_t> cnt(nv);
+    std::vector<uint64_t> flg(nv);
+    if ((rc = copy_results(all, (uint32_t)nv, k, rid.data(), sim.data(), cnt.data(), flg.data(), c->st)) != YAMS_OK) return rc;
+    for (uint64_t i = 0; i < nv; ++i) {
+        const uint64_t s = slot[i];
+        out_counts[s] = cnt[i];
+        if (out_flags) out_flags[s] = flg[i];
+        for (uint32_t j = 0; j < cnt[i]; ++j) {
+            out_rowids[s * k + j] = rid[i * k + j];
+            out_sims[s * k + j] = sim[i * k + j];
+        }
+    }
+    return YAMS_OK;
+    YB_CATCH
+}
+
+yams_status_t yams_b200_debug_semantic_stage1(yams_b200_corpus* c, const int64_t* source_rowids, uint32_t n_sources, int engine,
+                                              float* out_scores, float* out_eps) {
+    YB_ARG(c && source_rowids && out_scores && out_eps && n_sources > 0 && n_sources <= kGraphBatch, "bad argument");
+    std::lock_guard<std::mutex> corpus_lock(c->mu);
+    YB_ARG(c->metric == YAMS_B200_COSINE && c->n > 0, "needs a non-empty cosine corpus");
+    yams_status_t rc;
+    YB_BIND(c);
+    c->pending.active = false;
+    GraphRows g;
+    std::vector<float> h_inv;
+    std::vector<int64_t> h_rowids;
+    if ((rc = graph_rows(c, &g, &h_inv, &h_rowids)) != YAMS_OK) return rc;
+    std::vector<uint32_t> src_row(n_sources);
+    for (uint32_t i = 0; i < n_sources; ++i) {
+        const auto it = std::lower_bound(h_rowids.begin(), h_rowids.end(), source_rowids[i]);
+        YB_ARG(it != h_rowids.end() && *it == source_rowids[i] && h_inv[it - h_rowids.begin()] > 0.f, "every source must be a taken row");
+        src_row[i] = (uint32_t)(it - h_rowids.begin());
+    }
+    YB_CUDA(cudaMemcpyAsync(const_cast<uint32_t*>(g.src_row), src_row.data(), (size_t)n_sources * 4, cudaMemcpyHostToDevice, c->st));
+    ScanPlan p;
+    p.nq = n_sources; p.graph = &g;
+    if ((rc = prepare_sources(c, p)) != YAMS_OK) return rc;
+    if ((rc = c->dense.reserve((size_t)n_sources * c->n * 4)) != YAMS_OK) return rc;
+    if ((rc = c->eps.reserve((size_t)n_sources * 4)) != YAMS_OK) return rc;
+    Stage1Args a{};
+    fill_stage1_common(c, a, n_sources, &g);
+    a.row_start = 0; a.row_stride = 1; a.nrows = c->n;
+    a.out_scores = c->dense.as<float>(); a.ld = c->n;
+    Stage1Engine s1{c, engine == 1, false};
+    if ((rc = s1.run(a, false)) != YAMS_OK) return rc;
+    s1.launch_eps(n_sources);
+    YB_CUDA(cudaMemcpyAsync(out_scores, c->dense.p, (size_t)n_sources * c->n * 4, cudaMemcpyDeviceToHost, c->st));
+    YB_CUDA(cudaMemcpyAsync(out_eps, c->eps.p, (size_t)n_sources * 4, cudaMemcpyDeviceToHost, c->st));
+    YB_CUDA(cudaStreamSynchronize(c->st));
+    for (uint32_t i = 0; i < n_sources; ++i) out_eps[i] += graph_eps(h_inv[src_row[i]], g.uf);   // as final_kernel adds it
+    return YAMS_OK;
 }
 
 yams_status_t yams_b200_search_device(yams_b200_corpus* c, const float* d_queries, uint32_t nq, uint32_t k, float threshold,
@@ -2295,7 +2510,9 @@ yams_status_t yams_b200_debug_final(yams_b200_corpus* c, uint32_t nq, uint32_t K
     YB_CUDA(cudaMemcpyAsync(c->eps.p, eps, (size_t)nq * 4, cudaMemcpyHostToDevice, st));
     YB_CUDA(cudaMemcpyAsync(c->qnorm.p, qnorm, (size_t)nq * 8, cudaMemcpyHostToDevice, st));
     YB_CUDA(cudaMemsetAsync(c->status.p, 0, sizeof(ScanStatus) + (size_t)nq * 8, st));
-    CertArgs cert = cert_args(c, c->bound.as<float>(), c->eps.as<float>(), threshold, level, nq);
+    ScanPlan p;
+    p.nq = nq; p.threshold = threshold;
+    CertArgs cert = cert_args(c, p, c->bound.as<float>(), c->eps.as<float>(), level);
     cert.metric = metric;   // either result convention on any corpus
     launch_final(d_ex, ex_n ? d_ex_n : nullptr, Kp, k, c->rowids.as<int64_t>(), r, nq, nullptr, cert, st);
     YB_CUDA(cudaGetLastError());

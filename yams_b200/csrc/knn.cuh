@@ -37,6 +37,15 @@ struct DirectLists {
     uint32_t max_len = 0;
 };
 
+// The semantic-neighbour graph's rows (yams_b200_semantic_neighbors): its own row set and scales, which replace the search's
+// cached inv_norm and statistics in stage 1 and the exact score, and the source row of each query of a batch
+struct GraphRows {
+    const float* inv = nullptr;          // n: float(1 / sqrt(sum (double)r^2)) of the rows the graph takes, else 0
+    float r_max = 0.f, dr_abs_max = 0.f, dr_rel_max = 0.f, inv_max = 0.f;   // row_stats_kernel over those rows
+    float uf = 0.f;                      // the certificate's underflow term per unit of max(1/|s|, 1) (knn.cu graph_eps)
+    const uint32_t* src_row = nullptr;   // nq: corpus row of source q (never its own neighbour)
+};
+
 // one exact search (knn.cu): the candidate-set form it scans and the device results it writes, from the enqueue to the finish
 struct ScanPlan {
     uint32_t nq = 0, k = 0;
@@ -45,6 +54,7 @@ struct ScanPlan {
     DirectLists lists;
     const uint32_t* d_mask = nullptr;   // else nullable: bit matrix [nq][mask_ld*32] of allowed rows -> masked corpus pass
     uint64_t mask_ld = 0;
+    const GraphRows* graph = nullptr;   // a batch of semantic-graph sources instead of queries
     DeviceResults out;
 };
 
@@ -71,6 +81,7 @@ struct Corpus {
     DevBuf status;     // ScanStatus + bad[nq] + bad2[nq] of the call in flight
     DevBuf bound, eps, eps2;   // per query: certificate inputs (knn.cu final_kernel)
     DevBuf lvl;        // exhaustive level 1 workspace
+    DevBuf graph;      // semantic graph: inv[n] + stats[4] + the batch's source rows
     HostBuf h_pin;
     // the call enqueued by search_device and not yet finished (search_device_finish)
     struct Pending {

@@ -15,6 +15,7 @@
 #include <stdexcept>
 #include <algorithm>
 #include <cmath>
+#include <limits>
 #include <map>
 #include <optional>
 #include <string>
@@ -820,6 +821,79 @@ private:
         }
     }
     yams_b200_digest_set* s_ = nullptr;
+};
+
+// One document-level vector as forEachDocumentLevelVector streams it (sqlite_vec_backend.cpp:1818-1862): the fields the
+// semantic graph reads.
+struct SemanticDoc {
+    std::string hash;               // document_hash
+    std::vector<float> embedding;
+};
+
+// The pair loop of EmbeddingService::updateSemanticNeighborGraphUnlocked (EmbeddingService.cpp:856-1030) and of
+// rebuildSemanticNeighborGraphForCorpus (:1119-1156) on the device: every source document's top-k neighbour documents.  The
+// daemon keeps the edge weights, ranks and KG writes (:1038-1075).
+class B200SemanticGraph {
+public:
+    using Neighbors = std::vector<std::pair<std::string, float>>;   // (document_hash, similarity) in rank order
+    // docs: the streamed records (empty hashes and embeddings skipped, the first record per hash kept, :864-882); sources: the
+    // requested hashes (empty = every document, the rebuild).  out: one entry per source document that has an embedding with
+    // a positive norm, in hash order, with its neighbours (none above the threshold: an empty list).  explicitThreshold is
+    // YAMS_GRAPH_SEMANTIC_THRESHOLD (clamped to [0, 1] here, :395-403); nullopt is the adaptive mode (sim > 0).
+    // YAMS_ERR_UNSUPPORTED when the embeddings have more than one dimension: the reference scores those pairs 0, and the
+    // caller keeps its own loop.  Unlike the reference's streaming branch above 250 000 pairs (:555-610, HNSW), the answer is
+    // always exact.
+    static yams_status_t neighbors(const std::vector<SemanticDoc>& docs, const std::vector<std::string>& sources, size_t topK,
+                                   std::optional<float> explicitThreshold, std::vector<std::pair<std::string, Neighbors>>* out) {
+        out->clear();
+        std::unordered_set<std::string> seen;
+        std::vector<const SemanticDoc*> corpus;
+        for (const auto& d : docs)
+            if (!d.hash.empty() && !d.embedding.empty() && seen.insert(d.hash).second) corpus.push_back(&d);
+        if (corpus.empty() || topK == 0) return YAMS_OK;
+        const size_t dim = corpus[0]->embedding.size();
+        for (const auto* d : corpus)
+            if (d->embedding.size() != dim) return YAMS_ERR_UNSUPPORTED;
+        if (topK > 3072) return YAMS_ERR_INVALID_ARG;
+        std::sort(corpus.begin(), corpus.end(), [](const SemanticDoc* a, const SemanticDoc* b) { return a->hash < b->hash; });
+        // the daemon's own float values: an fp32 corpus (the tf32 tensor-core engine), rowid = position in hash order
+        std::vector<float> rows(corpus.size() * dim);
+        std::vector<int64_t> rowids(corpus.size());
+        for (size_t i = 0; i < corpus.size(); ++i) {
+            std::memcpy(rows.data() + i * dim, corpus[i]->embedding.data(), dim * sizeof(float));
+            rowids[i] = (int64_t)i;
+        }
+        std::vector<int64_t> src;
+        if (!sources.empty()) {
+            std::unordered_set<std::string> want(sources.begin(), sources.end());
+            for (size_t i = 0; i < corpus.size(); ++i)
+                if (want.count(corpus[i]->hash)) src.push_back((int64_t)i);
+            if (src.empty()) return YAMS_OK;
+        }
+        const float threshold = explicitThreshold ? std::clamp(*explicitThreshold, 0.0f, 1.0f) : std::numeric_limits<float>::denorm_min();
+        yams_b200_corpus* c = nullptr;
+        yams_status_t st = yams_b200_corpus_create(nullptr, (uint32_t)dim, YAMS_B200_F32, YAMS_B200_COSINE, corpus.size(), &c);
+        if (st != YAMS_OK) return st;
+        const size_t ns = sources.empty() ? corpus.size() : src.size();
+        std::vector<int64_t> nb(ns * topK);
+        std::vector<float> sims(ns * topK);
+        std::vector<uint32_t> counts(ns);
+        std::vector<uint64_t> flags(ns);
+        st = yams_b200_corpus_append(c, rows.data(), corpus.size(), rowids.data());
+        if (st == YAMS_OK)
+            st = yams_b200_semantic_neighbors(c, sources.empty() ? nullptr : src.data(), ns, (uint32_t)topK, threshold, nb.data(),
+                                              sims.data(), counts.data(), flags.data());
+        yams_b200_corpus_destroy(c);
+        if (st != YAMS_OK) return st;
+        for (size_t i = 0; i < ns; ++i) {
+            const size_t row = sources.empty() ? i : (size_t)src[i];
+            if (flags[i] & YAMS_B200_FLAG_NOT_A_SOURCE) continue;   // zero-norm or non-finite document (:904, 916)
+            Neighbors list;
+            for (uint32_t j = 0; j < counts[i]; ++j) list.emplace_back(corpus[(size_t)nb[i * topK + j]]->hash, sims[i * topK + j]);
+            out->emplace_back(corpus[row]->hash, std::move(list));
+        }
+        return YAMS_OK;
+    }
 };
 
 }  // namespace yams_b200::host
