@@ -384,6 +384,29 @@ YAMS_B200_API yams_status_t yams_b200_semantic_neighbors(yams_b200_corpus* c, co
 YAMS_B200_API yams_status_t yams_b200_debug_semantic_stage1(yams_b200_corpus* c, const int64_t* source_rowids, uint32_t n_sources,
                                                             int engine, float* out_scores, float* out_eps);
 
+/* The k-means topology engine's clustering (KMeansTopologyEngine, src/topology/topology_alternate_engines.cpp:341-478 runKMeans):
+ * a deterministic spherical k-means over document-level embeddings, bit-identical to the reference.  c is a cosine corpus
+ * (fp32 or fp16, defined on the stored values; L2 -> YAMS_ERR_INVALID_ARG) of one row per USABLE document, appended in document
+ * order (documents without an embedding of the first embedding's size are the caller's singletons, see B200TopologyKMeans).
+ *   k          k_requested, or round(sqrt(rows)) when 0, clamped to [2, rows]
+ *   distance   cosineDistance: dot, |a|^2, |b|^2 as sequential double sums; 2.0 when a norm is <= 0, else
+ *              1 - clamp(dot / (sqrt(|a|^2) * sqrt(|b|^2)), -1, 1), a NaN kept
+ *   init       farthest-first: centroid 0 = normalized(row 0), then k - 1 picks of the first unselected row with the largest
+ *              distance to its nearest centroid so far
+ *   iterate    max_iterations (0 means 10) rounds of: assignment to the first centroid with the strictly smallest distance (0
+ *              when all are NaN); centroid = normalized(float mean of the members in row order) for every non-empty cluster;
+ *              empty clusters repaired in order by the row farthest from its centroid among clusters of more than one member;
+ *              stop when nothing changed
+ * Outputs (HOST): out_assignment[rows] = the cluster of every row, numbered as runKMeans numbers them; out_centroids
+ * (nullable) [k][dim] the final centroids; *out_k = k; *out_iterations = the rounds run.  Fewer than 2 rows: out_assignment[i] =
+ * i, *out_k = *out_iterations = 0.  Every distance is computed exactly in fp64 on the device (DESIGN.md §4.10). */
+YAMS_B200_API yams_status_t yams_b200_topology_kmeans(yams_b200_corpus* c, uint32_t k_requested, uint32_t max_iterations,
+                                                      uint32_t* out_assignment, float* out_centroids, uint32_t* out_k,
+                                                      uint32_t* out_iterations);
+/* the last yams_b200_topology_kmeans call on c: out_ms[0..2] device ms of the init, the assignments and the centroid updates
+ * (repairs included), out_ms[3] the call's host wall time */
+YAMS_B200_API yams_status_t yams_b200_topology_kmeans_last_timings(yams_b200_corpus* c, float out_ms[4]);
+
 /* Device-pointer form for multi-GPU sharding: queries and outputs are DEVICE pointers, the whole pipeline is enqueued on
  * the corpus stream and the call returns WITHOUT synchronising (query validity, list overflow and the exactness
  * certificate are evaluated on the device and parked in a status block).  Outputs are the rank-local partial top-k in

@@ -113,6 +113,8 @@ SYMBOLS = {
     "yams_b200_search_all_matching": (C.c_int, [C.c_void_p, f32p, C.c_float, i64p, C.c_uint64, i64p, f32p, u64p]),
     "yams_b200_semantic_neighbors": (C.c_int, [C.c_void_p, i64p, C.c_uint64, C.c_uint32, C.c_float, i64p, f32p, u32p, u64p]),
     "yams_b200_debug_semantic_stage1": (C.c_int, [C.c_void_p, i64p, C.c_uint32, C.c_int, f32p, f32p]),
+    "yams_b200_topology_kmeans": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, u32p, f32p, u32p, u32p]),
+    "yams_b200_topology_kmeans_last_timings": (C.c_int, [C.c_void_p, f32p]),
     "yams_b200_search_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_float, C.c_void_p, C.c_void_p]),
     "yams_b200_search_device_finish": (C.c_int, [C.c_void_p, u32p]),
     "yams_b200_search_exhaustive": (C.c_int, [C.c_void_p, f32p, C.c_uint32, C.c_uint32, C.c_float, i64p, f32p, u32p, u64p]),
@@ -496,6 +498,24 @@ class Corpus:
         _check(lib().yams_b200_debug_semantic_stage1(self._h, src.ctypes.data_as(i64p), len(src), engine, out.ctypes.data_as(f32p),
                                                      eps.ctypes.data_as(f32p)), "debug_semantic_stage1")
         return out, eps
+
+    def topology_kmeans(self, k: int = 0, max_iterations: int = 0):
+        """The k-means topology engine's spherical k-means (runKMeans) over the rows, one usable document each in document order:
+        k = 0 is round(sqrt(rows)), max_iterations = 0 is 10.  -> (assignment u32[rows], centroids f32[k, dim], k, iterations)"""
+        n = len(self)
+        kk = 0 if n < 2 else min(max(k if k else int(np.floor(np.sqrt(n) + 0.5)), 2), n)
+        asg = np.empty(max(n, 1), dtype=np.uint32)
+        cent = np.empty((max(kk, 1), self.dim), dtype=np.float32)
+        k_out, it_out = C.c_uint32(), C.c_uint32()
+        _check(lib().yams_b200_topology_kmeans(self._h, k, max_iterations, asg.ctypes.data_as(u32p), cent.ctypes.data_as(f32p),
+                                               C.byref(k_out), C.byref(it_out)), "topology_kmeans")
+        assert k_out.value == kk
+        return asg[:n], cent[:kk], k_out.value, it_out.value
+
+    def topology_kmeans_last_timings(self) -> dict:
+        ms = (C.c_float * 4)()
+        _check(lib().yams_b200_topology_kmeans_last_timings(self._h, ms), "topology_kmeans_last_timings")
+        return {"init_ms": ms[0], "assign_ms": ms[1], "update_ms": ms[2], "total_ms": ms[3]}
 
     def search_device(self, d_queries: int, nq: int, k: int, threshold: float, d_out_rowids: int, d_out_scores: int):
         _check(lib().yams_b200_search_device(self._h, d_queries, nq, k, threshold, d_out_rowids, d_out_scores), "search_device")

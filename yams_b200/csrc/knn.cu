@@ -1662,7 +1662,7 @@ void yams_b200_corpus_destroy(yams_b200_corpus* c) {
     if (c->st) cudaStreamSynchronize(c->st);
     for (DevBuf* b : {&c->rows, &c->rowids, &c->inv_norm, &c->q32, &c->q16, &c->qinv, &c->tau, &c->counts, &c->cands,
                       &c->sample_scores, &c->sel, &c->outbuf, &c->dense, &c->mask, &c->misc, &c->qnorm, &c->dout, &c->stats, &c->status,
-                      &c->bound, &c->eps, &c->eps2, &c->lvl, &c->graph})
+                      &c->bound, &c->eps, &c->eps2, &c->lvl, &c->graph, &c->kmeans})
         b->release();
     c->h_pin.release();
     for (auto& e : c->ev)

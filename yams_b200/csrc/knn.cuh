@@ -82,6 +82,8 @@ struct Corpus {
     DevBuf bound, eps, eps2;   // per query: certificate inputs (knn.cu final_kernel)
     DevBuf lvl;        // exhaustive level 1 workspace
     DevBuf graph;      // semantic graph: inv[n] + stats[4] + the batch's source rows
+    DevBuf kmeans;     // topology k-means workspace (kmeans.cu)
+    float kmeans_ms[4] = {0, 0, 0, 0};   // the last k-means call: device ms of init, assignment, update; host wall ms
     HostBuf h_pin;
     // the call enqueued by search_device and not yet finished (search_device_finish)
     struct Pending {

@@ -896,4 +896,48 @@ public:
     }
 };
 
+// The k-means topology engine's clustering (KMeansTopologyEngine::buildArtifacts -> runKMeans,
+// src/topology/topology_alternate_engines.cpp:341-478): the per-document assignment runKMeans returns.  embeddings: each
+// document's embedding in span order (empty: none).  A usable document has a non-empty embedding of the first non-empty one's
+// size (:349-361); fewer than 2 usable -> every document is its own cluster (iota); the usable ones are clustered on the
+// device (yams_b200_topology_kmeans, an fp32 corpus of the daemon's own values), the others become singletons numbered k,
+// k + 1, ... in document order (:471-476).
+class B200TopologyKMeans {
+public:
+    static yams_status_t assign(const std::vector<std::span<const float>>& embeddings, size_t requestedK, size_t maxIterations,
+                                std::vector<int64_t>* out) {
+        const size_t n = embeddings.size();
+        out->assign(n, -1);
+        std::vector<size_t> usable;
+        size_t dim = 0;
+        for (size_t i = 0; i < n; ++i) {
+            if (embeddings[i].empty()) continue;
+            if (dim == 0) dim = embeddings[i].size();
+            if (embeddings[i].size() == dim) usable.push_back(i);
+        }
+        if (usable.size() < 2) {
+            for (size_t i = 0; i < n; ++i) (*out)[i] = (int64_t)i;
+            return YAMS_OK;
+        }
+        if (usable.size() >= 0xFFFFFFFFull || requestedK > 0xFFFFFFFFull || maxIterations > 0xFFFFFFFFull) return YAMS_ERR_INVALID_ARG;
+        std::vector<float> rows(usable.size() * dim);
+        for (size_t u = 0; u < usable.size(); ++u) std::memcpy(rows.data() + u * dim, embeddings[usable[u]].data(), dim * sizeof(float));
+        yams_b200_corpus* c = nullptr;
+        yams_status_t st = yams_b200_corpus_create(nullptr, (uint32_t)dim, YAMS_B200_F32, YAMS_B200_COSINE, usable.size(), &c);
+        if (st != YAMS_OK) return st;
+        std::vector<uint32_t> membership(usable.size());
+        uint32_t k = 0, iterations = 0;
+        st = yams_b200_corpus_append(c, rows.data(), usable.size(), nullptr);
+        if (st == YAMS_OK)
+            st = yams_b200_topology_kmeans(c, (uint32_t)requestedK, (uint32_t)maxIterations, membership.data(), nullptr, &k, &iterations);
+        yams_b200_corpus_destroy(c);
+        if (st != YAMS_OK) return st;
+        for (size_t u = 0; u < usable.size(); ++u) (*out)[usable[u]] = membership[u];
+        int64_t singleton = k;
+        for (size_t i = 0; i < n; ++i)
+            if ((*out)[i] < 0) (*out)[i] = singleton++;
+        return YAMS_OK;
+    }
+};
+
 }  // namespace yams_b200::host
