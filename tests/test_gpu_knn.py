@@ -474,6 +474,8 @@ def test_candidate_sets_direct_and_masked_paths(Y, oracle, dtype_name, d):
     n, nq, k = 150_000, 6, 10
     rows32 = O.gen_rows_f32(21, 0, n, d)
     rows32[500] = 0
+    rows32[501, 1] = np.nan                       # non-finite rows are skipped, also from the scalar loop (f16, d = 20)
+    rows32[502, d - 2] = np.inf
     if dtype_name == "f16":
         stored = O.f16_from_float(rows32).reshape(n, d)
         c = Y.Corpus(d, Y.F16, Y.COSINE)
@@ -494,11 +496,11 @@ def test_candidate_sets_direct_and_masked_paths(Y, oracle, dtype_name, d):
             assert cnt[qi] == len(wr) and list(rid[qi, :len(wr)]) == list(wr), (what, qi)
             assert np.array_equal(sc[qi, :len(wr)], ws), (what, qi)
 
-    # direct: ascending lists with repeats, ids that do not exist, a list shorter than k, an empty list, the zero row
+    # direct: ascending lists with repeats, ids that do not exist, a list shorter than k, an empty list, the zero and non-finite rows
     small = []
     for qi in range(nq):
         sel = np.sort(rng.choice(n, size=[3, 40, 700, 5000, 1, 2500][qi], replace=False))
-        small.append(np.sort(np.concatenate([sel, sel[:2], [500], [n + 5, n + 9]])).astype(np.int64))
+        small.append(np.sort(np.concatenate([sel, sel[:2], [500, 501, 502], [n + 5, n + 9]])).astype(np.int64))
     small[4] = np.zeros(0, dtype=np.int64)
     check(small, "direct")
     # masked pass, few allowed rows (unsorted lists cannot take the direct path): thresholds fall back to -inf

@@ -1,6 +1,6 @@
-// cosine.cuh -- device building blocks shared by the exact scan (knn.cu), the PQ engine (pq.cu) and the sqlite-vec operators
-// (operators.cu): the exact per-row similarity, the score keys every ordered path ranks by, the in-block key sort and the
-// rowid -> row lookup.
+// cosine.cuh -- device building blocks shared by the exact scan (knn.cu), the PQ engine (pq.cu), k-means (kmeans.cu) and the
+// sqlite-vec operators (operators.cu): the double-precision element walk over a row and the exact similarities built on it, the
+// score keys every ordered path ranks by, the in-block key sort and the rowid -> row lookup.
 #pragma once
 #include <cuda_fp16.h>
 #include <math.h>
@@ -59,59 +59,114 @@ __device__ __forceinline__ uint64_t find_row(const int64_t* __restrict__ rowids,
     return (a < n && rowids[a] == want) ? a : n;
 }
 
-// Sequential double sums of corpus row `row` against qv (fp32, 16-byte aligned): *norm_sq = sum r^2, *dot = sum r q, in the
-// reference's element order; -> false when the row holds a non-finite element (the sums are then partial).
+// f(x) for each element x of the N-element 16-byte chunk `raw` (fp16: N = 8, fp32: N = 4) that starts at element c; PAIR:
+// f(x, y), y the matching element of the fp32 vector v, read one element at a time: where the threads of a warp share the vector
+// (the re-scoring kernels, the k-means init) these reads are broadcasts, and 16-byte reads of it take pq_rerank_kernel past the
+// 32 registers of full occupancy
+template <bool PAIR, int N, typename F>
+__device__ __forceinline__ void visit_chunk(const uint4& raw, const float* __restrict__ v, uint32_t c, F& f) {
+    float x[N];
+    if constexpr (N == 8) {
+        const __half2* h2 = reinterpret_cast<const __half2*>(&raw);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const float2 p = __half22float2(h2[e]);
+            x[2 * e] = p.x;
+            x[2 * e + 1] = p.y;
+        }
+    } else {
+        x[0] = __uint_as_float(raw.x); x[1] = __uint_as_float(raw.y); x[2] = __uint_as_float(raw.z); x[3] = __uint_as_float(raw.w);
+    }
+    if constexpr (PAIR) {
+#pragma unroll
+        for (int e = 0; e < N; ++e) f(x[e], __ldg(v + c + e));
+    } else {
+#pragma unroll
+        for (int e = 0; e < N; ++e) f(x[e]);
+    }
+}
+
+// the d / N chunks of a row (d % N == 0), G per trip with their loads issued together, then the rest one per trip
+template <bool PAIR, int G, int N, typename F>
+__device__ __forceinline__ void walk_chunks(const uint4* __restrict__ rp, uint32_t d, const float* __restrict__ v, F& f) {
+    uint32_t c = 0;
+#pragma unroll 1
+    for (; c + G * N <= d; c += G * N) {
+        uint4 raw[G];
+#pragma unroll
+        for (int g = 0; g < G; ++g) raw[g] = __ldg(rp + c / N + g);
+#pragma unroll
+        for (int g = 0; g < G; ++g) visit_chunk<PAIR, N>(raw[g], v, c + g * N, f);
+    }
+#pragma unroll 1
+    for (; c < d; c += N) visit_chunk<PAIR, N>(__ldg(rp + c / N), v, c, f);
+}
+
+template <bool PAIR, int G, typename F>
+__device__ __forceinline__ void walk_elems(const void* __restrict__ rows, int dtype, uint32_t d, uint64_t row, const float* __restrict__ v,
+                                           F& f) {
+    const uint64_t base = row * d;
+    if (dtype == YAMS_B200_F16 && d % 8 == 0) {
+        walk_chunks<PAIR, G, 8>(reinterpret_cast<const uint4*>(static_cast<const __half*>(rows) + base), d, v, f);
+    } else if (dtype == YAMS_B200_F32 && d % 4 == 0) {
+        walk_chunks<PAIR, G, 4>(reinterpret_cast<const uint4*>(static_cast<const float*>(rows) + base), d, v, f);
+    } else {
+#pragma unroll 1
+        for (uint32_t c = 0; c < d; ++c) {
+            const float x = load_elem(rows, dtype, base + c);
+            if constexpr (PAIR) f(x, v[c]);
+            else f(x);
+        }
+    }
+}
+
+// The element walk of every exact path (the reference sums floats into a double in element order): f(x) for each element x of
+// row `row` of the [rows][d] fp16/fp32 array, widened exactly to float, in element order.  An fp32 query row is walked with
+// dtype F32.  Loads are 16 bytes wide where d keeps every row 16-byte aligned (fp16: d % 8 == 0, fp32: d % 4 == 0), and one
+// element at a time otherwise.  G > 1 issues the loads of G 16-byte chunks together, for callers whose kernels have the
+// registers to spare (one dependent load per trip leaves a thread latency-bound).  There is no early exit: f sees every
+// element and does the accumulating and any finiteness tracking.
+template <int G = 1, typename F>
+__device__ __forceinline__ void walk_row(const void* __restrict__ rows, int dtype, uint32_t d, uint64_t row, F&& f) {
+    walk_elems<false, G>(rows, dtype, d, row, nullptr, f);
+}
+// ... f(x, y) with y the matching element of the fp32 vector v
+template <int G = 1, typename F>
+__device__ __forceinline__ void walk_row_pair(const void* __restrict__ rows, int dtype, uint32_t d, uint64_t row, const float* __restrict__ v,
+                                              F&& f) {
+    walk_elems<true, G>(rows, dtype, d, row, v, f);
+}
+
+// Sequential double sums of corpus row `row` against qv (fp32): *norm_sq = sum r^2, *dot = sum r q, in the reference's element
+// order; -> false when the row holds a non-finite element (the sums then mean nothing).  Four chunks per trip: the re-scoring
+// kernels stay within the registers of their occupancy.
 __device__ __forceinline__ bool row_dot(const void* __restrict__ rows, int dtype, uint32_t d, uint32_t row, const float* __restrict__ qv,
                                         double* norm_sq_out, double* dot_out) {
-    const uint64_t base = (uint64_t)row * d;
     double norm_sq = 0.0, dot = 0.0;
     bool finite = true;
-    // same element order as the reference's loop; only the loads are widened (16-byte row and query chunks)
-    uint32_t c = 0;
-    if (dtype == YAMS_B200_F16 && d % 8 == 0) {
-        const uint4* rp = reinterpret_cast<const uint4*>(static_cast<const __half*>(rows) + base);
-        const float4* qp = reinterpret_cast<const float4*>(qv);
-        for (; c < d; c += 8) {
-            const uint4 raw = __ldg(rp + (c >> 3));
-            const float4 q0 = __ldg(qp + (c >> 2)), q1 = __ldg(qp + (c >> 2) + 1);
-            const __half2* h2 = reinterpret_cast<const __half2*>(&raw);
-            const float2 f0 = __half22float2(h2[0]), f1 = __half22float2(h2[1]), f2 = __half22float2(h2[2]), f3 = __half22float2(h2[3]);
-            const float rv[8] = {f0.x, f0.y, f1.x, f1.y, f2.x, f2.y, f3.x, f3.y};
-            const float qq[8] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w};
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-                if (!isfinite(rv[e])) finite = false;
-                const double sv = (double)rv[e];
-                norm_sq += sv * sv;
-                dot += sv * (double)qq[e];
-            }
-        }
-    } else if (dtype == YAMS_B200_F32 && d % 4 == 0) {
-        const float4* rp = reinterpret_cast<const float4*>(static_cast<const float*>(rows) + base);
-        const float4* qp = reinterpret_cast<const float4*>(qv);
-        for (; c < d; c += 4) {
-            const float4 r4 = __ldg(rp + (c >> 2)), q4 = __ldg(qp + (c >> 2));
-            const float rv[4] = {r4.x, r4.y, r4.z, r4.w};
-            const float qq[4] = {q4.x, q4.y, q4.z, q4.w};
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                if (!isfinite(rv[e])) finite = false;
-                const double sv = (double)rv[e];
-                norm_sq += sv * sv;
-                dot += sv * (double)qq[e];
-            }
-        }
-    }
-    for (; c < d; ++c) {
-        float v = load_elem(rows, dtype, base + c);
-        if (!isfinite(v)) { finite = false; break; }
-        double sv = (double)v, qd = (double)qv[c];
-        norm_sq += sv * sv;
-        dot += sv * qd;
-    }
+    walk_row_pair<4>(rows, dtype, d, row, qv, [&](float x, float y) {
+        if (!isfinite(x)) finite = false;
+        norm_sq += (double)x * x;
+        dot += (double)x * y;
+    });
     *norm_sq_out = norm_sq;
     *dot_out = dot;
     return finite;
+}
+
+// VectorDatabase::computeCosineSimilarity (vector_database.cpp:1786-1810) of the fp32 vector a against row `row`: double sums
+// of a.b, a^2 and b^2 in element order, 0 when either norm is 0, else dot / (|a| |b|)
+__device__ __forceinline__ double compute_cosine_similarity(const void* __restrict__ rows, int dtype, uint32_t d, uint64_t row,
+                                                            const float* __restrict__ a) {
+    double dp = 0.0, na = 0.0, nb = 0.0;
+    walk_row_pair(rows, dtype, d, row, a, [&](float y, float x) {   // the reference's names: x of a, y of the row (its b)
+        dp += (double)x * y;
+        na += (double)x * x;
+        nb += (double)y * y;
+    });
+    na = sqrt(na);
+    nb = sqrt(nb);
+    return (na == 0.0 || nb == 0.0) ? 0.0 : dp / (na * nb);
 }
 
 // bruteForceSearchUnlocked's cosine (sqlite_vec_backend.cpp:4253-4279) of corpus row `row` against the query qv (fp32, 16-byte

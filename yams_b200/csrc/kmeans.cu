@@ -33,46 +33,6 @@ constexpr uint32_t kNone = 0xFFFFFFFFu;
 constexpr int kRedThreads = 256;   // argmax kernels
 constexpr int kPickThreads = 1024;
 
-// sequential double dot of document row `row` with the fp32 vector v (v = nullptr: the row with itself), loads widened to
-// 16 bytes where the pitch allows it; element order untouched, no early exit (a non-finite element propagates as in the
-// reference)
-__device__ __forceinline__ double km_row_dot(const void* __restrict__ rows, int dtype, uint32_t d, uint32_t row,
-                                             const float* __restrict__ v) {
-    const uint64_t base = (uint64_t)row * d;
-    double acc = 0.0;
-    uint32_t c = 0;
-    if (dtype == YAMS_B200_F16 && d % 8 == 0) {
-        const uint4* rp = reinterpret_cast<const uint4*>(static_cast<const __half*>(rows) + base);
-        for (; c < d; c += 8) {
-            const uint4 raw = __ldg(rp + (c >> 3));
-            const __half2* h2 = reinterpret_cast<const __half2*>(&raw);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const float2 f = __half22float2(h2[e]);
-                const double a0 = f.x, a1 = f.y;
-                acc += a0 * (v ? (double)__ldg(v + c + 2 * e) : a0);
-                acc += a1 * (v ? (double)__ldg(v + c + 2 * e + 1) : a1);
-            }
-        }
-    } else if (dtype == YAMS_B200_F32 && d % 4 == 0) {
-        const float4* rp = reinterpret_cast<const float4*>(static_cast<const float*>(rows) + base);
-        for (; c < d; c += 4) {
-            const float4 r4 = __ldg(rp + (c >> 2));
-            const float rv[4] = {r4.x, r4.y, r4.z, r4.w};
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const double a = rv[e];
-                acc += a * (v ? (double)__ldg(v + c + e) : a);
-            }
-        }
-    }
-    for (; c < d; ++c) {
-        const double a = load_elem(rows, dtype, base + c);
-        acc += a * (v ? (double)v[c] : a);
-    }
-    return acc;
-}
-
 // cosineDistance from its three sums (std::clamp keeps a NaN)
 __device__ __forceinline__ double km_distance(double dot, double na, double nb) {
     if (na <= 0.0 || nb <= 0.0) return 2.0;
@@ -137,7 +97,10 @@ __device__ void block_normalize(float* v, uint32_t d, float* __restrict__ out, d
 
 __global__ void km_norms_kernel(const void* __restrict__ rows, int dtype, uint32_t d, uint32_t n, double* __restrict__ na) {
     const uint32_t u = blockIdx.x * blockDim.x + threadIdx.x;
-    if (u < n) na[u] = km_row_dot(rows, dtype, d, u, nullptr);
+    if (u >= n) return;
+    double a = 0.0;
+    walk_row(rows, dtype, d, u, [&](float x) { a += (double)x * x; });
+    na[u] = a;
 }
 
 // Farthest-first step against centroid `cent` (norm cnorm): minDist[u] = min(minDist[u], d) (strict <) for the unselected
@@ -149,7 +112,9 @@ __global__ void __launch_bounds__(kRedThreads) km_far_step_kernel(const void* __
     const uint32_t u = blockIdx.x * blockDim.x + threadIdx.x;
     ArgMax m{-1.0, kNone};
     if (u < n && !selected[u]) {
-        const double dist = km_distance(km_row_dot(rows, dtype, d, u, cent), na[u], *cnorm);
+        double dot = 0.0;
+        walk_row_pair(rows, dtype, d, u, cent, [&](float x, float y) { dot += (double)x * y; });
+        const double dist = km_distance(dot, na[u], *cnorm);
         double md = min_dist[u];
         if (dist < md) { md = dist; min_dist[u] = md; }
         m = {md, u};
@@ -332,7 +297,9 @@ __global__ void __launch_bounds__(kRedThreads) km_repair_scan_kernel(const void*
     if (u < n) {
         const uint32_t mc = membership[u];
         if (size[mc] > 1) {
-            const double dist = km_distance(km_row_dot(rows, dtype, d, u, cent + (uint64_t)mc * d), na[u], cnorm[mc]);
+            double dot = 0.0;
+            walk_row_pair(rows, dtype, d, u, cent + (uint64_t)mc * d, [&](float x, float y) { dot += (double)x * y; });
+            const double dist = km_distance(dot, na[u], cnorm[mc]);
             if (dist > -1.0) m = {dist, u};
         }
     }

@@ -104,18 +104,16 @@ __global__ void row_stats_kernel(const void* __restrict__ rows, int dtype, uint3
                                  float* __restrict__ inv_norm, int metric, float* __restrict__ stats, double min_sq) {
     uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= n) return;
-    uint64_t base = (first + r) * (uint64_t)d;
     double ss = 0.0, res = 0.0;
     bool finite = true;
-    for (uint32_t c = 0; c < d; ++c) {
-        float v = load_elem(rows, dtype, base + c);
-        if (!isfinite(v)) { finite = false; break; }
-        ss += (double)v * (double)v;
+    walk_row(rows, dtype, d, first + r, [&](float v) {
+        if (!isfinite(v)) finite = false;
+        ss += (double)v * v;
         if (dtype == YAMS_B200_F32) {
             float t = v - __uint_as_float(__float_as_uint(v) & 0xFFFFE000u);
-            res += (double)t * (double)t;
+            res += (double)t * t;
         }
-    }
+    });
     if (metric == YAMS_B200_L2) inv_norm[first + r] = finite ? (float)ss : INFINITY;
     else inv_norm[first + r] = (finite && ss > min_sq) ? (float)(1.0 / sqrt(ss)) : 0.0f;
     if (finite && ss > 0.0) {
@@ -143,36 +141,16 @@ struct ScanStatus {
 constexpr int QP_THREADS = 32;
 __global__ void __launch_bounds__(QP_THREADS) query_prep_kernel(const float* __restrict__ q, uint32_t nq, uint32_t d, double* __restrict__ qnorm,
                                                                 float* __restrict__ qinv, int metric, ScanStatus* __restrict__ status) {
-    // thread = query, the reference's sequential double sum (sqlite_vec_backend.cpp:4140-4150).  The row is read with 16-byte
-    // loads, four in flight (one 4-byte load per dependent trip cost 64 us for 1024 x 768 queries).
+    // thread = query, the reference's sequential double sum (sqlite_vec_backend.cpp:4140-4150).  The walk keeps four 16-byte
+    // loads in flight (one 4-byte load per dependent trip cost 64 us for 1024 x 768 queries).
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= nq) return;
-    const float* row = q + (uint64_t)i * d;
     double ss = 0.0;
     bool finite = true;
-    auto add = [&](float v) {
+    walk_row<4>(q, YAMS_B200_F32, d, i, [&](float v) {
         if (!isfinite(v)) finite = false;
-        ss += (double)v * (double)v;
-    };
-    uint32_t c = 0;
-    if ((reinterpret_cast<uintptr_t>(row) & 15u) == 0) {
-        const float4* r4 = reinterpret_cast<const float4*>(row);
-        const uint32_t n4 = d / 4;
-        uint32_t j = 0;
-        for (; j + 4 <= n4; j += 4) {
-            const float4 a0 = r4[j], a1 = r4[j + 1], a2 = r4[j + 2], a3 = r4[j + 3];
-            add(a0.x); add(a0.y); add(a0.z); add(a0.w);
-            add(a1.x); add(a1.y); add(a1.z); add(a1.w);
-            add(a2.x); add(a2.y); add(a2.z); add(a2.w);
-            add(a3.x); add(a3.y); add(a3.z); add(a3.w);
-        }
-        for (; j < n4; ++j) {
-            const float4 a0 = r4[j];
-            add(a0.x); add(a0.y); add(a0.z); add(a0.w);
-        }
-        c = n4 * 4;
-    }
-    for (; c < d; ++c) add(row[c]);
+        ss += (double)v * v;
+    });
     bool bad = !finite || (metric == YAMS_B200_COSINE && ss < 1e-10);
     if (bad) atomicAdd(&status->n_invalid, 1u);
     double nrm = sqrt(ss);

@@ -70,28 +70,17 @@ __global__ void dist_keys_kernel(const float* __restrict__ neg_dist, uint64_t n,
 __global__ void negate_kernel(float* p, uint64_t n) {
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) p[i] = -p[i];
 }
-// computeCosineSimilarity (vector_database.cpp:1786-1810): one thread, the reference's accumulation order
-__global__ void cosine_similarity_f64_kernel(const float* __restrict__ a_all, const float* __restrict__ b_all, uint64_t n, uint64_t d,
+// computeCosineSimilarity of pair p: row p of a_all against row p of b_all ([n][d] each, one after the other in a 256-byte-aligned
+// buffer, so every row is 16-byte aligned when d % 4 == 0)
+__global__ void cosine_similarity_f64_kernel(const float* __restrict__ a_all, const float* __restrict__ b_all, uint64_t n, uint32_t d,
                                              double* __restrict__ out_all) {
     const uint64_t p = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (p >= n) return;
-    const float* a = a_all + p * d;
-    const float* b = b_all + p * d;
-    double* out = out_all + p;
-    double dp = 0.0, na = 0.0, nb = 0.0;
-    for (uint64_t i = 0; i < d; ++i) {
-        double x = (double)a[i], y = (double)b[i];
-        dp += x * y;
-        na += x * x;
-        nb += y * y;
-    }
-    na = sqrt(na);
-    nb = sqrt(nb);
-    *out = (na == 0.0 || nb == 0.0) ? 0.0 : dp / (na * nb);
+    if (p < n) out_all[p] = compute_cosine_similarity(b_all, YAMS_B200_F32, d, p, a_all + p * d);
 }
 
 // n pairs (a_i, b_i) of d floats each -> n doubles; one thread per pair, the reference's accumulation order
 static yams_status_t cosine_similarity_pairs(const float* a, const float* b, size_t n, size_t d, double* out) {
+    YB_ARG(d < 0x100000000ull, "dim must be below 2^32");
     OpWsLease lease;
     OpWs* w = lease.w;
     if (!w) return YAMS_ERR_INTERNAL;
@@ -104,7 +93,7 @@ static yams_status_t cosine_similarity_pairs(const float* a, const float* b, siz
     double* dout = reinterpret_cast<double*>(w->d[0].as<uint8_t>() + ((2 * vb + 7) & ~(size_t)7));
     YB_CUDA(cudaMemcpyAsync(da, a, vb, cudaMemcpyHostToDevice, w->st));
     YB_CUDA(cudaMemcpyAsync(db, b, vb, cudaMemcpyHostToDevice, w->st));
-    cosine_similarity_f64_kernel<<<(unsigned)((n + 63) / 64), 64, 0, w->st>>>(da, db, n, d, dout);
+    cosine_similarity_f64_kernel<<<(unsigned)((n + 63) / 64), 64, 0, w->st>>>(da, db, n, (uint32_t)d, dout);
     YB_CUDA(cudaMemcpyAsync(w->h.p, dout, n * 8, cudaMemcpyDeviceToHost, w->st));
     YB_CUDA(cudaStreamSynchronize(w->st));
     memcpy(out, w->h.p, n * 8);

@@ -48,10 +48,7 @@ __global__ void pq_keep_kernel(const void* __restrict__ rows, int dtype, uint32_
     uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= n) return;
     double ss = 0.0;
-    for (uint32_t c = 0; c < d; ++c) {
-        float v = load_elem(rows, dtype, r * d + c);
-        ss += (double)v * (double)v;
-    }
+    walk_row(rows, dtype, d, r, [&](float v) { ss += (double)v * v; });
     keep[r] = ss <= 1e-20 ? 0u : 1u;
 }
 __global__ void pq_compact_kernel(const uint32_t* __restrict__ keep, const uint32_t* __restrict__ pos, uint64_t n, uint32_t* __restrict__ idx_rows) {
@@ -348,20 +345,11 @@ __global__ void pq_rank_to_row_kernel(Cand* __restrict__ sel, const uint32_t* __
     }
 }
 
-// VectorDatabase::computeCosineSimilarity (vector_database.cpp:1786-1810) of the ORIGINAL query a against corpus row `row`,
-// float cast, NaN and `similarity < threshold` dropped (sqlite_vec_backend.cpp:4022-4037).  -> true and *out = sim when kept.
+// compute_cosine_similarity of the ORIGINAL query a against corpus row `row`, float cast, NaN and `similarity < threshold`
+// dropped (sqlite_vec_backend.cpp:4022-4037).  -> true and *out = sim when kept.
 __device__ __forceinline__ bool pq_rerank_sim(const void* __restrict__ rows, int dtype, uint32_t d, uint32_t row, const float* __restrict__ a,
                                               float threshold, float* out) {
-    double dp = 0.0, na = 0.0, nb = 0.0;
-    for (uint32_t c = 0; c < d; ++c) {
-        const double x = (double)a[c], y = (double)load_elem(rows, dtype, (uint64_t)row * d + c);
-        dp += x * y;
-        na += x * x;
-        nb += y * y;
-    }
-    na = sqrt(na);
-    nb = sqrt(nb);
-    const float sim = (float)((na == 0.0 || nb == 0.0) ? 0.0 : dp / (na * nb));
+    const float sim = (float)compute_cosine_similarity(rows, dtype, d, row, a);
     if (sim == sim && !(sim < threshold)) {
         *out = sim;
         return true;
@@ -458,7 +446,7 @@ __global__ void pq_query_valid_kernel(const float* __restrict__ q32, uint32_t nq
     const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
     if (q >= nq) return;
     double ss = 0.0;
-    for (uint32_t c = 0; c < d; ++c) ss += (double)q32[(size_t)q * d + c] * (double)q32[(size_t)q * d + c];
+    walk_row(q32, YAMS_B200_F32, d, q, [&](float v) { ss += (double)v * v; });
     float inv;
     valid[q] = normalize_factor(ss, &inv) ? 1u : 0u;
 }
