@@ -70,7 +70,8 @@ YAMS_B200_API const char* yams_plugin_get_manifest_json(void);
 YAMS_B200_API int yams_plugin_init(const char* config_json, const void* host_context);
 YAMS_B200_API void yams_plugin_shutdown(void);
 YAMS_B200_API int yams_plugin_get_interface(const char* iface_id, uint32_t version, void** out_iface);
-/* *out_json is malloc'd (strdup), as s3_plugin.cpp does; release with free() */
+/* *out_json is malloc'd (strdup), as s3_plugin.cpp does; release with free().  "device_buffer_bytes" and
+ * "pinned_buffer_bytes" are the bytes the library's device and pinned host buffers hold in this process now. */
 YAMS_B200_API int yams_plugin_get_health_json(char** out_json);
 
 #define YAMS_IFACE_VECTOR_SCAN_V1 "vector_scan_v1"

@@ -17,6 +17,7 @@ static char g_global_error[512] = "";
 static DeviceCtx g_dev;
 static int g_requested_device = -1;
 static bool g_inited = false;
+std::atomic<uint64_t> g_device_buffer_bytes{0}, g_pinned_buffer_bytes{0};
 
 void set_last_error(const char* fmt, ...) {
     va_list ap;
@@ -105,9 +106,6 @@ void opws_release(OpWs* w) {
         g_ws_free.push_back(w);
         return;
     }
-    for (auto& b : w->d) b.release();
-    w->h.release();
-    cudaStreamDestroy(w->st);
     delete w;
 }
 
@@ -215,9 +213,10 @@ int yams_plugin_get_health_json(char** out_json) {
     esc[j] = 0;
     snprintf(buf, sizeof buf,
              "{\"status\": \"%s\", \"device\": %d, \"sm_count\": %d, \"compute_capability\": \"%d.%d\", "
-             "\"last_error\": \"%s\"}",
+             "\"device_buffer_bytes\": %llu, \"pinned_buffer_bytes\": %llu, \"last_error\": \"%s\"}",
              g_dev.ok ? "ok" : (g_inited ? "degraded" : "uninitialized"), g_dev.device, g_dev.sm_count,
-             g_dev.cc_major, g_dev.cc_minor, esc);
+             g_dev.cc_major, g_dev.cc_minor, (unsigned long long)g_device_buffer_bytes.load(),
+             (unsigned long long)g_pinned_buffer_bytes.load(), esc);
     *out_json = strdup(buf);
     return *out_json ? YAMS_PLUGIN_OK : YAMS_PLUGIN_ERR_INVALID;
 }

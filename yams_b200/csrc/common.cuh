@@ -5,8 +5,11 @@
 #include <stdio.h>
 #include <string.h>
 
+#include <atomic>
 #include <exception>
 #include <new>
+#include <type_traits>
+#include <utility>
 
 #include <string>
 
@@ -52,10 +55,26 @@ void note_global_error(const char* text);  // remembered for yams_plugin_get_hea
         return YAMS_ERR_INTERNAL;                                     \
     }
 
-// Growable device buffer (never shrinks); contents are NOT preserved across growth unless asked.
+// Bytes currently held by every DevBuf / HostBuf of the process (reported by yams_plugin_get_health_json): a GPU's free
+// memory is shared with other processes, these counters are exact for this one.
+extern std::atomic<uint64_t> g_device_buffer_bytes, g_pinned_buffer_bytes;
+
+// Growable device buffer (never shrinks); contents are NOT preserved across growth unless asked.  It owns its allocation:
+// freed on destruction, moved but never copied.
 struct DevBuf {
     void* p = nullptr;
     size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(DevBuf&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+    DevBuf& operator=(DevBuf&& o) noexcept {
+        if (this != &o) {
+            release();
+            p = o.p; cap = o.cap;
+            o.p = nullptr; o.cap = 0;
+        }
+        return *this;
+    }
+    ~DevBuf() { release(); }
     yams_status_t reserve(size_t bytes, bool preserve = false, cudaStream_t st = 0) {
         if (bytes <= cap) return YAMS_OK;
         size_t ncap = cap ? cap : 256;
@@ -63,44 +82,63 @@ struct DevBuf {
         ncap = (ncap + 255) & ~size_t(255);
         void* np = nullptr;
         YB_CUDA(cudaMalloc(&np, ncap));
+        g_device_buffer_bytes += ncap;
+        DevBuf nb;   // frees the new allocation if the copy below fails
+        nb.p = np;
+        nb.cap = ncap;
         if (preserve && p && cap) {
-            YB_CUDA(cudaMemcpyAsync(np, p, cap, cudaMemcpyDeviceToDevice, st));
+            YB_CUDA(cudaMemcpyAsync(nb.p, p, cap, cudaMemcpyDeviceToDevice, st));
             YB_CUDA(cudaStreamSynchronize(st));
         }
-        if (p) cudaFree(p);
-        p = np;
-        cap = ncap;
+        *this = std::move(nb);
         return YAMS_OK;
     }
     void release() {
         if (p) cudaFree(p);
+        g_device_buffer_bytes -= cap;
         p = nullptr;
         cap = 0;
     }
     template <typename T> T* as() const { return reinterpret_cast<T*>(p); }
 };
 
-// Pinned host buffer
+// Pinned host buffer; owns its allocation like DevBuf.
 struct HostBuf {
     void* p = nullptr;
     size_t cap = 0;
+    HostBuf() = default;
+    HostBuf(HostBuf&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+    HostBuf& operator=(HostBuf&& o) noexcept {
+        if (this != &o) {
+            release();
+            p = o.p; cap = o.cap;
+            o.p = nullptr; o.cap = 0;
+        }
+        return *this;
+    }
+    ~HostBuf() { release(); }
     yams_status_t reserve(size_t bytes) {
         if (bytes <= cap) return YAMS_OK;
-        if (p) cudaFreeHost(p);
-        p = nullptr;
-        cap = 0;
+        release();
         size_t ncap = (bytes + 4095) & ~size_t(4095);
         YB_CUDA(cudaMallocHost(&p, ncap));
         cap = ncap;
+        g_pinned_buffer_bytes += ncap;
         return YAMS_OK;
     }
     void release() {
         if (p) cudaFreeHost(p);
+        g_pinned_buffer_bytes -= cap;
         p = nullptr;
         cap = 0;
     }
     template <typename T> T* as() const { return reinterpret_cast<T*>(p); }
 };
+
+static_assert(!std::is_copy_constructible<DevBuf>::value && !std::is_copy_assignable<DevBuf>::value, "a DevBuf is never copied");
+static_assert(std::is_nothrow_move_constructible<DevBuf>::value && std::is_nothrow_move_assignable<DevBuf>::value, "DevBuf moves");
+static_assert(!std::is_copy_constructible<HostBuf>::value && !std::is_copy_assignable<HostBuf>::value, "a HostBuf is never copied");
+static_assert(std::is_nothrow_move_constructible<HostBuf>::value && std::is_nothrow_move_assignable<HostBuf>::value, "HostBuf moves");
 
 // Per-plugin device context: which GPU, SM count, init state.
 struct DeviceCtx {
@@ -128,6 +166,13 @@ struct OpWs {
     cudaStream_t st = nullptr;
     DevBuf d[8];
     HostBuf h;
+    // the stream is drained first, so the buffers may be freed after it is destroyed
+    ~OpWs() {
+        if (st) {
+            cudaStreamSynchronize(st);
+            cudaStreamDestroy(st);
+        }
+    }
 };
 OpWs* opws_acquire();             // nullptr (+ last error set) when no device / stream can be had
 void opws_release(OpWs* w);

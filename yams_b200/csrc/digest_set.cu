@@ -9,6 +9,7 @@
 // Batch semantics == the reference's sequential loop: digest i "existed" iff it was in the set before the call or an
 // EARLIER digest of the same batch equals it (the loop stores chunk j before it looks at chunk i > j).  The claim
 // kernel lets equal digests of one batch agree on their lowest index with atomicMin, so the answer is deterministic.
+#include <memory>
 #include <mutex>
 #include <new>
 
@@ -144,6 +145,13 @@ struct yams_b200_digest_set {
     float last_ms = 0.f;    // device time of the last insert/contains (staging + kernels, no PCIe)
     cudaEvent_t ev[2] = {nullptr, nullptr};
     std::mutex mu;
+    // the stream is drained first, so the buffers may be freed in any order after it is destroyed
+    ~yams_b200_digest_set() {
+        if (st) cudaStreamSynchronize(st);
+        for (auto& e : ev)
+            if (e) cudaEventDestroy(e);
+        if (st) cudaStreamDestroy(st);
+    }
 };
 
 static yams_status_t set_grow(yams_b200_digest_set* s, uint64_t need_entries) {
@@ -165,10 +173,7 @@ static yams_status_t set_grow(yams_b200_digest_set* s, uint64_t need_entries) {
             YB_CUDA(cudaGetLastError());
         }
         YB_CUDA(cudaStreamSynchronize(s->st));
-        s->table.release();
-        s->table = nt;
-        nt.p = nullptr;
-        nt.cap = 0;
+        s->table = std::move(nt);
         s->slots = want;
     }
     return YAMS_OK;
@@ -184,7 +189,7 @@ yams_status_t yams_b200_digest_set_create(void* self, uint64_t capacity_hint, ya
     DeviceCtx* dev = nullptr;
     yams_status_t rc = ensure_device(&dev);
     if (rc != YAMS_OK) return rc;
-    auto* s = new (std::nothrow) yams_b200_digest_set();
+    std::unique_ptr<yams_b200_digest_set> s(new (std::nothrow) yams_b200_digest_set());
     YB_ARG(s, "out of memory");
     s->dev = dev;
     cudaError_t e = cudaStreamCreateWithFlags(&s->st, cudaStreamNonBlocking);
@@ -192,35 +197,23 @@ yams_status_t yams_b200_digest_set_create(void* self, uint64_t capacity_hint, ya
     if (e == cudaSuccess) e = cudaEventCreate(&s->ev[1]);
     if (e != cudaSuccess) {
         set_last_error("digest_set_create: %s", cudaGetErrorString(e));
-        delete s;
         return YAMS_ERR_INTERNAL;
     }
-    if ((rc = s->counter.reserve(8)) != YAMS_OK || (rc = set_grow(s, capacity_hint ? capacity_hint : 1024)) != YAMS_OK) {
-        yams_b200_digest_set_destroy(s);
-        return rc;
-    }
-    *out = s;
+    if ((rc = s->counter.reserve(8)) != YAMS_OK || (rc = set_grow(s.get(), capacity_hint ? capacity_hint : 1024)) != YAMS_OK) return rc;
+    *out = s.release();
     return YAMS_OK;
     YB_CATCH
 }
 
-void yams_b200_digest_set_destroy(yams_b200_digest_set* s) {
-    if (!s) return;
-    if (s->st) cudaStreamSynchronize(s->st);
-    for (DevBuf* b : {&s->store, &s->table, &s->stage, &s->flags, &s->probe, &s->counter, &s->fresh, &s->pos, &s->index_of, &s->scan_scratch})
-        b->release();
-    s->pin.release();
-    for (auto& e : s->ev)
-        if (e) cudaEventDestroy(e);
-    if (s->st) cudaStreamDestroy(s->st);
-    delete s;
-}
+void yams_b200_digest_set_destroy(yams_b200_digest_set* s) { delete s; }
 
 yams_status_t yams_b200_digest_set_size(yams_b200_digest_set* s, uint64_t* out) {
+    YB_TRY
     YB_ARG(s && out, "null argument");
     std::lock_guard<std::mutex> lk(s->mu);
     *out = s->unique;
     return YAMS_OK;
+    YB_CATCH
 }
 
 yams_status_t yams_b200_digest_set_insert(yams_b200_digest_set* s, const uint8_t* digests, size_t stride, size_t n,

@@ -90,14 +90,10 @@ struct IngestRes {
         YB_CUDA(cudaMemcpyAsync(table.p, tbl, 256 * 8, cudaMemcpyHostToDevice, st));
         return YAMS_OK;
     }
-    void destroy() {
+    // both streams are drained first, so the buffers may be freed in any order after they are destroyed
+    ~IngestRes() {
         if (st) cudaStreamSynchronize(st);
         if (copy_st) cudaStreamSynchronize(copy_st);
-        for (DevBuf* b : {&table, &tile_counts, &tile_offsets, &cand, &cand_tmp, &next, &forced, &exit_, &entry, &onchain,
-                          &emit_counts, &emit_offsets, &scan_scratch, &descs, &scalars, &sha_order, &npos, &fileinfo, &first,
-                          &stage[0], &stage[1]})
-            b->release();
-        for (HostBuf* b : {&h_scalars, &pin[0], &pin[1]}) b->release();
         for (cudaEvent_t e : {ev[0], ev[1], ev[2], ev[3], call[0], call[1], call[2], copied[0], copied[1], freed[0], freed[1],
                               pin_done[0], pin_done[1]})
             if (e) cudaEventDestroy(e);
@@ -351,7 +347,6 @@ static yams_status_t acquire_res(const yams_cdc_config* cfg, IngestRes** out) {
     yams_status_t rc = r->create();
     if (rc == YAMS_OK) rc = cfg ? r->init(cfg) : YAMS_OK;
     if (rc != YAMS_OK) {
-        r->destroy();
         delete r;
         return rc;
     }
@@ -374,7 +369,6 @@ static void release_res(IngestRes* r) {
             return;
         }
     }
-    r->destroy();
     delete r;
 }
 
@@ -1005,7 +999,6 @@ yams_status_t yams_b200_dedup_stats(void* self, const yams_chunk_desc* chunks, s
             }
         }
     }
-    for (DevBuf* b : {&d_descs, &d_table, &d_out}) b->release();
     cudaStreamDestroy(st);
     return rc;
     YB_CATCH

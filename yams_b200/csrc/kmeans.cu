@@ -499,8 +499,10 @@ yams_status_t yams_b200_topology_kmeans(yams_b200_corpus* c, uint32_t k_requeste
 }
 
 yams_status_t yams_b200_topology_kmeans_last_timings(yams_b200_corpus* c, float out_ms[4]) {
+    YB_TRY
     YB_ARG(c && out_ms, "null argument");
     std::lock_guard<std::mutex> corpus_lock(c->mu);
     for (int i = 0; i < 4; ++i) out_ms[i] = c->kmeans_ms[i];
     return YAMS_OK;
+    YB_CATCH
 }

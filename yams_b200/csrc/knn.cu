@@ -20,6 +20,7 @@
 #include <math.h>
 
 #include <algorithm>
+#include <memory>
 #include <new>
 #include <vector>
 
@@ -1610,46 +1611,25 @@ yams_status_t yams_b200_corpus_create(void* self, uint32_t dim, int dtype, int m
     DeviceCtx* dev = nullptr;
     yams_status_t rc = ensure_device(&dev);
     if (rc != YAMS_OK) return rc;
-    yams_b200_corpus* c = new (std::nothrow) yams_b200_corpus();
+    std::unique_ptr<yams_b200_corpus> c(new (std::nothrow) yams_b200_corpus());
     if (!c) return YAMS_ERR_INTERNAL;
     c->dev = dev;
     c->dim = dim;
     c->dtype = dtype;
     c->metric = metric;
     if (cudaStreamCreateWithFlags(&c->st, cudaStreamNonBlocking) != cudaSuccess) {
-        delete c;
         set_last_error("cudaStreamCreate failed");
         return YAMS_ERR_INTERNAL;
     }
     for (auto& e : c->ev) cudaEventCreate(&e);
     for (auto& e : c->ev_scan) cudaEventCreate(&e);
-    if (capacity_hint) {
-        rc = corpus_reserve(c, capacity_hint);
-        if (rc != YAMS_OK) {
-            yams_b200_corpus_destroy(c);
-            return rc;
-        }
-    }
-    *out = c;
+    if (capacity_hint && (rc = corpus_reserve(c.get(), capacity_hint)) != YAMS_OK) return rc;
+    *out = c.release();
     return YAMS_OK;
     YB_CATCH
 }
 
-void yams_b200_corpus_destroy(yams_b200_corpus* c) {
-    if (!c) return;
-    if (c->st) cudaStreamSynchronize(c->st);
-    for (DevBuf* b : {&c->rows, &c->rowids, &c->inv_norm, &c->q32, &c->q16, &c->qinv, &c->tau, &c->counts, &c->cands,
-                      &c->sample_scores, &c->sel, &c->outbuf, &c->dense, &c->mask, &c->misc, &c->qnorm, &c->dout, &c->stats, &c->status,
-                      &c->bound, &c->eps, &c->eps2, &c->lvl, &c->graph, &c->kmeans})
-        b->release();
-    c->h_pin.release();
-    for (auto& e : c->ev)
-        if (e) cudaEventDestroy(e);
-    for (auto& e : c->ev_scan)
-        if (e) cudaEventDestroy(e);
-    if (c->st) cudaStreamDestroy(c->st);
-    delete c;
-}
+void yams_b200_corpus_destroy(yams_b200_corpus* c) { delete c; }
 
 yams_status_t yams_b200_corpus_append(yams_b200_corpus* c, const void* rows, uint64_t n, const int64_t* rowids) {
     YB_TRY
@@ -1755,6 +1735,7 @@ yams_status_t yams_b200_corpus_remove(yams_b200_corpus* c, const int64_t* rowids
 }
 
 yams_status_t yams_b200_corpus_clear(yams_b200_corpus* c) {
+    YB_TRY
     YB_ARG(c, "corpus is null");
     std::lock_guard<std::mutex> corpus_lock(c->mu);
     YB_BIND(c);
@@ -1766,6 +1747,7 @@ yams_status_t yams_b200_corpus_clear(yams_b200_corpus* c) {
     c->r_max = c->dr_abs_max = c->dr_rel_max = c->inv_max = 0.f;
     if (c->stats.p) YB_CUDA(cudaMemsetAsync(c->stats.p, 0, 16, c->st));
     return YAMS_OK;
+    YB_CATCH
 }
 
 yams_status_t yams_b200_corpus_size(const yams_b200_corpus* c, uint64_t* out_n) {
@@ -1775,11 +1757,13 @@ yams_status_t yams_b200_corpus_size(const yams_b200_corpus* c, uint64_t* out_n) 
 }
 
 yams_status_t yams_b200_corpus_sync(yams_b200_corpus* c) {
+    YB_TRY
     YB_ARG(c, "corpus is null");
     std::lock_guard<std::mutex> corpus_lock(c->mu);
     YB_BIND(c);
     YB_CUDA(cudaStreamSynchronize(c->st));
     return YAMS_OK;
+    YB_CATCH
 }
 
 void* yams_b200_corpus_stream(yams_b200_corpus* c) { return c ? (void*)c->st : nullptr; }
@@ -2164,6 +2148,7 @@ yams_status_t yams_b200_semantic_neighbors(yams_b200_corpus* c, const int64_t* s
 
 yams_status_t yams_b200_debug_semantic_stage1(yams_b200_corpus* c, const int64_t* source_rowids, uint32_t n_sources, int engine,
                                               float* out_scores, float* out_eps) {
+    YB_TRY
     YB_ARG(c && source_rowids && out_scores && out_eps && n_sources > 0 && n_sources <= kGraphBatch, "bad argument");
     std::lock_guard<std::mutex> corpus_lock(c->mu);
     YB_ARG(c->metric == YAMS_B200_COSINE && c->n > 0, "needs a non-empty cosine corpus");
@@ -2198,6 +2183,7 @@ yams_status_t yams_b200_debug_semantic_stage1(yams_b200_corpus* c, const int64_t
     YB_CUDA(cudaStreamSynchronize(c->st));
     for (uint32_t i = 0; i < n_sources; ++i) out_eps[i] += graph_eps(h_inv[src_row[i]], g.uf);   // as final_kernel adds it
     return YAMS_OK;
+    YB_CATCH
 }
 
 yams_status_t yams_b200_search_device(yams_b200_corpus* c, const float* d_queries, uint32_t nq, uint32_t k, float threshold,
@@ -2253,11 +2239,13 @@ static yams_status_t merge_launch(yams_b200_corpus* c, const int64_t* d_rowids, 
 yams_status_t yams_b200_merge_partials_device(yams_b200_corpus* c, const int64_t* d_rowids, const float* d_scores,
                                               uint32_t nranks, uint32_t nq, uint32_t k, int64_t* d_out_rowids,
                                               float* d_out_scores, uint32_t* d_out_counts) {
+    YB_TRY
     YB_ARG(c && d_rowids && d_scores && d_out_rowids && d_out_scores, "null argument");
     std::lock_guard<std::mutex> corpus_lock(c->mu);
     YB_BIND(c);
     return merge_launch(c, d_rowids, d_scores, (uint64_t)nq * k, (uint64_t)nq * k, nranks, nq, k, d_out_rowids, d_out_scores,
                         d_out_counts, c->st);
+    YB_CATCH
 }
 
 yams_status_t yams_b200_merge_packed_device(yams_b200_corpus* c, const void* d_packed, uint32_t nranks, uint32_t nq, uint32_t k,
@@ -2285,6 +2273,7 @@ yams_status_t yams_b200_search_last_timings(yams_b200_corpus* c, float out_ms[8]
 // chosen engine (0 cuda-core, 1 wgmma) -> out[q * nrows + i] (HOST). Used by the tests to compare engines.
 yams_status_t yams_b200_debug_stage1_scores(yams_b200_corpus* c, const float* queries, uint32_t nq, int engine,
                                             uint64_t row_start, uint64_t row_stride, uint64_t nrows, float* out) {
+    YB_TRY
     YB_ARG(c && queries && out && nq > 0 && nrows > 0 && row_stride > 0, "bad argument");
     std::lock_guard<std::mutex> corpus_lock(c->mu);
     YB_ARG(row_start + (nrows - 1) * row_stride < c->n, "rows out of range");
@@ -2305,6 +2294,7 @@ yams_status_t yams_b200_debug_stage1_scores(yams_b200_corpus* c, const float* qu
     YB_CUDA(cudaMemcpyAsync(out, c->dense.p, (size_t)nq * nrows * 4, cudaMemcpyDeviceToHost, c->st));
     YB_CUDA(cudaStreamSynchronize(c->st));
     return YAMS_OK;
+    YB_CATCH
 }
 
 // the filter-mode set-up of the stage-1 diagnostics: the queries prepared, tau[nq] uploaded, the list counters zeroed and `a`
@@ -2330,6 +2320,7 @@ yams_status_t yams_b200_debug_stage1_candidates(yams_b200_corpus* c, const float
                                                 uint64_t row_start, uint64_t row_stride, uint64_t nrows, const float* tau, uint32_t cap,
                                                 const int64_t* allowed_rowids, const uint64_t* allowed_offsets, uint32_t* out_counts,
                                                 void* out_cands) {
+    YB_TRY
     YB_ARG(c && queries && tau && out_counts && (out_cands || cap == 0) && nq > 0 && nrows > 0 && row_stride > 0, "bad argument");
     YB_ARG(!allowed_rowids || allowed_offsets, "allowed_offsets missing");
     YB_ARG(!allowed_offsets || allowed_rowids || allowed_offsets[nq] == 0, "allowed_rowids missing");
@@ -2366,12 +2357,14 @@ yams_status_t yams_b200_debug_stage1_candidates(yams_b200_corpus* c, const float
     if (cb) YB_CUDA(cudaMemcpyAsync(out_cands, c->cands.p, cb, cudaMemcpyDeviceToHost, c->st));
     YB_CUDA(cudaStreamSynchronize(c->st));
     return YAMS_OK;
+    YB_CATCH
 }
 
 // diagnostics: one pass of the profiling instantiation of the wgmma scan in filter mode over every row (the search's corpus
 // pass) -> per-CTA cycle counters, the launch's layout and its device time (HOST out), see include/yams_b200.h
 yams_status_t yams_b200_debug_stage1_profile(yams_b200_corpus* c, const float* queries, uint32_t nq, const float* tau, uint32_t cap,
                                              uint32_t max_ctas, uint64_t* out_cycles, uint32_t* out_info, float* out_ms) {
+    YB_TRY
     YB_ARG(c && queries && tau && out_cycles && out_info && out_ms && nq > 0, "bad argument");
     std::lock_guard<std::mutex> corpus_lock(c->mu);
     YB_ARG(c->n > 0, "empty corpus");
@@ -2394,6 +2387,7 @@ yams_status_t yams_b200_debug_stage1_profile(yams_b200_corpus* c, const float* q
     YB_CUDA(cudaEventElapsedTime(out_ms, c->ev_scan[0], c->ev_scan[1]));
     out_info[0] = c->wg_launch[0]; out_info[1] = c->wg_launch[1];
     return YAMS_OK;
+    YB_CATCH
 }
 
 // diagnostics: the top-K selection (topk_select_kernel) on caller-supplied scores, see include/yams_b200.h
@@ -2401,6 +2395,7 @@ yams_status_t yams_b200_debug_select(yams_b200_corpus* c, uint32_t nq, const flo
                                      uint64_t row_stride, uint32_t dense_shift, const void* cands, const uint32_t* counts, uint32_t cap,
                                      const float* tau, uint32_t K, int tau_only, float tau_margin, int fast_tau, void* out_sel,
                                      uint32_t* out_n, float* out_bound) {
+    YB_TRY
     YB_ARG(c && nq > 0 && out_bound && (tau_only || (out_sel && out_n)), "bad argument");
     YB_ARG(dense ? (ld >= len && dense_shift < 4) : (counts && (cands || cap == 0)), "bad input");
     YB_ARG(tau_only || K <= SEL_MAXK, "K > 4096");
@@ -2447,6 +2442,7 @@ yams_status_t yams_b200_debug_select(yams_b200_corpus* c, uint32_t nq, const flo
     YB_CUDA(cudaMemcpyAsync(out_bound, d_bound, (size_t)nq * 4, cudaMemcpyDeviceToHost, st));
     YB_CUDA(cudaStreamSynchronize(st));
     return YAMS_OK;
+    YB_CATCH
 }
 
 // diagnostics: the final ordering and the exactness certificate (final_kernel) on caller-supplied exact scores, see
@@ -2515,12 +2511,11 @@ yams_status_t yams_b200_synth_rows_device(uint64_t seed, uint64_t first_row, uin
     DeviceCtx* dev = nullptr;
     yams_status_t rc = ensure_device(&dev);
     if (rc != YAMS_OK) return rc;
-    float* d_inv = nullptr;
-    YB_CUDA(cudaMalloc(&d_inv, (size_t)n * 4));
-    synth_rownorm_kernel<<<(unsigned)((n + 127) / 128), 128>>>(seed, first_row, n, dim, d_inv);
-    synth_fill_kernel<<<dev->sm_count * 16, 256>>>(seed, first_row, n, dim, d_inv, d_out, YAMS_B200_F32);
+    DevBuf inv;
+    if ((rc = inv.reserve((size_t)n * 4)) != YAMS_OK) return rc;
+    synth_rownorm_kernel<<<(unsigned)((n + 127) / 128), 128>>>(seed, first_row, n, dim, inv.as<float>());
+    synth_fill_kernel<<<dev->sm_count * 16, 256>>>(seed, first_row, n, dim, inv.as<float>(), d_out, YAMS_B200_F32);
     cudaError_t e = cudaDeviceSynchronize();
-    cudaFree(d_inv);
     if (e != cudaSuccess) {
         set_last_error("synth_rows_device failed: %s", cudaGetErrorString(e));
         return YAMS_ERR_INTERNAL;
@@ -2532,6 +2527,7 @@ yams_status_t yams_b200_synth_rows_device(uint64_t seed, uint64_t first_row, uin
 // diagnostics: the per-query stage-1 error bound eps[q] (certificate input) computed by the last search /
 // debug_stage1_scores call on this corpus
 yams_status_t yams_b200_debug_last_eps(yams_b200_corpus* c, uint32_t nq, float* out) {
+    YB_TRY
     YB_ARG(c && out && nq > 0, "bad argument");
     std::lock_guard<std::mutex> corpus_lock(c->mu);
     YB_BIND(c);
@@ -2539,6 +2535,7 @@ yams_status_t yams_b200_debug_last_eps(yams_b200_corpus* c, uint32_t nq, float* 
     YB_CUDA(cudaMemcpyAsync(out, c->eps.p, (size_t)nq * 4, cudaMemcpyDeviceToHost, c->st));
     YB_CUDA(cudaStreamSynchronize(c->st));
     return YAMS_OK;
+    YB_CATCH
 }
 
 }  // extern "C"

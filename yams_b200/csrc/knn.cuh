@@ -97,6 +97,15 @@ struct Corpus {
     uint32_t wg_launch[2] = {0, 0};   // the last wgmma scan launch: query-tile columns, CTAs
     std::mutex mu;   // public entry points on one corpus are serialised (the workspace buffers are per corpus)
     size_t elem() const { return dtype == YAMS_B200_F16 ? 2 : 4; }
+    // the stream is drained first, so the buffers may be freed in any order after it is destroyed
+    ~Corpus() {
+        if (st) cudaStreamSynchronize(st);
+        for (auto& e : ev)
+            if (e) cudaEventDestroy(e);
+        for (auto& e : ev_scan)
+            if (e) cudaEventDestroy(e);
+        if (st) cudaStreamDestroy(st);
+    }
 };
 
 // Stage-1 engine interface: approximate scores of `nrows` corpus rows (row_start + i*row_stride) against nq queries.

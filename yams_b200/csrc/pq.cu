@@ -23,6 +23,7 @@
 #include <cuda_fp16.h>
 
 #include <algorithm>
+#include <memory>
 #include <new>
 #include <vector>
 
@@ -577,9 +578,8 @@ yams_status_t yams_b200_pq_build(yams_b200_corpus* c, uint32_t m, uint32_t k, co
     YB_ARG((size_t)m * k * 4 + PQ_TILE * 8 + 64 <= 200 * 1024, "m * k too large for the shared-memory lookup table");
     const uint64_t n = c->n;
     YB_ARG(n < 0xFFFFFFFFull, "too many rows");
-    yams_b200_pq* p = new (std::nothrow) yams_b200_pq();
+    std::unique_ptr<yams_b200_pq> p(new (std::nothrow) yams_b200_pq());
     if (!p) return YAMS_ERR_INTERNAL;
-    struct Guard { yams_b200_pq* p; ~Guard() { if (p) yams_b200_pq_destroy(p); } } guard{p};
     p->corpus = c;
     p->corpus_generation = c->generation;
     p->m = m; p->k = k; p->dim = c->dim;
@@ -592,7 +592,6 @@ yams_status_t yams_b200_pq_build(yams_b200_corpus* c, uint32_t m, uint32_t k, co
     if (n) {
         // rows the index holds: those normalizeEmbeddingInPlace accepts (:3569-3577)
         DevBuf keep, pos, scratch, total;
-        struct Rel { DevBuf *a, *b, *c2, *d; ~Rel() { a->release(); b->release(); c2->release(); d->release(); } } rel{&keep, &pos, &scratch, &total};
         if ((rc = keep.reserve(n * 4)) != YAMS_OK || (rc = pos.reserve(n * 4)) != YAMS_OK || (rc = total.reserve(8)) != YAMS_OK) return rc;
         pq_keep_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(c->rows.p, c->dtype, c->dim, n, keep.as<uint32_t>());
         if ((rc = exclusive_scan_u32(keep.as<uint32_t>(), pos.as<uint32_t>(), n, total.as<uint64_t>(), scratch, st)) != YAMS_OK) return rc;
@@ -625,19 +624,12 @@ yams_status_t yams_b200_pq_build(yams_b200_corpus* c, uint32_t m, uint32_t k, co
         }
         YB_CUDA(cudaStreamSynchronize(st));
     }
-    guard.p = nullptr;
-    *out = p;
+    *out = p.release();
     return YAMS_OK;
     YB_CATCH
 }
 
-void yams_b200_pq_destroy(yams_b200_pq* p) {
-    if (!p) return;
-    for (DevBuf* b : {&p->codebooks, &p->codes, &p->idx_rows, &p->tie_rank, &p->rank_to_idx, &p->row_to_idx, &p->q32, &p->lut, &p->valid, &p->lists,
-                      &p->counts, &p->sel, &p->exact, &p->dout, &p->tau, &p->cin, &p->mapped, &p->cidx, &p->bits})
-        b->release();
-    delete p;
-}
+void yams_b200_pq_destroy(yams_b200_pq* p) { delete p; }
 
 yams_status_t yams_b200_pq_codes(yams_b200_pq* p, uint8_t* out_codes, int64_t* out_rowids, uint64_t* out_n) {
     YB_TRY

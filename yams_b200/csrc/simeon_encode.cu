@@ -28,6 +28,7 @@
 // One CTA per text.  The sign matrix is tabulated once per encoder, 2 bits per entry, column-major (for one sketch column the
 // 384 row signs are 96 contiguous bytes): the projection walks the NON-ZERO sketch columns only.
 #include <algorithm>
+#include <memory>
 #include <mutex>
 #include <new>
 #include <vector>
@@ -290,7 +291,7 @@ yams_status_t yams_b200_simeon_create(void* self, const yams_simeon_config* cfg_
     DeviceCtx* dev = nullptr;
     yams_status_t rc = ensure_device(&dev);
     if (rc != YAMS_OK) return rc;
-    yams_b200_encoder* e = new (std::nothrow) yams_b200_encoder();
+    std::unique_ptr<yams_b200_encoder> e(new (std::nothrow) yams_b200_encoder());
     if (!e) return YAMS_ERR_INTERNAL;
     e->dev = dev;
     e->cfg = cfg;
@@ -318,39 +319,27 @@ yams_status_t yams_b200_simeon_create(void* self, const yams_simeon_config* cfg_
             const uint32_t pick = i + (uint32_t)(srng % (uint64_t)(pad_n - i));
             std::swap(idx[i], idx[pick]);
         }
-        if ((rc = e->signs.reserve((size_t)pad_n * 4)) != YAMS_OK || (rc = e->sample.reserve((size_t)cfg.output_dim * 4)) != YAMS_OK) {
-            e->signs.release(); e->sample.release();
-            delete e;
-            return rc;
-        }
+        if ((rc = e->signs.reserve((size_t)pad_n * 4)) != YAMS_OK || (rc = e->sample.reserve((size_t)cfg.output_dim * 4)) != YAMS_OK) return rc;
         ce = cudaMemcpy(e->signs.p, signs.data(), (size_t)pad_n * 4, cudaMemcpyHostToDevice);
         if (ce == cudaSuccess) ce = cudaMemcpy(e->sample.p, idx.data(), (size_t)cfg.output_dim * 4, cudaMemcpyHostToDevice);
     } else {
     const size_t words = (size_t)cfg.sketch_dim * e->words_per_col;
     rc = e->table.reserve(words * 4);
-    if (rc != YAMS_OK) { delete e; return rc; }
+    if (rc != YAMS_OK) return rc;
     achlioptas_table_kernel<<<(unsigned)((words + 255) / 256), 256>>>(cfg.sketch_dim, cfg.output_dim, cfg.projection_seed, e->words_per_col,
                                                                       e->table.as<uint32_t>());
     }
     if (ce == cudaSuccess) ce = cudaDeviceSynchronize();
     if (ce != cudaSuccess) {
         set_last_error("encoder table build failed: %s", cudaGetErrorString(ce));
-        e->table.release(); e->signs.release(); e->sample.release();
-        delete e;
         return YAMS_ERR_INTERNAL;
     }
-    *out = e;
+    *out = e.release();
     return YAMS_OK;
     YB_CATCH
 }
 
-void yams_b200_simeon_destroy(yams_b200_encoder* e) {
-    if (!e) return;
-    e->table.release();
-    e->signs.release();
-    e->sample.release();
-    delete e;
-}
+void yams_b200_simeon_destroy(yams_b200_encoder* e) { delete e; }
 
 yams_status_t yams_b200_simeon_encode(yams_b200_encoder* e, const char* const* texts, const size_t* lens, size_t n, float* out) {
     YB_TRY
