@@ -578,6 +578,69 @@ YAMS_B200_API yams_status_t yams_b200_simeon_encode(yams_b200_encoder* e, const 
                                                     size_t n, float* out);
 YAMS_B200_API void yams_b200_simeon_destroy(yams_b200_encoder* e);
 
+/* ---- Simeon BM25 lexical index (DESIGN.md §4.11) ----------------------------------------------------------------
+ * third_party/simeon Bm25Index (src/bm25.cpp), as the lexical backend builds and scores it (SimeonLexicalBackend:
+ * src/search/simeon_lexical_backend.cpp), for the two variants that backend selects: Atire and SubwordAwareBackoff.
+ *   build  add_doc(text) for each document in order, then finalize(): words are the maximal runs of [A-Za-z0-9_] (bytes >= 0x80
+ *          separate words), ASCII-lowercased and hashed with SplitMix64; dl = words of the document; SubwordAwareBackoff also
+ *          indexes every n-gram (k = ngram_min..ngram_max, every position) of every lowercased word, ngram_dl = their count,
+ *          and drops n-grams whose df exceeds size_t(double(prune_ratio) * n) (prune_ratio 0: none).  Posting lists are in
+ *          document order; idf = logf((n - df + 0.5f) / (df + 0.5f) + 1.0f), avg_dl = float(double(sum dl) / n).
+ *   score  for each query word in order (duplicates kept), Atire adds score_atire to every document of its posting list;
+ *          SubwordAwareBackoff adds alpha * bm25plus over the word's list (alpha = df / (df + gamma), 0 when df = 0) when
+ *          alpha > 0, and (1 - alpha) * bm25plus over the list of each distinct n-gram of the word still in the index when
+ *          alpha < 1.  Every float operation is the reference's, in its order, without fused multiply-adds.
+ * Scores are bit-identical to the reference.  Out of scope (the caller's, as today): the concept blend
+ * (ConceptIndex::blend_into) applied to the returned vector, fragment geometry, the strategy router, RRF, the BM25F aux field,
+ * SDM / word bigrams, PRF, and the caller's document windowing (buildEnhancementText). */
+#define YAMS_BM25_ATIRE 0                    /* simeon::Bm25Variant::Atire */
+#define YAMS_BM25_SUBWORD_AWARE_BACKOFF 7    /* simeon::Bm25Variant::SubwordAwareBackoff */
+typedef struct yams_bm25_config {
+    float k1, b, delta;           /* 1.2, 0.75, 1.0 */
+    float subword_gamma;          /* 5 (the lexical backend's); alpha = df / (df + gamma) */
+    uint32_t variant;             /* YAMS_BM25_*; any other value -> YAMS_ERR_UNSUPPORTED */
+    uint32_t ngram_min, ngram_max;   /* 3, 4 */
+    float ngram_df_prune_ratio;   /* 0.5 */
+    uint64_t hash_seed;           /* 0xB252B252B252B252 */
+} yams_bm25_config;
+typedef struct yams_b200_bm25 yams_b200_bm25;
+/* the lexical backend's configuration: SubwordAwareBackoff, gamma 5, Bm25Config's defaults otherwise */
+YAMS_B200_API void yams_b200_bm25_default_config(yams_bm25_config* cfg);
+/* builds and finalizes an index of n_docs HOST texts (bytes, not NUL-terminated; a NULL text of length 0 is an empty document;
+ * n_docs = 0 is an empty index).  Corpora larger than one device pass are built in document slices; beyond device memory the
+ * call fails with YAMS_ERR_INTERNAL and says so.  n_docs < 2^32 - 1. */
+YAMS_B200_API yams_status_t yams_b200_bm25_build(void* self, const yams_bm25_config* cfg /* NULL = default */,
+                                                 const char* const* texts, const size_t* lens, uint64_t n_docs,
+                                                 yams_b200_bm25** out);
+/* Bm25Index::score for nq HOST queries.  out_scores (nullable): [nq][n_docs] HOST floats, the full score vectors.  k > 0
+ * (<= 4096): the documents of score > 0, best first (score descending, then document ascending), k of them at most ->
+ * out_docs[nq][k] (padded with 0xFFFFFFFF), out_topk_scores[nq][k] (padded with 0), out_counts[nq]. */
+YAMS_B200_API yams_status_t yams_b200_bm25_score(yams_b200_bm25* idx, const char* const* queries, const size_t* qlens, uint32_t nq,
+                                                 float* out_scores, uint32_t k, uint32_t* out_docs, float* out_topk_scores,
+                                                 uint32_t* out_counts);
+typedef struct yams_bm25_stats {
+    uint64_t n_docs;
+    float avg_dl, ngram_avg_dl;   /* ngram_avg_dl: 0 for Atire */
+    uint64_t total_tokens;        /* sum of dl */
+    uint64_t terms[2];            /* distinct hashes of field 0 (words) and 1 (n-grams, after pruning) */
+    uint64_t postings[2];         /* (term, document) entries per field */
+    uint64_t pruned;              /* n-grams dropped by the df rule */
+} yams_bm25_stats;
+YAMS_B200_API yams_status_t yams_b200_bm25_stats(yams_b200_bm25* idx, yams_bm25_stats* out);
+/* the posting list of term_hash in field 0 (words) or 1 (n-grams): *out_df (0 when absent), *out_idf, *out_total_tf, and the
+ * first min(df, cap) (document, tf) entries in document order (out_docs / out_tfs nullable when cap = 0).  Bm25Index::df /
+ * idf / total_tf of a term are these of field 0 for the term's hash. */
+YAMS_B200_API yams_status_t yams_b200_bm25_postings(yams_b200_bm25* idx, uint32_t field, uint64_t term_hash, uint32_t* out_df,
+                                                    float* out_idf, uint64_t* out_total_tf, uint32_t* out_docs, uint32_t* out_tfs,
+                                                    uint64_t cap);
+/* dl (field 0) or ngram_dl (field 1, zeros for Atire) of every document -> out[n_docs] (HOST) */
+YAMS_B200_API yams_status_t yams_b200_bm25_doc_lengths(yams_b200_bm25* idx, uint32_t field, uint32_t* out);
+/* out_ms[0..3]: the last build's device ms of the upload, the tokenising (per-document counts, words, n-gram pairs), the sorts,
+ * the posting lists (runs, pruning, dictionary), [4] its host wall ms, [5] its document slices; [6] the last score call's
+ * device ms, [7] its host wall ms */
+YAMS_B200_API yams_status_t yams_b200_bm25_last_timings(yams_b200_bm25* idx, float out_ms[8]);
+YAMS_B200_API void yams_b200_bm25_destroy(yams_b200_bm25* idx);
+
 /* [0] stage-1 scan ms, [1] rescoring+select ms, [2] total device ms of the last yams_b200_search or
  * yams_b200_search_device on this corpus (the latter's once its work is done); [3] unused (0);
  * [4] = which stage-1 kernel ran (0 cuda-core, 1 wgmma);

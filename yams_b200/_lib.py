@@ -51,6 +51,18 @@ class SimeonConfig(C.Structure):
                 ("hash_seed", C.c_uint64), ("projection_seed", C.c_uint64), ("l2_normalize", C.c_int32), ("flags", C.c_int32)]
 
 
+class Bm25Config(C.Structure):
+    _fields_ = [("k1", C.c_float), ("b", C.c_float), ("delta", C.c_float), ("subword_gamma", C.c_float), ("variant", C.c_uint32),
+                ("ngram_min", C.c_uint32), ("ngram_max", C.c_uint32), ("ngram_df_prune_ratio", C.c_float), ("hash_seed", C.c_uint64)]
+
+
+class Bm25Stats(C.Structure):
+    _fields_ = [("n_docs", C.c_uint64), ("avg_dl", C.c_float), ("ngram_avg_dl", C.c_float), ("total_tokens", C.c_uint64),
+                ("terms", C.c_uint64 * 2), ("postings", C.c_uint64 * 2), ("pruned", C.c_uint64)]
+
+
+BM25_ATIRE, BM25_SUBWORD_AWARE_BACKOFF = 0, 7   # simeon::Bm25Variant numbering
+
 SIMEON_WORD_TOKENS = 1        # NGramMode::CharAndWord
 SIMEON_PROJECTION_FWHT = 2    # ProjectionMode::Fwht (default projection: AchlioptasSparse)
 
@@ -140,6 +152,16 @@ SYMBOLS = {
     "yams_b200_simeon_create": (C.c_int, [C.c_void_p, C.POINTER(SimeonConfig), C.POINTER(C.c_void_p)]),
     "yams_b200_simeon_encode": (C.c_int, [C.c_void_p, C.POINTER(C.c_char_p), C.POINTER(C.c_size_t), C.c_size_t, f32p]),
     "yams_b200_simeon_destroy": (None, [C.c_void_p]),
+    "yams_b200_bm25_default_config": (None, [C.POINTER(Bm25Config)]),
+    "yams_b200_bm25_build": (C.c_int, [C.c_void_p, C.POINTER(Bm25Config), C.POINTER(C.c_char_p), C.POINTER(C.c_size_t), C.c_uint64,
+                                       C.POINTER(C.c_void_p)]),
+    "yams_b200_bm25_score": (C.c_int, [C.c_void_p, C.POINTER(C.c_char_p), C.POINTER(C.c_size_t), C.c_uint32, f32p, C.c_uint32, u32p, f32p,
+                                       u32p]),
+    "yams_b200_bm25_stats": (C.c_int, [C.c_void_p, C.POINTER(Bm25Stats)]),
+    "yams_b200_bm25_postings": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint64, u32p, f32p, u64p, u32p, u32p, C.c_uint64]),
+    "yams_b200_bm25_doc_lengths": (C.c_int, [C.c_void_p, C.c_uint32, u32p]),
+    "yams_b200_bm25_last_timings": (C.c_int, [C.c_void_p, f32p]),
+    "yams_b200_bm25_destroy": (None, [C.c_void_p]),
     "yams_b200_pq_build": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, f32p, u64p, C.POINTER(C.c_void_p)]),
     "yams_b200_pq_search": (C.c_int, [C.c_void_p, f32p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_float, i64p, f32p, u32p, u64p]),
     "yams_b200_pq_search_candidates": (C.c_int, [C.c_void_p, f32p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_float, i64p, u64p, i64p, f32p,
@@ -749,6 +771,85 @@ class SimeonEncoder:
     def close(self):
         if getattr(self, "_h", None):
             lib().yams_b200_simeon_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def _texts(texts):
+    raw = [t.encode("utf-8") if isinstance(t, str) else bytes(t) for t in texts]
+    n = len(raw)
+    return raw, (C.c_char_p * max(n, 1))(*raw), (C.c_size_t * max(n, 1))(*[len(r) for r in raw])
+
+
+class Bm25Index:
+    """simeon's Bm25Index built on the device over `texts` (add_doc for each, then finalize), as the lexical backend configures it
+    unless overridden: SubwordAwareBackoff, gamma 5.  `variant` is BM25_ATIRE or BM25_SUBWORD_AWARE_BACKOFF."""
+
+    def __init__(self, texts, **overrides):
+        cfg = Bm25Config()
+        lib().yams_b200_bm25_default_config(C.byref(cfg))
+        for k, v in overrides.items():
+            setattr(cfg, k, v)
+        self.cfg = cfg
+        raw, ptrs, lens = _texts(texts)
+        self.n = len(raw)
+        self._h = C.c_void_p()
+        _check(lib().yams_b200_bm25_build(None, C.byref(cfg), ptrs, lens, self.n, C.byref(self._h)), "bm25_build")
+
+    def score(self, queries, k: int = 0, full: bool = True):
+        """Bm25Index::score of every query: {"scores": [nq][n_docs] (full=True)}, and for k > 0 the best k documents of score > 0
+        ("docs", "topk_scores" padded with 0xFFFFFFFF / 0, "counts")."""
+        raw, ptrs, lens = _texts(queries)
+        nq = len(raw)
+        out = {}
+        scores = np.zeros((nq, self.n), np.float32) if full else None
+        docs = np.zeros((nq, max(k, 1)), np.uint32)
+        tops = np.zeros((nq, max(k, 1)), np.float32)
+        counts = np.zeros(max(nq, 1), np.uint32)
+        _check(lib().yams_b200_bm25_score(self._h, ptrs, lens, nq, scores.ctypes.data_as(f32p) if full else None, k,
+                                          docs.ctypes.data_as(u32p), tops.ctypes.data_as(f32p), counts.ctypes.data_as(u32p)),
+               "bm25_score")
+        if full:
+            out["scores"] = scores
+        if k:
+            out.update(docs=docs, topk_scores=tops, counts=counts[:nq])
+        return out
+
+    def stats(self) -> dict:
+        s = Bm25Stats()
+        _check(lib().yams_b200_bm25_stats(self._h, C.byref(s)), "bm25_stats")
+        return {"n_docs": s.n_docs, "avg_dl": np.float32(s.avg_dl), "ngram_avg_dl": np.float32(s.ngram_avg_dl),
+                "total_tokens": s.total_tokens, "terms": tuple(s.terms), "postings": tuple(s.postings), "pruned": s.pruned}
+
+    def postings(self, field: int, term_hash: int):
+        """(docs, tfs, idf, total_tf) of a hash in field 0 (words) or 1 (n-grams); empty lists and 0 when absent."""
+        df, idf, ttf = C.c_uint32(), C.c_float(), C.c_uint64()
+        _check(lib().yams_b200_bm25_postings(self._h, field, term_hash, C.byref(df), C.byref(idf), C.byref(ttf), None, None, 0), "bm25_postings")
+        docs = np.zeros(max(df.value, 1), np.uint32)
+        tfs = np.zeros(max(df.value, 1), np.uint32)
+        _check(lib().yams_b200_bm25_postings(self._h, field, term_hash, C.byref(df), C.byref(idf), C.byref(ttf), docs.ctypes.data_as(u32p),
+                                             tfs.ctypes.data_as(u32p), df.value), "bm25_postings")
+        return docs[:df.value], tfs[:df.value], np.float32(idf.value), ttf.value
+
+    def doc_lengths(self, field: int = 0) -> np.ndarray:
+        out = np.zeros(max(self.n, 1), np.uint32)
+        _check(lib().yams_b200_bm25_doc_lengths(self._h, field, out.ctypes.data_as(u32p)), "bm25_doc_lengths")
+        return out[:self.n]
+
+    def last_timings(self) -> dict:
+        ms = (C.c_float * 8)()
+        _check(lib().yams_b200_bm25_last_timings(self._h, ms), "bm25_last_timings")
+        return {"build_upload_ms": ms[0], "build_tokenise_ms": ms[1], "build_sort_ms": ms[2], "build_postings_ms": ms[3],
+                "build_wall_ms": ms[4], "build_slices": int(ms[5]), "score_device_ms": ms[6], "score_wall_ms": ms[7]}
+
+    def close(self):
+        if getattr(self, "_h", None):
+            lib().yams_b200_bm25_destroy(self._h)
             self._h = None
 
     def __del__(self):

@@ -17,6 +17,7 @@
 #include <vector>
 
 #include "cdc_kernels.cuh"
+#include "upload.cuh"
 
 namespace yb {
 
@@ -429,11 +430,6 @@ static yams_status_t run_device(const uint8_t* d_data, size_t len, const yams_cd
     return YAMS_OK;
 }
 
-// One piece of a packed layout: `len` bytes from host memory `src` at layout position `pos`.
-struct LayoutPiece {
-    uint64_t pos, len;
-    const uint8_t* src;
-};
 // Writes the image of layout positions [lo, hi) to dst: the bytes of the pieces (ascending, disjoint), zeros elsewhere.
 static void layout_image(const std::vector<LayoutPiece>& pieces, uint8_t* dst, uint64_t lo, uint64_t hi) {
     // first piece that ends beyond lo
@@ -471,19 +467,19 @@ static unsigned stage_threads() {
     }();
     return v;
 }
-static yams_status_t staged_upload(IngestRes& r, uint8_t* d_dst, uint64_t total, const std::vector<LayoutPiece>& pieces,
-                                   cudaStream_t st) {
+yams_status_t staged_upload(HostBuf pin[2], cudaEvent_t pin_done[2], uint8_t* d_dst, uint64_t total,
+                            const std::vector<LayoutPiece>& pieces, cudaStream_t st) {
     if (total == 0) return YAMS_OK;
     yams_status_t rc;
     const uint64_t S = std::min<uint64_t>(stage_slice_bytes(), (total + 255) & ~255ull);
     for (int b = 0; b < 2; ++b)
-        if ((rc = r.pin[b].reserve((size_t)S)) != YAMS_OK) return rc;
+        if ((rc = pin[b].reserve((size_t)S)) != YAMS_OK) return rc;
     const unsigned T = total < (4u << 20) ? 1u : stage_threads();
     int b = 0;
     for (uint64_t lo = 0; lo < total; lo += S, b ^= 1) {
         const uint64_t hi = std::min<uint64_t>(total, lo + S);
-        YB_CUDA(cudaEventSynchronize(r.pin_done[b]));   // the copy that last used this pinned buffer has finished
-        uint8_t* img = r.pin[b].as<uint8_t>();
+        YB_CUDA(cudaEventSynchronize(pin_done[b]));   // the copy that last used this pinned buffer has finished
+        uint8_t* img = pin[b].as<uint8_t>();
         if (T == 1) {
             layout_image(pieces, img, lo, hi);
         } else {
@@ -496,7 +492,7 @@ static yams_status_t staged_upload(IngestRes& r, uint8_t* d_dst, uint64_t total,
             for (auto& x : th) x.join();
         }
         YB_CUDA(cudaMemcpyAsync(d_dst + lo, img, (size_t)(hi - lo), cudaMemcpyHostToDevice, st));
-        YB_CUDA(cudaEventRecord(r.pin_done[b], st));
+        YB_CUDA(cudaEventRecord(pin_done[b], st));
     }
     return YAMS_OK;
 }
@@ -541,7 +537,7 @@ static yams_status_t run_batch_group(IngestRes& r, const uint8_t* const* files, 
     if ((rc = r.first.reserve(((size_t)nf + 1) * 8)) != YAMS_OK) return rc;
     YB_CUDA(cudaEventRecord(r.call[0], st));
     // the whole buffer is uploaded, file bytes and zero gaps alike
-    if ((rc = staged_upload(r, d_buf, L + 256, pieces, st)) != YAMS_OK) return rc;
+    if ((rc = staged_upload(r.pin, r.pin_done, d_buf, L + 256, pieces, st)) != YAMS_OK) return rc;
     YB_CUDA(cudaMemcpyAsync(r.fileinfo.p, lay.data(), (size_t)nf * 16, cudaMemcpyHostToDevice, st));
     YB_CUDA(cudaEventRecord(r.ev[0], st));
     uint32_t ncand = 0;
@@ -680,7 +676,7 @@ static yams_status_t session_feed(yams_b200_ingest* s, const uint8_t* data, size
         const uint8_t* src = data + i * kFeedSlice;
         if (pageable && sl >= (4u << 20)) {
             // ordinary host memory: pinned double-buffered upload filled by host threads (see staged_upload)
-            yams_status_t ur = staged_upload(r, r.stage[b].as<uint8_t>() + s->head, sl, {{0, (uint64_t)sl, src}}, r.copy_st);
+            yams_status_t ur = staged_upload(r.pin, r.pin_done, r.stage[b].as<uint8_t>() + s->head, sl, {{0, (uint64_t)sl, src}}, r.copy_st);
             if (ur != YAMS_OK) return ur;
         } else {
             YB_CUDA(cudaMemcpyAsync(r.stage[b].as<uint8_t>() + s->head, src, sl, cudaMemcpyHostToDevice, r.copy_st));
@@ -958,7 +954,7 @@ yams_status_t yams_b200_sha256_many(void* self, const uint8_t* const* msgs, cons
             ++i1;
         }
         if ((rc = r.stage[0].reserve((size_t)tot + 256)) != YAMS_OK) return rc;
-        if ((rc = staged_upload(r, r.stage[0].as<uint8_t>(), tot, pieces, r.st)) != YAMS_OK) return rc;
+        if ((rc = staged_upload(r.pin, r.pin_done, r.stage[0].as<uint8_t>(), tot, pieces, r.st)) != YAMS_OK) return rc;
         if ((rc = r.hash_table(r.stage[0].as<uint8_t>(), h, tot, digests + 32 * i0)) != YAMS_OK) return rc;
     }
     return YAMS_OK;

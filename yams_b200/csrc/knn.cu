@@ -328,6 +328,7 @@ yams_status_t stage1_cuda_core(const Stage1Args& a, bool filter, cudaStream_t st
 // fkey / fkey_inv: cosine.cuh
 constexpr int SEL_THREADS = 256;
 constexpr int SEL_MAXK = 4096;       // survivors per query the select / final kernels can order in shared memory
+static_assert(TOPK_MAX == SEL_MAXK, "launch_topk_dense takes K <= TOPK_MAX");
 
 struct SelectIn {
     const float* dense;     // mode dense: scores[q * ld + i], row = row_start + i * row_stride
@@ -1423,6 +1424,13 @@ void launch_topk_lists(const Cand* lists, const uint32_t* counts, uint32_t cap, 
                        cudaStream_t st) {
     SelectIn in{};
     in.cands = lists; in.counts = counts; in.cap = cap;
+    topk_select_kernel<<<nq, SEL_THREADS, 0, st>>>(in, K, 0, nullptr, out_sel, out_n, nullptr);
+}
+// top-K of dense score rows: row q of `dense` holds the n scores of documents 0..n-1; out_sel[q * K ..] best first (score
+// descending, then document ascending), out_n[q] = min(n, K)
+void launch_topk_dense(const float* dense, uint64_t n, uint32_t nq, uint32_t K, Cand* out_sel, uint32_t* out_n, cudaStream_t st) {
+    SelectIn in{};
+    in.dense = dense; in.ld = n; in.row_start = 0; in.row_stride = 1; in.dense_len = n;
     topk_select_kernel<<<nq, SEL_THREADS, 0, st>>>(in, K, 0, nullptr, out_sel, out_n, nullptr);
 }
 void launch_final_plain(const Exact* exact, uint32_t Kp, uint32_t k, uint32_t nq, const int64_t* rowids, const DeviceResults& out,

@@ -147,6 +147,8 @@ yams_status_t stage1_cuda_core(const Stage1Args& a, bool filter, cudaStream_t st
 // Stages of the exact scan that the other engines (pq.cu) launch on their own lists; each is described at its definition in knn.cu
 void launch_topk_lists(const Cand* lists, const uint32_t* counts, uint32_t cap, uint32_t nq, uint32_t K, Cand* out_sel, uint32_t* out_n,
                        cudaStream_t st);
+void launch_topk_dense(const float* dense, uint64_t n, uint32_t nq, uint32_t K, Cand* out_sel, uint32_t* out_n, cudaStream_t st);
+constexpr uint32_t TOPK_MAX = 4096;   // the largest K the selection orders in shared memory (knn.cu SEL_MAXK)
 void launch_final_plain(const Exact* exact, uint32_t Kp, uint32_t k, uint32_t nq, const int64_t* rowids, const DeviceResults& out,
                         cudaStream_t st);
 void launch_map_rowids(const int64_t* rowids_in, uint64_t n_in, const int64_t* corpus_rowids, uint64_t n, Cand* out, cudaStream_t st);

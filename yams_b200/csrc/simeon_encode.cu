@@ -34,36 +34,11 @@
 #include <vector>
 
 #include "common.cuh"
+#include "text_hash.cuh"
 
 namespace yb {
 
 constexpr int ENC_THREADS = 256;
-
-__host__ __device__ __forceinline__ uint64_t sm64_mix(uint64_t z) {
-    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL;
-    z = (z ^ (z >> 27)) * 0x94D049BB133111EBULL;
-    return z ^ (z >> 31);
-}
-
-// splitmix64_hash of k bytes at p (hasher.cpp:33-47); h0 = splitmix64_mix(seed ^ 0x9E37...) is precomputed
-__device__ __forceinline__ uint64_t gram_hash(const uint8_t* __restrict__ p, uint32_t k, uint64_t h0) {
-    uint64_t h = h0;
-    uint32_t i = 0;
-    while (i + 8 <= k) {
-        uint64_t chunk = 0;
-#pragma unroll
-        for (int b = 0; b < 8; ++b) chunk |= (uint64_t)p[i + b] << (8 * b);
-        h = sm64_mix(h ^ chunk);
-        i += 8;
-    }
-    if (i < k) {
-        uint64_t tail = 0;
-        for (uint32_t j = 0; i + j < k; ++j) tail |= (uint64_t)p[i + j] << (8 * j);
-        tail ^= (uint64_t)(k - i) << 56;
-        h = sm64_mix(h ^ tail);
-    }
-    return sm64_mix(h ^ (uint64_t)k);
-}
 
 // achlioptas_entry (projection.cpp:22-34) as a 2-bit code: 0 zero, 1 plus, 2 minus
 __global__ void achlioptas_table_kernel(uint32_t sketch_dim, uint32_t output_dim, uint64_t seed, uint32_t words_per_col, uint32_t* __restrict__ table) {
@@ -89,7 +64,7 @@ struct EncArgs {
     const uint64_t* offsets;    // n + 1
     uint32_t n;
     uint32_t kmin, kmax, sketch_dim, output_dim, words_per_col;
-    uint64_t h0;                // splitmix64_mix(hash_seed ^ 0x9E3779B97F4A7C15)
+    uint64_t h0;                // gram_hash_h0(hash_seed)
     const uint32_t* table;
     float scale;                // sqrt(3.0f) * (1.0f / sqrt((float)output_dim)), evaluated on the host in float like projection.cpp:128-129
     int l2_normalize;
@@ -100,11 +75,6 @@ struct EncArgs {
     const uint32_t* sample;     // Fwht: output_dim distinct coordinates of the transformed vector
     float fwht_scale;           // Fwht: 1.0f / sqrt((float)output_dim)
 };
-
-// std::isalnum in the "C" locale, or '_' (tokenizer.cpp:13-15)
-__device__ __forceinline__ bool is_word_char(uint8_t c) {
-    return (c >= '0' && c <= '9') || (c >= 'A' && c <= 'Z') || (c >= 'a' && c <= 'z') || c == '_';
-}
 
 __global__ void __launch_bounds__(ENC_THREADS) simeon_encode_kernel(EncArgs a) {
     extern __shared__ unsigned char sm[];
@@ -375,7 +345,7 @@ yams_status_t yams_b200_simeon_encode(yams_b200_encoder* e, const char* const* t
     a.n = (uint32_t)n;
     a.kmin = e->cfg.ngram_min; a.kmax = e->cfg.ngram_max;
     a.sketch_dim = e->cfg.sketch_dim; a.output_dim = D; a.words_per_col = e->words_per_col;
-    a.h0 = sm64_mix(e->cfg.hash_seed ^ 0x9E3779B97F4A7C15ULL);
+    a.h0 = gram_hash_h0(e->cfg.hash_seed);
     a.table = e->table.as<uint32_t>();
     a.scale = e->scale;
     a.l2_normalize = e->cfg.l2_normalize;

@@ -19,6 +19,7 @@
 #include <map>
 #include <optional>
 #include <string>
+#include <string_view>
 #include <unordered_map>
 #include <unordered_set>
 #include <vector>
@@ -938,6 +939,98 @@ public:
             if ((*out)[i] < 0) (*out)[i] = singleton++;
         return YAMS_OK;
     }
+};
+
+// simeon::Bm25Index (third_party/simeon/include/simeon/bm25.hpp) as SimeonLexicalBackend uses it
+// (src/search/simeon_lexical_backend.cpp: buildAsync adds every document then finalizes; score fills a vector of all document
+// scores): add_doc buffers the text, finalize() makes one device build (yams_b200_bm25_build), score() runs on the device.
+// Errors the reference reports by throwing (add_doc after finalize, score before it or into a span of the wrong size) throw
+// std::runtime_error here too, as does a failed device call.  Atire and SubwordAwareBackoff only (yams_bm25_config).
+class B200Bm25Index {
+public:
+    explicit B200Bm25Index(const yams_bm25_config* cfg = nullptr) {
+        if (cfg) cfg_ = *cfg; else yams_b200_bm25_default_config(&cfg_);
+    }
+    ~B200Bm25Index() { yams_b200_bm25_destroy(idx_); }
+    B200Bm25Index(const B200Bm25Index&) = delete;
+    B200Bm25Index& operator=(const B200Bm25Index&) = delete;
+
+    void add_doc(std::string_view text) {
+        if (idx_) throw std::runtime_error("Bm25Index::add_doc after finalize()");
+        texts_.emplace_back(text);
+    }
+    void finalize() {
+        if (idx_) return;
+        std::vector<const char*> ptrs;
+        std::vector<size_t> lens;
+        for (const auto& t : texts_) { ptrs.push_back(t.data()); lens.push_back(t.size()); }
+        check(yams_b200_bm25_build(nullptr, &cfg_, ptrs.data(), lens.data(), texts_.size(), &idx_), "build");
+        n_ = texts_.size();
+        texts_.clear();
+        texts_.shrink_to_fit();
+        check(yams_b200_bm25_stats(idx_, &stats_), "stats");
+        doc_lengths_.resize(n_);
+        check(yams_b200_bm25_doc_lengths(idx_, 0, doc_lengths_.data()), "doc_lengths");
+    }
+    void score(std::string_view query, std::span<float> out_scores) const {
+        if (!idx_) throw std::runtime_error("Bm25Index::score before finalize()");
+        if (out_scores.size() != n_) throw std::runtime_error("Bm25Index::score out_scores size mismatch");
+        const char* q = query.data();
+        const size_t len = query.size();
+        check(yams_b200_bm25_score(idx_, &q, &len, 1, out_scores.data(), 0, nullptr, nullptr, nullptr), "score");
+    }
+    uint32_t doc_count() const noexcept { return (uint32_t)(idx_ ? n_ : texts_.size()); }
+    float avg_dl() const noexcept { return idx_ ? stats_.avg_dl : 0.0f; }
+    uint32_t doc_length(uint32_t doc_id) const noexcept { return doc_id < doc_lengths_.size() ? doc_lengths_[doc_id] : 0u; }
+    uint64_t total_tokens() const noexcept { return idx_ ? stats_.total_tokens : 0; }
+    // Bm25Index::df / idf / total_tf: the raw term's hash (no tokenising, no case folding), 0 when unknown or not finalized
+    uint32_t df(std::string_view term) const { return lookup(term).df; }
+    float idf(std::string_view term) const { return lookup(term).idf; }
+    uint64_t total_tf(std::string_view term) const { return lookup(term).total_tf; }
+    uint64_t hash_term(std::string_view term) const noexcept {
+        // splitmix64_hash (simeon src/hasher.cpp:33-47)
+        auto mix = [](uint64_t z) {
+            z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL;
+            z = (z ^ (z >> 27)) * 0x94D049BB133111EBULL;
+            return z ^ (z >> 31);
+        };
+        uint64_t h = mix(cfg_.hash_seed ^ 0x9E3779B97F4A7C15ULL);
+        const size_t n = term.size();
+        size_t i = 0;
+        for (; i + 8 <= n; i += 8) {
+            uint64_t chunk = 0;
+            for (int b = 0; b < 8; ++b) chunk |= (uint64_t)(uint8_t)term[i + b] << (8 * b);
+            h = mix(h ^ chunk);
+        }
+        if (i < n) {
+            uint64_t tail = 0;
+            for (size_t j = 0; i + j < n; ++j) tail |= (uint64_t)(uint8_t)term[i + j] << (8 * j);
+            h = mix(h ^ (tail ^ ((uint64_t)(n - i) << 56)));
+        }
+        return mix(h ^ (uint64_t)n);
+    }
+
+private:
+    struct Term {
+        uint32_t df = 0;
+        float idf = 0.0f;
+        uint64_t total_tf = 0;
+    };
+    Term lookup(std::string_view term) const {
+        Term t;
+        if (!idx_ || term.empty()) return t;
+        check(yams_b200_bm25_postings(idx_, 0, hash_term(term), &t.df, &t.idf, &t.total_tf, nullptr, nullptr, 0), "postings");
+        return t;
+    }
+    static void check(yams_status_t st, const char* what) {
+        if (st != YAMS_OK) throw std::runtime_error(std::string("yams_b200_bm25 ") + what + ": " + yams_b200_last_error());
+    }
+    yams_bm25_config cfg_{};
+    std::vector<std::string> texts_;
+    yams_b200_bm25* idx_ = nullptr;
+    uint64_t n_ = 0;
+    yams_bm25_stats stats_{};
+    std::vector<uint32_t> doc_lengths_;
 };
 
 }  // namespace yams_b200::host
