@@ -506,8 +506,13 @@ static yams_status_t bm25_build(yams_b200_bm25* x, const char* const* texts, con
     // ---- document slices: pairs of one slice (words + n-grams) within what the device can hold ----
     size_t free_b = 0, total_b = 0;
     YB_CUDA(cudaMemGetInfo(&free_b, &total_b));
-    // per pair of a slice: keys and values twice, run starts, the word arrays, postings and the sort's scratch: ~96 bytes
-    const uint64_t budget = std::max<uint64_t>(1ull << 20, std::min<uint64_t>((uint64_t)free_b / 2 / 96, 1ull << 31));
+    // per pair of a slice: keys and values twice, run starts, the word arrays, postings and the sort's scratch: ~96 bytes.
+    // YAMS_B200_BM25_SLICE_PAIRS = N >= 1 lowers the budget to N pairs, read at every build (the index is the same at any cut).
+    uint64_t budget = std::max<uint64_t>(1ull << 20, std::min<uint64_t>((uint64_t)free_b / 2 / 96, 1ull << 31));
+    if (const char* e = getenv("YAMS_B200_BM25_SLICE_PAIRS")) {
+        const uint64_t cap = strtoull(e, nullptr, 10);
+        if (cap) budget = std::min(budget, cap);
+    }
     std::vector<uint64_t> cuts{0};
     uint64_t acc = 0;
     for (uint64_t d = 0; d < n; ++d) {
