@@ -590,9 +590,9 @@ YAMS_B200_API void yams_b200_simeon_destroy(yams_b200_encoder* e);
  *          SubwordAwareBackoff adds alpha * bm25plus over the word's list (alpha = df / (df + gamma), 0 when df = 0) when
  *          alpha > 0, and (1 - alpha) * bm25plus over the list of each distinct n-gram of the word still in the index when
  *          alpha < 1.  Every float operation is the reference's, in its order, without fused multiply-adds.
- * Scores are bit-identical to the reference.  Out of scope (the caller's, as today): the concept blend
- * (ConceptIndex::blend_into) applied to the returned vector, fragment geometry, the strategy router, RRF, the BM25F aux field,
- * SDM / word bigrams, PRF, and the caller's document windowing (buildEnhancementText). */
+ * Scores are bit-identical to the reference.  The concept blend (ConceptIndex::blend_into) is the concepts block below.  Out of
+ * scope (the caller's, as today): fragment geometry, the strategy router, RRF, the BM25F aux field, SDM / word bigrams, PRF, and
+ * the caller's document windowing (buildEnhancementText). */
 #define YAMS_BM25_ATIRE 0                    /* simeon::Bm25Variant::Atire */
 #define YAMS_BM25_SUBWORD_AWARE_BACKOFF 7    /* simeon::Bm25Variant::SubwordAwareBackoff */
 typedef struct yams_bm25_config {
@@ -640,6 +640,68 @@ YAMS_B200_API yams_status_t yams_b200_bm25_doc_lengths(yams_b200_bm25* idx, uint
  * device ms, [7] its host wall ms */
 YAMS_B200_API yams_status_t yams_b200_bm25_last_timings(yams_b200_bm25* idx, float out_ms[8]);
 YAMS_B200_API void yams_b200_bm25_destroy(yams_b200_bm25* idx);
+
+/* ---- Simeon word-bigram concepts (DESIGN.md §4.12) ---------------------------------------------------------------
+ * third_party/simeon ConceptIndex (src/concept_mining.cpp) mined against a BM25 index, and its blend into BM25 scores, as the
+ * lexical backend configures them (concept mining on, concept_weight 0.5).
+ *   mine   words as in the index but hashed WITHOUT case folding; a document of w >= 2 words has the w - 1 ordered bigrams
+ *          hash_bigram(a, b) and bigram_dl = w - 1 (else 0); avg = float(double(sum bigram_dl) / n).  Nothing is kept when the
+ *          index has no tokens or no document has a bigram.  A bigram is kept when total_tf >= min_ttf, both words of its first
+ *          occurrence are in the index (their index total_tf: an uppercase word never is), and pmi = log((ttf / sum_bdl) /
+ *          ((tf_a / T) * (tf_b / T))) is finite and >= pmi_floor (T = the index's total_tokens); over max_concepts, the highest
+ *          float pmi are kept, and a tie across the cut is settled as the reference settles it (std::nth_element over its map's
+ *          order).  idf = logf((n - df + 0.5f) / (df + 0.5f) + 1.0f).
+ *   blend  for queries of >= 2 (unfolded) words, each distinct adjacent bigram that is a concept, in the reference's order, adds
+ *          weight * pmi * score_atire(tf, bigram_dl, idf, k1, b, avg) to each document of its posting list.
+ * Everything is bit-identical to the reference.  One device pass: beyond device memory the call fails with YAMS_ERR_INTERNAL
+ * (about 16 bytes per word pair plus the sort's double buffer and the postings). */
+typedef struct yams_concept_config {
+    uint32_t min_ttf;             /* 5 */
+    float pmi_floor;              /* 2.0 */
+    uint32_t max_concepts;        /* 200 000 */
+    float k1, b;                  /* 1.2, 0.75 */
+} yams_concept_config;
+typedef struct yams_b200_concepts yams_b200_concepts;
+YAMS_B200_API void yams_b200_concepts_default_config(yams_concept_config* cfg);
+/* mine_concepts(idx, texts, cfg) over n_docs HOST texts (they may differ from the index's, as the backend's raw texts do; NULL
+ * text of length 0 = empty).  The handle owns what it needs (hash seed included) and may outlive idx.  n_docs < 2^32 - 1. */
+YAMS_B200_API yams_status_t yams_b200_concepts_mine(yams_b200_bm25* idx, const yams_concept_config* cfg /* NULL = default */,
+                                                    const char* const* texts, const size_t* lens, uint64_t n_docs,
+                                                    yams_b200_concepts** out);
+/* yams_b200_bm25_score, then ConceptIndex::blend_into(query, scores, weight) of each query before the top-k: the same outputs
+ * and limits.  concepts NULL, empty, or of another document count than idx: no blend (the reference's size test). */
+YAMS_B200_API yams_status_t yams_b200_bm25_score_blended(yams_b200_bm25* idx, const yams_b200_concepts* concepts, float weight,
+                                                         const char* const* queries, const size_t* qlens, uint32_t nq,
+                                                         float* out_scores, uint32_t k, uint32_t* out_docs, float* out_topk_scores,
+                                                         uint32_t* out_counts);
+/* ConceptIndex::blend_into(query, inout_scores[n], weight) on a HOST vector: a no-op unless n == doc_count */
+YAMS_B200_API yams_status_t yams_b200_concepts_blend(yams_b200_concepts* concepts, const char* query, size_t qlen, float weight,
+                                                     float* inout_scores, uint64_t n);
+typedef struct yams_concepts_stats {
+    uint64_t size;                /* kept concepts */
+    uint64_t doc_count;
+    float avg_bigram_dl;
+    uint32_t replayed;            /* 1: a pmi tie crossed max_concepts and the reference's selection order was replayed */
+    uint64_t sum_bigram_dl;
+    uint64_t distinct;            /* distinct bigram hashes */
+    uint64_t passed_min_ttf;      /* of these, total_tf >= min_ttf */
+    uint64_t accepted;            /* accepted before the cap */
+} yams_concepts_stats;
+YAMS_B200_API yams_status_t yams_b200_concepts_stats(yams_b200_concepts* concepts, yams_concepts_stats* out);
+/* ConceptIndex::find(hash): *found 0/1; pmi, idf, total_tf, a_hash, b_hash, df and the first min(df, cap) (document, tf)
+ * postings in document order (out_docs / out_tfs nullable when cap = 0) */
+YAMS_B200_API yams_status_t yams_b200_concepts_find(yams_b200_concepts* concepts, uint64_t hash, uint32_t* found, float* pmi, float* idf,
+                                                    uint64_t* total_tf, uint64_t* a_hash, uint64_t* b_hash, uint32_t* df,
+                                                    uint32_t* out_docs, uint32_t* out_tfs, uint64_t cap);
+/* the kept concepts' hashes, ascending -> out[size] (HOST) */
+YAMS_B200_API yams_status_t yams_b200_concepts_hashes(yams_b200_concepts* concepts, uint64_t* out);
+/* bigram_dl of every document -> out[doc_count] (HOST) */
+YAMS_B200_API yams_status_t yams_b200_concepts_bigram_lengths(yams_b200_concepts* concepts, uint32_t* out);
+/* out_ms: the mining's device ms of [0] the upload, [1] the tokenising (words, pairs), [2] the sort, [3] the runs and the filter,
+ * [4] the gather of the kept postings; [5] its host ms of the log, the floor and the cap, [6] of the replay alone (0 when it did
+ * not run), [7] its host wall ms */
+YAMS_B200_API yams_status_t yams_b200_concepts_last_timings(yams_b200_concepts* concepts, float out_ms[8]);
+YAMS_B200_API void yams_b200_concepts_destroy(yams_b200_concepts* concepts);
 
 /* [0] stage-1 scan ms, [1] rescoring+select ms, [2] total device ms of the last yams_b200_search or
  * yams_b200_search_device on this corpus (the latter's once its work is done); [3] unused (0);

@@ -61,6 +61,15 @@ class Bm25Stats(C.Structure):
                 ("terms", C.c_uint64 * 2), ("postings", C.c_uint64 * 2), ("pruned", C.c_uint64)]
 
 
+class ConceptConfig(C.Structure):
+    _fields_ = [("min_ttf", C.c_uint32), ("pmi_floor", C.c_float), ("max_concepts", C.c_uint32), ("k1", C.c_float), ("b", C.c_float)]
+
+
+class ConceptStats(C.Structure):
+    _fields_ = [("size", C.c_uint64), ("doc_count", C.c_uint64), ("avg_bigram_dl", C.c_float), ("replayed", C.c_uint32),
+                ("sum_bigram_dl", C.c_uint64), ("distinct", C.c_uint64), ("passed_min_ttf", C.c_uint64), ("accepted", C.c_uint64)]
+
+
 BM25_ATIRE, BM25_SUBWORD_AWARE_BACKOFF = 0, 7   # simeon::Bm25Variant numbering
 
 SIMEON_WORD_TOKENS = 1        # NGramMode::CharAndWord
@@ -162,6 +171,18 @@ SYMBOLS = {
     "yams_b200_bm25_doc_lengths": (C.c_int, [C.c_void_p, C.c_uint32, u32p]),
     "yams_b200_bm25_last_timings": (C.c_int, [C.c_void_p, f32p]),
     "yams_b200_bm25_destroy": (None, [C.c_void_p]),
+    "yams_b200_concepts_default_config": (None, [C.POINTER(ConceptConfig)]),
+    "yams_b200_concepts_mine": (C.c_int, [C.c_void_p, C.POINTER(ConceptConfig), C.POINTER(C.c_char_p), C.POINTER(C.c_size_t), C.c_uint64,
+                                          C.POINTER(C.c_void_p)]),
+    "yams_b200_bm25_score_blended": (C.c_int, [C.c_void_p, C.c_void_p, C.c_float, C.POINTER(C.c_char_p), C.POINTER(C.c_size_t), C.c_uint32,
+                                               f32p, C.c_uint32, u32p, f32p, u32p]),
+    "yams_b200_concepts_blend": (C.c_int, [C.c_void_p, C.c_char_p, C.c_size_t, C.c_float, f32p, C.c_uint64]),
+    "yams_b200_concepts_stats": (C.c_int, [C.c_void_p, C.POINTER(ConceptStats)]),
+    "yams_b200_concepts_find": (C.c_int, [C.c_void_p, C.c_uint64, u32p, f32p, f32p, u64p, u64p, u64p, u32p, u32p, u32p, C.c_uint64]),
+    "yams_b200_concepts_hashes": (C.c_int, [C.c_void_p, u64p]),
+    "yams_b200_concepts_bigram_lengths": (C.c_int, [C.c_void_p, u32p]),
+    "yams_b200_concepts_last_timings": (C.c_int, [C.c_void_p, f32p]),
+    "yams_b200_concepts_destroy": (None, [C.c_void_p]),
     "yams_b200_pq_build": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, f32p, u64p, C.POINTER(C.c_void_p)]),
     "yams_b200_pq_search": (C.c_int, [C.c_void_p, f32p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_float, i64p, f32p, u32p, u64p]),
     "yams_b200_pq_search_candidates": (C.c_int, [C.c_void_p, f32p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_float, i64p, u64p, i64p, f32p,
@@ -801,9 +822,10 @@ class Bm25Index:
         self._h = C.c_void_p()
         _check(lib().yams_b200_bm25_build(None, C.byref(cfg), ptrs, lens, self.n, C.byref(self._h)), "bm25_build")
 
-    def score(self, queries, k: int = 0, full: bool = True):
+    def score(self, queries, k: int = 0, full: bool = True, concepts: Optional["ConceptIndex"] = None, weight: float = 0.5):
         """Bm25Index::score of every query: {"scores": [nq][n_docs] (full=True)}, and for k > 0 the best k documents of score > 0
-        ("docs", "topk_scores" padded with 0xFFFFFFFF / 0, "counts")."""
+        ("docs", "topk_scores" padded with 0xFFFFFFFF / 0, "counts").  With `concepts`, each query's scores are then blended
+        with ConceptIndex::blend_into(query, scores, weight) before the top-k, as the lexical backend scores."""
         raw, ptrs, lens = _texts(queries)
         nq = len(raw)
         out = {}
@@ -811,14 +833,21 @@ class Bm25Index:
         docs = np.zeros((nq, max(k, 1)), np.uint32)
         tops = np.zeros((nq, max(k, 1)), np.float32)
         counts = np.zeros(max(nq, 1), np.uint32)
-        _check(lib().yams_b200_bm25_score(self._h, ptrs, lens, nq, scores.ctypes.data_as(f32p) if full else None, k,
-                                          docs.ctypes.data_as(u32p), tops.ctypes.data_as(f32p), counts.ctypes.data_as(u32p)),
-               "bm25_score")
+        args = (ptrs, lens, nq, scores.ctypes.data_as(f32p) if full else None, k, docs.ctypes.data_as(u32p), tops.ctypes.data_as(f32p),
+                counts.ctypes.data_as(u32p))
+        if concepts is None:
+            _check(lib().yams_b200_bm25_score(self._h, *args), "bm25_score")
+        else:
+            _check(lib().yams_b200_bm25_score_blended(self._h, concepts._h, weight, *args), "bm25_score_blended")
         if full:
             out["scores"] = scores
         if k:
             out.update(docs=docs, topk_scores=tops, counts=counts[:nq])
         return out
+
+    def mine_concepts(self, texts, **overrides) -> "ConceptIndex":
+        """mine_concepts(this index, texts, ConceptConfig) on the device; overrides: min_ttf, pmi_floor, max_concepts, k1, b."""
+        return ConceptIndex(self, texts, **overrides)
 
     def stats(self) -> dict:
         s = Bm25Stats()
@@ -1071,3 +1100,77 @@ def vec_distance_cosine(a, b):
 
 def vec_distance_l1(a, b):
     return _pair(lib().yams_b200_vec_distance_l1, a, b)
+
+
+class ConceptIndex:
+    """simeon's ConceptIndex mined on the device against a Bm25Index (Bm25Index.mine_concepts).  It holds what it scores with and
+    may outlive the index."""
+
+    def __init__(self, index: Bm25Index, texts, **overrides):
+        cfg = ConceptConfig()
+        lib().yams_b200_concepts_default_config(C.byref(cfg))
+        for k, v in overrides.items():
+            setattr(cfg, k, v)
+        self.cfg = cfg
+        raw, ptrs, lens = _texts(texts)
+        self.n = len(raw)
+        self._h = C.c_void_p()
+        _check(lib().yams_b200_concepts_mine(index._h, C.byref(cfg), ptrs, lens, self.n, C.byref(self._h)), "concepts_mine")
+
+    def stats(self) -> dict:
+        s = ConceptStats()
+        _check(lib().yams_b200_concepts_stats(self._h, C.byref(s)), "concepts_stats")
+        return {"size": s.size, "doc_count": s.doc_count, "avg_bigram_dl": np.float32(s.avg_bigram_dl), "replayed": bool(s.replayed),
+                "sum_bigram_dl": s.sum_bigram_dl, "distinct": s.distinct, "passed_min_ttf": s.passed_min_ttf, "accepted": s.accepted}
+
+    def find(self, concept_hash: int):
+        """ConceptIndex::find: None when absent, else {"pmi", "idf", "total_tf", "a_hash", "b_hash", "docs", "tfs"}."""
+        found, df = C.c_uint32(), C.c_uint32()
+        pmi, idf = C.c_float(), C.c_float()
+        ttf, a, b = C.c_uint64(), C.c_uint64(), C.c_uint64()
+        refs = [C.byref(v) for v in (found, pmi, idf, ttf, a, b, df)]
+        _check(lib().yams_b200_concepts_find(self._h, concept_hash, *refs, None, None, 0), "concepts_find")
+        if not found.value:
+            return None
+        docs = np.zeros(max(df.value, 1), np.uint32)
+        tfs = np.zeros(max(df.value, 1), np.uint32)
+        _check(lib().yams_b200_concepts_find(self._h, concept_hash, *refs, docs.ctypes.data_as(u32p), tfs.ctypes.data_as(u32p), df.value),
+               "concepts_find")
+        return {"pmi": np.float32(pmi.value), "idf": np.float32(idf.value), "total_tf": ttf.value, "a_hash": a.value, "b_hash": b.value,
+                "docs": docs[:df.value], "tfs": tfs[:df.value]}
+
+    def hashes(self) -> np.ndarray:
+        """the kept concepts' hashes, ascending"""
+        size = self.stats()["size"]
+        out = np.zeros(max(size, 1), np.uint64)
+        _check(lib().yams_b200_concepts_hashes(self._h, out.ctypes.data_as(u64p)), "concepts_hashes")
+        return out[:size]
+
+    def bigram_lengths(self) -> np.ndarray:
+        out = np.zeros(max(self.n, 1), np.uint32)
+        _check(lib().yams_b200_concepts_bigram_lengths(self._h, out.ctypes.data_as(u32p)), "concepts_bigram_lengths")
+        return out[:self.n]
+
+    def blend(self, query, scores: np.ndarray, weight: float = 0.5) -> np.ndarray:
+        """ConceptIndex::blend_into(query, scores, weight) on a copy of the float32 vector `scores`, which is returned."""
+        q = query.encode("utf-8") if isinstance(query, str) else bytes(query)
+        out = np.array(scores, dtype=np.float32, copy=True).reshape(-1)
+        _check(lib().yams_b200_concepts_blend(self._h, q, len(q), weight, out.ctypes.data_as(f32p), out.size), "concepts_blend")
+        return out
+
+    def last_timings(self) -> dict:
+        ms = (C.c_float * 8)()
+        _check(lib().yams_b200_concepts_last_timings(self._h, ms), "concepts_last_timings")
+        return {"upload_ms": ms[0], "tokenise_ms": ms[1], "sort_ms": ms[2], "runs_filter_ms": ms[3], "gather_ms": ms[4],
+                "host_ms": ms[5], "replay_ms": ms[6], "wall_ms": ms[7]}
+
+    def close(self):
+        if getattr(self, "_h", None):
+            lib().yams_b200_concepts_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass

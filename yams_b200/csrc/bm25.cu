@@ -29,9 +29,11 @@
 #include <algorithm>
 #include <chrono>
 #include <cmath>
+#include <functional>
 #include <memory>
 #include <mutex>
 #include <new>
+#include <unordered_map>
 #include <unordered_set>
 #include <vector>
 
@@ -86,6 +88,9 @@ __device__ __forceinline__ uint64_t word_end(const uint8_t* t, uint64_t i) {
     return i;
 }
 
+// ConceptIndex::hash_bigram: ordered (a, b) (concept_mining.cpp:40-44)
+__host__ __device__ __forceinline__ uint64_t hash_bigram(uint64_t a, uint64_t b) { return sm64_mix(a ^ sm64_mix(b + 0x9E3779B97F4A7C15ULL)); }
+
 // dl and ngram_dl of every document: the thread at a word's first byte counts the word and its n-grams
 __global__ void bm_doc_counts_kernel(const uint8_t* __restrict__ t, uint64_t len, const uint64_t* __restrict__ pos, uint64_t n,
                                      int sab, uint32_t kmin, uint32_t kmax, uint32_t* __restrict__ dl, uint32_t* __restrict__ gdl) {
@@ -98,16 +103,17 @@ __global__ void bm_doc_counts_kernel(const uint8_t* __restrict__ t, uint64_t len
     }
 }
 
-// one word: its hash, document, length and n-gram count
+// one word: its hash (FOLD: of the ASCII-lowercased bytes), document, length and n-gram count
+template <bool FOLD>
 __global__ void bm_words_kernel(const uint8_t* __restrict__ t, const uint64_t* __restrict__ wstart, uint64_t nw,
                                 const uint64_t* __restrict__ pos, uint64_t n, uint64_t h0, uint32_t kmin, uint32_t kmax,
                                 uint64_t* __restrict__ whash, uint32_t* __restrict__ wdoc, uint32_t* __restrict__ wlen,
                                 uint64_t* __restrict__ gcnt) {
     for (uint64_t w = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; w < nw; w += (uint64_t)gridDim.x * blockDim.x) {
         const uint64_t s = wstart[w], L = word_end(t, s) - s;
-        whash[w] = gram_hash<true>(t + s, L, h0);
+        whash[w] = gram_hash<FOLD>(t + s, L, h0);
         wdoc[w] = (uint32_t)last_le(pos, n + 1, s);
-        wlen[w] = (uint32_t)L;
+        if (wlen) wlen[w] = (uint32_t)L;
         if (gcnt) gcnt[w] = ngram_count(L, kmin, kmax);
     }
 }
@@ -189,7 +195,11 @@ __global__ void bm_unpack_kernel(const uint64_t* __restrict__ pv, uint64_t m, ui
 }
 
 // ---- score ----
-struct RawLeg {        // one query word (field 0) or one distinct n-gram of it (field 1)
+// Field kinds of a leg: 0 the words, 1 the n-grams (the index's two fields), 2 a mined concept (ConceptIndex, blended after the
+// BM25 legs of its query).
+constexpr uint32_t BM_CONCEPT = 2;
+
+struct RawLeg {        // one query word (field 0), one distinct n-gram of it (field 1), or one matched concept (field 2)
     uint64_t hash;
     uint64_t term_hash;
     uint32_t field;
@@ -206,24 +216,34 @@ struct Dict {
     const uint64_t* offs;
     uint64_t terms;
 };
+struct ConceptDict {   // the kept concepts of a ConceptIndex: sorted hashes, posting offsets, pmi and idf; the blend's weight
+    Dict d;
+    const float* pmi;
+    const float* idf;
+    float weight;
+};
 
-__device__ __forceinline__ bool dict_find(const Dict& D, uint64_t h, uint64_t* b, uint64_t* e) {
+__device__ __forceinline__ bool dict_find(const Dict& D, uint64_t h, uint64_t* b, uint64_t* e, uint64_t* t_out = nullptr) {
     if (D.terms == 0 || h < D.hashes[0]) return false;
     const uint64_t t = last_le(D.hashes, D.terms, h);
     if (D.hashes[t] != h) return false;
     *b = D.offs[t];
     *e = D.offs[t + 1];
+    if (t_out) *t_out = t;
     return true;
 }
 
 __global__ void bm_plan_kernel(const RawLeg* __restrict__ raw, uint64_t nlegs, Dict w, Dict g, const float* __restrict__ idf,
-                               int sab, float gamma, Leg* __restrict__ legs) {
+                               int sab, float gamma, ConceptDict c, Leg* __restrict__ legs) {
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nlegs; i += (uint64_t)gridDim.x * blockDim.x) {
         const RawLeg r = raw[i];
         Leg L{};
         L.field = r.field;
-        uint64_t b = 0, e = 0;
-        if (!sab) {
+        uint64_t b = 0, e = 0, t = 0;
+        if (r.field == BM_CONCEPT) {
+            // wpmi = weight * pmi (concept_mining.cpp:106); the host only emits concepts the index keeps
+            if (dict_find(c.d, r.hash, &b, &e, &t)) { L.b = b; L.e = e; L.w = __fmul_rn(c.weight, c.pmi[t]); L.idf = c.idf[t]; }
+        } else if (!sab) {
             if (dict_find(w, r.hash, &b, &e)) { L.b = b; L.e = e; L.idf = idf[e - b]; }
         } else {
             // alpha = float(df) / (float(df) + gamma), 0 when the word is unknown (bm25.cpp:805-807)
@@ -243,14 +263,16 @@ struct ScoreArgs {
     const Leg* legs;
     const uint64_t* qoff;     // legs of query q: [qoff[q], qoff[q + 1])
     uint32_t q0;              // first query of the batch
-    const uint32_t* docs[2];
-    const uint32_t* tfs[2];
-    const uint32_t* dl[2];
-    float avg[2];             // avg_dl > 0 ? avg_dl : 1
+    const uint32_t* docs[3];
+    const uint32_t* tfs[3];
+    const uint32_t* dl[3];
+    float avg[3];             // fields 0, 1: avg_dl > 0 ? avg_dl : 1; field 2: avg_bigram_dl (> 0 whenever a concept exists)
+    float k1[3], b[3];        // fields 0, 1: Bm25Config's; field 2: ConceptConfig's
     uint64_t n;
-    float k1, b, delta;
+    float delta;
     int sab;
-    float* out;               // [batch][n]
+    const float* init;        // nullable: [batch][n] starting scores (the standalone blend), else zeros
+    float* out;               // [batch][n]; may be init
 };
 
 __device__ __forceinline__ uint64_t first_ge(const uint32_t* a, uint64_t lo, uint64_t hi, uint64_t x) {
@@ -266,9 +288,9 @@ __global__ void __launch_bounds__(BM_THREADS) bm_score_kernel(ScoreArgs a) {
     const uint32_t q = a.q0 + blockIdx.y;
     const uint64_t lo = (uint64_t)blockIdx.x * BM_TILE;
     const uint32_t len = (uint32_t)min((uint64_t)BM_TILE, a.n - lo);
-    for (uint32_t i = threadIdx.x; i < len; i += BM_THREADS) s[i] = 0.0f;
+    const float* init = a.init ? a.init + (uint64_t)blockIdx.y * a.n + lo : nullptr;
+    for (uint32_t i = threadIdx.x; i < len; i += BM_THREADS) s[i] = init ? init[i] : 0.0f;
     __syncthreads();
-    const float k1p1 = __fadd_rn(a.k1, 1.0f), omb = __fsub_rn(1.0f, a.b);
     for (uint64_t l = a.qoff[q]; l < a.qoff[q + 1]; ++l) {
         const Leg g = a.legs[l];
         if (g.b == g.e) continue;
@@ -277,17 +299,22 @@ __global__ void __launch_bounds__(BM_THREADS) bm_score_kernel(ScoreArgs a) {
         if (sb == se) continue;   // the same for every thread of the CTA
         const uint32_t* tfs = a.tfs[g.field];
         const uint32_t* dlv = a.dl[g.field];
-        const float avg = a.avg[g.field];
+        const float avg = a.avg[g.field], k1 = a.k1[g.field], b = a.b[g.field];
+        const float k1p1 = __fadd_rn(k1, 1.0f), omb = __fsub_rn(1.0f, b);
         for (uint64_t i = sb + threadIdx.x; i < se; i += BM_THREADS) {
             const uint32_t d = docs[i];
             const float tf = __uint2float_rn(tfs[i]), dl = __uint2float_rn(dlv[d]);
             // tf + k1 * (1 - b + b * dl / avg)
-            const float denom = __fadd_rn(tf, __fmul_rn(a.k1, __fadd_rn(omb, __fdiv_rn(__fmul_rn(a.b, dl), avg))));
+            const float denom = __fadd_rn(tf, __fmul_rn(k1, __fadd_rn(omb, __fdiv_rn(__fmul_rn(b, dl), avg))));
+            // idf * tf * (k1 + 1) / denom: Atire, and a concept's score_atire (concept_mining.cpp:31-36)
+            const float atire = __fdiv_rn(__fmul_rn(__fmul_rn(g.idf, tf), k1p1), denom);
             float add;
-            if (a.sab)   // alpha * (idf * (tf * (k1 + 1) / denom + delta))
+            if (g.field == BM_CONCEPT)   // wpmi * score_atire
+                add = __fmul_rn(g.w, atire);
+            else if (a.sab)              // alpha * (idf * (tf * (k1 + 1) / denom + delta))
                 add = __fmul_rn(g.w, __fmul_rn(g.idf, __fadd_rn(__fdiv_rn(__fmul_rn(tf, k1p1), denom), a.delta)));
-            else         // idf * tf * (k1 + 1) / denom
-                add = __fdiv_rn(__fmul_rn(__fmul_rn(g.idf, tf), k1p1), denom);
+            else
+                add = atire;
             s[d - lo] = __fadd_rn(s[d - lo], add);
         }
         __syncthreads();
@@ -357,15 +384,44 @@ struct yams_b200_bm25 {
     }
 };
 
+// simeon::ConceptIndex mined against an index (DESIGN.md §4.12).  It owns everything it scores with, the hash seed included, and
+// may outlive the index.
+struct yams_b200_concepts {
+    DeviceCtx* dev = nullptr;
+    yams_concept_config cfg{};
+    uint64_t h0 = 0;                 // gram_hash_h0 of the index's hash seed
+    uint64_t n = 0, sum_bdl = 0, distinct = 0, passed_ttf = 0, accepted = 0;
+    float avg = 0.f;
+    uint32_t replayed = 0;
+    DevBuf bdl;                      // n: bigram_dl
+    std::vector<uint32_t> h_bdl;
+    // the kept concepts, by hash ascending: device dictionary and postings, host copies of what find() and the blend read
+    uint64_t size = 0;
+    DevBuf hashes, offs, docs, tfs, pmi, idf;
+    std::vector<uint64_t> h_hashes, h_offs, h_ttf, h_a, h_b;
+    std::vector<float> h_pmi, h_idf;
+    cudaStream_t st = nullptr;
+    cudaEvent_t ev[2] = {nullptr, nullptr};
+    DevBuf raw, legs, qoff, dense;   // standalone blend workspace
+    float ms[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    std::mutex mu;
+    ~yams_b200_concepts() {
+        if (st) cudaStreamSynchronize(st);
+        for (auto& e : ev)
+            if (e) cudaEventDestroy(e);
+        if (st) cudaStreamDestroy(st);
+    }
+};
+
 namespace yb {
 
 static double wall_ms() {
     return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count();
 }
 
-// device ms of the work `fn` enqueues on the index's stream (waits for it)
-template <typename F>
-static yams_status_t timed(yams_b200_bm25* x, float* acc, F&& fn) {
+// device ms of the work `fn` enqueues on the handle's stream (waits for it)
+template <typename H, typename F>
+static yams_status_t timed(H* x, float* acc, F&& fn) {
     YB_CUDA(cudaEventRecord(x->ev[0], x->st));
     yams_status_t rc = fn();
     if (rc != YAMS_OK) return rc;
@@ -450,6 +506,32 @@ static yams_status_t pair_runs(CubTmp& tmp, DevBuf& k, DevBuf& v, uint64_t m, De
     return YAMS_OK;
 }
 
+// texts -> one device layout, document d at pos[d] with one zero byte after it (so no word crosses a document), 16 more zero
+// bytes at the end; d_pos = pos[0..n]
+static yams_status_t upload_texts(const char* const* texts, const size_t* lens, uint64_t n, std::vector<uint64_t>& pos, DevBuf& text,
+                                  DevBuf& d_pos, cudaStream_t st) {
+    pos.assign(n + 1, 0);
+    std::vector<LayoutPiece> pieces;
+    pieces.reserve(n);
+    for (uint64_t d = 0; d < n; ++d) {
+        if (lens[d]) pieces.push_back({pos[d], (uint64_t)lens[d], reinterpret_cast<const uint8_t*>(texts[d])});
+        pos[d + 1] = pos[d] + lens[d] + 1;
+    }
+    const uint64_t L = pos[n];
+    yams_status_t r;
+    if ((r = text.reserve(L + 16)) != YAMS_OK || (r = d_pos.reserve((n + 1) * 8)) != YAMS_OK) return r;
+    HostBuf pin[2];
+    cudaEvent_t done[2] = {nullptr, nullptr};
+    for (auto& e : done) YB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    r = staged_upload(pin, done, text.as<uint8_t>(), L, pieces, st);
+    if (r == YAMS_OK && cudaMemsetAsync(text.as<uint8_t>() + L, 0, 16, st) != cudaSuccess) r = YAMS_ERR_INTERNAL;
+    if (r == YAMS_OK && cudaMemcpyAsync(d_pos.p, pos.data(), (n + 1) * 8, cudaMemcpyHostToDevice, st) != cudaSuccess) r = YAMS_ERR_INTERNAL;
+    cudaStreamSynchronize(st);   // the pinned buffers and pos are read until here
+    for (auto& e : done) cudaEventDestroy(e);
+    if (r == YAMS_ERR_INTERNAL) set_last_error("text upload failed");
+    return r;
+}
+
 static yams_status_t bm25_build(yams_b200_bm25* x, const char* const* texts, const size_t* lens) {
     const double t0 = wall_ms();
     cudaStream_t st = x->st;
@@ -458,35 +540,16 @@ static yams_status_t bm25_build(yams_b200_bm25* x, const char* const* texts, con
     const uint32_t kmin = x->cfg.ngram_min, kmax = x->cfg.ngram_max;
     const uint64_t h0 = gram_hash_h0(x->cfg.hash_seed);
     yams_status_t rc;
-    // ---- layout: document d at pos[d], one zero byte after it ----
-    std::vector<uint64_t> pos(n + 1, 0);
-    std::vector<LayoutPiece> pieces;
-    pieces.reserve(n);
-    for (uint64_t d = 0; d < n; ++d) {
-        if (lens[d]) pieces.push_back({pos[d], (uint64_t)lens[d], reinterpret_cast<const uint8_t*>(texts[d])});
-        pos[d + 1] = pos[d] + lens[d] + 1;
-    }
-    const uint64_t L = pos[n];
+    std::vector<uint64_t> pos;
     DevBuf text, d_pos;
-    if ((rc = text.reserve(L + 16)) != YAMS_OK || (rc = d_pos.reserve((n + 1) * 8)) != YAMS_OK) return rc;
     for (Bm25Field& F : x->f) {
         if ((rc = F.dl.reserve(std::max<uint64_t>(n, 1) * 4)) != YAMS_OK) return rc;
         YB_CUDA(cudaMemsetAsync(F.dl.p, 0, std::max<uint64_t>(n, 1) * 4, st));
         F.h_dl.assign(n, 0);
     }
-    rc = timed(x, &x->ms[0], [&]() -> yams_status_t {
-        HostBuf pin[2];
-        cudaEvent_t done[2] = {nullptr, nullptr};
-        for (auto& e : done) YB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-        yams_status_t r = staged_upload(pin, done, text.as<uint8_t>(), L, pieces, st);
-        if (r == YAMS_OK && cudaMemsetAsync(text.as<uint8_t>() + L, 0, 16, st) != cudaSuccess) r = YAMS_ERR_INTERNAL;
-        if (r == YAMS_OK && cudaMemcpyAsync(d_pos.p, pos.data(), (n + 1) * 8, cudaMemcpyHostToDevice, st) != cudaSuccess) r = YAMS_ERR_INTERNAL;
-        cudaStreamSynchronize(st);   // the pinned buffers are freed on return
-        for (auto& e : done) cudaEventDestroy(e);
-        if (r == YAMS_ERR_INTERNAL) set_last_error("bm25 upload failed");
-        return r;
-    });
+    rc = timed(x, &x->ms[0], [&] { return upload_texts(texts, lens, n, pos, text, d_pos, st); });
     if (rc != YAMS_OK) return rc;
+    const uint64_t L = pos[n];
     // ---- dl / ngram_dl ----
     rc = timed(x, &x->ms[1], [&]() -> yams_status_t {
         if (L) bm_doc_counts_kernel<<<bm_grid(L), BM_THREADS, 0, st>>>(text.as<uint8_t>(), L, d_pos.as<uint64_t>(), n, sab, kmin, kmax,
@@ -536,7 +599,7 @@ static yams_status_t bm25_build(yams_b200_bm25* x, const char* const* texts, con
                 (r = wlen.reserve(std::max<uint64_t>(nw, 1) * 4)) != YAMS_OK || (r = gcnt.reserve(std::max<uint64_t>(nw, 1) * 8)) != YAMS_OK)
                 return r;
             if (nw)
-                bm_words_kernel<<<bm_grid(nw), BM_THREADS, 0, st>>>(text.as<uint8_t>(), wstart.as<uint64_t>(), nw, d_pos.as<uint64_t>(), n, h0,
+                bm_words_kernel<true><<<bm_grid(nw), BM_THREADS, 0, st>>>(text.as<uint8_t>(), wstart.as<uint64_t>(), nw, d_pos.as<uint64_t>(), n, h0,
                                                                     kmin, kmax, whash.as<uint64_t>(), wdoc.as<uint32_t>(), wlen.as<uint32_t>(),
                                                                     sab ? gcnt.as<uint64_t>() : nullptr);
             YB_CUDA(cudaGetLastError());
@@ -613,8 +676,47 @@ static void query_words(const uint8_t* p, size_t len, std::vector<std::pair<size
     }
 }
 
-static yams_status_t bm25_score(yams_b200_bm25* x, const char* const* queries, const size_t* qlens, uint32_t nq, float* out_scores,
-                                uint32_t k, uint32_t* out_docs, float* out_topk, uint32_t* out_counts) {
+// ConceptIndex::blend_into's concept order for one query: its unfolded words' adjacent bigrams that are kept concepts, emplaced
+// into an unordered_map reserved for the word count, in that map's iteration order (concept_mining.cpp:82-104).  The additions
+// of a document in several matched concepts are made in this order.
+static void concept_order(const yams_b200_concepts* c, const uint8_t* p, size_t len, std::vector<std::pair<size_t, size_t>>& ws,
+                          std::vector<uint64_t>& out) {
+    out.clear();
+    query_words(p, len, ws);
+    if (c->size == 0 || ws.size() < 2) return;
+    std::vector<uint64_t> qw(ws.size());
+    for (size_t i = 0; i < ws.size(); ++i) qw[i] = gram_hash(p + ws[i].first, ws[i].second, c->h0);
+    std::unordered_map<uint64_t, uint32_t> matched;
+    matched.reserve(qw.size());
+    for (size_t i = 1; i < qw.size(); ++i) {
+        const uint64_t bh = hash_bigram(qw[i - 1], qw[i]);
+        const auto it = std::lower_bound(c->h_hashes.begin(), c->h_hashes.end(), bh);
+        if (it != c->h_hashes.end() && *it == bh) matched.emplace(bh, (uint32_t)(it - c->h_hashes.begin()));
+    }
+    for (const auto& [bh, j] : matched) {
+        (void)j;
+        out.push_back(bh);
+    }
+}
+
+// the concept field of the score kernel's arguments, and the plan kernel's concept dictionary
+static void concept_field(const yams_b200_concepts* c, ScoreArgs& a) {
+    a.docs[BM_CONCEPT] = c->docs.as<uint32_t>();
+    a.tfs[BM_CONCEPT] = c->tfs.as<uint32_t>();
+    a.dl[BM_CONCEPT] = c->bdl.as<uint32_t>();
+    a.avg[BM_CONCEPT] = c->avg;
+    a.k1[BM_CONCEPT] = c->cfg.k1;
+    a.b[BM_CONCEPT] = c->cfg.b;
+}
+static ConceptDict concept_dict(const yams_b200_concepts* c, float weight) {
+    return ConceptDict{Dict{c->hashes.as<uint64_t>(), c->offs.as<uint64_t>(), c->size}, c->pmi.as<float>(), c->idf.as<float>(), weight};
+}
+
+// Bm25Index::score of every query; with a concept index `c` of the same document count, then ConceptIndex::blend_into(query,
+// scores, weight) of each (SimeonLexicalBackend::score).
+static yams_status_t bm25_score(yams_b200_bm25* x, const yams_b200_concepts* c, float weight, const char* const* queries,
+                                const size_t* qlens, uint32_t nq, float* out_scores, uint32_t k, uint32_t* out_docs, float* out_topk,
+                                uint32_t* out_counts) {
     const double t0 = wall_ms();
     cudaStream_t st = x->st;
     const uint64_t n = x->n;
@@ -627,6 +729,9 @@ static yams_status_t bm25_score(yams_b200_bm25* x, const char* const* queries, c
     std::vector<std::pair<size_t, size_t>> ws;
     std::vector<uint8_t> low;
     std::unordered_set<uint64_t> seen;
+    // the blend is a no-op when the concept index is empty or of another document count (blend_into's size test)
+    const bool blend = c && c->size && c->n == n;
+    std::vector<uint64_t> corder;
     for (uint32_t q = 0; q < nq; ++q) {
         const uint8_t* p = reinterpret_cast<const uint8_t*>(queries[q]);
         query_words(p, qlens[q], ws);
@@ -643,6 +748,10 @@ static yams_status_t bm25_score(yams_b200_bm25* x, const char* const* queries, c
                     const uint64_t gh = gram_hash(low.data() + i, kk, h0);
                     if (seen.insert(gh).second) raw.push_back({gh, th, 1, 0});
                 }
+        }
+        if (blend) {
+            concept_order(c, p, qlens[q], ws, corder);
+            for (uint64_t bh : corder) raw.push_back({bh, bh, BM_CONCEPT, 0});
         }
         qoff[q + 1] = raw.size();
     }
@@ -672,8 +781,9 @@ static yams_status_t bm25_score(yams_b200_bm25* x, const char* const* queries, c
             YB_CUDA(cudaMemcpyAsync(x->raw.p, raw.data(), nlegs * sizeof(RawLeg), cudaMemcpyHostToDevice, st));
             Dict w{x->f[0].hashes.as<uint64_t>(), x->f[0].offs.as<uint64_t>(), x->f[0].terms};
             Dict g{x->f[1].hashes.as<uint64_t>(), x->f[1].offs.as<uint64_t>(), x->f[1].terms};
+            const ConceptDict cd = blend ? concept_dict(c, weight) : ConceptDict{};
             bm_plan_kernel<<<bm_grid(nlegs), BM_THREADS, 0, st>>>(x->raw.as<RawLeg>(), nlegs, w, g, x->idf.as<float>(), sab,
-                                                                  x->cfg.subword_gamma, x->legs.as<Leg>());
+                                                                  x->cfg.subword_gamma, cd, x->legs.as<Leg>());
             YB_CUDA(cudaGetLastError());
         }
         YB_CUDA(cudaMemcpyAsync(x->qoff.p, qoff.data(), (nq + 1) * 8, cudaMemcpyHostToDevice, st));
@@ -685,9 +795,12 @@ static yams_status_t bm25_score(yams_b200_bm25* x, const char* const* queries, c
             a.tfs[fi] = x->f[fi].tfs.as<uint32_t>();
             a.dl[fi] = x->f[fi].dl.as<uint32_t>();
             a.avg[fi] = x->f[fi].avg > 0.0f ? x->f[fi].avg : 1.0f;
+            a.k1[fi] = x->cfg.k1;
+            a.b[fi] = x->cfg.b;
         }
+        if (blend) concept_field(c, a);
         a.n = n;
-        a.k1 = x->cfg.k1; a.b = x->cfg.b; a.delta = x->cfg.delta;
+        a.delta = x->cfg.delta;
         a.sab = sab;
         a.out = x->dense.as<float>();
         const unsigned tiles = (unsigned)((n + BM_TILE - 1) / BM_TILE);
@@ -726,6 +839,361 @@ static yams_status_t bm25_score(yams_b200_bm25* x, const char* const* queries, c
     if (rc != YAMS_OK) return rc;
     x->ms[6] = dev_ms;
     x->ms[7] = (float)(wall_ms() - t0);
+    return YAMS_OK;
+}
+
+// ---- concept mining (mine_concepts, concept_mining.cpp:117-258) ----
+// words per document (integer atomics: exact)
+__global__ void cm_doc_words_kernel(const uint32_t* __restrict__ wdoc, uint64_t nw, uint32_t* __restrict__ cnt) {
+    for (uint64_t w = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; w < nw; w += (uint64_t)gridDim.x * blockDim.x)
+        atomicAdd(&cnt[wdoc[w]], 1u);
+}
+
+// word w starts a bigram: the next word is of the same document
+struct StartsBigram {
+    const uint32_t* wdoc;
+    uint64_t nw;
+    __device__ bool operator()(uint64_t w) const { return w + 1 < nw && wdoc[w + 1] == wdoc[w]; }
+};
+
+// pair j (first word pw[j]): its bigram hash, and j itself, which is its corpus position
+__global__ void cm_pairs_kernel(const uint64_t* __restrict__ pw, uint64_t np, const uint64_t* __restrict__ whash,
+                                uint64_t* __restrict__ key, uint32_t* __restrict__ val) {
+    for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < np; j += (uint64_t)gridDim.x * blockDim.x) {
+        const uint64_t w = pw[j];
+        key[j] = hash_bigram(whash[w], whash[w + 1]);
+        val[j] = (uint32_t)j;
+    }
+}
+
+// the document of every sorted pair
+__global__ void cm_pair_docs_kernel(const uint32_t* __restrict__ pj, uint64_t np, const uint64_t* __restrict__ pw,
+                                    const uint32_t* __restrict__ wdoc, uint32_t* __restrict__ pdoc) {
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < np; i += (uint64_t)gridDim.x * blockDim.x)
+        pdoc[i] = wdoc[pw[pj[i]]];
+}
+
+enum : uint8_t { CM_UNDER_TTF = 0, CM_NO_WORD = 1, CM_CANDIDATE = 2 };
+
+// one distinct bigram (its pairs start at pstart[b] of the sorted pairs, a run of total_tf): the first occurrence (the run's
+// first pair) gives (a, b); under min_ttf or with a word the index lacks it is dropped, else the PMI ratio
+// p_ab / (p_a * p_b) is formed in double, each operation rounded once as the reference's (concept_mining.cpp:211-220)
+__global__ void cm_bigrams_kernel(const uint64_t* __restrict__ pstart, uint64_t nb, uint64_t np, const uint32_t* __restrict__ pj,
+                                  const uint64_t* __restrict__ pw, const uint64_t* __restrict__ whash, Dict words,
+                                  const uint64_t* __restrict__ wttf, uint32_t min_ttf, double sum_bdl, double total_tokens,
+                                  uint32_t* __restrict__ first, uint64_t* __restrict__ ab, uint8_t* __restrict__ status,
+                                  double* __restrict__ ratio) {
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nb; i += (uint64_t)gridDim.x * blockDim.x) {
+        const uint64_t s = pstart[i], e = i + 1 < nb ? pstart[i + 1] : np, ttf = e - s;
+        const uint32_t j = pj[s];
+        const uint64_t a = whash[pw[j]], b = whash[pw[j] + 1];
+        first[i] = j;
+        ab[2 * i] = a;
+        ab[2 * i + 1] = b;
+        ratio[i] = 0.0;
+        if (ttf < min_ttf) { status[i] = CM_UNDER_TTF; continue; }
+        uint64_t lo = 0, hi = 0, t = 0;
+        const uint64_t tf_a = dict_find(words, a, &lo, &hi, &t) ? wttf[t] : 0;
+        const uint64_t tf_b = dict_find(words, b, &lo, &hi, &t) ? wttf[t] : 0;
+        if (tf_a == 0 || tf_b == 0) { status[i] = CM_NO_WORD; continue; }
+        status[i] = CM_CANDIDATE;
+        const double p_ab = __ddiv_rn((double)ttf, sum_bdl);
+        const double p_a = __ddiv_rn((double)tf_a, total_tokens), p_b = __ddiv_rn((double)tf_b, total_tokens);
+        ratio[i] = __ddiv_rn(p_ab, __dmul_rn(p_a, p_b));
+    }
+}
+
+struct IsCandidate {
+    const uint8_t* status;
+    __device__ bool operator()(uint64_t i) const { return status[i] == CM_CANDIDATE; }
+};
+struct PassedTtf {
+    const uint8_t* status;
+    __device__ bool operator()(uint64_t i) const { return status[i] != CM_UNDER_TTF; }
+};
+
+__global__ void cm_candidates_kernel(const uint64_t* __restrict__ cand, uint64_t nc, const uint64_t* __restrict__ bhash,
+                                     const double* __restrict__ ratio, uint64_t* __restrict__ ch, double* __restrict__ cr) {
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nc; i += (uint64_t)gridDim.x * blockDim.x) {
+        ch[i] = bhash[cand[i]];
+        cr[i] = ratio[cand[i]];
+    }
+}
+
+// kept concept j (distinct bigram kb[j]): hash, total_tf, a, b, df
+__global__ void cm_kept_kernel(const uint64_t* __restrict__ kb, uint64_t nk, const uint64_t* __restrict__ bhash,
+                               const uint64_t* __restrict__ boffs, const uint64_t* __restrict__ bttf, const uint64_t* __restrict__ ab,
+                               uint64_t* __restrict__ out) {
+    for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < nk; j += (uint64_t)gridDim.x * blockDim.x) {
+        const uint64_t b = kb[j];
+        out[5 * j] = bhash[b];
+        out[5 * j + 1] = bttf[b];
+        out[5 * j + 2] = ab[2 * b];
+        out[5 * j + 3] = ab[2 * b + 1];
+        out[5 * j + 4] = boffs[b + 1] - boffs[b];
+    }
+}
+
+// posting i of the kept concepts (koffs: their offsets) from the packed postings (document << 32 | tf) of every bigram
+__global__ void cm_gather_kernel(const uint64_t* __restrict__ kb, const uint64_t* __restrict__ koffs, uint64_t nk, uint64_t total,
+                                 const uint64_t* __restrict__ boffs, const uint64_t* __restrict__ pv, uint32_t* __restrict__ docs,
+                                 uint32_t* __restrict__ tfs) {
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (uint64_t)gridDim.x * blockDim.x) {
+        const uint64_t j = last_le(koffs, nk, i);
+        const uint64_t v = pv[boffs[kb[j]] + (i - koffs[j])];
+        docs[i] = (uint32_t)(v >> 32);
+        tfs[i] = (uint32_t)v;
+    }
+}
+
+template <typename K, typename V>
+static yams_status_t radix_sort(CubTmp& tmp, DevBuf& k, DevBuf& v, DevBuf& k2, DevBuf& v2, uint64_t m, cudaStream_t st) {
+    yams_status_t rc;
+    if ((rc = k2.reserve(std::max<uint64_t>(m, 1) * sizeof(K))) != YAMS_OK || (rc = v2.reserve(std::max<uint64_t>(m, 1) * sizeof(V))) != YAMS_OK)
+        return rc;
+    tmp.bytes = 0;
+    YB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp.bytes, k.as<K>(), k2.as<K>(), v.as<V>(), v2.as<V>(), (int64_t)m, 0, 8 * (int)sizeof(K), st));
+    if ((rc = tmp.grow()) != YAMS_OK) return rc;
+    YB_CUDA(cub::DeviceRadixSort::SortPairs(tmp.buf.p, tmp.bytes, k.as<K>(), k2.as<K>(), v.as<V>(), v2.as<V>(), (int64_t)m, 0, 8 * (int)sizeof(K),
+                                            st));
+    std::swap(k, k2);
+    std::swap(v, v2);
+    return YAMS_OK;
+}
+
+// The cap (concept_mining.cpp:228-234) when a PMI tie crosses it.  The reference collects its accepted bigrams in the iteration
+// order of unordered_map<uint64_t, RawEntry> raw, whose keys were inserted in first-occurrence order (the map's order depends
+// on that sequence of keys alone), then keeps the first max_concepts after std::nth_element by PMI descending.  `order` is
+// every distinct bigram hash by first occurrence; `acc` maps an accepted hash to its (PMI, distinct-bigram index).
+static void replay_cap(const std::vector<uint64_t>& order, const std::unordered_map<uint64_t, std::pair<float, uint64_t>>& acc,
+                       uint32_t max_concepts, std::vector<std::pair<uint64_t, float>>& kept) {
+    std::unordered_map<uint64_t, char> raw;
+    for (uint64_t h : order) raw[h];
+    std::vector<std::pair<uint64_t, float>> accepted;   // (hash, PMI), as the reference's vector
+    accepted.reserve(acc.size());
+    for (const auto& [h, unused] : raw) {
+        (void)unused;
+        const auto it = acc.find(h);
+        if (it != acc.end()) accepted.emplace_back(h, it->second.first);
+    }
+    std::nth_element(accepted.begin(), accepted.begin() + static_cast<std::ptrdiff_t>(max_concepts), accepted.end(),
+                     [](const auto& x, const auto& y) { return x.second > y.second; });
+    accepted.resize(max_concepts);
+    kept.clear();
+    for (const auto& [h, pmi] : accepted) kept.emplace_back(acc.at(h).second, pmi);
+}
+
+static yams_status_t concepts_mine(yams_b200_concepts* c, yams_b200_bm25* x, const char* const* texts, const size_t* lens) {
+    const double t0 = wall_ms();
+    cudaStream_t st = c->st;
+    const uint64_t n = c->n;
+    yams_status_t rc;
+    c->h_bdl.assign(n, 0);
+    if ((rc = c->bdl.reserve(std::max<uint64_t>(n, 1) * 4)) != YAMS_OK || (rc = c->offs.reserve(8)) != YAMS_OK) return rc;
+    YB_CUDA(cudaMemsetAsync(c->bdl.p, 0, std::max<uint64_t>(n, 1) * 4, st));
+    YB_CUDA(cudaMemsetAsync(c->offs.p, 0, 8, st));
+    std::vector<uint64_t> pos;
+    DevBuf text, d_pos;
+    rc = timed(c, &c->ms[0], [&] { return upload_texts(texts, lens, n, pos, text, d_pos, st); });
+    if (rc != YAMS_OK) return rc;
+    const uint64_t L = pos[n];
+    // ---- words (unfolded hashes), words per document, pairs of adjacent words of one document ----
+    CubTmp tmp;
+    DevBuf wstart, cnt, whash, wdoc, dcount, pw, key, val, k2, v2;
+    uint64_t nw = 0, np = 0;
+    rc = timed(c, &c->ms[1], [&]() -> yams_status_t {
+        yams_status_t r;
+        if ((r = select_indices(tmp, 0, L, IsWordStart{text.as<uint8_t>()}, wstart, cnt, &nw, st)) != YAMS_OK) return r;
+        if ((r = whash.reserve(std::max<uint64_t>(nw, 1) * 8)) != YAMS_OK || (r = wdoc.reserve(std::max<uint64_t>(nw, 1) * 4)) != YAMS_OK ||
+            (r = dcount.reserve(std::max<uint64_t>(n, 1) * 4)) != YAMS_OK)
+            return r;
+        YB_CUDA(cudaMemsetAsync(dcount.p, 0, std::max<uint64_t>(n, 1) * 4, st));
+        if (nw) {
+            bm_words_kernel<false><<<bm_grid(nw), BM_THREADS, 0, st>>>(text.as<uint8_t>(), wstart.as<uint64_t>(), nw, d_pos.as<uint64_t>(), n,
+                                                                       c->h0, 0, 0, whash.as<uint64_t>(), wdoc.as<uint32_t>(), nullptr, nullptr);
+            cm_doc_words_kernel<<<bm_grid(nw), BM_THREADS, 0, st>>>(wdoc.as<uint32_t>(), nw, dcount.as<uint32_t>());
+        }
+        YB_CUDA(cudaGetLastError());
+        if (n) YB_CUDA(cudaMemcpyAsync(c->h_bdl.data(), dcount.p, n * 4, cudaMemcpyDeviceToHost, st));
+        if (nw && (r = select_indices(tmp, 0, nw, StartsBigram{wdoc.as<uint32_t>(), nw}, pw, cnt, &np, st)) != YAMS_OK) return r;
+        if (np >= 0xFFFFFFFFull) {
+            set_last_error("concept mining: %llu word pairs, at most 2^32 - 2 are served", (unsigned long long)np);
+            return YAMS_ERR_INVALID_ARG;
+        }
+        if ((r = key.reserve(std::max<uint64_t>(np, 1) * 8)) != YAMS_OK || (r = val.reserve(std::max<uint64_t>(np, 1) * 4)) != YAMS_OK) return r;
+        if (np) cm_pairs_kernel<<<bm_grid(np), BM_THREADS, 0, st>>>(pw.as<uint64_t>(), np, whash.as<uint64_t>(), key.as<uint64_t>(), val.as<uint32_t>());
+        YB_CUDA(cudaGetLastError());
+        return YAMS_OK;
+    });
+    if (rc != YAMS_OK) return rc;
+    text = DevBuf();
+    wstart = DevBuf();
+    dcount = DevBuf();
+    // bigram_dl = words - 1 for documents of >= 2 words (concept_mining.cpp:154-159)
+    for (uint64_t d = 0; d < n; ++d) {
+        c->h_bdl[d] = c->h_bdl[d] >= 2 ? c->h_bdl[d] - 1 : 0;
+        c->sum_bdl += c->h_bdl[d];
+    }
+    c->avg = n == 0 ? 0.0f : (float)((double)c->sum_bdl / (double)n);
+    if (n) YB_CUDA(cudaMemcpyAsync(c->bdl.p, c->h_bdl.data(), n * 4, cudaMemcpyHostToDevice, st));
+    // ---- stable sort by bigram hash: each hash's pairs in corpus order ----
+    rc = timed(c, &c->ms[2], [&] { return np ? radix_sort<uint64_t, uint32_t>(tmp, key, val, k2, v2, np, st) : YAMS_OK; });
+    if (rc != YAMS_OK) return rc;
+    k2 = DevBuf();
+    v2 = DevBuf();
+    // ---- runs: (hash, document) -> postings; hash -> distinct bigrams (total_tf, first occurrence); the filter ----
+    DevBuf ph, pv, bhash, boffs, bttf, pstart, first, ab, status, ratio, cand, ch, cr;
+    uint64_t nposts = 0, nb = 0, nc = 0;
+    const uint64_t T = x->total_tokens;
+    std::vector<uint64_t> h_ch;
+    std::vector<double> h_cr;
+    rc = timed(c, &c->ms[3], [&]() -> yams_status_t {
+        yams_status_t r;
+        if (np == 0) return YAMS_OK;
+        DevBuf pdoc, sc;
+        if ((r = pdoc.reserve(np * 4)) != YAMS_OK) return r;
+        cm_pair_docs_kernel<<<bm_grid(np), BM_THREADS, 0, st>>>(val.as<uint32_t>(), np, pw.as<uint64_t>(), wdoc.as<uint32_t>(), pdoc.as<uint32_t>());
+        YB_CUDA(cudaGetLastError());
+        if ((r = pair_runs(tmp, key, pdoc, np, ph, pv, &nposts, st)) != YAMS_OK) return r;
+        if ((r = select_indices(tmp, 0, nposts, NewTerm{ph.as<uint64_t>()}, sc, cnt, &nb, st)) != YAMS_OK) return r;
+        if ((r = bhash.reserve(nb * 8)) != YAMS_OK || (r = boffs.reserve((nb + 1) * 8)) != YAMS_OK || (r = bttf.reserve(nb * 8)) != YAMS_OK)
+            return r;
+        bm_terms_kernel<<<bm_grid(nb), BM_THREADS, 0, st>>>(ph.as<uint64_t>(), pv.as<uint64_t>(), nposts, sc.as<uint64_t>(), nb,
+                                                            bhash.as<uint64_t>(), boffs.as<uint64_t>(), bttf.as<uint64_t>());
+        YB_CUDA(cudaGetLastError());
+        uint64_t nb2 = 0;
+        if ((r = select_indices(tmp, 0, np, NewTerm{key.as<uint64_t>()}, pstart, cnt, &nb2, st)) != YAMS_OK) return r;
+        if ((r = first.reserve(nb * 4)) != YAMS_OK || (r = ab.reserve(nb * 16)) != YAMS_OK || (r = status.reserve(nb)) != YAMS_OK ||
+            (r = ratio.reserve(nb * 8)) != YAMS_OK)
+            return r;
+        const Dict words{x->f[0].hashes.as<uint64_t>(), x->f[0].offs.as<uint64_t>(), x->f[0].terms};
+        cm_bigrams_kernel<<<bm_grid(nb), BM_THREADS, 0, st>>>(pstart.as<uint64_t>(), nb, np, val.as<uint32_t>(), pw.as<uint64_t>(),
+                                                              whash.as<uint64_t>(), words, x->f[0].ttf.as<uint64_t>(), c->cfg.min_ttf,
+                                                              (double)c->sum_bdl, (double)T, first.as<uint32_t>(), ab.as<uint64_t>(),
+                                                              status.as<uint8_t>(), ratio.as<double>());
+        YB_CUDA(cudaGetLastError());
+        if ((r = select_indices(tmp, 0, nb, PassedTtf{status.as<uint8_t>()}, cand, cnt, &c->passed_ttf, st)) != YAMS_OK) return r;
+        // the reference returns before the filter when the index has no tokens (concept_mining.cpp:193-195); sum_bdl > 0 here
+        if (T == 0) return YAMS_OK;
+        if ((r = select_indices(tmp, 0, nb, IsCandidate{status.as<uint8_t>()}, cand, cnt, &nc, st)) != YAMS_OK) return r;
+        if ((r = ch.reserve(std::max<uint64_t>(nc, 1) * 8)) != YAMS_OK || (r = cr.reserve(std::max<uint64_t>(nc, 1) * 8)) != YAMS_OK) return r;
+        if (nc) cm_candidates_kernel<<<bm_grid(nc), BM_THREADS, 0, st>>>(cand.as<uint64_t>(), nc, bhash.as<uint64_t>(), ratio.as<double>(),
+                                                                         ch.as<uint64_t>(), cr.as<double>());
+        YB_CUDA(cudaGetLastError());
+        h_ch.resize(nc);
+        h_cr.resize(nc);
+        if (nc) {
+            YB_CUDA(cudaMemcpyAsync(h_ch.data(), ch.p, nc * 8, cudaMemcpyDeviceToHost, st));
+            YB_CUDA(cudaMemcpyAsync(h_cr.data(), cr.p, nc * 8, cudaMemcpyDeviceToHost, st));
+        }
+        return YAMS_OK;
+    });
+    if (rc != YAMS_OK) return rc;
+    c->distinct = nb;
+    key = DevBuf();
+    // ---- host: std::log of each ratio, the finiteness and floor tests, float(pmi); the cap ----
+    const double th = wall_ms();
+    std::vector<uint64_t> h_cand(nc);
+    if (nc) {
+        YB_CUDA(cudaMemcpyAsync(h_cand.data(), cand.p, nc * 8, cudaMemcpyDeviceToHost, st));
+        YB_CUDA(cudaStreamSynchronize(st));
+    }
+    std::vector<std::pair<uint64_t, float>> kept;   // (distinct-bigram index, PMI)
+    std::vector<uint64_t> khash;                     // the hash of each
+    std::vector<float> apmi;
+    for (uint64_t i = 0; i < nc; ++i) {
+        const double pmi = std::log(h_cr[i]);
+        if (!std::isfinite(pmi) || pmi < (double)c->cfg.pmi_floor) continue;
+        kept.emplace_back(h_cand[i], (float)pmi);
+        khash.push_back(h_ch[i]);
+    }
+    c->accepted = kept.size();
+    const uint64_t cap = c->cfg.max_concepts;
+    double replay_ms = 0.0;
+    if (kept.size() > cap) {
+        apmi.resize(kept.size());
+        for (size_t i = 0; i < kept.size(); ++i) apmi[i] = kept[i].second;
+        std::nth_element(apmi.begin(), apmi.begin() + cap, apmi.end(), std::greater<float>());
+        const float at_cut = apmi[cap];                                  // rank max_concepts
+        const float last_in = cap ? *std::min_element(apmi.begin(), apmi.begin() + cap) : at_cut;   // rank max_concepts - 1
+        if (cap == 0) {
+            kept.clear();
+        } else if (last_in != at_cut) {
+            // no tie across the cut: the top max_concepts are the same in any order
+            std::vector<std::pair<uint64_t, float>> top;
+            top.reserve(cap);
+            for (const auto& kv : kept)
+                if (kv.second >= last_in) top.push_back(kv);
+            kept.swap(top);
+        } else {
+            const double tr = wall_ms();
+            std::vector<uint64_t> order(nb);
+            DevBuf k1, v1, k3, v3;
+            if ((rc = k1.reserve(nb * 4)) != YAMS_OK || (rc = v1.reserve(nb * 8)) != YAMS_OK) return rc;
+            YB_CUDA(cudaMemcpyAsync(k1.p, first.p, nb * 4, cudaMemcpyDeviceToDevice, st));
+            YB_CUDA(cudaMemcpyAsync(v1.p, bhash.p, nb * 8, cudaMemcpyDeviceToDevice, st));
+            if ((rc = radix_sort<uint32_t, uint64_t>(tmp, k1, v1, k3, v3, nb, st)) != YAMS_OK) return rc;
+            YB_CUDA(cudaMemcpyAsync(order.data(), v1.p, nb * 8, cudaMemcpyDeviceToHost, st));
+            YB_CUDA(cudaStreamSynchronize(st));
+            std::unordered_map<uint64_t, std::pair<float, uint64_t>> acc;
+            acc.reserve(kept.size());
+            for (size_t i = 0; i < kept.size(); ++i) acc.emplace(khash[i], std::make_pair(kept[i].second, kept[i].first));
+            replay_cap(order, acc, c->cfg.max_concepts, kept);
+            c->replayed = 1;
+            replay_ms = wall_ms() - tr;
+        }
+    }
+    std::sort(kept.begin(), kept.end());   // by distinct-bigram index: hash ascending
+    const uint64_t nk = kept.size();
+    c->size = nk;
+    c->ms[5] = (float)(wall_ms() - th - replay_ms);
+    c->ms[6] = (float)replay_ms;
+    // ---- gather the kept concepts: dictionary, postings, pmi, idf ----
+    rc = timed(c, &c->ms[4], [&]() -> yams_status_t {
+        yams_status_t r;
+        if (nk == 0) return YAMS_OK;
+        std::vector<uint64_t> kb(nk), info(5 * nk);
+        for (uint64_t j = 0; j < nk; ++j) kb[j] = kept[j].first;
+        DevBuf d_kb, d_info;
+        if ((r = d_kb.reserve(nk * 8)) != YAMS_OK || (r = d_info.reserve(nk * 40)) != YAMS_OK) return r;
+        YB_CUDA(cudaMemcpyAsync(d_kb.p, kb.data(), nk * 8, cudaMemcpyHostToDevice, st));
+        cm_kept_kernel<<<bm_grid(nk), BM_THREADS, 0, st>>>(d_kb.as<uint64_t>(), nk, bhash.as<uint64_t>(), boffs.as<uint64_t>(),
+                                                           bttf.as<uint64_t>(), ab.as<uint64_t>(), d_info.as<uint64_t>());
+        YB_CUDA(cudaGetLastError());
+        YB_CUDA(cudaMemcpyAsync(info.data(), d_info.p, nk * 40, cudaMemcpyDeviceToHost, st));
+        YB_CUDA(cudaStreamSynchronize(st));
+        c->h_hashes.resize(nk); c->h_ttf.resize(nk); c->h_a.resize(nk); c->h_b.resize(nk);
+        c->h_offs.assign(nk + 1, 0); c->h_pmi.resize(nk); c->h_idf.resize(nk);
+        const float nf = (float)n;
+        for (uint64_t j = 0; j < nk; ++j) {
+            c->h_hashes[j] = info[5 * j];
+            c->h_ttf[j] = info[5 * j + 1];
+            c->h_a[j] = info[5 * j + 2];
+            c->h_b[j] = info[5 * j + 3];
+            c->h_offs[j + 1] = c->h_offs[j] + info[5 * j + 4];
+            c->h_pmi[j] = kept[j].second;
+            // the BM25 idf expression for this concept's df (concept_mining.cpp:252-253)
+            const float df = (float)info[5 * j + 4];
+            c->h_idf[j] = std::log((nf - df + 0.5f) / (df + 0.5f) + 1.0f);
+        }
+        const uint64_t total = c->h_offs[nk];
+        if ((r = c->hashes.reserve(nk * 8)) != YAMS_OK || (r = c->offs.reserve((nk + 1) * 8)) != YAMS_OK ||
+            (r = c->pmi.reserve(nk * 4)) != YAMS_OK || (r = c->idf.reserve(nk * 4)) != YAMS_OK ||
+            (r = c->docs.reserve(total * 4)) != YAMS_OK || (r = c->tfs.reserve(total * 4)) != YAMS_OK)
+            return r;
+        YB_CUDA(cudaMemcpyAsync(c->hashes.p, c->h_hashes.data(), nk * 8, cudaMemcpyHostToDevice, st));
+        YB_CUDA(cudaMemcpyAsync(c->offs.p, c->h_offs.data(), (nk + 1) * 8, cudaMemcpyHostToDevice, st));
+        YB_CUDA(cudaMemcpyAsync(c->pmi.p, c->h_pmi.data(), nk * 4, cudaMemcpyHostToDevice, st));
+        YB_CUDA(cudaMemcpyAsync(c->idf.p, c->h_idf.data(), nk * 4, cudaMemcpyHostToDevice, st));
+        cm_gather_kernel<<<bm_grid(total), BM_THREADS, 0, st>>>(d_kb.as<uint64_t>(), c->offs.as<uint64_t>(), nk, total, boffs.as<uint64_t>(),
+                                                                pv.as<uint64_t>(), c->docs.as<uint32_t>(), c->tfs.as<uint32_t>());
+        YB_CUDA(cudaGetLastError());
+        YB_CUDA(cudaStreamSynchronize(st));   // the host vectors and d_kb are read until here
+        return YAMS_OK;
+    });
+    if (rc != YAMS_OK) return rc;
+    YB_CUDA(cudaStreamSynchronize(st));
+    c->ms[7] = (float)(wall_ms() - t0);
     return YAMS_OK;
 }
 
@@ -802,7 +1270,7 @@ yams_status_t yams_b200_bm25_score(yams_b200_bm25* idx, const char* const* queri
     for (uint32_t q = 0; q < nq; ++q) YB_ARG(queries[q] || qlens[q] == 0, "null query");
     YB_BIND(idx);
     std::lock_guard<std::mutex> g(idx->mu);
-    return bm25_score(idx, queries, qlens, nq, out_scores, k, out_docs, out_topk_scores, out_counts);
+    return bm25_score(idx, nullptr, 0.0f, queries, qlens, nq, out_scores, k, out_docs, out_topk_scores, out_counts);
     YB_CATCH
 }
 
@@ -885,5 +1353,168 @@ yams_status_t yams_b200_bm25_last_timings(yams_b200_bm25* idx, float out_ms[8]) 
 }
 
 void yams_b200_bm25_destroy(yams_b200_bm25* idx) { delete idx; }
+
+void yams_b200_concepts_default_config(yams_concept_config* cfg) {
+    if (!cfg) return;
+    // ConceptConfig defaults (include/simeon/concept_mining.hpp:16-23)
+    cfg->min_ttf = 5;
+    cfg->pmi_floor = 2.0f;
+    cfg->max_concepts = 200000;
+    cfg->k1 = 1.2f;
+    cfg->b = 0.75f;
+}
+
+yams_status_t yams_b200_concepts_mine(yams_b200_bm25* idx, const yams_concept_config* cfg_in, const char* const* texts, const size_t* lens,
+                                      uint64_t n_docs, yams_b200_concepts** out) {
+    YB_TRY
+    DeviceCtx* dev = nullptr;
+    yams_status_t rc = ensure_device(&dev);
+    if (rc != YAMS_OK) return rc;
+    YB_ARG(idx && out, "null argument");
+    *out = nullptr;
+    YB_ARG(n_docs < 0xFFFFFFFFull, "too many documents");
+    YB_ARG(n_docs == 0 || (texts && lens), "null argument");
+    for (uint64_t i = 0; i < n_docs; ++i) YB_ARG(texts[i] || lens[i] == 0, "null text");
+    YB_BIND(idx);
+    std::unique_ptr<yams_b200_concepts> c(new (std::nothrow) yams_b200_concepts());
+    if (!c) return YAMS_ERR_INTERNAL;
+    c->dev = dev;
+    if (cfg_in) c->cfg = *cfg_in; else yams_b200_concepts_default_config(&c->cfg);
+    c->n = n_docs;
+    YB_CUDA(cudaStreamCreateWithFlags(&c->st, cudaStreamNonBlocking));
+    for (auto& e : c->ev) YB_CUDA(cudaEventCreate(&e));
+    std::lock_guard<std::mutex> g(idx->mu);
+    c->h0 = gram_hash_h0(idx->cfg.hash_seed);
+    if ((rc = concepts_mine(c.get(), idx, texts, lens)) != YAMS_OK) return rc;
+    *out = c.release();
+    return YAMS_OK;
+    YB_CATCH
+}
+
+yams_status_t yams_b200_bm25_score_blended(yams_b200_bm25* idx, const yams_b200_concepts* concepts, float weight, const char* const* queries,
+                                           const size_t* qlens, uint32_t nq, float* out_scores, uint32_t k, uint32_t* out_docs,
+                                           float* out_topk_scores, uint32_t* out_counts) {
+    YB_TRY
+    DeviceCtx* dev = nullptr;
+    yams_status_t rc = ensure_device(&dev);
+    if (rc != YAMS_OK) return rc;
+    YB_ARG(idx, "index is null");
+    YB_ARG(k <= TOPK_MAX, "k must be <= 4096");
+    YB_ARG(k == 0 || (out_docs && out_topk_scores && out_counts), "null top-k output");
+    if (nq == 0) return YAMS_OK;
+    YB_ARG(queries && qlens, "null argument");
+    for (uint32_t q = 0; q < nq; ++q) YB_ARG(queries[q] || qlens[q] == 0, "null query");
+    YB_BIND(idx);
+    std::lock_guard<std::mutex> g(idx->mu);
+    return bm25_score(idx, concepts, weight, queries, qlens, nq, out_scores, k, out_docs, out_topk_scores, out_counts);
+    YB_CATCH
+}
+
+yams_status_t yams_b200_concepts_blend(yams_b200_concepts* c, const char* query, size_t qlen, float weight, float* inout, uint64_t n) {
+    YB_TRY
+    DeviceCtx* dev = nullptr;
+    yams_status_t rc = ensure_device(&dev);
+    if (rc != YAMS_OK) return rc;
+    YB_ARG(c, "concept index is null");
+    YB_ARG(query || qlen == 0, "null query");
+    YB_ARG(inout || n == 0, "null score vector");
+    if (n != c->n || c->size == 0) return YAMS_OK;
+    YB_BIND(c);
+    std::lock_guard<std::mutex> g(c->mu);
+    std::vector<std::pair<size_t, size_t>> ws;
+    std::vector<uint64_t> order;
+    concept_order(c, reinterpret_cast<const uint8_t*>(query), qlen, ws, order);
+    if (order.empty()) return YAMS_OK;
+    std::vector<RawLeg> raw;
+    for (uint64_t bh : order) raw.push_back({bh, bh, BM_CONCEPT, 0});
+    const uint64_t nlegs = raw.size(), qoff[2] = {0, nlegs};
+    cudaStream_t st = c->st;
+    if ((rc = c->raw.reserve(nlegs * sizeof(RawLeg))) != YAMS_OK || (rc = c->legs.reserve(nlegs * sizeof(Leg))) != YAMS_OK ||
+        (rc = c->qoff.reserve(16)) != YAMS_OK || (rc = c->dense.reserve(n * 4)) != YAMS_OK)
+        return rc;
+    float dev_ms = 0.f;   // timed() also waits for the copy back
+    return timed(c, &dev_ms, [&]() -> yams_status_t {
+        YB_CUDA(cudaMemcpyAsync(c->raw.p, raw.data(), nlegs * sizeof(RawLeg), cudaMemcpyHostToDevice, st));
+        YB_CUDA(cudaMemcpyAsync(c->qoff.p, qoff, 16, cudaMemcpyHostToDevice, st));
+        YB_CUDA(cudaMemcpyAsync(c->dense.p, inout, n * 4, cudaMemcpyHostToDevice, st));
+        bm_plan_kernel<<<bm_grid(nlegs), BM_THREADS, 0, st>>>(c->raw.as<RawLeg>(), nlegs, Dict{}, Dict{}, nullptr, 0, 0.0f,
+                                                              concept_dict(c, weight), c->legs.as<Leg>());
+        ScoreArgs a{};
+        a.legs = c->legs.as<Leg>();
+        a.qoff = c->qoff.as<uint64_t>();
+        concept_field(c, a);
+        a.n = n;
+        a.init = c->dense.as<float>();   // in place: each CTA reads and writes its own tile
+        a.out = c->dense.as<float>();
+        bm_score_kernel<<<dim3((unsigned)((n + BM_TILE - 1) / BM_TILE), 1), BM_THREADS, 0, st>>>(a);
+        YB_CUDA(cudaGetLastError());
+        YB_CUDA(cudaMemcpyAsync(inout, c->dense.p, n * 4, cudaMemcpyDeviceToHost, st));
+        return YAMS_OK;
+    });
+    YB_CATCH
+}
+
+yams_status_t yams_b200_concepts_stats(yams_b200_concepts* c, yams_concepts_stats* out) {
+    YB_ARG(c && out, "null argument");
+    out->size = c->size;
+    out->doc_count = c->n;
+    out->avg_bigram_dl = c->avg;
+    out->replayed = c->replayed;
+    out->sum_bigram_dl = c->sum_bdl;
+    out->distinct = c->distinct;
+    out->passed_min_ttf = c->passed_ttf;
+    out->accepted = c->accepted;
+    return YAMS_OK;
+}
+
+yams_status_t yams_b200_concepts_find(yams_b200_concepts* c, uint64_t hash, uint32_t* found, float* pmi, float* idf, uint64_t* total_tf,
+                                      uint64_t* a_hash, uint64_t* b_hash, uint32_t* df, uint32_t* out_docs, uint32_t* out_tfs, uint64_t cap) {
+    YB_TRY
+    DeviceCtx* dev = nullptr;
+    yams_status_t rc = ensure_device(&dev);
+    if (rc != YAMS_OK) return rc;
+    YB_ARG(c && found && pmi && idf && total_tf && a_hash && b_hash && df, "null argument");
+    YB_ARG(cap == 0 || (out_docs && out_tfs), "null posting output");
+    *found = 0; *pmi = 0.0f; *idf = 0.0f; *total_tf = 0; *a_hash = 0; *b_hash = 0; *df = 0;
+    const auto it = std::lower_bound(c->h_hashes.begin(), c->h_hashes.end(), hash);
+    if (it == c->h_hashes.end() || *it != hash) return YAMS_OK;
+    const uint64_t j = (uint64_t)(it - c->h_hashes.begin());
+    *found = 1;
+    *pmi = c->h_pmi[j];
+    *idf = c->h_idf[j];
+    *total_tf = c->h_ttf[j];
+    *a_hash = c->h_a[j];
+    *b_hash = c->h_b[j];
+    *df = (uint32_t)(c->h_offs[j + 1] - c->h_offs[j]);
+    const uint64_t m = std::min<uint64_t>(*df, cap);
+    if (m) {
+        YB_BIND(c);
+        YB_CUDA(cudaMemcpy(out_docs, c->docs.as<uint32_t>() + c->h_offs[j], m * 4, cudaMemcpyDeviceToHost));
+        YB_CUDA(cudaMemcpy(out_tfs, c->tfs.as<uint32_t>() + c->h_offs[j], m * 4, cudaMemcpyDeviceToHost));
+    }
+    return YAMS_OK;
+    YB_CATCH
+}
+
+yams_status_t yams_b200_concepts_hashes(yams_b200_concepts* c, uint64_t* out) {
+    YB_ARG(c && (out || c->size == 0), "null argument");
+    if (c->size) memcpy(out, c->h_hashes.data(), c->size * 8);
+    return YAMS_OK;
+}
+
+yams_status_t yams_b200_concepts_bigram_lengths(yams_b200_concepts* c, uint32_t* out) {
+    YB_ARG(c && (out || c->n == 0), "null argument");
+    if (c->n) memcpy(out, c->h_bdl.data(), c->n * 4);
+    return YAMS_OK;
+}
+
+yams_status_t yams_b200_concepts_last_timings(yams_b200_concepts* c, float out_ms[8]) {
+    YB_ARG(c && out_ms, "null argument");
+    std::lock_guard<std::mutex> g(c->mu);
+    for (int i = 0; i < 8; ++i) out_ms[i] = c->ms[i];
+    return YAMS_OK;
+}
+
+void yams_b200_concepts_destroy(yams_b200_concepts* c) { delete c; }
 
 }  // extern "C"

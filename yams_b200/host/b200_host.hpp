@@ -946,6 +946,8 @@ public:
 // scores): add_doc buffers the text, finalize() makes one device build (yams_b200_bm25_build), score() runs on the device.
 // Errors the reference reports by throwing (add_doc after finalize, score before it or into a span of the wrong size) throw
 // std::runtime_error here too, as does a failed device call.  Atire and SubwordAwareBackoff only (yams_bm25_config).
+class B200ConceptIndex;
+
 class B200Bm25Index {
 public:
     explicit B200Bm25Index(const yams_bm25_config* cfg = nullptr) {
@@ -979,8 +981,12 @@ public:
         const size_t len = query.size();
         check(yams_b200_bm25_score(idx_, &q, &len, 1, out_scores.data(), 0, nullptr, nullptr, nullptr), "score");
     }
+    // SimeonLexicalBackend::score with its concept index: the BM25 scores, then concepts->blend_into(query, scores, weight), fused
+    // on the device (a null or empty concept index, or one of another document count, adds nothing)
+    void score(std::string_view query, std::span<float> out_scores, const B200ConceptIndex* concepts, float weight) const;
     uint32_t doc_count() const noexcept { return (uint32_t)(idx_ ? n_ : texts_.size()); }
     float avg_dl() const noexcept { return idx_ ? stats_.avg_dl : 0.0f; }
+    yams_b200_bm25* handle() const noexcept { return idx_; }
     uint32_t doc_length(uint32_t doc_id) const noexcept { return doc_id < doc_lengths_.size() ? doc_lengths_[doc_id] : 0u; }
     uint64_t total_tokens() const noexcept { return idx_ ? stats_.total_tokens : 0; }
     // Bm25Index::df / idf / total_tf: the raw term's hash (no tokenising, no case folding), 0 when unknown or not finalized
@@ -1032,5 +1038,92 @@ private:
     yams_bm25_stats stats_{};
     std::vector<uint32_t> doc_lengths_;
 };
+
+// simeon::ConceptEntry / ConceptIndex (include/simeon/concept_mining.hpp) mined on the device: size, doc_count, avg_dl, find,
+// score and blend_into as the lexical backend calls them.  It owns its device state and may outlive the index it was mined
+// against.
+struct B200ConceptEntry {
+    float pmi = 0.0f;
+    float idf = 0.0f;
+    uint64_t total_tf = 0;
+    uint64_t a_hash = 0;
+    uint64_t b_hash = 0;
+    std::vector<std::pair<uint32_t, uint32_t>> docs;
+};
+
+class B200ConceptIndex {
+public:
+    B200ConceptIndex() = default;
+    ~B200ConceptIndex() { yams_b200_concepts_destroy(c_); }
+    B200ConceptIndex(B200ConceptIndex&& o) noexcept : c_(o.c_), stats_(o.stats_) { o.c_ = nullptr; o.stats_ = {}; }
+    B200ConceptIndex& operator=(B200ConceptIndex&& o) noexcept {
+        if (this != &o) {
+            yams_b200_concepts_destroy(c_);
+            c_ = o.c_;
+            stats_ = o.stats_;
+            o.c_ = nullptr;
+            o.stats_ = {};
+        }
+        return *this;
+    }
+    B200ConceptIndex(const B200ConceptIndex&) = delete;
+    B200ConceptIndex& operator=(const B200ConceptIndex&) = delete;
+
+    uint32_t size() const noexcept { return (uint32_t)stats_.size; }
+    uint32_t doc_count() const noexcept { return (uint32_t)stats_.doc_count; }
+    float avg_dl() const noexcept { return stats_.avg_bigram_dl; }
+    // ConceptIndex::find: nullopt when the hash is not a kept concept
+    std::optional<B200ConceptEntry> find(uint64_t concept_hash) const {
+        if (!c_) return std::nullopt;
+        uint32_t found = 0, df = 0;
+        B200ConceptEntry e;
+        check(yams_b200_concepts_find(c_, concept_hash, &found, &e.pmi, &e.idf, &e.total_tf, &e.a_hash, &e.b_hash, &df, nullptr, nullptr, 0),
+              "find");
+        if (!found) return std::nullopt;
+        std::vector<uint32_t> docs(df), tfs(df);
+        check(yams_b200_concepts_find(c_, concept_hash, &found, &e.pmi, &e.idf, &e.total_tf, &e.a_hash, &e.b_hash, &df, docs.data(),
+                                      tfs.data(), df),
+              "find");
+        for (uint32_t i = 0; i < df; ++i) e.docs.emplace_back(docs[i], tfs[i]);
+        return e;
+    }
+    void score(std::string_view query, std::span<float> out_scores) const { blend_into(query, out_scores, 1.0f); }
+    void blend_into(std::string_view query, std::span<float> out_scores, float weight) const {
+        if (!c_) return;
+        check(yams_b200_concepts_blend(c_, query.data(), query.size(), weight, out_scores.data(), out_scores.size()), "blend");
+    }
+    const yams_b200_concepts* handle() const noexcept { return c_; }
+
+private:
+    friend B200ConceptIndex mine_concepts(const B200Bm25Index&, std::span<const std::string_view>, const yams_concept_config&);
+    static void check(yams_status_t st, const char* what) {
+        if (st != YAMS_OK) throw std::runtime_error(std::string("yams_b200_concepts ") + what + ": " + yams_b200_last_error());
+    }
+    yams_b200_concepts* c_ = nullptr;
+    yams_concepts_stats stats_{};
+};
+
+// simeon::mine_concepts(idx, docs, cfg) on the device.  The backend mines only corpora of 100 documents or more
+// (simeon_lexical_backend.cpp:507); that rule stays the caller's, as in INTEGRATION §11.
+inline B200ConceptIndex mine_concepts(const B200Bm25Index& idx, std::span<const std::string_view> docs, const yams_concept_config& cfg) {
+    if (!idx.handle()) throw std::runtime_error("mine_concepts before finalize()");
+    std::vector<const char*> ptrs;
+    std::vector<size_t> lens;
+    for (const auto& d : docs) { ptrs.push_back(d.data()); lens.push_back(d.size()); }
+    B200ConceptIndex out;
+    B200ConceptIndex::check(yams_b200_concepts_mine(idx.handle(), &cfg, ptrs.data(), lens.data(), docs.size(), &out.c_), "mine");
+    B200ConceptIndex::check(yams_b200_concepts_stats(out.c_, &out.stats_), "stats");
+    return out;
+}
+
+inline void B200Bm25Index::score(std::string_view query, std::span<float> out_scores, const B200ConceptIndex* concepts, float weight) const {
+    if (!idx_) throw std::runtime_error("Bm25Index::score before finalize()");
+    if (out_scores.size() != n_) throw std::runtime_error("Bm25Index::score out_scores size mismatch");
+    const char* q = query.data();
+    const size_t len = query.size();
+    check(yams_b200_bm25_score_blended(idx_, concepts ? concepts->handle() : nullptr, weight, &q, &len, 1, out_scores.data(), 0, nullptr,
+                                       nullptr, nullptr),
+          "score_blended");
+}
 
 }  // namespace yams_b200::host
