@@ -415,7 +415,12 @@ YAMS_B200_API yams_status_t yams_b200_topology_kmeans_last_timings(yams_b200_cor
  * yams_b200_search_device_finish waits for the stream, returns YAMS_ERR_INVALID_ARG if a query was non-finite / zero,
  * and re-runs the queries the certificate rejected through the exhaustive levels, patching the device outputs in place
  * (*out_resolved = how many; 0 for ordinary data).  A caller that pipelines batches calls it before it consumes the
- * outputs of that batch; only the most recent search_device of a corpus can be finished. */
+ * outputs of that batch.  A pending search is finished against the corpus it was enqueued on before any other call on that
+ * corpus runs (an append, remove or clear, a search of any form, the graph, k-means, document search, a diagnostic): that
+ * call first waits for the stream and runs the exhaustive levels, and search_device_finish later returns what they returned
+ * and resolved.  The output buffers must therefore stay valid until search_device_finish or until the next call on the
+ * corpus.  Only a later search_device supersedes a pending search, without waiting for it: its finish then reports
+ * nothing for the superseded batch, whose rejected queries are never re-run. */
 YAMS_B200_API yams_status_t yams_b200_search_device(yams_b200_corpus* c, const float* d_queries,
                                                     uint32_t nq, uint32_t k, float threshold,
                                                     int64_t* d_out_rowids, float* d_out_scores);

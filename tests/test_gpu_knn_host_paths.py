@@ -1,7 +1,8 @@
 """GPU tests of the exact scan's two host routes: the blocking search and search_device + search_device_finish enqueue and
 finish the same plan, so they must return the same bytes and report the same resolution counts on every path of the scan
-(dense, sampled threshold, exhaustive level 1, full exact pass).  A pending search_device must also survive a corpus
-mutator that reuses the corpus's scratch buffers before it is finished."""
+(dense, sampled threshold, exhaustive level 1, full exact pass).  A pending search_device is finished against the corpus
+it was enqueued on before any other call on that corpus runs, so it also survives a remove that changes nothing
+(test_gpu_corpus_lifecycle.py puts every other call between a search_device and its finish)."""
 import numpy as np
 import pytest
 

@@ -346,6 +346,7 @@ yams_status_t yams_b200_topology_kmeans(yams_b200_corpus* c, uint32_t k_requeste
     YB_ARG(c && out_assignment && out_k && out_iterations, "null argument");
     std::lock_guard<std::mutex> corpus_lock(c->mu);
     YB_BIND(c);
+    settle_pending(c);
     YB_ARG(c->metric == YAMS_B200_COSINE, "k-means clusters a cosine corpus");
     YB_ARG(c->n < 0xFFFFFFFFull, "at most 2^32 - 2 documents");
     const uint32_t n = (uint32_t)c->n, d = c->dim;
@@ -357,7 +358,6 @@ yams_status_t yams_b200_topology_kmeans(yams_b200_corpus* c, uint32_t k_requeste
         return YAMS_OK;
     }
     const auto t0 = std::chrono::steady_clock::now();
-    c->pending.active = false;
     uint64_t k64 = k_requested ? k_requested : (uint64_t)std::llround(std::sqrt((double)n));
     const uint32_t k = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(k64, 2), n);
     const uint32_t iterations = max_iterations == 0 ? 10 : max_iterations;

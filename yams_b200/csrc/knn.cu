@@ -1644,6 +1644,7 @@ yams_status_t yams_b200_corpus_append(yams_b200_corpus* c, const void* rows, uin
     YB_ARG(c, "corpus is null");
     std::lock_guard<std::mutex> corpus_lock(c->mu);
     YB_BIND(c);
+    settle_pending(c);
     if (n == 0) return YAMS_OK;
     YB_ARG(rows, "rows is null");
     YB_ARG(c->n + n < 0xFFFFFFFFull, "corpus is limited to 2^32-1 rows per GPU");
@@ -1660,6 +1661,7 @@ yams_status_t yams_b200_corpus_append_f32_as_f16(yams_b200_corpus* c, const floa
     YB_ARG(c, "corpus is null");
     std::lock_guard<std::mutex> corpus_lock(c->mu);
     YB_BIND(c);
+    settle_pending(c);
     YB_ARG(c->dtype == YAMS_B200_F16, "corpus is not fp16");
     if (n == 0) return YAMS_OK;
     YB_ARG(rows, "rows is null");
@@ -1680,6 +1682,7 @@ yams_status_t yams_b200_corpus_append_synthetic(yams_b200_corpus* c, uint64_t se
     YB_ARG(c, "corpus is null");
     std::lock_guard<std::mutex> corpus_lock(c->mu);
     YB_BIND(c);
+    settle_pending(c);
     if (n == 0) return YAMS_OK;
     YB_ARG(c->n + n < 0xFFFFFFFFull, "corpus is limited to 2^32-1 rows per GPU");
     yams_status_t rc = corpus_reserve(c, c->n + n);
@@ -1701,6 +1704,7 @@ yams_status_t yams_b200_corpus_remove(yams_b200_corpus* c, const int64_t* rowids
     YB_ARG(c, "corpus is null");
     std::lock_guard<std::mutex> corpus_lock(c->mu);
     YB_BIND(c);
+    settle_pending(c);
     if (out_removed) *out_removed = 0;
     if (n == 0 || c->n == 0) return YAMS_OK;
     YB_ARG(rowids, "rowids is null");
@@ -1747,11 +1751,11 @@ yams_status_t yams_b200_corpus_clear(yams_b200_corpus* c) {
     YB_ARG(c, "corpus is null");
     std::lock_guard<std::mutex> corpus_lock(c->mu);
     YB_BIND(c);
+    settle_pending(c);
     c->n = 0;
     ++c->generation;
     c->last_rowid = INT64_MIN;
     c->rowids_dense = true;
-    c->pending.active = false;
     c->r_max = c->dr_abs_max = c->dr_rel_max = c->inv_max = 0.f;
     if (c->stats.p) YB_CUDA(cudaMemsetAsync(c->stats.p, 0, 16, c->st));
     return YAMS_OK;
@@ -1904,6 +1908,24 @@ static yams_status_t finish_search(yams_b200_corpus* c, ScanPlan& p, const int64
     return rc;
 }
 
+}  // extern "C"
+
+void yb::settle_pending(Corpus* c) {
+    if (!c->pending.active) return;
+    c->pending.active = false;
+    uint32_t resolved = 0;
+    yams_status_t rc = YAMS_ERR_INTERNAL;
+    const cudaError_t e = cudaStreamSynchronize(c->st);
+    if (e == cudaSuccess) rc = finish_search(static_cast<yams_b200_corpus*>(c), c->pending.plan, nullptr, nullptr, &resolved);
+    else set_last_error("cudaStreamSynchronize failed: %s", cudaGetErrorString(e));
+    c->pending.settled = true;
+    c->pending.status = rc;
+    c->pending.resolved = resolved;
+    c->pending.error = rc == YAMS_OK ? "" : last_error();
+}
+
+extern "C" {
+
 // the blocking paths: prepare the queries and reject an invalid one before any search work is enqueued
 static yams_status_t prepare_valid_queries(yams_b200_corpus* c, const float* queries, uint32_t nq) {
     yams_status_t rc;
@@ -1922,6 +1944,7 @@ yams_status_t yams_b200_search(yams_b200_corpus* c, const float* queries, uint32
     YB_ARG(c, "corpus is null");
     std::lock_guard<std::mutex> corpus_lock(c->mu);
     YB_BIND(c);
+    settle_pending(c);
     if (nq == 0) return YAMS_OK;
     YB_ARG(queries && out_counts, "null argument");
     YB_ARG(!allowed_rowids || allowed_offsets, "allowed_offsets missing");
@@ -1935,7 +1958,6 @@ yams_status_t yams_b200_search(yams_b200_corpus* c, const float* queries, uint32
     YB_ARG(k <= kMaxK, "k > 3072 is not supported by the fused top-k path (page larger requests)");
     YB_ARG(nq <= 65535, "at most 65535 queries per call (split larger batches)");   // per-query grid dimensions
     YB_ARG(!allowed_offsets || c->metric == YAMS_B200_COSINE, "candidate sets are only supported for the cosine metric");
-    c->pending.active = false;
     yams_status_t rc;
     ScanPlan plan;
     plan.nq = nq; plan.k = k; plan.threshold = threshold;
@@ -1974,12 +1996,12 @@ yams_status_t yams_b200_search_exhaustive(yams_b200_corpus* c, const float* quer
     YB_ARG(c, "corpus is null");
     std::lock_guard<std::mutex> corpus_lock(c->mu);
     YB_BIND(c);
+    settle_pending(c);
     if (nq == 0) return YAMS_OK;
     YB_ARG(queries && out_counts && out_rowids && out_scores, "null argument");
     YB_ARG(k > 0 && k <= kMaxK, "k must be in 1..3072");
     YB_ARG(nq <= 65535, "at most 65535 queries per call");
     yams_status_t rc;
-    c->pending.active = false;
     if ((rc = prepare_valid_queries(c, queries, nq)) != YAMS_OK) return rc;
     ScanPlan plan;
     plan.nq = nq; plan.k = k; plan.threshold = threshold;
@@ -1997,8 +2019,8 @@ yams_status_t yams_b200_search_all_matching(yams_b200_corpus* c, const float* qu
     YB_ARG(c && query && out_count, "null argument");
     std::lock_guard<std::mutex> corpus_lock(c->mu);
     YB_BIND(c);
+    settle_pending(c);
     *out_count = 0;
-    c->pending.active = false;
     YB_ARG(c->metric == YAMS_B200_COSINE, "all-matching selection is defined for the cosine scan");
     // the reference gathers the candidate rowids into a set (:4412-4448): duplicates count once
     std::vector<int64_t> uniq;
@@ -2084,6 +2106,7 @@ yams_status_t yams_b200_semantic_neighbors(yams_b200_corpus* c, const int64_t* s
     YB_ARG(c, "corpus is null");
     std::lock_guard<std::mutex> corpus_lock(c->mu);
     YB_BIND(c);
+    settle_pending(c);
     YB_ARG(c->metric == YAMS_B200_COSINE, "the semantic graph needs a cosine corpus");
     YB_ARG(source_rowids || n_sources == c->n, "without source_rowids, n_sources must equal the corpus size");
     YB_ARG(k <= kMaxK, "k > 3072 is not supported by the fused top-k path");
@@ -2098,7 +2121,6 @@ yams_status_t yams_b200_semantic_neighbors(yams_b200_corpus* c, const int64_t* s
     YB_ARG(out_rowids && out_sims, "null output");
     if (out_flags) for (uint64_t i = 0; i < n_sources; ++i) out_flags[i] = YAMS_B200_FLAG_NOT_A_SOURCE;   // until answered
     for (uint64_t i = 0; i < n_sources * k; ++i) { out_rowids[i] = -1; out_sims[i] = 0.f; }
-    c->pending.active = false;
     yams_status_t rc;
     GraphRows g;
     std::vector<float> h_inv;
@@ -2162,7 +2184,7 @@ yams_status_t yams_b200_debug_semantic_stage1(yams_b200_corpus* c, const int64_t
     YB_ARG(c->metric == YAMS_B200_COSINE && c->n > 0, "needs a non-empty cosine corpus");
     yams_status_t rc;
     YB_BIND(c);
-    c->pending.active = false;
+    settle_pending(c);
     GraphRows g;
     std::vector<float> h_inv;
     std::vector<int64_t> h_rowids;
@@ -2203,7 +2225,8 @@ yams_status_t yams_b200_search_device(yams_b200_corpus* c, const float* d_querie
     YB_ARG(k > 0 && k <= 768, "k must be in 1..768");
     YB_ARG(nq <= 65535, "at most 65535 queries per call (split larger batches)");
     if (nq == 0) return YAMS_OK;
-    c->pending.active = false;
+    // supersedes a pending search without waiting for it (a pipelined caller enqueues its next batch before the last is done)
+    c->pending.active = c->pending.settled = false;
     ScanPlan plan;
     plan.nq = nq; plan.k = k; plan.threshold = threshold;
     plan.out.rowids = d_out_rowids; plan.out.scores = d_out_scores;
@@ -2221,13 +2244,12 @@ yams_status_t yams_b200_search_device_finish(yams_b200_corpus* c, uint32_t* out_
     std::lock_guard<std::mutex> corpus_lock(c->mu);
     YB_BIND(c);
     if (out_resolved) *out_resolved = 0;
-    if (!c->pending.active) return YAMS_OK;
-    YB_CUDA(cudaStreamSynchronize(c->st));
-    c->pending.active = false;
-    uint32_t resolved = 0;
-    yams_status_t rc = finish_search(c, c->pending.plan, nullptr, nullptr, &resolved);
-    if (out_resolved) *out_resolved = resolved;
-    return rc;
+    settle_pending(c);
+    if (!c->pending.settled) return YAMS_OK;
+    c->pending.settled = false;
+    if (out_resolved) *out_resolved = c->pending.resolved;
+    if (c->pending.status != YAMS_OK) set_last_error("%s", c->pending.error.c_str());
+    return c->pending.status;
     YB_CATCH
 }
 
@@ -2287,7 +2309,7 @@ yams_status_t yams_b200_debug_stage1_scores(yams_b200_corpus* c, const float* qu
     YB_ARG(row_start + (nrows - 1) * row_stride < c->n, "rows out of range");
     yams_status_t rc;
     YB_BIND(c);
-    c->pending.active = false;
+    settle_pending(c);
     if ((rc = prepare_queries(c, queries, false, nq)) != YAMS_OK) return rc;
     if ((rc = c->dense.reserve((size_t)nq * nrows * 4)) != YAMS_OK) return rc;
     if ((rc = c->eps.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
@@ -2310,7 +2332,6 @@ yams_status_t yams_b200_debug_stage1_scores(yams_b200_corpus* c, const float* qu
 static yams_status_t debug_filter_setup(yams_b200_corpus* c, const float* queries, uint32_t nq, const float* tau, uint32_t cap,
                                         Stage1Args& a) {
     yams_status_t rc;
-    c->pending.active = false;
     if ((rc = prepare_queries(c, queries, false, nq)) != YAMS_OK) return rc;
     if ((rc = c->eps.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
     if ((rc = c->tau.reserve((size_t)nq * 4)) != YAMS_OK) return rc;
@@ -2336,6 +2357,7 @@ yams_status_t yams_b200_debug_stage1_candidates(yams_b200_corpus* c, const float
     YB_ARG(row_start + (nrows - 1) * row_stride < c->n, "rows out of range");
     yams_status_t rc;
     YB_BIND(c);
+    settle_pending(c);
     Stage1Args a{};
     if ((rc = debug_filter_setup(c, queries, nq, tau, cap, a)) != YAMS_OK) return rc;
     const size_t cb = (size_t)nq * cap * sizeof(Cand);
@@ -2378,6 +2400,7 @@ yams_status_t yams_b200_debug_stage1_profile(yams_b200_corpus* c, const float* q
     YB_ARG(c->n > 0, "empty corpus");
     yams_status_t rc;
     YB_BIND(c);
+    settle_pending(c);
     Stage1Args a{};
     if ((rc = debug_filter_setup(c, queries, nq, tau, cap, a)) != YAMS_OK) return rc;
     const size_t pb = (size_t)c->dev->sm_count * 4 * sizeof(unsigned long long);
@@ -2409,7 +2432,7 @@ yams_status_t yams_b200_debug_select(yams_b200_corpus* c, uint32_t nq, const flo
     YB_ARG(tau_only || K <= SEL_MAXK, "K > 4096");
     std::lock_guard<std::mutex> corpus_lock(c->mu);
     YB_BIND(c);
-    c->pending.active = false;
+    settle_pending(c);
     yams_status_t rc;
     cudaStream_t st = c->st;
     SelectIn in{};
@@ -2465,7 +2488,7 @@ yams_status_t yams_b200_debug_final(yams_b200_corpus* c, uint32_t nq, uint32_t K
     YB_ARG(metric == YAMS_B200_COSINE || metric == YAMS_B200_L2, "unknown metric");
     std::lock_guard<std::mutex> corpus_lock(c->mu);
     YB_BIND(c);
-    c->pending.active = false;
+    settle_pending(c);
     const Exact* ex = static_cast<const Exact*>(exact);
     for (uint32_t b = 0; b < nq; ++b) {   // entries final_kernel reads must index the rowid table
         const uint32_t m = ex_n ? std::min(ex_n[b], Kp) : Kp;

@@ -2,6 +2,7 @@
 #pragma once
 #include <algorithm>
 #include <mutex>
+#include <string>
 
 #include "common.cuh"
 
@@ -89,6 +90,11 @@ struct Corpus {
     struct Pending {
         ScanPlan plan;
         bool active = false;
+        // finished by settle_pending before another call ran on the corpus: what search_device_finish reports
+        bool settled = false;
+        yams_status_t status = YAMS_OK;
+        uint32_t resolved = 0;
+        std::string error;
     } pending;
     cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};
     cudaEvent_t ev_scan[2] = {nullptr, nullptr};  // around the full-corpus filtered scan launch
@@ -143,6 +149,11 @@ struct Stage1Args {
 };
 
 yams_status_t stage1_cuda_core(const Stage1Args& a, bool filter, cudaStream_t st);
+
+// Finishes a pending search_device (knn.cu) on the corpus it was enqueued on and keeps its outcome for search_device_finish.
+// Every entry point on a corpus but search_device calls it first, under the corpus lock: a mutator would otherwise change the
+// rows its exhaustive levels re-score, and any call reuses the workspace its finish reads.
+void settle_pending(Corpus* c);
 
 // Stages of the exact scan that the other engines (pq.cu) launch on their own lists; each is described at its definition in knn.cu
 void launch_topk_lists(const Cand* lists, const uint32_t* counts, uint32_t cap, uint32_t nq, uint32_t K, Cand* out_sel, uint32_t* out_n,

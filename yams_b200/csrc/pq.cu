@@ -1091,6 +1091,7 @@ yams_status_t yams_b200_search_documents(yams_b200_corpus* c, yams_b200_pq* pq, 
     if (pq) pq_lock = std::unique_lock<std::mutex>(pq->mu);
     std::lock_guard<std::mutex> corpus_lock(c->mu);
     YB_BIND(c);
+    settle_pending(c);
     zero_outputs(nq, out_counts, nullptr);
     if (nq == 0) return YAMS_OK;
     YB_ARG(queries && query_docs && out_docs && out_rowids && out_scores, "null argument");
@@ -1113,7 +1114,6 @@ yams_status_t yams_b200_search_documents(yams_b200_corpus* c, yams_b200_pq* pq, 
     YB_ARG(total == 0 || rowids_unique_per_query(doc_rowids, doc_offsets, query_docs, nq),
            "a rowid appears twice among one query's documents (documents are disjoint row sets)");
     if (k == 0) return YAMS_OK;
-    c->pending.active = false;
     // slices of <= kPqMaxBatch queries and a bounded number of (query, row) pairs; one host synchronisation each
     const uint64_t kMaxPairs = 1ull << 26;
     for (uint32_t q0 = 0; q0 < nq;) {
