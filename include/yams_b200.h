@@ -596,8 +596,8 @@ YAMS_B200_API void yams_b200_simeon_destroy(yams_b200_encoder* e);
  *          alpha > 0, and (1 - alpha) * bm25plus over the list of each distinct n-gram of the word still in the index when
  *          alpha < 1.  Every float operation is the reference's, in its order, without fused multiply-adds.
  * Scores are bit-identical to the reference.  The concept blend (ConceptIndex::blend_into) is the concepts block below.  Out of
- * scope (the caller's, as today): fragment geometry, the strategy router, RRF, the BM25F aux field, SDM / word bigrams, PRF, and
- * the caller's document windowing (buildEnhancementText). */
+ * scope (the caller's, as today): fragment geometry, the strategy router, the query router, the BM25F aux field, SDM / word
+ * bigrams, PRF, and the caller's document windowing (buildEnhancementText).  RRF over variants is yams_b200_bm25_score_rrf. */
 #define YAMS_BM25_ATIRE 0                    /* simeon::Bm25Variant::Atire */
 #define YAMS_BM25_SUBWORD_AWARE_BACKOFF 7    /* simeon::Bm25Variant::SubwordAwareBackoff */
 typedef struct yams_bm25_config {
@@ -645,6 +645,14 @@ YAMS_B200_API yams_status_t yams_b200_bm25_doc_lengths(yams_b200_bm25* idx, uint
  * device ms, [7] its host wall ms */
 YAMS_B200_API yams_status_t yams_b200_bm25_last_timings(yams_b200_bm25* idx, float out_ms[8]);
 YAMS_B200_API void yams_b200_bm25_destroy(yams_b200_bm25* idx);
+/* An Atire view of idx -> *out: a handle that answers every yams_b200_bm25_* call and yams_b200_concepts_mine exactly as an
+ * Atire index built from the same texts with idx's k1, b and hash_seed would (SimeonLexicalBackend's second index for RRF, built
+ * with Bm25Config's defaults otherwise).  Such an index's word field and idf table are idx's, whatever idx's variant: n-grams
+ * and their pruning never touch words.  The view reads them in place, with no copy and no build; its n-gram field is empty
+ * (stats: ngram_avg_dl, terms[1], postings[1] and pruned 0; field 1 postings and doc lengths empty and zero).  A view of an
+ * Atire index is equivalent to the index.  The view has its own stream, lock and score workspace, so it may be scored
+ * concurrently with idx, and the two may be destroyed in either order. */
+YAMS_B200_API yams_status_t yams_b200_bm25_atire_view(yams_b200_bm25* idx, yams_b200_bm25** out);
 
 /* ---- Simeon word-bigram concepts (DESIGN.md §4.12) ---------------------------------------------------------------
  * third_party/simeon ConceptIndex (src/concept_mining.cpp) mined against a BM25 index, and its blend into BM25 scores, as the
@@ -707,6 +715,25 @@ YAMS_B200_API yams_status_t yams_b200_concepts_bigram_lengths(yams_b200_concepts
  * not run), [7] its host wall ms */
 YAMS_B200_API yams_status_t yams_b200_concepts_last_timings(yams_b200_concepts* concepts, float out_ms[8]);
 YAMS_B200_API void yams_b200_concepts_destroy(yams_b200_concepts* concepts);
+
+/* ---- reciprocal-rank fusion of BM25 variants (DESIGN.md §4.13) ---------------------------------------------------
+ * score_bm25_variants_rrf(variants, query, scores, k_rrf) of each of nq HOST queries (fusion.cpp), then, with concepts,
+ * ConceptIndex::blend_into(query, scores, weight): SimeonLexicalBackend::score with bm25_variants_rrf on.  Each variant, in the
+ * given order, ranks the documents of finite score > 0 by score descending, then document ascending; rank r (1, 2, ...) adds
+ * 1.0f / (k_rrf + (float)r) to its document, the variants' additions in their order from 0.0f (an unranked document stays 0).
+ * The blend adds onto the fused scores.  Outputs and limits are yams_b200_bm25_score's.  Bit-identical to the reference; ranks
+ * above 2^24, where (float)r rounds, need more than 16.7 M documents and are not tested.
+ *   - The same index may appear more than once (its ranks then count twice).  Every distinct index is locked for the call, in
+ *     an order that cannot deadlock; the work runs on the first variant's stream and workspace, whose last_timings [6] and [7]
+ *     record it.  Queries are batched so that the score rows, ranked keys and the sort's double buffer stay within 1 GiB.
+ *   - YAMS_ERR_INVALID_ARG: a null index, indexes of different document counts, k_rrf not finite or < 0 (the backend passes
+ *     60), k > 4096, nv * n_docs >= 2^32.  YAMS_ERR_UNSUPPORTED: indexes on different devices.
+ *   - nv = 0: nothing is ranked and there is no document count: no score row is written, every count is 0.
+ *   - concepts NULL, empty or of another document count: no blend (as yams_b200_bm25_score_blended). */
+YAMS_B200_API yams_status_t yams_b200_bm25_score_rrf(const yams_b200_bm25* const* variants, uint32_t nv, float k_rrf,
+                                                     const yams_b200_concepts* concepts, float weight, const char* const* queries,
+                                                     const size_t* qlens, uint32_t nq, float* out_scores, uint32_t k,
+                                                     uint32_t* out_docs, float* out_topk_scores, uint32_t* out_counts);
 
 /* [0] stage-1 scan ms, [1] rescoring+select ms, [2] total device ms of the last yams_b200_search or
  * yams_b200_search_device on this corpus (the latter's once its work is done); [3] unused (0);

@@ -183,6 +183,9 @@ SYMBOLS = {
     "yams_b200_concepts_bigram_lengths": (C.c_int, [C.c_void_p, u32p]),
     "yams_b200_concepts_last_timings": (C.c_int, [C.c_void_p, f32p]),
     "yams_b200_concepts_destroy": (None, [C.c_void_p]),
+    "yams_b200_bm25_atire_view": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p)]),
+    "yams_b200_bm25_score_rrf": (C.c_int, [C.POINTER(C.c_void_p), C.c_uint32, C.c_float, C.c_void_p, C.c_float, C.POINTER(C.c_char_p),
+                                           C.POINTER(C.c_size_t), C.c_uint32, f32p, C.c_uint32, u32p, f32p, u32p]),
     "yams_b200_pq_build": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, f32p, u64p, C.POINTER(C.c_void_p)]),
     "yams_b200_pq_search": (C.c_int, [C.c_void_p, f32p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_float, i64p, f32p, u32p, u64p]),
     "yams_b200_pq_search_candidates": (C.c_int, [C.c_void_p, f32p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_float, i64p, u64p, i64p, f32p,
@@ -807,6 +810,24 @@ def _texts(texts):
     return raw, (C.c_char_p * max(n, 1))(*raw), (C.c_size_t * max(n, 1))(*[len(r) for r in raw])
 
 
+def _score_call(call, n, queries, k, full):
+    """the outputs of one score call over `queries`: call(ptrs, lens, nq, scores, k, docs, topk_scores, counts)"""
+    raw, ptrs, lens = _texts(queries)
+    nq = len(raw)
+    out = {}
+    scores = np.zeros((nq, n), np.float32) if full else None
+    docs = np.zeros((nq, max(k, 1)), np.uint32)
+    tops = np.zeros((nq, max(k, 1)), np.float32)
+    counts = np.zeros(max(nq, 1), np.uint32)
+    call(ptrs, lens, nq, scores.ctypes.data_as(f32p) if full else None, k, docs.ctypes.data_as(u32p), tops.ctypes.data_as(f32p),
+         counts.ctypes.data_as(u32p))
+    if full:
+        out["scores"] = scores
+    if k:
+        out.update(docs=docs, topk_scores=tops, counts=counts[:nq])
+    return out
+
+
 class Bm25Index:
     """simeon's Bm25Index built on the device over `texts` (add_doc for each, then finalize), as the lexical backend configures it
     unless overridden: SubwordAwareBackoff, gamma 5.  `variant` is BM25_ATIRE or BM25_SUBWORD_AWARE_BACKOFF."""
@@ -826,24 +847,21 @@ class Bm25Index:
         """Bm25Index::score of every query: {"scores": [nq][n_docs] (full=True)}, and for k > 0 the best k documents of score > 0
         ("docs", "topk_scores" padded with 0xFFFFFFFF / 0, "counts").  With `concepts`, each query's scores are then blended
         with ConceptIndex::blend_into(query, scores, weight) before the top-k, as the lexical backend scores."""
-        raw, ptrs, lens = _texts(queries)
-        nq = len(raw)
-        out = {}
-        scores = np.zeros((nq, self.n), np.float32) if full else None
-        docs = np.zeros((nq, max(k, 1)), np.uint32)
-        tops = np.zeros((nq, max(k, 1)), np.float32)
-        counts = np.zeros(max(nq, 1), np.uint32)
-        args = (ptrs, lens, nq, scores.ctypes.data_as(f32p) if full else None, k, docs.ctypes.data_as(u32p), tops.ctypes.data_as(f32p),
-                counts.ctypes.data_as(u32p))
         if concepts is None:
-            _check(lib().yams_b200_bm25_score(self._h, *args), "bm25_score")
-        else:
-            _check(lib().yams_b200_bm25_score_blended(self._h, concepts._h, weight, *args), "bm25_score_blended")
-        if full:
-            out["scores"] = scores
-        if k:
-            out.update(docs=docs, topk_scores=tops, counts=counts[:nq])
-        return out
+            return _score_call(lambda *args: _check(lib().yams_b200_bm25_score(self._h, *args), "bm25_score"), self.n, queries, k, full)
+        return _score_call(lambda *args: _check(lib().yams_b200_bm25_score_blended(self._h, concepts._h, weight, *args), "bm25_score_blended"),
+                           self.n, queries, k, full)
+
+    def atire_view(self) -> "Bm25Index":
+        """The Atire index of the same texts with this index's k1, b and hash seed, served from this index's word field in place
+        (yams_b200_bm25_atire_view): no copy, no build.  Either may be closed first."""
+        v = object.__new__(Bm25Index)
+        v.cfg = Bm25Config.from_buffer_copy(self.cfg)
+        v.cfg.variant = BM25_ATIRE
+        v.n = self.n
+        v._h = C.c_void_p()
+        _check(lib().yams_b200_bm25_atire_view(self._h, C.byref(v._h)), "bm25_atire_view")
+        return v
 
     def mine_concepts(self, texts, **overrides) -> "ConceptIndex":
         """mine_concepts(this index, texts, ConceptConfig) on the device; overrides: min_ttf, pmi_floor, max_concepts, k1, b."""
@@ -1174,3 +1192,15 @@ class ConceptIndex:
             self.close()
         except Exception:
             pass
+
+
+def bm25_score_rrf(indexes, queries, k: int = 0, full: bool = True, k_rrf: float = 60.0, concepts: Optional[ConceptIndex] = None,
+                   weight: float = 0.5):
+    """score_bm25_variants_rrf(indexes, query, scores, k_rrf) of every query, then with `concepts` ConceptIndex::blend_into(query,
+    scores, weight): the lexical backend's score with bm25_variants_rrf on (yams_b200_bm25_score_rrf).  The outputs of
+    Bm25Index.score; the score rows have the indexes' document count (0 without indexes)."""
+    nv = len(indexes)
+    hs = (C.c_void_p * max(nv, 1))(*[i._h for i in indexes])
+    n = indexes[0].n if nv else 0
+    return _score_call(lambda *args: _check(lib().yams_b200_bm25_score_rrf(hs, nv, k_rrf, concepts._h if concepts is not None else None,
+                                                                            weight, *args), "bm25_score_rrf"), n, queries, k, full)

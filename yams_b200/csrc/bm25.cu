@@ -23,8 +23,13 @@
 // part of the posting list inside the tile by binary search and adds each document's contribution -- a document appears once
 // per leg, so no atomics, and each document receives its additions in the reference's order.  Every float operation is an
 // explicit _rn intrinsic: the reference is compiled without -mfma, so nothing may be fused.
+//
+// RRF (score_bm25_variants_rrf, fusion.cpp; DESIGN.md §4.13): the variants' score rows, their ranked entries as sortable keys,
+// one segmented sort per batch, one scatter of 1 / (k + r) per variant in order.  An Atire view shares its parent's word field
+// and idf table, which an Atire build of the same texts would reproduce exactly.
 #include <cub/cub.cuh>
 #include <thrust/iterator/counting_iterator.h>
+#include <thrust/iterator/transform_iterator.h>
 
 #include <algorithm>
 #include <chrono>
@@ -369,11 +374,15 @@ struct yams_b200_bm25 {
     DeviceCtx* dev = nullptr;
     yams_bm25_config cfg{};
     uint64_t n = 0, total_tokens = 0, pruned = 0;
-    Bm25Field f[2];
-    DevBuf idf;                   // n + 1 floats: idf of df = 0..n
+    // The fields and the idf table are shared with the index's Atire views (yams_b200_bm25_atire_view), which read the word
+    // field and the table in place; whichever handle goes last frees them.  Nothing writes them after the build.
+    std::shared_ptr<Bm25Field> f[2] = {std::make_shared<Bm25Field>(), std::make_shared<Bm25Field>()};
+    std::shared_ptr<DevBuf> idf = std::make_shared<DevBuf>();   // n + 1 floats: idf of df = 0..n
     cudaStream_t st = nullptr;
     cudaEvent_t ev[2] = {nullptr, nullptr};
     DevBuf raw, legs, qoff, dense, sel, seln;   // score workspace
+    DevBuf fused, keys, keys2, cnt, base;       // RRF workspace (the call runs on its first variant's)
+    CubTmp tmp;
     float ms[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     std::mutex mu;
     ~yams_b200_bm25() {
@@ -542,7 +551,8 @@ static yams_status_t bm25_build(yams_b200_bm25* x, const char* const* texts, con
     yams_status_t rc;
     std::vector<uint64_t> pos;
     DevBuf text, d_pos;
-    for (Bm25Field& F : x->f) {
+    for (auto& pf : x->f) {
+        Bm25Field& F = *pf;
         if ((rc = F.dl.reserve(std::max<uint64_t>(n, 1) * 4)) != YAMS_OK) return rc;
         YB_CUDA(cudaMemsetAsync(F.dl.p, 0, std::max<uint64_t>(n, 1) * 4, st));
         F.h_dl.assign(n, 0);
@@ -553,17 +563,17 @@ static yams_status_t bm25_build(yams_b200_bm25* x, const char* const* texts, con
     // ---- dl / ngram_dl ----
     rc = timed(x, &x->ms[1], [&]() -> yams_status_t {
         if (L) bm_doc_counts_kernel<<<bm_grid(L), BM_THREADS, 0, st>>>(text.as<uint8_t>(), L, d_pos.as<uint64_t>(), n, sab, kmin, kmax,
-                                                                       x->f[0].dl.as<uint32_t>(), x->f[1].dl.as<uint32_t>());
+                                                                       x->f[0]->dl.as<uint32_t>(), x->f[1]->dl.as<uint32_t>());
         YB_CUDA(cudaGetLastError());
-        for (Bm25Field& F : x->f)
-            if (n) YB_CUDA(cudaMemcpyAsync(F.h_dl.data(), F.dl.p, n * 4, cudaMemcpyDeviceToHost, st));
+        for (auto& pf : x->f)
+            if (n) YB_CUDA(cudaMemcpyAsync(pf->h_dl.data(), pf->dl.p, n * 4, cudaMemcpyDeviceToHost, st));
         return YAMS_OK;
     });
     if (rc != YAMS_OK) return rc;
     uint64_t sums[2] = {0, 0};
     for (int fi = 0; fi < 2; ++fi) {
-        for (uint32_t v : x->f[fi].h_dl) sums[fi] += v;
-        x->f[fi].avg = n == 0 ? 0.0f : (float)((double)sums[fi] / (double)n);   // finalize_word_field (bm25.cpp:668-676)
+        for (uint32_t v : x->f[fi]->h_dl) sums[fi] += v;
+        x->f[fi]->avg = n == 0 ? 0.0f : (float)((double)sums[fi] / (double)n);   // finalize_word_field (bm25.cpp:668-676)
     }
     x->total_tokens = sums[0];
     // ---- document slices: pairs of one slice (words + n-grams) within what the device can hold ----
@@ -579,7 +589,7 @@ static yams_status_t bm25_build(yams_b200_bm25* x, const char* const* texts, con
     std::vector<uint64_t> cuts{0};
     uint64_t acc = 0;
     for (uint64_t d = 0; d < n; ++d) {
-        const uint64_t c = (uint64_t)x->f[0].h_dl[d] + (sab ? (uint64_t)x->f[1].h_dl[d] : 0);
+        const uint64_t c = (uint64_t)x->f[0]->h_dl[d] + (sab ? (uint64_t)x->f[1]->h_dl[d] : 0);
         if (acc && acc + c > budget) { cuts.push_back(d); acc = 0; }
         acc += c;
     }
@@ -645,7 +655,7 @@ static yams_status_t bm25_build(yams_b200_bm25* x, const char* const* texts, con
     text = DevBuf();
     for (int fi = 0; fi < (sab ? 2 : 1); ++fi) {
         rc = timed(x, &x->ms[3], [&] {
-            return finish_field(x, x->f[fi], ph[fi], pv[fi], np[fi], nslices > 1, fi == 1 && x->cfg.ngram_df_prune_ratio > 0.0f && n > 0, tmp);
+            return finish_field(x, *x->f[fi], ph[fi], pv[fi], np[fi], nslices > 1, fi == 1 && x->cfg.ngram_df_prune_ratio > 0.0f && n > 0, tmp);
         });
         if (rc != YAMS_OK) return rc;
     }
@@ -656,8 +666,8 @@ static yams_status_t bm25_build(yams_b200_bm25* x, const char* const* texts, con
         const float d = (float)df;
         idf[df] = std::log((nf - d + 0.5f) / (d + 0.5f) + 1.0f);
     }
-    if ((rc = x->idf.reserve((n + 1) * 4)) != YAMS_OK) return rc;
-    YB_CUDA(cudaMemcpyAsync(x->idf.p, idf.data(), (n + 1) * 4, cudaMemcpyHostToDevice, st));
+    if ((rc = x->idf->reserve((n + 1) * 4)) != YAMS_OK) return rc;
+    YB_CUDA(cudaMemcpyAsync(x->idf->p, idf.data(), (n + 1) * 4, cudaMemcpyHostToDevice, st));
     YB_CUDA(cudaStreamSynchronize(st));
     x->ms[4] = (float)(wall_ms() - t0);
     x->ms[5] = (float)nslices;
@@ -712,29 +722,20 @@ static ConceptDict concept_dict(const yams_b200_concepts* c, float weight) {
     return ConceptDict{Dict{c->hashes.as<uint64_t>(), c->offs.as<uint64_t>(), c->size}, c->pmi.as<float>(), c->idf.as<float>(), weight};
 }
 
-// Bm25Index::score of every query; with a concept index `c` of the same document count, then ConceptIndex::blend_into(query,
-// scores, weight) of each (SimeonLexicalBackend::score).
-static yams_status_t bm25_score(yams_b200_bm25* x, const yams_b200_concepts* c, float weight, const char* const* queries,
-                                const size_t* qlens, uint32_t nq, float* out_scores, uint32_t k, uint32_t* out_docs, float* out_topk,
-                                uint32_t* out_counts) {
-    const double t0 = wall_ms();
-    cudaStream_t st = x->st;
-    const uint64_t n = x->n;
-    const bool sab = x->cfg.variant == YAMS_BM25_SUBWORD_AWARE_BACKOFF;
-    const uint64_t h0 = gram_hash_h0(x->cfg.hash_seed);
-    yams_status_t rc;
-    // ---- host: the legs of every query, in the reference's order ----
-    std::vector<RawLeg> raw;
-    std::vector<uint64_t> qoff(nq + 1, 0);
+// The legs of queries [0, nq), in the reference's order, appended to raw: the BM25 legs of index x (nullable: none), then, with a
+// concept index c, the concepts each query matches in blend_into's order.  qoff[q] .. qoff[q + 1] are query q's (absolute).
+static void query_legs(const yams_b200_bm25* x, const yams_b200_concepts* c, const char* const* queries, const size_t* qlens,
+                       uint32_t nq, std::vector<RawLeg>& raw, uint64_t* qoff) {
+    const bool sab = x && x->cfg.variant == YAMS_BM25_SUBWORD_AWARE_BACKOFF;
+    const uint64_t h0 = x ? gram_hash_h0(x->cfg.hash_seed) : 0;
     std::vector<std::pair<size_t, size_t>> ws;
     std::vector<uint8_t> low;
     std::unordered_set<uint64_t> seen;
-    // the blend is a no-op when the concept index is empty or of another document count (blend_into's size test)
-    const bool blend = c && c->size && c->n == n;
     std::vector<uint64_t> corder;
+    qoff[0] = raw.size();
     for (uint32_t q = 0; q < nq; ++q) {
         const uint8_t* p = reinterpret_cast<const uint8_t*>(queries[q]);
-        query_words(p, qlens[q], ws);
+        if (x) query_words(p, qlens[q], ws); else ws.clear();
         for (const auto& [s, l] : ws) {
             low.resize(l);
             for (size_t i = 0; i < l; ++i) low[i] = ascii_lower(p[s + i]);
@@ -749,12 +750,99 @@ static yams_status_t bm25_score(yams_b200_bm25* x, const yams_b200_concepts* c, 
                     if (seen.insert(gh).second) raw.push_back({gh, th, 1, 0});
                 }
         }
-        if (blend) {
+        if (c) {
             concept_order(c, p, qlens[q], ws, corder);
             for (uint64_t bh : corder) raw.push_back({bh, bh, BM_CONCEPT, 0});
         }
         qoff[q + 1] = raw.size();
     }
+}
+
+// the plan kernel over raw legs [0, nlegs) of index x (nullable: concept legs only) and concept index c (nullable)
+static yams_status_t plan_legs(const yams_b200_bm25* x, const yams_b200_concepts* c, float weight, const RawLeg* raw, uint64_t nlegs,
+                               Leg* legs, cudaStream_t st) {
+    if (nlegs == 0) return YAMS_OK;
+    const Dict w = x ? Dict{x->f[0]->hashes.as<uint64_t>(), x->f[0]->offs.as<uint64_t>(), x->f[0]->terms} : Dict{};
+    const Dict g = x ? Dict{x->f[1]->hashes.as<uint64_t>(), x->f[1]->offs.as<uint64_t>(), x->f[1]->terms} : Dict{};
+    const ConceptDict cd = c ? concept_dict(c, weight) : ConceptDict{};
+    bm_plan_kernel<<<bm_grid(nlegs), BM_THREADS, 0, st>>>(raw, nlegs, w, g, x ? x->idf->as<float>() : nullptr,
+                                                          x && x->cfg.variant == YAMS_BM25_SUBWORD_AWARE_BACKOFF,
+                                                          x ? x->cfg.subword_gamma : 0.0f, cd, legs);
+    YB_CUDA(cudaGetLastError());
+    return YAMS_OK;
+}
+
+// the score kernel's arguments of index x's two fields
+static ScoreArgs bm25_args(const yams_b200_bm25* x) {
+    ScoreArgs a{};
+    for (int fi = 0; fi < 2; ++fi) {
+        a.docs[fi] = x->f[fi]->docs.as<uint32_t>();
+        a.tfs[fi] = x->f[fi]->tfs.as<uint32_t>();
+        a.dl[fi] = x->f[fi]->dl.as<uint32_t>();
+        a.avg[fi] = x->f[fi]->avg > 0.0f ? x->f[fi]->avg : 1.0f;
+        a.k1[fi] = x->cfg.k1;
+        a.b[fi] = x->cfg.b;
+    }
+    a.n = x->n;
+    a.delta = x->cfg.delta;
+    a.sab = x->cfg.variant == YAMS_BM25_SUBWORD_AWARE_BACKOFF;
+    return a;
+}
+
+// The outputs of one batch: queries q0 .. q0 + qb, whose score rows are rows[qb][n] on x's stream -- the full vectors, and the
+// best K (k <= 4096 asked) of score > 0 through x's selection workspace.  Returns with the rows free for the next batch.
+static yams_status_t emit_batch(yams_b200_bm25* x, const float* rows, uint64_t n, uint32_t q0, uint32_t qb, uint32_t nq, uint32_t K,
+                                uint32_t k, float* out_scores, uint32_t* out_docs, float* out_topk, uint32_t* out_counts,
+                                std::vector<Cand>& h_sel, std::vector<uint32_t>& h_n) {
+    cudaStream_t st = x->st;
+    if (out_scores) YB_CUDA(cudaMemcpyAsync(out_scores + (uint64_t)q0 * n, rows, (uint64_t)qb * n * 4, cudaMemcpyDeviceToHost, st));
+    if (K) {
+        launch_topk_dense(rows, n, qb, K, x->sel.as<Cand>(), x->seln.as<uint32_t>(), st);
+        YB_CUDA(cudaGetLastError());
+        h_sel.resize((uint64_t)qb * K);
+        h_n.resize(qb);
+        YB_CUDA(cudaMemcpyAsync(h_sel.data(), x->sel.p, (uint64_t)qb * K * sizeof(Cand), cudaMemcpyDeviceToHost, st));
+        YB_CUDA(cudaMemcpyAsync(h_n.data(), x->seln.p, (uint64_t)qb * 4, cudaMemcpyDeviceToHost, st));
+        YB_CUDA(cudaStreamSynchronize(st));
+        // best first: the documents of score > 0 lead the selection
+        for (uint32_t j = 0; j < qb; ++j) {
+            uint32_t c = 0;
+            const uint32_t m = std::min(h_n[j], K);
+            while (c < m && h_sel[(uint64_t)j * K + c].score > 0.0f) {
+                out_docs[(uint64_t)(q0 + j) * k + c] = h_sel[(uint64_t)j * K + c].row;
+                out_topk[(uint64_t)(q0 + j) * k + c] = h_sel[(uint64_t)j * K + c].score;
+                ++c;
+            }
+            out_counts[q0 + j] = c;
+        }
+    } else if (q0 + qb < nq) {
+        YB_CUDA(cudaStreamSynchronize(st));   // the next batch overwrites the score rows
+    }
+    return YAMS_OK;
+}
+
+// the top-k outputs before any batch: padding, counts 0
+static void clear_topk(uint32_t nq, uint32_t k, uint32_t* out_docs, float* out_topk, uint32_t* out_counts) {
+    if (!k) return;
+    for (uint64_t i = 0; i < (uint64_t)nq * k; ++i) { out_docs[i] = 0xFFFFFFFFu; out_topk[i] = 0.0f; }
+    for (uint32_t q = 0; q < nq; ++q) out_counts[q] = 0;
+}
+
+// Bm25Index::score of every query; with a concept index `c` of the same document count, then ConceptIndex::blend_into(query,
+// scores, weight) of each (SimeonLexicalBackend::score).
+static yams_status_t bm25_score(yams_b200_bm25* x, const yams_b200_concepts* c, float weight, const char* const* queries,
+                                const size_t* qlens, uint32_t nq, float* out_scores, uint32_t k, uint32_t* out_docs, float* out_topk,
+                                uint32_t* out_counts) {
+    const double t0 = wall_ms();
+    cudaStream_t st = x->st;
+    const uint64_t n = x->n;
+    yams_status_t rc;
+    // ---- host: the legs of every query, in the reference's order ----
+    // the blend is a no-op when the concept index is empty or of another document count (blend_into's size test)
+    const bool blend = c && c->size && c->n == n;
+    std::vector<RawLeg> raw;
+    std::vector<uint64_t> qoff(nq + 1, 0);
+    query_legs(x, blend ? c : nullptr, queries, qlens, nq, raw, qoff.data());
     const uint64_t nlegs = raw.size();
     const uint32_t K = std::min<uint64_t>(k, n);
     if ((rc = x->raw.reserve(std::max<uint64_t>(nlegs, 1) * sizeof(RawLeg))) != YAMS_OK) return rc;
@@ -764,10 +852,7 @@ static yams_status_t bm25_score(yams_b200_bm25* x, const yams_b200_concepts* c, 
     if (n && (rc = x->dense.reserve(qb_max * n * 4)) != YAMS_OK) return rc;
     if (K && (rc = x->sel.reserve(qb_max * K * sizeof(Cand))) != YAMS_OK) return rc;
     if (K && (rc = x->seln.reserve(qb_max * 4)) != YAMS_OK) return rc;
-    if (k) {
-        for (uint64_t i = 0; i < (uint64_t)nq * k; ++i) { out_docs[i] = 0xFFFFFFFFu; out_topk[i] = 0.0f; }
-        for (uint32_t q = 0; q < nq; ++q) out_counts[q] = 0;
-    }
+    clear_topk(nq, k, out_docs, out_topk, out_counts);
     if (n == 0) {
         x->ms[6] = 0.f;
         x->ms[7] = (float)(wall_ms() - t0);
@@ -777,31 +862,16 @@ static yams_status_t bm25_score(yams_b200_bm25* x, const yams_b200_concepts* c, 
     std::vector<Cand> h_sel;
     std::vector<uint32_t> h_n;
     rc = timed(x, &dev_ms, [&]() -> yams_status_t {
+        yams_status_t r;
         if (nlegs) {
             YB_CUDA(cudaMemcpyAsync(x->raw.p, raw.data(), nlegs * sizeof(RawLeg), cudaMemcpyHostToDevice, st));
-            Dict w{x->f[0].hashes.as<uint64_t>(), x->f[0].offs.as<uint64_t>(), x->f[0].terms};
-            Dict g{x->f[1].hashes.as<uint64_t>(), x->f[1].offs.as<uint64_t>(), x->f[1].terms};
-            const ConceptDict cd = blend ? concept_dict(c, weight) : ConceptDict{};
-            bm_plan_kernel<<<bm_grid(nlegs), BM_THREADS, 0, st>>>(x->raw.as<RawLeg>(), nlegs, w, g, x->idf.as<float>(), sab,
-                                                                  x->cfg.subword_gamma, cd, x->legs.as<Leg>());
-            YB_CUDA(cudaGetLastError());
+            if ((r = plan_legs(x, blend ? c : nullptr, weight, x->raw.as<RawLeg>(), nlegs, x->legs.as<Leg>(), st)) != YAMS_OK) return r;
         }
         YB_CUDA(cudaMemcpyAsync(x->qoff.p, qoff.data(), (nq + 1) * 8, cudaMemcpyHostToDevice, st));
-        ScoreArgs a{};
+        ScoreArgs a = bm25_args(x);
         a.legs = x->legs.as<Leg>();
         a.qoff = x->qoff.as<uint64_t>();
-        for (int fi = 0; fi < 2; ++fi) {
-            a.docs[fi] = x->f[fi].docs.as<uint32_t>();
-            a.tfs[fi] = x->f[fi].tfs.as<uint32_t>();
-            a.dl[fi] = x->f[fi].dl.as<uint32_t>();
-            a.avg[fi] = x->f[fi].avg > 0.0f ? x->f[fi].avg : 1.0f;
-            a.k1[fi] = x->cfg.k1;
-            a.b[fi] = x->cfg.b;
-        }
         if (blend) concept_field(c, a);
-        a.n = n;
-        a.delta = x->cfg.delta;
-        a.sab = sab;
         a.out = x->dense.as<float>();
         const unsigned tiles = (unsigned)((n + BM_TILE - 1) / BM_TILE);
         for (uint32_t q0 = 0; q0 < nq; q0 += (uint32_t)qb_max) {
@@ -809,30 +879,193 @@ static yams_status_t bm25_score(yams_b200_bm25* x, const yams_b200_concepts* c, 
             a.q0 = q0;
             bm_score_kernel<<<dim3(tiles, qb), BM_THREADS, 0, st>>>(a);
             YB_CUDA(cudaGetLastError());
-            if (out_scores)
-                YB_CUDA(cudaMemcpyAsync(out_scores + (uint64_t)q0 * n, x->dense.p, (uint64_t)qb * n * 4, cudaMemcpyDeviceToHost, st));
-            if (K) {
-                launch_topk_dense(x->dense.as<float>(), n, qb, K, x->sel.as<Cand>(), x->seln.as<uint32_t>(), st);
-                YB_CUDA(cudaGetLastError());
-                h_sel.resize((uint64_t)qb * K);
-                h_n.resize(qb);
-                YB_CUDA(cudaMemcpyAsync(h_sel.data(), x->sel.p, (uint64_t)qb * K * sizeof(Cand), cudaMemcpyDeviceToHost, st));
-                YB_CUDA(cudaMemcpyAsync(h_n.data(), x->seln.p, (uint64_t)qb * 4, cudaMemcpyDeviceToHost, st));
-                YB_CUDA(cudaStreamSynchronize(st));
-                // best first: the documents of score > 0 lead the selection
-                for (uint32_t j = 0; j < qb; ++j) {
-                    uint32_t c = 0;
-                    const uint32_t m = std::min(h_n[j], K);
-                    while (c < m && h_sel[(uint64_t)j * K + c].score > 0.0f) {
-                        out_docs[(uint64_t)(q0 + j) * k + c] = h_sel[(uint64_t)j * K + c].row;
-                        out_topk[(uint64_t)(q0 + j) * k + c] = h_sel[(uint64_t)j * K + c].score;
-                        ++c;
-                    }
-                    out_counts[q0 + j] = c;
-                }
-            } else if (q0 + qb < nq) {
-                YB_CUDA(cudaStreamSynchronize(st));   // the next batch overwrites the score rows
+            if ((r = emit_batch(x, x->dense.as<float>(), n, q0, qb, nq, K, k, out_scores, out_docs, out_topk, out_counts, h_sel, h_n)) != YAMS_OK)
+                return r;
+        }
+        return YAMS_OK;
+    });
+    if (rc != YAMS_OK) return rc;
+    x->ms[6] = dev_ms;
+    x->ms[7] = (float)(wall_ms() - t0);
+    return YAMS_OK;
+}
+
+// ---- reciprocal-rank fusion of BM25 variants (score_bm25_variants_rrf, fusion.cpp:24-63) ----
+// A ranked entry: the key (~score_bits << 32) | document sorts ascending as the reference's ranking (score descending, then
+// document ascending, fusion.cpp:14-20); only positive finite scores are ranked, whose bits order as their values.
+__device__ __forceinline__ bool rrf_ranked(float s) { return __float_as_uint(s) - 1u < 0x7F7FFFFFu; }
+
+// ranked entries of each (row, tile of BM_TILE documents); block b = row * tiles + tile
+__global__ void __launch_bounds__(BM_THREADS) rrf_count_kernel(const float* __restrict__ rows, uint64_t n, uint32_t tiles,
+                                                               uint32_t* __restrict__ cnt) {
+    const uint64_t row = blockIdx.x / tiles, lo = (uint64_t)(blockIdx.x % tiles) * BM_TILE;
+    const uint32_t len = (uint32_t)min((uint64_t)BM_TILE, n - lo);
+    const float* s = rows + row * n + lo;
+    uint32_t c = 0;
+    for (uint32_t i0 = 0; i0 < len; i0 += BM_THREADS)
+        c += __syncthreads_count(i0 + threadIdx.x < len && rrf_ranked(s[i0 + threadIdx.x]));
+    if (threadIdx.x == 0) cnt[blockIdx.x] = c;
+}
+
+// the ranked entries' keys, each (row, tile) at its exclusive-scan base, in document order
+__global__ void __launch_bounds__(BM_THREADS) rrf_keys_kernel(const float* __restrict__ rows, uint64_t n, uint32_t tiles,
+                                                              const uint32_t* __restrict__ base, uint64_t* __restrict__ keys) {
+    using Scan = cub::BlockScan<uint32_t, BM_THREADS>;
+    __shared__ typename Scan::TempStorage ts;
+    const uint64_t row = blockIdx.x / tiles, lo = (uint64_t)(blockIdx.x % tiles) * BM_TILE;
+    const uint32_t len = (uint32_t)min((uint64_t)BM_TILE, n - lo);
+    const float* s = rows + row * n + lo;
+    uint32_t at = base[blockIdx.x];
+    for (uint32_t i0 = 0; i0 < len; i0 += BM_THREADS) {
+        const uint32_t i = i0 + threadIdx.x;
+        const float v = i < len ? s[i] : 0.0f;
+        const uint32_t f = rrf_ranked(v) ? 1u : 0u;
+        uint32_t pre, total;
+        Scan(ts).ExclusiveSum(f, pre, total);
+        if (f) keys[at + pre] = ((uint64_t)~__float_as_uint(v) << 32) | (uint32_t)(lo + i);
+        at += total;
+        __syncthreads();   // ts is reused
+    }
+}
+
+// segment r (a (variant, query) row) of the sorted keys: [base[r * tiles], base[(r + 1) * tiles])
+struct RowStart {
+    const uint32_t* base;
+    uint32_t tiles;
+    __host__ __device__ uint32_t operator()(uint64_t r) const { return base[r * tiles]; }
+};
+
+// one variant's contributions, in rank order r = 1, 2, ...: fused[q][doc] += 1.0f / (k + float(r)) (fusion.cpp:31-33), each
+// operation rounded once.  A document appears once per segment and one launch serves one variant, so the additions of a
+// document follow the variant order with no atomics.
+__global__ void rrf_scatter_kernel(const uint64_t* __restrict__ keys, const uint32_t* __restrict__ base, uint32_t tiles, uint64_t row0,
+                                   float k_rrf, uint64_t n, float* __restrict__ fused) {
+    const uint64_t r = row0 + blockIdx.y;
+    const uint32_t b = base[r * tiles], e = base[(r + 1) * tiles];
+    float* out = fused + (uint64_t)blockIdx.y * n;
+    for (uint32_t i = b + blockIdx.x * blockDim.x + threadIdx.x; i < e; i += gridDim.x * blockDim.x) {
+        const uint32_t d = (uint32_t)keys[i];
+        out[d] = __fadd_rn(out[d], __fdiv_rn(1.0f, __fadd_rn(k_rrf, __ull2float_rn((uint64_t)(i - b) + 1))));
+    }
+}
+
+// score_bm25_variants_rrf(v[0..nv), query, out, k_rrf) of every query, then, with a concept index c of the same document count,
+// ConceptIndex::blend_into(query, out, weight) (SimeonLexicalBackend::score with bm25_variants_rrf), on v[0]'s stream and
+// workspace.  Per batch of queries: every variant's score rows, their ranked keys, one segmented sort of the (variant, query)
+// segments, one scatter per variant in order onto zeroed fused rows, the blend's concept legs, the outputs.
+static yams_status_t bm25_score_rrf(const yams_b200_bm25* const* v, uint32_t nv, float k_rrf, const yams_b200_concepts* c, float weight,
+                                    const char* const* queries, const size_t* qlens, uint32_t nq, float* out_scores, uint32_t k,
+                                    uint32_t* out_docs, float* out_topk, uint32_t* out_counts) {
+    const double t0 = wall_ms();
+    yams_b200_bm25* x = const_cast<yams_b200_bm25*>(v[0]);
+    cudaStream_t st = x->st;
+    const uint64_t n = x->n;
+    yams_status_t rc;
+    const bool blend = c && c->size && c->n == n;
+    // ---- host: each variant's legs, then the concepts' (offsets: nv + 1 blocks of nq + 1) ----
+    std::vector<RawLeg> raw;
+    std::vector<uint64_t> qoff((uint64_t)(nv + 1) * (nq + 1), 0);
+    for (uint32_t j = 0; j < nv; ++j) query_legs(v[j], nullptr, queries, qlens, nq, raw, qoff.data() + (uint64_t)j * (nq + 1));
+    if (blend) query_legs(nullptr, c, queries, qlens, nq, raw, qoff.data() + (uint64_t)nv * (nq + 1));
+    const uint64_t nlegs = raw.size();
+    const uint32_t K = std::min<uint64_t>(k, n);
+    const uint64_t tiles = (n + BM_TILE - 1) / BM_TILE;
+    // per query: nv score rows (4 bytes a document), at most n keys per row twice (the sort's double buffer), one fused row
+    const uint64_t per_q = n * (20ull * nv + 4);
+    const uint64_t qb_max = n ? std::max<uint64_t>(1, std::min<uint64_t>({BM_DENSE_BYTES / per_q, (uint64_t)nq, 4096})) : 0;
+    if ((rc = x->raw.reserve(std::max<uint64_t>(nlegs, 1) * sizeof(RawLeg))) != YAMS_OK) return rc;
+    if ((rc = x->legs.reserve(std::max<uint64_t>(nlegs, 1) * sizeof(Leg))) != YAMS_OK) return rc;
+    if ((rc = x->qoff.reserve(qoff.size() * 8)) != YAMS_OK) return rc;
+    if (n) {
+        if ((rc = x->dense.reserve(qb_max * nv * n * 4)) != YAMS_OK || (rc = x->fused.reserve(qb_max * n * 4)) != YAMS_OK ||
+            (rc = x->keys.reserve(qb_max * nv * n * 8)) != YAMS_OK || (rc = x->keys2.reserve(qb_max * nv * n * 8)) != YAMS_OK ||
+            (rc = x->cnt.reserve((qb_max * nv * tiles + 1) * 4)) != YAMS_OK || (rc = x->base.reserve((qb_max * nv * tiles + 1) * 4)) != YAMS_OK)
+            return rc;
+    }
+    if (K && (rc = x->sel.reserve(qb_max * K * sizeof(Cand))) != YAMS_OK) return rc;
+    if (K && (rc = x->seln.reserve(qb_max * 4)) != YAMS_OK) return rc;
+    clear_topk(nq, k, out_docs, out_topk, out_counts);
+    if (n == 0) {
+        x->ms[6] = 0.f;
+        x->ms[7] = (float)(wall_ms() - t0);
+        return YAMS_OK;
+    }
+    float dev_ms = 0.f;
+    std::vector<Cand> h_sel;
+    std::vector<uint32_t> h_n;
+    rc = timed(x, &dev_ms, [&]() -> yams_status_t {
+        yams_status_t r;
+        if (nlegs) {
+            YB_CUDA(cudaMemcpyAsync(x->raw.p, raw.data(), nlegs * sizeof(RawLeg), cudaMemcpyHostToDevice, st));
+            for (uint32_t j = 0; j <= nv; ++j) {
+                if (j == nv && !blend) break;
+                const uint64_t lb = qoff[(uint64_t)j * (nq + 1)], le = qoff[(uint64_t)j * (nq + 1) + nq];
+                if ((r = plan_legs(j < nv ? v[j] : nullptr, j < nv ? nullptr : c, weight, x->raw.as<RawLeg>() + lb, le - lb,
+                                   x->legs.as<Leg>() + lb, st)) != YAMS_OK)
+                    return r;
             }
+        }
+        YB_CUDA(cudaMemcpyAsync(x->qoff.p, qoff.data(), qoff.size() * 8, cudaMemcpyHostToDevice, st));
+        for (uint32_t q0 = 0; q0 < nq; q0 += (uint32_t)qb_max) {
+            const uint32_t qb = (uint32_t)std::min<uint64_t>(qb_max, nq - q0);
+            const uint64_t rows = (uint64_t)nv * qb, blocks = rows * tiles;
+            // every variant's rows: variant j's queries at rows j * qb ..
+            for (uint32_t j = 0; j < nv; ++j) {
+                ScoreArgs a = bm25_args(v[j]);
+                a.legs = x->legs.as<Leg>();
+                a.qoff = x->qoff.as<uint64_t>() + (uint64_t)j * (nq + 1);
+                a.q0 = q0;
+                a.out = x->dense.as<float>() + (uint64_t)j * qb * n;
+                bm_score_kernel<<<dim3((unsigned)tiles, qb), BM_THREADS, 0, st>>>(a);
+                YB_CUDA(cudaGetLastError());
+            }
+            // the ranked keys of each row, the rows' segments, one segmented sort
+            rrf_count_kernel<<<(unsigned)blocks, BM_THREADS, 0, st>>>(x->dense.as<float>(), n, (uint32_t)tiles, x->cnt.as<uint32_t>());
+            YB_CUDA(cudaGetLastError());
+            YB_CUDA(cudaMemsetAsync(x->cnt.as<uint32_t>() + blocks, 0, 4, st));
+            x->tmp.bytes = 0;
+            YB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, x->tmp.bytes, x->cnt.as<uint32_t>(), x->base.as<uint32_t>(), (int64_t)blocks + 1, st));
+            if ((r = x->tmp.grow()) != YAMS_OK) return r;
+            YB_CUDA(cub::DeviceScan::ExclusiveSum(x->tmp.buf.p, x->tmp.bytes, x->cnt.as<uint32_t>(), x->base.as<uint32_t>(), (int64_t)blocks + 1, st));
+            uint32_t items = 0;
+            YB_CUDA(cudaMemcpyAsync(&items, x->base.as<uint32_t>() + blocks, 4, cudaMemcpyDeviceToHost, st));
+            rrf_keys_kernel<<<(unsigned)blocks, BM_THREADS, 0, st>>>(x->dense.as<float>(), n, (uint32_t)tiles, x->base.as<uint32_t>(),
+                                                                     x->keys.as<uint64_t>());
+            YB_CUDA(cudaGetLastError());
+            YB_CUDA(cudaStreamSynchronize(st));   // items
+            const uint64_t* sorted = x->keys.as<uint64_t>();
+            if (items) {
+                cub::DoubleBuffer<uint64_t> db(x->keys.as<uint64_t>(), x->keys2.as<uint64_t>());
+                const auto begins = thrust::make_transform_iterator(thrust::counting_iterator<uint64_t>(0), RowStart{x->base.as<uint32_t>(), (uint32_t)tiles});
+                x->tmp.bytes = 0;
+                YB_CUDA(cub::DeviceSegmentedSort::SortKeys(nullptr, x->tmp.bytes, db, (int64_t)items, (int64_t)rows, begins, begins + 1, st));
+                if ((r = x->tmp.grow()) != YAMS_OK) return r;
+                YB_CUDA(cub::DeviceSegmentedSort::SortKeys(x->tmp.buf.p, x->tmp.bytes, db, (int64_t)items, (int64_t)rows, begins, begins + 1, st));
+                sorted = db.Current();
+            }
+            // the fusion: zeros, then each variant's ranks in order
+            YB_CUDA(cudaMemsetAsync(x->fused.p, 0, (uint64_t)qb * n * 4, st));
+            const unsigned gx = (unsigned)std::min<uint64_t>((n + 4 * BM_THREADS - 1) / (4 * BM_THREADS), 64);
+            for (uint32_t j = 0; items && j < nv; ++j) {
+                rrf_scatter_kernel<<<dim3(gx, qb), BM_THREADS, 0, st>>>(sorted, x->base.as<uint32_t>(), (uint32_t)tiles, (uint64_t)j * qb,
+                                                                        k_rrf, n, x->fused.as<float>());
+                YB_CUDA(cudaGetLastError());
+            }
+            // the blend adds onto the fused rows in place (its init rows)
+            if (blend) {
+                ScoreArgs a{};
+                a.legs = x->legs.as<Leg>();
+                a.qoff = x->qoff.as<uint64_t>() + (uint64_t)nv * (nq + 1);
+                a.q0 = q0;
+                concept_field(c, a);
+                a.n = n;
+                a.init = x->fused.as<float>();
+                a.out = x->fused.as<float>();
+                bm_score_kernel<<<dim3((unsigned)tiles, qb), BM_THREADS, 0, st>>>(a);
+                YB_CUDA(cudaGetLastError());
+            }
+            if ((r = emit_batch(x, x->fused.as<float>(), n, q0, qb, nq, K, k, out_scores, out_docs, out_topk, out_counts, h_sel, h_n)) != YAMS_OK)
+                return r;
         }
         return YAMS_OK;
     });
@@ -1066,9 +1299,9 @@ static yams_status_t concepts_mine(yams_b200_concepts* c, yams_b200_bm25* x, con
         if ((r = first.reserve(nb * 4)) != YAMS_OK || (r = ab.reserve(nb * 16)) != YAMS_OK || (r = status.reserve(nb)) != YAMS_OK ||
             (r = ratio.reserve(nb * 8)) != YAMS_OK)
             return r;
-        const Dict words{x->f[0].hashes.as<uint64_t>(), x->f[0].offs.as<uint64_t>(), x->f[0].terms};
+        const Dict words{x->f[0]->hashes.as<uint64_t>(), x->f[0]->offs.as<uint64_t>(), x->f[0]->terms};
         cm_bigrams_kernel<<<bm_grid(nb), BM_THREADS, 0, st>>>(pstart.as<uint64_t>(), nb, np, val.as<uint32_t>(), pw.as<uint64_t>(),
-                                                              whash.as<uint64_t>(), words, x->f[0].ttf.as<uint64_t>(), c->cfg.min_ttf,
+                                                              whash.as<uint64_t>(), words, x->f[0]->ttf.as<uint64_t>(), c->cfg.min_ttf,
                                                               (double)c->sum_bdl, (double)T, first.as<uint32_t>(), ab.as<uint64_t>(),
                                                               status.as<uint8_t>(), ratio.as<double>());
         YB_CUDA(cudaGetLastError());
@@ -1280,12 +1513,12 @@ yams_status_t yams_b200_bm25_stats(yams_b200_bm25* idx, yams_bm25_stats* out) {
     if (rc != YAMS_OK) return rc;
     YB_ARG(idx && out, "null argument");
     out->n_docs = idx->n;
-    out->avg_dl = idx->f[0].avg;
-    out->ngram_avg_dl = idx->f[1].avg;
+    out->avg_dl = idx->f[0]->avg;
+    out->ngram_avg_dl = idx->f[1]->avg;
     out->total_tokens = idx->total_tokens;
     for (int fi = 0; fi < 2; ++fi) {
-        out->terms[fi] = idx->f[fi].terms;
-        out->postings[fi] = idx->f[fi].posts;
+        out->terms[fi] = idx->f[fi]->terms;
+        out->postings[fi] = idx->f[fi]->posts;
     }
     out->pruned = idx->pruned;
     return YAMS_OK;
@@ -1302,7 +1535,7 @@ yams_status_t yams_b200_bm25_postings(yams_b200_bm25* idx, uint32_t field, uint6
     YB_ARG(cap == 0 || (out_docs && out_tfs), "null posting output");
     YB_BIND(idx);
     std::lock_guard<std::mutex> g(idx->mu);
-    const Bm25Field& F = idx->f[field];
+    const Bm25Field& F = *idx->f[field];
     *out_df = 0;
     *out_idf = 0.0f;
     *out_total_tf = 0;
@@ -1320,7 +1553,7 @@ yams_status_t yams_b200_bm25_postings(yams_b200_bm25* idx, uint32_t field, uint6
     const uint64_t df = r[1] - r[0];
     if (df == 0) return YAMS_OK;
     *out_df = (uint32_t)df;
-    YB_CUDA(cudaMemcpy(out_idf, idx->idf.as<float>() + df, 4, cudaMemcpyDeviceToHost));
+    YB_CUDA(cudaMemcpy(out_idf, idx->idf->as<float>() + df, 4, cudaMemcpyDeviceToHost));
     *out_total_tf = r[2];
     const uint64_t m = std::min(df, cap);
     if (m) {
@@ -1338,7 +1571,7 @@ yams_status_t yams_b200_bm25_doc_lengths(yams_b200_bm25* idx, uint32_t field, ui
     YB_ARG(idx, "index is null");
     YB_ARG(field < 2, "field must be 0 (words) or 1 (n-grams)");
     YB_ARG(out || idx->n == 0, "out is null");
-    if (idx->n) memcpy(out, idx->f[field].h_dl.data(), idx->n * 4);
+    if (idx->n) memcpy(out, idx->f[field]->h_dl.data(), idx->n * 4);
     return YAMS_OK;
 }
 
@@ -1353,6 +1586,71 @@ yams_status_t yams_b200_bm25_last_timings(yams_b200_bm25* idx, float out_ms[8]) 
 }
 
 void yams_b200_bm25_destroy(yams_b200_bm25* idx) { delete idx; }
+
+yams_status_t yams_b200_bm25_atire_view(yams_b200_bm25* idx, yams_b200_bm25** out) {
+    YB_TRY
+    DeviceCtx* dev = nullptr;
+    yams_status_t rc = ensure_device(&dev);
+    if (rc != YAMS_OK) return rc;
+    YB_ARG(idx && out, "null argument");
+    *out = nullptr;
+    YB_BIND(idx);
+    std::unique_ptr<yams_b200_bm25> v(new (std::nothrow) yams_b200_bm25());
+    if (!v) return YAMS_ERR_INTERNAL;
+    // An Atire build of the same texts, k1, b and hash seed has exactly this word field (n-grams and their pruning never touch
+    // words) and the same idf table (it depends on n alone); its n-gram field is empty.
+    v->dev = idx->dev;
+    v->cfg = idx->cfg;
+    v->cfg.variant = YAMS_BM25_ATIRE;
+    v->n = idx->n;
+    v->total_tokens = idx->total_tokens;
+    v->f[0] = idx->f[0];
+    v->f[1]->h_dl.assign(idx->n, 0);
+    v->idf = idx->idf;
+    YB_CUDA(cudaStreamCreateWithFlags(&v->st, cudaStreamNonBlocking));
+    for (auto& e : v->ev) YB_CUDA(cudaEventCreate(&e));
+    *out = v.release();
+    return YAMS_OK;
+    YB_CATCH
+}
+
+yams_status_t yams_b200_bm25_score_rrf(const yams_b200_bm25* const* variants, uint32_t nv, float k_rrf, const yams_b200_concepts* concepts,
+                                       float weight, const char* const* queries, const size_t* qlens, uint32_t nq, float* out_scores,
+                                       uint32_t k, uint32_t* out_docs, float* out_topk_scores, uint32_t* out_counts) {
+    YB_TRY
+    DeviceCtx* dev = nullptr;
+    yams_status_t rc = ensure_device(&dev);
+    if (rc != YAMS_OK) return rc;
+    YB_ARG(nv == 0 || variants, "variants is null");
+    for (uint32_t j = 0; j < nv; ++j) YB_ARG(variants[j], "an index is null");
+    for (uint32_t j = 1; j < nv; ++j) YB_ARG(variants[j]->n == variants[0]->n, "the indexes differ in document count");
+    for (uint32_t j = 1; j < nv; ++j)
+        if (variants[j]->dev && variants[0]->dev && variants[j]->dev->device != variants[0]->dev->device) {
+            set_last_error("the indexes are on different devices");
+            return YAMS_ERR_UNSUPPORTED;
+        }
+    YB_ARG(std::isfinite(k_rrf) && k_rrf >= 0.0f, "k_rrf must be finite and >= 0");
+    YB_ARG(k <= TOPK_MAX, "k must be <= 4096");
+    YB_ARG(k == 0 || (out_docs && out_topk_scores && out_counts), "null top-k output");
+    YB_ARG(nv == 0 || (uint64_t)nv * variants[0]->n < (1ull << 32), "more than 2^32 - 1 ranked entries per query");
+    if (nq == 0) return YAMS_OK;
+    YB_ARG(queries && qlens, "null argument");
+    for (uint32_t q = 0; q < nq; ++q) YB_ARG(queries[q] || qlens[q] == 0, "null query");
+    if (nv == 0) {   // nothing ranks a document; there is no document count, so no score row
+        clear_topk(nq, k, out_docs, out_topk_scores, out_counts);
+        return YAMS_OK;
+    }
+    YB_BIND(variants[0]);
+    // every distinct index, locked in address order (the same index may be passed twice; callers may pass them in any order)
+    std::vector<yams_b200_bm25*> hs;
+    for (uint32_t j = 0; j < nv; ++j) hs.push_back(const_cast<yams_b200_bm25*>(variants[j]));
+    std::sort(hs.begin(), hs.end());
+    hs.erase(std::unique(hs.begin(), hs.end()), hs.end());
+    std::vector<std::unique_lock<std::mutex>> locks;
+    for (yams_b200_bm25* h : hs) locks.emplace_back(h->mu);
+    return bm25_score_rrf(variants, nv, k_rrf, concepts, weight, queries, qlens, nq, out_scores, k, out_docs, out_topk_scores, out_counts);
+    YB_CATCH
+}
 
 void yams_b200_concepts_default_config(yams_concept_config* cfg) {
     if (!cfg) return;

@@ -17,6 +17,7 @@
 #include <cmath>
 #include <limits>
 #include <map>
+#include <memory>
 #include <optional>
 #include <string>
 #include <string_view>
@@ -984,6 +985,18 @@ public:
     // SimeonLexicalBackend::score with its concept index: the BM25 scores, then concepts->blend_into(query, scores, weight), fused
     // on the device (a null or empty concept index, or one of another document count, adds nothing)
     void score(std::string_view query, std::span<float> out_scores, const B200ConceptIndex* concepts, float weight) const;
+    // The Atire index SimeonLexicalBackend builds beside a SubwordAwareBackoff primary for RRF (and its router), served from this
+    // index's word field without a second build (yams_b200_bm25_atire_view).  The view and this index may go in either order.
+    std::unique_ptr<B200Bm25Index> atire_view() const {
+        if (!idx_) throw std::runtime_error("Bm25Index::atire_view before finalize()");
+        std::unique_ptr<B200Bm25Index> v(new B200Bm25Index(&cfg_));
+        v->cfg_.variant = YAMS_BM25_ATIRE;
+        check(yams_b200_bm25_atire_view(idx_, &v->idx_), "atire_view");
+        v->n_ = n_;
+        check(yams_b200_bm25_stats(v->idx_, &v->stats_), "stats");
+        v->doc_lengths_ = doc_lengths_;
+        return v;
+    }
     uint32_t doc_count() const noexcept { return (uint32_t)(idx_ ? n_ : texts_.size()); }
     float avg_dl() const noexcept { return idx_ ? stats_.avg_dl : 0.0f; }
     yams_b200_bm25* handle() const noexcept { return idx_; }
@@ -1124,6 +1137,34 @@ inline void B200Bm25Index::score(std::string_view query, std::span<float> out_sc
     check(yams_b200_bm25_score_blended(idx_, concepts ? concepts->handle() : nullptr, weight, &q, &len, 1, out_scores.data(), 0, nullptr,
                                        nullptr, nullptr),
           "score_blended");
+}
+
+// simeon::score_bm25_variants_rrf(variants, query, out_scores, k_rrf) (fusion.hpp) on the device, and SimeonLexicalBackend::score
+// with bm25_variants_rrf: the fusion, then concepts->blend_into(query, out_scores, weight), in one call
+// (yams_b200_bm25_score_rrf).  out_scores must have the variants' document count; a variant not finalized, variants of
+// different document counts or k_rrf < 0 throw std::runtime_error.  No variants: zeros (then the blend), as the reference.
+inline void score_bm25_variants_rrf(std::span<const B200Bm25Index* const> variants, std::string_view query, std::span<float> out_scores,
+                                    const B200ConceptIndex* concepts, float weight, float k_rrf = 60.0f) {
+    std::fill(out_scores.begin(), out_scores.end(), 0.0f);
+    if (variants.empty()) {
+        if (concepts) concepts->blend_into(query, out_scores, weight);
+        return;
+    }
+    std::vector<const yams_b200_bm25*> hs;
+    for (const B200Bm25Index* v : variants) {
+        if (!v || !v->handle()) throw std::runtime_error("score_bm25_variants_rrf: a variant is not finalized");
+        hs.push_back(v->handle());
+    }
+    if (out_scores.size() != variants[0]->doc_count()) throw std::runtime_error("score_bm25_variants_rrf: out_scores size mismatch");
+    const char* q = query.data();
+    const size_t len = query.size();
+    const yams_status_t st = yams_b200_bm25_score_rrf(hs.data(), (uint32_t)hs.size(), k_rrf, concepts ? concepts->handle() : nullptr, weight,
+                                                      &q, &len, 1, out_scores.data(), 0, nullptr, nullptr, nullptr);
+    if (st != YAMS_OK) throw std::runtime_error(std::string("yams_b200_bm25 score_rrf: ") + yams_b200_last_error());
+}
+inline void score_bm25_variants_rrf(std::span<const B200Bm25Index* const> variants, std::string_view query, std::span<float> out_scores,
+                                    float k_rrf = 60.0f) {
+    score_bm25_variants_rrf(variants, query, out_scores, nullptr, 0.0f, k_rrf);
 }
 
 }  // namespace yams_b200::host
