@@ -595,9 +595,10 @@ YAMS_B200_API void yams_b200_simeon_destroy(yams_b200_encoder* e);
  *          SubwordAwareBackoff adds alpha * bm25plus over the word's list (alpha = df / (df + gamma), 0 when df = 0) when
  *          alpha > 0, and (1 - alpha) * bm25plus over the list of each distinct n-gram of the word still in the index when
  *          alpha < 1.  Every float operation is the reference's, in its order, without fused multiply-adds.
- * Scores are bit-identical to the reference.  The concept blend (ConceptIndex::blend_into) is the concepts block below.  Out of
- * scope (the caller's, as today): fragment geometry, the strategy router, the query router, the BM25F aux field, SDM / word
- * bigrams, PRF, and the caller's document windowing (buildEnhancementText).  RRF over variants is yams_b200_bm25_score_rrf. */
+ * Scores are bit-identical to the reference.  The concept blend (ConceptIndex::blend_into) is the concepts block below.  The lead-text
+ * aux field and the strategy router are yams_b200_bm25_build_lead and yams_b200_bm25_score_strategy.  Out of scope (the
+ * caller's, as today): fragment geometry, the query router, SDM / word bigrams, PRF, and the caller's document windowing (buildEnhancementText).  RRF over variants is
+ * yams_b200_bm25_score_rrf. */
 #define YAMS_BM25_ATIRE 0                    /* simeon::Bm25Variant::Atire */
 #define YAMS_BM25_SUBWORD_AWARE_BACKOFF 7    /* simeon::Bm25Variant::SubwordAwareBackoff */
 typedef struct yams_bm25_config {
@@ -632,13 +633,14 @@ typedef struct yams_bm25_stats {
     uint64_t pruned;              /* n-grams dropped by the df rule */
 } yams_bm25_stats;
 YAMS_B200_API yams_status_t yams_b200_bm25_stats(yams_b200_bm25* idx, yams_bm25_stats* out);
-/* the posting list of term_hash in field 0 (words) or 1 (n-grams): *out_df (0 when absent), *out_idf, *out_total_tf, and the
+/* the posting list of term_hash in field 0 (words), 1 (n-grams), 2 (lead words) or 3 (lead n-grams): *out_df (0 when absent), *out_idf, *out_total_tf, and the
  * first min(df, cap) (document, tf) entries in document order (out_docs / out_tfs nullable when cap = 0).  Bm25Index::df /
  * idf / total_tf of a term are these of field 0 for the term's hash. */
 YAMS_B200_API yams_status_t yams_b200_bm25_postings(yams_b200_bm25* idx, uint32_t field, uint64_t term_hash, uint32_t* out_df,
                                                     float* out_idf, uint64_t* out_total_tf, uint32_t* out_docs, uint32_t* out_tfs,
                                                     uint64_t cap);
-/* dl (field 0) or ngram_dl (field 1, zeros for Atire) of every document -> out[n_docs] (HOST) */
+/* dl (field 0), ngram_dl (field 1, zeros for Atire) or the lead field's (2, 3; zeros without an active lead field) of every
+ * document -> out[n_docs] (HOST) */
 YAMS_B200_API yams_status_t yams_b200_bm25_doc_lengths(yams_b200_bm25* idx, uint32_t field, uint32_t* out);
 /* out_ms[0..3]: the last build's device ms of the upload, the tokenising (per-document counts, words, n-gram pairs), the sorts,
  * the posting lists (runs, pruning, dictionary), [4] its host wall ms, [5] its document slices; [6] the last score call's
@@ -653,6 +655,21 @@ YAMS_B200_API void yams_b200_bm25_destroy(yams_b200_bm25* idx);
  * Atire index is equivalent to the index.  The view has its own stream, lock and score workspace, so it may be scored
  * concurrently with idx, and the two may be destroyed in either order. */
 YAMS_B200_API yams_status_t yams_b200_bm25_atire_view(yams_b200_bm25* idx, yams_b200_bm25** out);
+
+/* ---- the lead-text field (DESIGN.md §4.14) ----------------------------------------------------------------------
+ * yams_b200_bm25_build with Bm25Index::add_doc(text, extract_lead_tokens(text, lead_tokens)) for each document, as the lexical
+ * backend builds with strategy_router_enabled (lead_tokens 64).  The lead text is the text up to the whitespace byte (C-locale
+ * isspace) that ends its lead_tokens-th whitespace-delimited token (all of it when it has fewer), whitespace turned into ' ',
+ * trailing spaces trimmed.  It is indexed as an aux word field (field 2) and, for SubwordAwareBackoff, an aux n-gram field
+ * (field 3), with their own lengths, averages and n-gram pruning.  The aux field is active from the first document whose lead
+ * text is non-empty, earlier documents counting length 0, so it exists for all documents or for none (every lead text empty).
+ * lead_tokens = 0 is yams_b200_bm25_build.  An Atire view (yams_b200_bm25_atire_view) shares the aux word field. */
+YAMS_B200_API yams_status_t yams_b200_bm25_build_lead(void* self, const yams_bm25_config* cfg /* NULL = default */,
+                                                      const char* const* texts, const size_t* lens, uint64_t n_docs,
+                                                      uint32_t lead_tokens, yams_b200_bm25** out);
+/* the aux fields' yams_bm25_stats: n_docs (n_docs when the aux field is active, else 0), avg_dl / ngram_avg_dl, total_tokens,
+ * terms / postings of fields 2 and 3, and the aux n-grams the df rule dropped */
+YAMS_B200_API yams_status_t yams_b200_bm25_aux_stats(yams_b200_bm25* idx, yams_bm25_stats* out);
 
 /* ---- Simeon word-bigram concepts (DESIGN.md §4.12) ---------------------------------------------------------------
  * third_party/simeon ConceptIndex (src/concept_mining.cpp) mined against a BM25 index, and its blend into BM25 scores, as the
@@ -734,6 +751,50 @@ YAMS_B200_API yams_status_t yams_b200_bm25_score_rrf(const yams_b200_bm25* const
                                                      const yams_b200_concepts* concepts, float weight, const char* const* queries,
                                                      const size_t* qlens, uint32_t nq, float* out_scores, uint32_t k,
                                                      uint32_t* out_docs, float* out_topk_scores, uint32_t* out_counts);
+
+/* ---- the strategy router (DESIGN.md §4.14) ----------------------------------------------------------------------
+ * The strategy router's pools over an index built with the lead field and its route, as the lexical backend constructs them (simeon_lexical_backend.cpp:563-580):
+ *   YAMS_BM25_STRATEGY_BM25        pool 0, Bm25Strategy: score_bm25f(q, lead(q, 64), 0.85, 0.15), or Bm25Index::score(q) when
+ *                                  the query's lead text is empty;
+ *   YAMS_BM25_STRATEGY_LEAD_FIELD  pool 2, LeadFieldStrategy (the "lead_field" bandit arm): score_bm25f(q, q, 0.85, 0.15).
+ * score_bm25f(body, aux, wb, wa): the body score, times wb, then the aux legs -- SubwordAwareBackoff adds (wa * alpha) *
+ * bm25plus over the aux query's words in field 2 and (wa * (1 - alpha)) * bm25plus over their n-grams in field 3, alpha from the
+ * field-2 df; Atire adds wa * score_atire over field 2.  An index built without the lead field has empty aux fields: wb * body.
+ *   YAMS_BM25_STRATEGY_KEYPHRASE   pool 1, KeyphraseStrategy(0.25, 0.30) (the "keyphrase" bandit arm): the plain score; the
+ *                                  normalised softmax entropy (double) of simeon::top_k(scores, 10), which keeps zero scores;
+ *                                  below 0.30f, or without keyphrases (alphabetic runs of >= 2 bytes, lowercased, stopwords
+ *                                  dropped), the plain score; else the z-score (two sequential double sums over the n scores)
+ *                                  plus (lam * 0.25f) * (matches / keyphrases), lam = 1 / (1 + expf(-(entropy - 0.48f) * 8)), a
+ *                                  document matching a keyphrase when its single-term score is > 0.  Scores may be negative.
+ *   YAMS_BM25_STRATEGY_ROUTED      SimeonLexicalBackend::scoreStrategyRouted: bm25_entropy = float(sum over the documents of
+ *                                  plain score s > 0, in document order, of sn * -log(sn), sn = (double)(s / max), over their
+ *                                  count); < 0.05f -> pool 0, > 0.50f -> pool 2, else pool 1.  The device's profile comes with a
+ *                                  bound on its distance from the reference's; a row whose route the bound cannot settle is
+ *                                  copied back and the backend's loop replayed with std::log.  YAMS_B200_BM25_ROUTE_MARGIN = w > 0,
+ *                                  read at every call, widens the entropy's interval by w (1 replays every row with a positive score).
+ * score_bm25f(body, aux, wb, wa): the body score, times wb, then the aux legs -- SubwordAwareBackoff adds (wa * alpha) *
+ * bm25plus over the aux query's words in field 2 and (wa * (1 - alpha)) * bm25plus over their n-grams in field 3, alpha from the
+ * field-2 df; Atire adds wa * score_atire over field 2.  An index built without the lead field has empty aux fields: wb * body. */
+#define YAMS_BM25_STRATEGY_BM25 0
+#define YAMS_BM25_STRATEGY_KEYPHRASE 1
+#define YAMS_BM25_STRATEGY_LEAD_FIELD 2
+#define YAMS_BM25_STRATEGY_ROUTED 3
+/* The strategy's scores of nq HOST queries, then, with concepts, ConceptIndex::blend_into(query, scores, weight): the outputs,
+ * limits and locking of yams_b200_bm25_score_blended, bit-identical to the reference.  out_chosen (nullable): [nq] the pool
+ * each query took.  KEYPHRASE and ROUTED batch queries so that their score rows and match rows stay within 1 GiB; all pools
+ * of a batch run together, each row getting its own pool's legs.  strategy > 3: YAMS_ERR_INVALID_ARG. */
+YAMS_B200_API yams_status_t yams_b200_bm25_score_strategy(yams_b200_bm25* idx, uint32_t strategy, const yams_b200_concepts* concepts,
+                                                          float weight, const char* const* queries, const size_t* qlens, uint32_t nq,
+                                                          float* out_scores, uint32_t k, uint32_t* out_docs, float* out_topk_scores,
+                                                          uint32_t* out_counts, uint32_t* out_chosen);
+typedef struct yams_bm25_strategy_stats {   /* of the index's last yams_b200_bm25_score_strategy call */
+    uint32_t queries[3];          /* queries scored by pool 0, 1, 2 */
+    uint32_t replayed;            /* ROUTED rows whose route was replayed on the host */
+    uint32_t keyphrase_boosted;   /* pool-1 rows past the gate (z-scored and boosted) */
+    float zscore_ms;              /* device ms of the z-score kernel */
+    float device_ms, wall_ms;     /* the call's device and host wall ms */
+} yams_bm25_strategy_stats;
+YAMS_B200_API yams_status_t yams_b200_bm25_strategy_stats(yams_b200_bm25* idx, yams_bm25_strategy_stats* out);
 
 /* [0] stage-1 scan ms, [1] rescoring+select ms, [2] total device ms of the last yams_b200_search or
  * yams_b200_search_device on this corpus (the latter's once its work is done); [3] unused (0);

@@ -61,6 +61,11 @@ class Bm25Stats(C.Structure):
                 ("terms", C.c_uint64 * 2), ("postings", C.c_uint64 * 2), ("pruned", C.c_uint64)]
 
 
+class Bm25StrategyStats(C.Structure):
+    _fields_ = [("queries", C.c_uint32 * 3), ("replayed", C.c_uint32), ("keyphrase_boosted", C.c_uint32), ("zscore_ms", C.c_float),
+                ("device_ms", C.c_float), ("wall_ms", C.c_float)]
+
+
 class ConceptConfig(C.Structure):
     _fields_ = [("min_ttf", C.c_uint32), ("pmi_floor", C.c_float), ("max_concepts", C.c_uint32), ("k1", C.c_float), ("b", C.c_float)]
 
@@ -71,6 +76,8 @@ class ConceptStats(C.Structure):
 
 
 BM25_ATIRE, BM25_SUBWORD_AWARE_BACKOFF = 0, 7   # simeon::Bm25Variant numbering
+BM25_STRATEGY_BM25, BM25_STRATEGY_KEYPHRASE, BM25_STRATEGY_LEAD_FIELD = 0, 1, 2   # the strategy router's pool numbers
+BM25_STRATEGY_ROUTED = 3
 
 SIMEON_WORD_TOKENS = 1        # NGramMode::CharAndWord
 SIMEON_PROJECTION_FWHT = 2    # ProjectionMode::Fwht (default projection: AchlioptasSparse)
@@ -186,6 +193,12 @@ SYMBOLS = {
     "yams_b200_bm25_atire_view": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p)]),
     "yams_b200_bm25_score_rrf": (C.c_int, [C.POINTER(C.c_void_p), C.c_uint32, C.c_float, C.c_void_p, C.c_float, C.POINTER(C.c_char_p),
                                            C.POINTER(C.c_size_t), C.c_uint32, f32p, C.c_uint32, u32p, f32p, u32p]),
+    "yams_b200_bm25_build_lead": (C.c_int, [C.c_void_p, C.POINTER(Bm25Config), C.POINTER(C.c_char_p), C.POINTER(C.c_size_t), C.c_uint64,
+                                            C.c_uint32, C.POINTER(C.c_void_p)]),
+    "yams_b200_bm25_aux_stats": (C.c_int, [C.c_void_p, C.POINTER(Bm25Stats)]),
+    "yams_b200_bm25_strategy_stats": (C.c_int, [C.c_void_p, C.POINTER(Bm25StrategyStats)]),
+    "yams_b200_bm25_score_strategy": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_float, C.POINTER(C.c_char_p), C.POINTER(C.c_size_t),
+                                                C.c_uint32, f32p, C.c_uint32, u32p, f32p, u32p, u32p]),
     "yams_b200_pq_build": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, f32p, u64p, C.POINTER(C.c_void_p)]),
     "yams_b200_pq_search": (C.c_int, [C.c_void_p, f32p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_float, i64p, f32p, u32p, u64p]),
     "yams_b200_pq_search_candidates": (C.c_int, [C.c_void_p, f32p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_float, i64p, u64p, i64p, f32p,
@@ -830,9 +843,11 @@ def _score_call(call, n, queries, k, full):
 
 class Bm25Index:
     """simeon's Bm25Index built on the device over `texts` (add_doc for each, then finalize), as the lexical backend configures it
-    unless overridden: SubwordAwareBackoff, gamma 5.  `variant` is BM25_ATIRE or BM25_SUBWORD_AWARE_BACKOFF."""
+    unless overridden: SubwordAwareBackoff, gamma 5.  `variant` is BM25_ATIRE or BM25_SUBWORD_AWARE_BACKOFF.  With lead_tokens > 0
+    each document also gets its lead text (extract_lead_tokens(text, lead_tokens)) as the aux field, as the backend builds with
+    the strategy router on (64)."""
 
-    def __init__(self, texts, **overrides):
+    def __init__(self, texts, lead_tokens: int = 0, **overrides):
         cfg = Bm25Config()
         lib().yams_b200_bm25_default_config(C.byref(cfg))
         for k, v in overrides.items():
@@ -840,8 +855,9 @@ class Bm25Index:
         self.cfg = cfg
         raw, ptrs, lens = _texts(texts)
         self.n = len(raw)
+        self.lead_tokens = lead_tokens
         self._h = C.c_void_p()
-        _check(lib().yams_b200_bm25_build(None, C.byref(cfg), ptrs, lens, self.n, C.byref(self._h)), "bm25_build")
+        _check(lib().yams_b200_bm25_build_lead(None, C.byref(cfg), ptrs, lens, self.n, lead_tokens, C.byref(self._h)), "bm25_build_lead")
 
     def score(self, queries, k: int = 0, full: bool = True, concepts: Optional["ConceptIndex"] = None, weight: float = 0.5):
         """Bm25Index::score of every query: {"scores": [nq][n_docs] (full=True)}, and for k > 0 the best k documents of score > 0
@@ -852,6 +868,33 @@ class Bm25Index:
         return _score_call(lambda *args: _check(lib().yams_b200_bm25_score_blended(self._h, concepts._h, weight, *args), "bm25_score_blended"),
                            self.n, queries, k, full)
 
+    def score_strategy(self, queries, strategy: int, k: int = 0, full: bool = True, concepts: Optional["ConceptIndex"] = None,
+                       weight: float = 0.5):
+        """The strategy router's pool `strategy` (BM25_STRATEGY_BM25: Bm25Strategy, BM25_STRATEGY_KEYPHRASE: KeyphraseStrategy,
+        BM25_STRATEGY_LEAD_FIELD: LeadFieldStrategy) or its routed choice (BM25_STRATEGY_ROUTED) for every query, then with
+        `concepts` blend_into(query, scores, weight): the outputs of score, and "chosen" [nq], the pool each query took."""
+        nq = len(queries)
+        chosen = np.zeros(max(nq, 1), np.uint32)
+        out = _score_call(lambda *args: _check(lib().yams_b200_bm25_score_strategy(self._h, strategy, concepts._h if concepts is not None
+                                                                                    else None, weight, *args, chosen.ctypes.data_as(u32p)),
+                                               "bm25_score_strategy"), self.n, queries, k, full)
+        out["chosen"] = chosen[:nq]
+        return out
+
+    def strategy_stats(self) -> dict:
+        """the last score_strategy call's pools, replayed routes, boosted keyphrase rows and times"""
+        s = Bm25StrategyStats()
+        _check(lib().yams_b200_bm25_strategy_stats(self._h, C.byref(s)), "bm25_strategy_stats")
+        return {"queries": tuple(s.queries), "replayed": s.replayed, "keyphrase_boosted": s.keyphrase_boosted, "zscore_ms": s.zscore_ms,
+                "device_ms": s.device_ms, "wall_ms": s.wall_ms}
+
+    def aux_stats(self) -> dict:
+        """stats() of the lead-text fields (2 and 3); n_docs 0 when no document has a lead text"""
+        s = Bm25Stats()
+        _check(lib().yams_b200_bm25_aux_stats(self._h, C.byref(s)), "bm25_aux_stats")
+        return {"n_docs": s.n_docs, "avg_dl": np.float32(s.avg_dl), "ngram_avg_dl": np.float32(s.ngram_avg_dl),
+                "total_tokens": s.total_tokens, "terms": tuple(s.terms), "postings": tuple(s.postings), "pruned": s.pruned}
+
     def atire_view(self) -> "Bm25Index":
         """The Atire index of the same texts with this index's k1, b and hash seed, served from this index's word field in place
         (yams_b200_bm25_atire_view): no copy, no build.  Either may be closed first."""
@@ -859,6 +902,7 @@ class Bm25Index:
         v.cfg = Bm25Config.from_buffer_copy(self.cfg)
         v.cfg.variant = BM25_ATIRE
         v.n = self.n
+        v.lead_tokens = self.lead_tokens
         v._h = C.c_void_p()
         _check(lib().yams_b200_bm25_atire_view(self._h, C.byref(v._h)), "bm25_atire_view")
         return v
@@ -874,7 +918,8 @@ class Bm25Index:
                 "total_tokens": s.total_tokens, "terms": tuple(s.terms), "postings": tuple(s.postings), "pruned": s.pruned}
 
     def postings(self, field: int, term_hash: int):
-        """(docs, tfs, idf, total_tf) of a hash in field 0 (words) or 1 (n-grams); empty lists and 0 when absent."""
+        """(docs, tfs, idf, total_tf) of a hash in field 0 (words), 1 (n-grams), 2 (lead words) or 3 (lead n-grams); empty lists
+        and 0 when absent."""
         df, idf, ttf = C.c_uint32(), C.c_float(), C.c_uint64()
         _check(lib().yams_b200_bm25_postings(self._h, field, term_hash, C.byref(df), C.byref(idf), C.byref(ttf), None, None, 0), "bm25_postings")
         docs = np.zeros(max(df.value, 1), np.uint32)

@@ -27,6 +27,13 @@
 // RRF (score_bm25_variants_rrf, fusion.cpp; DESIGN.md §4.13): the variants' score rows, their ranked entries as sortable keys,
 // one segmented sort per batch, one scatter of 1 / (k + r) per variant in order.  An Atire view shares its parent's word field
 // and idf table, which an Atire build of the same texts would reproduce exactly.
+//
+// Lead field and strategy router (extract_lead_tokens, add_doc(text, aux), score_bm25f, KeyphraseStrategy, the backend's entropy
+// route; DESIGN.md §4.14): one warp per document cuts its lead prefix in the uploaded text, the build's own pipeline makes the aux
+// fields 2 and 3 from the cut text, and BM25F is more legs: a body-scale leg, then aux legs whose weight is fl(wa * alpha).  The
+// keyphrase strategy counts matches with presence legs and z-scores a row with one lane's sequential double sums; the route
+// reduces each row's profile on the device with a bound on its distance from the reference's, replaying the row on the host
+// when the bound cannot settle it.
 #include <cub/cub.cuh>
 #include <thrust/iterator/counting_iterator.h>
 #include <thrust/iterator/transform_iterator.h>
@@ -39,6 +46,7 @@
 #include <mutex>
 #include <new>
 #include <unordered_map>
+#include <string>
 #include <unordered_set>
 #include <vector>
 
@@ -60,12 +68,47 @@ struct Bm25Field {
     DevBuf docs;     // postings: document ids, ascending per term
     DevBuf tfs;      // postings: tf
     DevBuf dl;       // n_docs: dl / ngram_dl
-    uint64_t terms = 0, posts = 0;
+    uint64_t terms = 0, posts = 0, sum = 0;   // sum: of dl
     float avg = 0.f;
     std::vector<uint32_t> h_dl;
 };
 
 // ---- build kernels ----
+__host__ __device__ __forceinline__ bool is_space(uint8_t c) { return c == ' ' || (c >= '\t' && c <= '\r'); }   // isspace, C locale
+
+// The lead-text field (extract_lead_tokens(text, lead), corpus_adapter.cpp:16-39): one warp per document finds the whitespace
+// byte that ends its lead-th whitespace-delimited token (none: the document's end) and zeroes the bytes from there to the
+// document's end, so the field's words are the prefix's.  *active = 1 when some document's lead text is non-empty (a
+// non-whitespace byte before its cut), which activates the reference's aux field.
+__global__ void bm_lead_cut_kernel(uint8_t* __restrict__ t, const uint64_t* __restrict__ pos, uint64_t n, uint32_t lead,
+                                   uint32_t* __restrict__ active) {
+    const uint32_t lane = threadIdx.x & 31;
+    const uint64_t warps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
+    for (uint64_t d = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; d < n; d += warps) {
+        const uint64_t s = pos[d], e = pos[d + 1] - 1;   // the document's bytes; the zero byte after it is not one
+        uint64_t cut = e;
+        uint32_t count = 0;
+        bool any = false;
+        for (uint64_t c0 = s; c0 < e; c0 += 32) {
+            const uint64_t i = c0 + lane;
+            const bool in = i < e, sp = in && is_space(t[i]);
+            const unsigned ends = __ballot_sync(0xFFFFFFFFu, sp && i > s && !is_space(t[i - 1]));   // a token ends at i
+            const unsigned chars = __ballot_sync(0xFFFFFFFFu, in && !sp);
+            const uint32_t m = __popc(ends);
+            if (count + m >= lead) {
+                const uint32_t bit = __fns(ends, 0, (int)(lead - count));
+                cut = c0 + bit;
+                any = any || (chars & ((1u << bit) - 1u)) != 0;
+                break;
+            }
+            count += m;
+            any = any || chars != 0;
+        }
+        for (uint64_t i = cut + lane; i < e; i += 32) t[i] = 0;
+        if (lane == 0 && any) *active = 1;
+    }
+}
+
 struct IsWordStart {
     const uint8_t* t;
     __device__ bool operator()(uint64_t i) const { return is_word_char(t[i]) && (i == 0 || !is_word_char(t[i - 1])); }
@@ -200,21 +243,27 @@ __global__ void bm_unpack_kernel(const uint64_t* __restrict__ pv, uint64_t m, ui
 }
 
 // ---- score ----
-// Field kinds of a leg: 0 the words, 1 the n-grams (the index's two fields), 2 a mined concept (ConceptIndex, blended after the
-// BM25 legs of its query).
-constexpr uint32_t BM_CONCEPT = 2;
+// Field kinds of a leg: 0 the words, 1 the n-grams, 2 the lead-text words, 3 the lead-text n-grams (the index's four fields),
+// 4 a mined concept (ConceptIndex, blended after the BM25 legs of its query), 5 BM25F's body scale (every score of the row
+// times the leg's weight, between the body legs and the aux legs).
+constexpr uint32_t BM_AUX = 2;
+constexpr uint32_t BM_CONCEPT = 4;
+constexpr uint32_t BM_SCALE = 5;
+// A presence leg (RawLeg / Leg pad of a field-0 leg): adds 1.0f to each document of a keyphrase's word list whose single-term
+// score (score_weighted_hashes with weight 1: bm25plus, or score_atire for Atire) is > 0, counting KeyphraseStrategy's matches.
+constexpr uint32_t BM_PRESENCE = 1;
 
-struct RawLeg {        // one query word (field 0), one distinct n-gram of it (field 1), or one matched concept (field 2)
+struct RawLeg {        // one query word (field 0 / 2), one distinct n-gram of it (1 / 3), one matched concept, or a scale
     uint64_t hash;
     uint64_t term_hash;
     uint32_t field;
-    uint32_t pad;
+    uint32_t pad;      // BM_SCALE: the scale's float bits
 };
 struct Leg {           // an addition over documents docs[b, e) of `field`; empty when b == e
     uint64_t b, e;
     float w, idf;
     uint32_t field;
-    uint32_t pad;
+    uint32_t pad;      // BM_PRESENCE: a presence leg
 };
 struct Dict {
     const uint64_t* hashes;
@@ -238,26 +287,41 @@ __device__ __forceinline__ bool dict_find(const Dict& D, uint64_t h, uint64_t* b
     return true;
 }
 
-__global__ void bm_plan_kernel(const RawLeg* __restrict__ raw, uint64_t nlegs, Dict w, Dict g, const float* __restrict__ idf,
-                               int sab, float gamma, ConceptDict c, Leg* __restrict__ legs) {
+struct FieldDicts {     // the index's fields 0..3
+    Dict d[4];
+};
+
+// An aux leg's weight is fl(wa * alpha), fl(wa * (1 - alpha)) or wa (Atire), taken before the product with the score, as
+// score_bm25f's `weight_aux * alpha * bm25plus` (bm25.cpp:1041-1060, 1087); alpha comes from the aux field's df.
+__global__ void bm_plan_kernel(const RawLeg* __restrict__ raw, uint64_t nlegs, FieldDicts f, const float* __restrict__ idf,
+                               int sab, float gamma, float wa, ConceptDict c, Leg* __restrict__ legs) {
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nlegs; i += (uint64_t)gridDim.x * blockDim.x) {
         const RawLeg r = raw[i];
         Leg L{};
         L.field = r.field;
         uint64_t b = 0, e = 0, t = 0;
-        if (r.field == BM_CONCEPT) {
+        if (r.field == BM_SCALE) {
+            L.w = __uint_as_float(r.pad);
+        } else if (r.field == BM_CONCEPT) {
             // wpmi = weight * pmi (concept_mining.cpp:106); the host only emits concepts the index keeps
             if (dict_find(c.d, r.hash, &b, &e, &t)) { L.b = b; L.e = e; L.w = __fmul_rn(c.weight, c.pmi[t]); L.idf = c.idf[t]; }
-        } else if (!sab) {
-            if (dict_find(w, r.hash, &b, &e)) { L.b = b; L.e = e; L.idf = idf[e - b]; }
         } else {
-            // alpha = float(df) / (float(df) + gamma), 0 when the word is unknown (bm25.cpp:805-807)
-            const uint64_t df = dict_find(w, r.term_hash, &b, &e) ? e - b : 0;
-            const float alpha = df > 0 ? __fdiv_rn(__ull2float_rn(df), __fadd_rn(__ull2float_rn(df), gamma)) : 0.0f;
-            if (r.field == 0) {
-                if (alpha > 0.0f) { L.b = b; L.e = e; L.w = alpha; L.idf = idf[df]; }
-            } else if (alpha < 1.0f && dict_find(g, r.hash, &b, &e)) {
-                L.b = b; L.e = e; L.w = __fsub_rn(1.0f, alpha); L.idf = idf[e - b];
+            const bool aux = r.field >= BM_AUX;
+            const Dict& w = f.d[r.field & BM_AUX];
+            if (r.pad == BM_PRESENCE) {   // a keyphrase's word list, whatever the variant
+                if (dict_find(w, r.hash, &b, &e)) { L.b = b; L.e = e; L.idf = idf[e - b]; L.pad = BM_PRESENCE; }
+            } else if (!sab) {
+                if (dict_find(w, r.hash, &b, &e)) { L.b = b; L.e = e; L.w = aux ? wa : 0.0f; L.idf = idf[e - b]; }
+            } else {
+                // alpha = float(df) / (float(df) + gamma), 0 when the word is unknown (bm25.cpp:805-807)
+                const uint64_t df = dict_find(w, r.term_hash, &b, &e) ? e - b : 0;
+                const float alpha = df > 0 ? __fdiv_rn(__ull2float_rn(df), __fadd_rn(__ull2float_rn(df), gamma)) : 0.0f;
+                if ((r.field & 1) == 0) {
+                    if (alpha > 0.0f) { L.b = b; L.e = e; L.w = aux ? __fmul_rn(wa, alpha) : alpha; L.idf = idf[df]; }
+                } else if (alpha < 1.0f && dict_find(f.d[r.field], r.hash, &b, &e)) {
+                    const float w1 = __fsub_rn(1.0f, alpha);
+                    L.b = b; L.e = e; L.w = aux ? __fmul_rn(wa, w1) : w1; L.idf = idf[e - b];
+                }
             }
         }
         legs[i] = L;
@@ -268,11 +332,11 @@ struct ScoreArgs {
     const Leg* legs;
     const uint64_t* qoff;     // legs of query q: [qoff[q], qoff[q + 1])
     uint32_t q0;              // first query of the batch
-    const uint32_t* docs[3];
-    const uint32_t* tfs[3];
-    const uint32_t* dl[3];
-    float avg[3];             // fields 0, 1: avg_dl > 0 ? avg_dl : 1; field 2: avg_bigram_dl (> 0 whenever a concept exists)
-    float k1[3], b[3];        // fields 0, 1: Bm25Config's; field 2: ConceptConfig's
+    const uint32_t* docs[5];
+    const uint32_t* tfs[5];
+    const uint32_t* dl[5];
+    float avg[5];             // fields 0..3: avg_dl > 0 ? avg_dl : 1; concepts: avg_bigram_dl (> 0 whenever a concept exists)
+    float k1[5], b[5];        // fields 0..3: Bm25Config's; concepts: ConceptConfig's
     uint64_t n;
     float delta;
     int sab;
@@ -298,6 +362,11 @@ __global__ void __launch_bounds__(BM_THREADS) bm_score_kernel(ScoreArgs a) {
     __syncthreads();
     for (uint64_t l = a.qoff[q]; l < a.qoff[q + 1]; ++l) {
         const Leg g = a.legs[l];
+        if (g.field == BM_SCALE) {   // score_bm25f's `s *= weight_body` over the whole row (bm25.cpp:993-996)
+            for (uint32_t i = threadIdx.x; i < len; i += BM_THREADS) s[i] = __fmul_rn(s[i], g.w);
+            __syncthreads();
+            continue;
+        }
         if (g.b == g.e) continue;
         const uint32_t* docs = a.docs[g.field];
         const uint64_t sb = first_ge(docs, g.b, g.e, lo), se = first_ge(docs, sb, g.e, lo + len);
@@ -313,11 +382,15 @@ __global__ void __launch_bounds__(BM_THREADS) bm_score_kernel(ScoreArgs a) {
             const float denom = __fadd_rn(tf, __fmul_rn(k1, __fadd_rn(omb, __fdiv_rn(__fmul_rn(b, dl), avg))));
             // idf * tf * (k1 + 1) / denom: Atire, and a concept's score_atire (concept_mining.cpp:31-36)
             const float atire = __fdiv_rn(__fmul_rn(__fmul_rn(g.idf, tf), k1p1), denom);
+            // idf * (tf * (k1 + 1) / denom + delta)
+            const float plus = __fmul_rn(g.idf, __fadd_rn(__fdiv_rn(__fmul_rn(tf, k1p1), denom), a.delta));
             float add;
-            if (g.field == BM_CONCEPT)   // wpmi * score_atire
+            if (g.pad == BM_PRESENCE)    // 1.0f * the single-term score > 0
+                add = (a.sab ? plus : atire) > 0.0f ? 1.0f : 0.0f;
+            else if (g.field == BM_CONCEPT || (!a.sab && g.field == BM_AUX))   // wpmi * score_atire; weight_aux * score_atire
                 add = __fmul_rn(g.w, atire);
-            else if (a.sab)              // alpha * (idf * (tf * (k1 + 1) / denom + delta))
-                add = __fmul_rn(g.w, __fmul_rn(g.idf, __fadd_rn(__fdiv_rn(__fmul_rn(tf, k1p1), denom), a.delta)));
+            else if (a.sab)              // alpha * bm25plus
+                add = __fmul_rn(g.w, plus);
             else
                 add = atire;
             s[d - lo] = __fadd_rn(s[d - lo], add);
@@ -326,6 +399,88 @@ __global__ void __launch_bounds__(BM_THREADS) bm_score_kernel(ScoreArgs a) {
     }
     float* out = a.out + (uint64_t)blockIdx.y * a.n + lo;
     for (uint32_t i = threadIdx.x; i < len; i += BM_THREADS) out[i] = s[i];
+}
+
+// The strategy router's entropy profile of one score row per block (SimeonLexicalBackend::scoreStrategyRouted,
+// simeon_lexical_backend.cpp:1000-1017): out[3 * row] = max, [+1] = the documents of score > 0, [+2] = the sum over them of
+// sn * -log(sn), sn = (double)(s / max), 0 when max <= 0.  The sum is a tree in double with the device's log; the host bounds
+// its distance from the reference's sequential sum with glibc's log (route_pool).
+__global__ void __launch_bounds__(BM_THREADS) bm_route_kernel(const float* __restrict__ rows, uint64_t n, double* __restrict__ out) {
+    using RF = cub::BlockReduce<float, BM_THREADS>;
+    using RD = cub::BlockReduce<double, BM_THREADS>;
+    __shared__ union { typename RF::TempStorage f; typename RD::TempStorage d; } ts;
+    __shared__ float top;
+    const float* s = rows + (uint64_t)blockIdx.x * n;
+    float m = 0.0f;
+    for (uint64_t i = threadIdx.x; i < n; i += BM_THREADS) m = fmaxf(m, s[i]);
+    m = RF(ts.f).Reduce(m, cub::Max());
+    if (threadIdx.x == 0) top = m;
+    __syncthreads();
+    m = top;
+    double sum = 0.0, cnt = 0.0;
+    if (m > 0.0f)
+        for (uint64_t i = threadIdx.x; i < n; i += BM_THREADS) {
+            const float v = s[i];
+            if (!(v > 0.0f)) continue;
+            const double sn = (double)__fdiv_rn(v, m);
+            if (sn > 0.0) sum = __dadd_rn(sum, __dmul_rn(sn, -log(sn)));
+            cnt += 1.0;
+        }
+    sum = RD(ts.d).Sum(sum);
+    __syncthreads();
+    cnt = RD(ts.d).Sum(cnt);
+    if (threadIdx.x == 0) {
+        out[3 * blockIdx.x] = (double)m;
+        out[3 * blockIdx.x + 1] = cnt;
+        out[3 * blockIdx.x + 2] = sum;
+    }
+}
+
+// KeyphraseStrategy's boost of one gated row per block (retrieval_strategy.cpp:17-30, 243-250): zscore_inplace's two sums in
+// double over the n scores in document order -- one lane adds while its warp stages the row through shared memory (adding +0.0
+// is exact, so the mean's pass skips zeros; the variance's may not) -- then every document's
+// float((x - mean) / sd) + lw * (float(matches) / nkp).  zrow[b] is the row, zp[2 b] lw = fl(lam * 0.25f), zp[2 b + 1] nkp.
+__global__ void __launch_bounds__(BM_THREADS) bm_zscore_kernel(float* __restrict__ rows, const float* __restrict__ counts, uint64_t n,
+                                                               const uint32_t* __restrict__ zrow, const float* __restrict__ zp) {
+    constexpr uint32_t CH = 1024;
+    __shared__ float buf[CH];
+    __shared__ double stat[2];
+    float* x = rows + (uint64_t)zrow[blockIdx.x] * n;
+    const float* cnt = counts + (uint64_t)zrow[blockIdx.x] * n;
+    if (threadIdx.x < 32) {
+        const uint32_t lane = threadIdx.x;
+        double mean = 0.0;
+        for (int pass = 0; pass < 2; ++pass) {
+            double acc = 0.0;
+            for (uint64_t c0 = 0; c0 < n; c0 += CH) {
+                const uint32_t len = (uint32_t)min((uint64_t)CH, n - c0);
+                for (uint32_t j = lane; j < len; j += 32) buf[j] = x[c0 + j];
+                __syncwarp();
+                if (lane == 0) {
+                    if (pass == 0) {
+                        for (uint32_t j = 0; j < len; ++j)
+                            if (buf[j] != 0.0f) acc = __dadd_rn(acc, (double)buf[j]);
+                    } else {
+                        for (uint32_t j = 0; j < len; ++j) {
+                            const double d = __dsub_rn((double)buf[j], mean);
+                            acc = __dadd_rn(acc, __dmul_rn(d, d));
+                        }
+                    }
+                }
+                __syncwarp();
+            }
+            if (pass == 0) mean = __shfl_sync(0xFFFFFFFFu, __ddiv_rn(acc, (double)n), 0);
+            else if (lane == 0) {
+                stat[0] = mean;
+                stat[1] = (double)__double2float_rn(__dadd_rn(__dsqrt_rn(__ddiv_rn(acc, (double)n)), 1e-12));
+            }
+        }
+    }
+    __syncthreads();
+    const double mean = stat[0], sd = stat[1];
+    const float lw = zp[2 * blockIdx.x], nkp = zp[2 * blockIdx.x + 1];
+    for (uint64_t i = threadIdx.x; i < n; i += BM_THREADS)
+        x[i] = __fadd_rn(__double2float_rn(__ddiv_rn(__dsub_rn((double)x[i], mean), sd)), __fmul_rn(lw, __fdiv_rn(cnt[i], nkp)));
 }
 
 inline unsigned bm_grid(uint64_t n) { return (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((n + BM_THREADS - 1) / BM_THREADS, 65535ull * 4)); }
@@ -373,14 +528,21 @@ using namespace yb;
 struct yams_b200_bm25 {
     DeviceCtx* dev = nullptr;
     yams_bm25_config cfg{};
-    uint64_t n = 0, total_tokens = 0, pruned = 0;
-    // The fields and the idf table are shared with the index's Atire views (yams_b200_bm25_atire_view), which read the word
-    // field and the table in place; whichever handle goes last frees them.  Nothing writes them after the build.
-    std::shared_ptr<Bm25Field> f[2] = {std::make_shared<Bm25Field>(), std::make_shared<Bm25Field>()};
+    uint64_t n = 0, total_tokens = 0, pruned = 0, aux_pruned = 0;
+    uint32_t lead = 0;        // the lead-text field's token count (0: no lead field)
+    bool aux_active = false;  // some document's lead text is non-empty: the reference's aux field exists for all n documents
+    // Fields 0 words, 1 n-grams, 2 lead-text words, 3 lead-text n-grams.  The fields and the idf table are shared with the
+    // index's Atire views (yams_b200_bm25_atire_view), which read the word fields and the table in place; whichever handle goes
+    // last frees them.  Nothing writes them after the build.
+    std::shared_ptr<Bm25Field> f[4] = {std::make_shared<Bm25Field>(), std::make_shared<Bm25Field>(), std::make_shared<Bm25Field>(),
+                                       std::make_shared<Bm25Field>()};
     std::shared_ptr<DevBuf> idf = std::make_shared<DevBuf>();   // n + 1 floats: idf of df = 0..n
     cudaStream_t st = nullptr;
     cudaEvent_t ev[2] = {nullptr, nullptr};
     DevBuf raw, legs, qoff, dense, sel, seln;   // score workspace
+    DevBuf counts, route, zrow, zp;             // strategy workspace: keyphrase matches, route profiles, z-score rows
+    cudaEvent_t zev[2] = {nullptr, nullptr};
+    yams_bm25_strategy_stats sstats{};
     DevBuf fused, keys, keys2, cnt, base;       // RRF workspace (the call runs on its first variant's)
     CubTmp tmp;
     float ms[8] = {0, 0, 0, 0, 0, 0, 0, 0};
@@ -388,6 +550,8 @@ struct yams_b200_bm25 {
     ~yams_b200_bm25() {
         if (st) cudaStreamSynchronize(st);
         for (auto& e : ev)
+            if (e) cudaEventDestroy(e);
+        for (auto& e : zev)
             if (e) cudaEventDestroy(e);
         if (st) cudaStreamDestroy(st);
     }
@@ -445,7 +609,7 @@ static yams_status_t timed(H* x, float* acc, F&& fn) {
 // postings (hash, document << 32 | tf) of one field, slices appended in document order -> the field's dictionary and lists.
 // N-grams over the df limit are dropped first (finalize_ngram_field).
 static yams_status_t finish_field(yams_b200_bm25* x, Bm25Field& F, DevBuf& ph, DevBuf& pv, uint64_t np, bool merge, bool prune,
-                                  CubTmp& tmp) {
+                                  uint64_t* pruned, CubTmp& tmp) {
     cudaStream_t st = x->st;
     yams_status_t rc;
     DevBuf ph2, pv2, starts, cnt;
@@ -480,9 +644,9 @@ static yams_status_t finish_field(yams_b200_bm25* x, Bm25Field& F, DevBuf& ph, D
         std::swap(ph, ph2);
         std::swap(pv, pv2);
         np = kept;
-        x->pruned = nterms;   // minus the terms left, below
+        *pruned = nterms;   // minus the terms left, below
     }
-    if (prune && x->pruned) x->pruned -= F.terms;
+    if (prune && *pruned) *pruned -= F.terms;
     if ((rc = F.docs.reserve(std::max<uint64_t>(np, 1) * 4)) != YAMS_OK || (rc = F.tfs.reserve(std::max<uint64_t>(np, 1) * 4)) != YAMS_OK)
         return rc;
     if (np) bm_unpack_kernel<<<bm_grid(np), BM_THREADS, 0, st>>>(pv.as<uint64_t>(), np, F.docs.as<uint32_t>(), F.tfs.as<uint32_t>());
@@ -541,41 +705,39 @@ static yams_status_t upload_texts(const char* const* texts, const size_t* lens, 
     return r;
 }
 
-static yams_status_t bm25_build(yams_b200_bm25* x, const char* const* texts, const size_t* lens) {
-    const double t0 = wall_ms();
+// The word field fw and the n-gram field fw + 1 of the texts laid out in `text` (upload_texts): per-document lengths and
+// averages, then the slices' pairs, sorts and runs, then each field's dictionary.  *pruned gets the n-grams the df rule drops,
+// *nslices the document slices.  The last pass frees the text before the dictionaries, the build's most memory-hungry stage.
+static yams_status_t build_fields(yams_b200_bm25* x, DevBuf& text, const DevBuf& d_pos, const std::vector<uint64_t>& pos, int fw,
+                                  uint64_t* pruned, uint64_t* nslices_out, bool last) {
     cudaStream_t st = x->st;
     const uint64_t n = x->n;
     const bool sab = x->cfg.variant == YAMS_BM25_SUBWORD_AWARE_BACKOFF;
     const uint32_t kmin = x->cfg.ngram_min, kmax = x->cfg.ngram_max;
     const uint64_t h0 = gram_hash_h0(x->cfg.hash_seed);
+    Bm25Field* fs[2] = {x->f[fw].get(), x->f[fw + 1].get()};
     yams_status_t rc;
-    std::vector<uint64_t> pos;
-    DevBuf text, d_pos;
-    for (auto& pf : x->f) {
-        Bm25Field& F = *pf;
-        if ((rc = F.dl.reserve(std::max<uint64_t>(n, 1) * 4)) != YAMS_OK) return rc;
-        YB_CUDA(cudaMemsetAsync(F.dl.p, 0, std::max<uint64_t>(n, 1) * 4, st));
-        F.h_dl.assign(n, 0);
+    for (Bm25Field* pf : fs) {
+        if ((rc = pf->dl.reserve(std::max<uint64_t>(n, 1) * 4)) != YAMS_OK) return rc;
+        YB_CUDA(cudaMemsetAsync(pf->dl.p, 0, std::max<uint64_t>(n, 1) * 4, st));
+        pf->h_dl.assign(n, 0);
     }
-    rc = timed(x, &x->ms[0], [&] { return upload_texts(texts, lens, n, pos, text, d_pos, st); });
-    if (rc != YAMS_OK) return rc;
     const uint64_t L = pos[n];
     // ---- dl / ngram_dl ----
     rc = timed(x, &x->ms[1], [&]() -> yams_status_t {
         if (L) bm_doc_counts_kernel<<<bm_grid(L), BM_THREADS, 0, st>>>(text.as<uint8_t>(), L, d_pos.as<uint64_t>(), n, sab, kmin, kmax,
-                                                                       x->f[0]->dl.as<uint32_t>(), x->f[1]->dl.as<uint32_t>());
+                                                                       fs[0]->dl.as<uint32_t>(), fs[1]->dl.as<uint32_t>());
         YB_CUDA(cudaGetLastError());
-        for (auto& pf : x->f)
+        for (Bm25Field* pf : fs)
             if (n) YB_CUDA(cudaMemcpyAsync(pf->h_dl.data(), pf->dl.p, n * 4, cudaMemcpyDeviceToHost, st));
         return YAMS_OK;
     });
     if (rc != YAMS_OK) return rc;
-    uint64_t sums[2] = {0, 0};
-    for (int fi = 0; fi < 2; ++fi) {
-        for (uint32_t v : x->f[fi]->h_dl) sums[fi] += v;
-        x->f[fi]->avg = n == 0 ? 0.0f : (float)((double)sums[fi] / (double)n);   // finalize_word_field (bm25.cpp:668-676)
+    for (Bm25Field* pf : fs) {
+        pf->sum = 0;
+        for (uint32_t v : pf->h_dl) pf->sum += v;
+        pf->avg = n == 0 ? 0.0f : (float)((double)pf->sum / (double)n);   // finalize_word_field (bm25.cpp:668-676)
     }
-    x->total_tokens = sums[0];
     // ---- document slices: pairs of one slice (words + n-grams) within what the device can hold ----
     size_t free_b = 0, total_b = 0;
     YB_CUDA(cudaMemGetInfo(&free_b, &total_b));
@@ -589,7 +751,7 @@ static yams_status_t bm25_build(yams_b200_bm25* x, const char* const* texts, con
     std::vector<uint64_t> cuts{0};
     uint64_t acc = 0;
     for (uint64_t d = 0; d < n; ++d) {
-        const uint64_t c = (uint64_t)x->f[0]->h_dl[d] + (sab ? (uint64_t)x->f[1]->h_dl[d] : 0);
+        const uint64_t c = (uint64_t)fs[0]->h_dl[d] + (sab ? (uint64_t)fs[1]->h_dl[d] : 0);
         if (acc && acc + c > budget) { cuts.push_back(d); acc = 0; }
         acc += c;
     }
@@ -652,13 +814,53 @@ static yams_status_t bm25_build(yams_b200_bm25* x, const char* const* texts, con
         rc = timed(x, &x->ms[3], [&] { return pair_runs(tmp, ghash, gdoc, ng, ph[1], pv[1], &np[1], st); });
         if (rc != YAMS_OK) return rc;
     }
-    text = DevBuf();
+    if (last) text = DevBuf();
     for (int fi = 0; fi < (sab ? 2 : 1); ++fi) {
         rc = timed(x, &x->ms[3], [&] {
-            return finish_field(x, *x->f[fi], ph[fi], pv[fi], np[fi], nslices > 1, fi == 1 && x->cfg.ngram_df_prune_ratio > 0.0f && n > 0, tmp);
+            return finish_field(x, *fs[fi], ph[fi], pv[fi], np[fi], nslices > 1, fi == 1 && x->cfg.ngram_df_prune_ratio > 0.0f && n > 0,
+                                pruned, tmp);
         });
         if (rc != YAMS_OK) return rc;
     }
+    *nslices_out = nslices;
+    return YAMS_OK;
+}
+
+// Bm25Index::add_doc(text, aux) for every document, then finalize(): the body's fields, then, with a lead length, the same
+// pipeline over the texts cut to their lead prefixes (bytes past the cut zeroed, so they separate words) for the aux fields.
+// An inactive aux field has no words, hence no terms (nothing of it is read) and zero lengths, as the reference's.  The aux
+// fields have the body's document count whenever they are active, so they share its idf table (which depends on n alone).
+static yams_status_t bm25_build(yams_b200_bm25* x, const char* const* texts, const size_t* lens) {
+    const double t0 = wall_ms();
+    cudaStream_t st = x->st;
+    const uint64_t n = x->n;
+    yams_status_t rc;
+    std::vector<uint64_t> pos;
+    DevBuf text, d_pos;
+    rc = timed(x, &x->ms[0], [&] { return upload_texts(texts, lens, n, pos, text, d_pos, st); });
+    if (rc != YAMS_OK) return rc;
+    uint64_t slices = 0, aux_slices = 0;
+    if ((rc = build_fields(x, text, d_pos, pos, 0, &x->pruned, &slices, !(x->lead && n))) != YAMS_OK) return rc;
+    x->total_tokens = x->f[0]->sum;
+    for (int fi = 2; fi < 4; ++fi) x->f[fi]->h_dl.assign(n, 0);
+    if (x->lead && n) {
+        DevBuf flag;
+        uint32_t active = 0;
+        rc = timed(x, &x->ms[1], [&]() -> yams_status_t {
+            yams_status_t r;
+            if ((r = flag.reserve(4)) != YAMS_OK) return r;
+            YB_CUDA(cudaMemsetAsync(flag.p, 0, 4, st));
+            bm_lead_cut_kernel<<<(unsigned)std::min<uint64_t>((n + 7) / 8, 65535ull * 4), BM_THREADS, 0, st>>>(
+                text.as<uint8_t>(), d_pos.as<uint64_t>(), n, x->lead, flag.as<uint32_t>());
+            YB_CUDA(cudaGetLastError());
+            YB_CUDA(cudaMemcpyAsync(&active, flag.p, 4, cudaMemcpyDeviceToHost, st));
+            return YAMS_OK;
+        });
+        if (rc != YAMS_OK) return rc;
+        x->aux_active = active != 0;
+        if (x->aux_active && (rc = build_fields(x, text, d_pos, pos, 2, &x->aux_pruned, &aux_slices, true)) != YAMS_OK) return rc;
+    }
+    text = DevBuf();
     // ---- idf of df = 0..n: the reference's float expression and std::log(float) (bm25.cpp:680-682, 729-731) ----
     std::vector<float> idf(n + 1);
     const float nf = (float)n;
@@ -670,7 +872,7 @@ static yams_status_t bm25_build(yams_b200_bm25* x, const char* const* texts, con
     YB_CUDA(cudaMemcpyAsync(x->idf->p, idf.data(), (n + 1) * 4, cudaMemcpyHostToDevice, st));
     YB_CUDA(cudaStreamSynchronize(st));
     x->ms[4] = (float)(wall_ms() - t0);
-    x->ms[5] = (float)nslices;
+    x->ms[5] = (float)(slices + aux_slices);
     return YAMS_OK;
 }
 
@@ -722,33 +924,82 @@ static ConceptDict concept_dict(const yams_b200_concepts* c, float weight) {
     return ConceptDict{Dict{c->hashes.as<uint64_t>(), c->offs.as<uint64_t>(), c->size}, c->pmi.as<float>(), c->idf.as<float>(), weight};
 }
 
-// The legs of queries [0, nq), in the reference's order, appended to raw: the BM25 legs of index x (nullable: none), then, with a
-// concept index c, the concepts each query matches in blend_into's order.  qoff[q] .. qoff[q + 1] are query q's (absolute).
-static void query_legs(const yams_b200_bm25* x, const yams_b200_concepts* c, const char* const* queries, const size_t* qlens,
-                       uint32_t nq, std::vector<RawLeg>& raw, uint64_t* qoff) {
-    const bool sab = x && x->cfg.variant == YAMS_BM25_SUBWORD_AWARE_BACKOFF;
-    const uint64_t h0 = x ? gram_hash_h0(x->cfg.hash_seed) : 0;
+// The end of the lead prefix of p[0, len): the whitespace byte that ends its lead-th token, else len (extract_lead_tokens,
+// corpus_adapter.cpp:16-39).  The prefix's words are the lead text's: the reference only turns whitespace into ' ' and trims.
+static size_t lead_cut(const uint8_t* p, size_t len, uint32_t lead) {
+    uint32_t tokens = 0;
+    bool in_token = false;
+    for (size_t i = 0; i < len; ++i) {
+        if (is_space(p[i])) {
+            if (in_token) { ++tokens; in_token = false; }
+            if (tokens >= lead) return i;
+        } else {
+            in_token = true;
+        }
+    }
+    return len;
+}
+
+// The BM25 legs of the words of p[0, len) over fields fw (words) and fw + 1 (n-grams), in Bm25Index::score's order
+struct WordLegs {
+    const yams_b200_bm25* x;
     std::vector<std::pair<size_t, size_t>> ws;
     std::vector<uint8_t> low;
     std::unordered_set<uint64_t> seen;
-    std::vector<uint64_t> corder;
-    qoff[0] = raw.size();
-    for (uint32_t q = 0; q < nq; ++q) {
-        const uint8_t* p = reinterpret_cast<const uint8_t*>(queries[q]);
-        if (x) query_words(p, qlens[q], ws); else ws.clear();
+    void operator()(const uint8_t* p, size_t len, uint32_t fw, std::vector<RawLeg>& raw) {
+        const bool sab = x->cfg.variant == YAMS_BM25_SUBWORD_AWARE_BACKOFF;
+        const uint64_t h0 = gram_hash_h0(x->cfg.hash_seed);
+        query_words(p, len, ws);
         for (const auto& [s, l] : ws) {
             low.resize(l);
             for (size_t i = 0; i < l; ++i) low[i] = ascii_lower(p[s + i]);
             const uint64_t th = gram_hash(low.data(), l, h0);
-            raw.push_back({th, th, 0, 0});
+            raw.push_back({th, th, fw, 0});
             if (!sab) continue;
             // collect_unique_query_ngrams (bm25.cpp:151-161): k ascending, position ascending, first occurrence of each hash
             seen.clear();
             for (uint64_t kk = x->cfg.ngram_min; kk <= x->cfg.ngram_max && kk <= l; ++kk)
                 for (uint64_t i = 0; i + kk <= l; ++i) {
                     const uint64_t gh = gram_hash(low.data() + i, kk, h0);
-                    if (seen.insert(gh).second) raw.push_back({gh, th, 1, 0});
+                    if (seen.insert(gh).second) raw.push_back({gh, th, fw + 1, 0});
                 }
+        }
+    }
+};
+
+// The lexical backend's strategies over its primary index (SimeonLexicalBackend, simeon_lexical_backend.cpp:563-580): Bm25Strategy
+// scores score_bm25f(q, lead(q, 64), 0.85, 0.15), or score(q) when that lead text is empty; LeadFieldStrategy scores
+// score_bm25f(q, q, 0.85, 0.15) (retrieval_strategy.cpp:84-127).
+constexpr uint32_t STRATEGY_LEAD = 64;
+constexpr float STRATEGY_WB = 0.85f, STRATEGY_WA = 0.15f;
+
+// The legs of queries [0, nq), in the reference's order, appended to raw: the BM25 legs of index x (nullable: none) -- with
+// strategy >= 0, score_bm25f's: the body's, the body scale, the aux query's over the aux fields -- then, with a concept index c,
+// the concepts each query matches in blend_into's order.  qoff[q] .. qoff[q + 1] are query q's (absolute).
+static void query_legs(const yams_b200_bm25* x, const yams_b200_concepts* c, const char* const* queries, const size_t* qlens,
+                       uint32_t nq, std::vector<RawLeg>& raw, uint64_t* qoff, int strategy = -1) {
+    WordLegs word_legs{x, {}, {}, {}};
+    std::vector<std::pair<size_t, size_t>> ws;
+    std::vector<uint64_t> corder;
+    uint32_t wb_bits;
+    memcpy(&wb_bits, &STRATEGY_WB, 4);
+    qoff[0] = raw.size();
+    for (uint32_t q = 0; q < nq; ++q) {
+        const uint8_t* p = reinterpret_cast<const uint8_t*>(queries[q]);
+        if (x) word_legs(p, qlens[q], 0, raw);
+        if (x && strategy >= 0) {
+            // the aux query: the query's lead prefix (Bm25Strategy) or the query (LeadFieldStrategy)
+            size_t aux_len = qlens[q];
+            if (strategy == YAMS_BM25_STRATEGY_BM25) {
+                aux_len = lead_cut(p, qlens[q], STRATEGY_LEAD);
+                bool empty = true;
+                for (size_t i = 0; i < aux_len && empty; ++i) empty = is_space(p[i]);
+                if (empty) aux_len = SIZE_MAX;   // no evidence: Bm25Index::score alone
+            }
+            if (aux_len != SIZE_MAX) {
+                raw.push_back({0, 0, BM_SCALE, wb_bits});   // weight_body != 1 (bm25.cpp:993-996)
+                word_legs(p, aux_len, BM_AUX, raw);
+            }
         }
         if (c) {
             concept_order(c, p, qlens[q], ws, corder);
@@ -762,20 +1013,20 @@ static void query_legs(const yams_b200_bm25* x, const yams_b200_concepts* c, con
 static yams_status_t plan_legs(const yams_b200_bm25* x, const yams_b200_concepts* c, float weight, const RawLeg* raw, uint64_t nlegs,
                                Leg* legs, cudaStream_t st) {
     if (nlegs == 0) return YAMS_OK;
-    const Dict w = x ? Dict{x->f[0]->hashes.as<uint64_t>(), x->f[0]->offs.as<uint64_t>(), x->f[0]->terms} : Dict{};
-    const Dict g = x ? Dict{x->f[1]->hashes.as<uint64_t>(), x->f[1]->offs.as<uint64_t>(), x->f[1]->terms} : Dict{};
+    FieldDicts f{};
+    for (int fi = 0; x && fi < 4; ++fi) f.d[fi] = Dict{x->f[fi]->hashes.as<uint64_t>(), x->f[fi]->offs.as<uint64_t>(), x->f[fi]->terms};
     const ConceptDict cd = c ? concept_dict(c, weight) : ConceptDict{};
-    bm_plan_kernel<<<bm_grid(nlegs), BM_THREADS, 0, st>>>(raw, nlegs, w, g, x ? x->idf->as<float>() : nullptr,
+    bm_plan_kernel<<<bm_grid(nlegs), BM_THREADS, 0, st>>>(raw, nlegs, f, x ? x->idf->as<float>() : nullptr,
                                                           x && x->cfg.variant == YAMS_BM25_SUBWORD_AWARE_BACKOFF,
-                                                          x ? x->cfg.subword_gamma : 0.0f, cd, legs);
+                                                          x ? x->cfg.subword_gamma : 0.0f, STRATEGY_WA, cd, legs);
     YB_CUDA(cudaGetLastError());
     return YAMS_OK;
 }
 
-// the score kernel's arguments of index x's two fields
+// the score kernel's arguments of index x's four fields
 static ScoreArgs bm25_args(const yams_b200_bm25* x) {
     ScoreArgs a{};
-    for (int fi = 0; fi < 2; ++fi) {
+    for (int fi = 0; fi < 4; ++fi) {
         a.docs[fi] = x->f[fi]->docs.as<uint32_t>();
         a.tfs[fi] = x->f[fi]->tfs.as<uint32_t>();
         a.dl[fi] = x->f[fi]->dl.as<uint32_t>();
@@ -830,9 +1081,10 @@ static void clear_topk(uint32_t nq, uint32_t k, uint32_t* out_docs, float* out_t
 
 // Bm25Index::score of every query; with a concept index `c` of the same document count, then ConceptIndex::blend_into(query,
 // scores, weight) of each (SimeonLexicalBackend::score).
+// With strategy >= 0, the strategy's score_bm25f replaces Bm25Index::score (the strategy router's pools 0 and 2).
 static yams_status_t bm25_score(yams_b200_bm25* x, const yams_b200_concepts* c, float weight, const char* const* queries,
                                 const size_t* qlens, uint32_t nq, float* out_scores, uint32_t k, uint32_t* out_docs, float* out_topk,
-                                uint32_t* out_counts) {
+                                uint32_t* out_counts, int strategy = -1) {
     const double t0 = wall_ms();
     cudaStream_t st = x->st;
     const uint64_t n = x->n;
@@ -842,7 +1094,7 @@ static yams_status_t bm25_score(yams_b200_bm25* x, const yams_b200_concepts* c, 
     const bool blend = c && c->size && c->n == n;
     std::vector<RawLeg> raw;
     std::vector<uint64_t> qoff(nq + 1, 0);
-    query_legs(x, blend ? c : nullptr, queries, qlens, nq, raw, qoff.data());
+    query_legs(x, blend ? c : nullptr, queries, qlens, nq, raw, qoff.data(), strategy);
     const uint64_t nlegs = raw.size();
     const uint32_t K = std::min<uint64_t>(k, n);
     if ((rc = x->raw.reserve(std::max<uint64_t>(nlegs, 1) * sizeof(RawLeg))) != YAMS_OK) return rc;
@@ -887,6 +1139,270 @@ static yams_status_t bm25_score(yams_b200_bm25* x, const yams_b200_concepts* c, 
     if (rc != YAMS_OK) return rc;
     x->ms[6] = dev_ms;
     x->ms[7] = (float)(wall_ms() - t0);
+    return YAMS_OK;
+}
+
+// ---- the keyphrase strategy and the entropy route (DESIGN.md §4.14) ----
+// extract_keyphrases (retrieval_strategy.cpp:152-186): alphabetic runs (C locale) of >= 2 bytes, lowercased, stopwords dropped,
+// sorted and de-duplicated; each hashed as Bm25Index::hash_term hashes it
+static void keyphrase_hashes(const yams_b200_bm25* x, const uint8_t* p, size_t len, std::vector<uint64_t>& out) {
+    static const std::unordered_set<std::string> stop = {
+        "a", "an", "the", "and", "or", "but", "in", "on", "at", "to", "for", "of", "with", "by", "from", "is", "are", "was", "were",
+        "be", "been", "being", "have", "has", "had", "do", "does", "did", "will", "would", "could", "should", "may", "might", "can",
+        "shall", "this", "that", "these", "those", "it", "its", "they", "them", "we", "us", "he", "she", "his", "her", "their", "our",
+        "my", "your", "not", "no", "nor", "so", "as", "if", "than", "then", "also", "very", "just", "about", "into", "over", "after",
+        "before", "between", "under", "during", "without"};
+    auto alpha = [](uint8_t c) { return (c >= 'A' && c <= 'Z') || (c >= 'a' && c <= 'z'); };
+    std::vector<std::string> kps;
+    for (size_t i = 0; i < len;) {
+        while (i < len && !alpha(p[i])) ++i;
+        const size_t st = i;
+        while (i < len && alpha(p[i])) ++i;
+        if (i - st < 2) continue;
+        std::string w(reinterpret_cast<const char*>(p + st), i - st);
+        for (char& ch : w) ch = (char)ascii_lower((uint8_t)ch);
+        if (!stop.count(w)) kps.push_back(std::move(w));
+    }
+    std::sort(kps.begin(), kps.end());
+    kps.erase(std::unique(kps.begin(), kps.end()), kps.end());
+    const uint64_t h0 = gram_hash_h0(x->cfg.hash_seed);
+    out.clear();
+    for (const auto& w : kps) out.push_back(gram_hash(reinterpret_cast<const uint8_t*>(w.data()), w.size(), h0));
+}
+
+// The route of one row: the backend's bm25_entropy < 0.05f -> pool 0, > 0.50f -> pool 2, else pool 1.  The device's profile
+// (bm_route_kernel) differs from the reference's by the order of the sum and device against glibc log: every term
+// sn * -log(sn) >= 0 is within 8u of the reference's (each log within 1 ulp, one rounding of the product on each side), and
+// each order's rounding is within (count)u of the exact sum, so |S_dev - S_ref| <= S_dev (8u + 2 count u)(1 + 1%) (u = 2^-53).
+// When every value in that interval, divided by count, rounds to a float on one side of both thresholds, the route is certain;
+// otherwise the row is copied back and the backend's loop replayed with std::log.  `margin` widens the entropy's interval.
+static int route_pool(const double* prof, const float* row_dev, uint64_t n, double margin, cudaStream_t st, bool* replayed) {
+    *replayed = false;
+    const double m = prof[0], cnt = prof[1], sum = prof[2];
+    if (!(m > 0.0) || cnt == 0.0) return 0;   // bm25_entropy = 0
+    const double u = 0x1p-53;
+    const double E = sum * (8.0 * u + 2.0 * cnt * u) * 1.01;
+    const double lo = (sum - E) / cnt * (1.0 - 4.0 * u) - margin, hi = (sum + E) / cnt * (1.0 + 4.0 * u) + margin;
+    const double t0 = 0.05f, t1 = 0.50f;
+    if (hi < (double)std::nextafter(0.05f, 0.0f)) return 0;
+    if (lo >= t0 && hi <= t1) return 1;
+    if (lo >= (double)std::nextafter(0.50f, 1.0f)) return 2;
+    *replayed = true;
+    std::vector<float> tmp(n);
+    if (cudaMemcpyAsync(tmp.data(), row_dev, n * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess)
+        return -1;
+    const float top = *std::max_element(tmp.begin(), tmp.end());
+    float e = 0.0f;
+    if (top > 0.0f) {
+        double acc = 0.0, positives = 0.0;
+        for (float v : tmp) {
+            if (v <= 0.0f) continue;
+            const double sn = v / top;
+            if (sn > 0.0) acc += sn * (-std::log(sn));
+            positives += 1.0;
+        }
+        e = positives > 0.0 ? (float)(acc / positives) : 0.0f;
+    }
+    return e < 0.05f ? 0 : e > 0.50f ? 2 : 1;
+}
+
+// raw legs [qoff[j], qoff[j + 1]) of the batch's rows j = 0 .. qb: planned and scored onto rows (init: in place; null: from 0)
+static yams_status_t run_legs(yams_b200_bm25* x, const yams_b200_concepts* c, float weight, const std::vector<RawLeg>& raw,
+                              const std::vector<uint64_t>& qoff, uint32_t qb, bool init, float* rows) {
+    cudaStream_t st = x->st;
+    yams_status_t rc;
+    const uint64_t nlegs = raw.size();
+    if (nlegs == 0) {
+        if (!init) YB_CUDA(cudaMemsetAsync(rows, 0, (uint64_t)qb * x->n * 4, st));
+        return YAMS_OK;
+    }
+    if ((rc = x->raw.reserve(nlegs * sizeof(RawLeg))) != YAMS_OK || (rc = x->legs.reserve(nlegs * sizeof(Leg))) != YAMS_OK ||
+        (rc = x->qoff.reserve((qb + 1) * 8)) != YAMS_OK)
+        return rc;
+    YB_CUDA(cudaMemcpyAsync(x->raw.p, raw.data(), nlegs * sizeof(RawLeg), cudaMemcpyHostToDevice, st));
+    YB_CUDA(cudaMemcpyAsync(x->qoff.p, qoff.data(), (qb + 1) * 8, cudaMemcpyHostToDevice, st));
+    if ((rc = plan_legs(x, c, weight, x->raw.as<RawLeg>(), nlegs, x->legs.as<Leg>(), st)) != YAMS_OK) return rc;
+    ScoreArgs a = bm25_args(x);
+    a.legs = x->legs.as<Leg>();
+    a.qoff = x->qoff.as<uint64_t>();
+    if (c) concept_field(c, a);
+    a.init = init ? rows : nullptr;
+    a.out = rows;
+    bm_score_kernel<<<dim3((unsigned)((x->n + BM_TILE - 1) / BM_TILE), qb), BM_THREADS, 0, st>>>(a);
+    YB_CUDA(cudaGetLastError());
+    YB_CUDA(cudaStreamSynchronize(st));   // raw and qoff are the caller's until here
+    return YAMS_OK;
+}
+
+// The strategy router's KEYPHRASE pool or its ROUTED choice for every query, then ConceptIndex::blend_into.  Per batch: the
+// plain score rows; with ROUTED, each row's profile and pool; the BM25F legs of rows routed to pools 0 and 2 onto their rows; for
+// rows of pool 1 the top-10 (padded with zero scores as simeon::top_k keeps them), the gate, the matches of each gated row's
+// keyphrases and the z-score; the concept legs; the outputs.
+static yams_status_t bm25_score_staged(yams_b200_bm25* x, const yams_b200_concepts* c, float weight, uint32_t strategy,
+                                       const char* const* queries, const size_t* qlens, uint32_t nq, float* out_scores, uint32_t k,
+                                       uint32_t* out_docs, float* out_topk, uint32_t* out_counts, uint32_t* out_chosen) {
+    const double t0 = wall_ms();
+    cudaStream_t st = x->st;
+    const uint64_t n = x->n;
+    yams_status_t rc;
+    const bool blend = c && c->size && c->n == n;
+    const uint32_t K = std::min<uint64_t>(k, n), K10 = (uint32_t)std::min<uint64_t>(10, n);
+    double margin = 0.0;   // YAMS_B200_BM25_ROUTE_MARGIN = w > 0 widens the certified interval by w, read at every call
+    if (const char* e = getenv("YAMS_B200_BM25_ROUTE_MARGIN")) margin = std::max(0.0, strtod(e, nullptr));
+    // per query: its score row and its row of keyphrase matches
+    const uint64_t qb_max = n ? std::max<uint64_t>(1, std::min<uint64_t>({BM_DENSE_BYTES / (n * 8), (uint64_t)nq, 4096})) : 0;
+    x->sstats = yams_bm25_strategy_stats{};
+    clear_topk(nq, k, out_docs, out_topk, out_counts);
+    if (n == 0) {
+        if (out_chosen)
+            for (uint32_t q = 0; q < nq; ++q) out_chosen[q] = strategy == YAMS_BM25_STRATEGY_ROUTED ? 0 : strategy;
+        x->ms[6] = 0.f;
+        x->ms[7] = (float)(wall_ms() - t0);
+        return YAMS_OK;
+    }
+    if ((rc = x->dense.reserve(qb_max * n * 4)) != YAMS_OK || (rc = x->counts.reserve(qb_max * n * 4)) != YAMS_OK ||
+        (rc = x->route.reserve(qb_max * 24)) != YAMS_OK || (rc = x->zrow.reserve(qb_max * 4)) != YAMS_OK ||
+        (rc = x->zp.reserve(qb_max * 8)) != YAMS_OK || (rc = x->sel.reserve(qb_max * std::max<uint32_t>(std::max(K, K10), 1) * sizeof(Cand))) != YAMS_OK ||
+        (rc = x->seln.reserve(qb_max * 4)) != YAMS_OK)
+        return rc;
+    float dev_ms = 0.f;
+    std::vector<Cand> h_sel;
+    std::vector<uint32_t> h_n;
+    std::vector<RawLeg> raw;
+    std::vector<uint64_t> qoff(qb_max + 1), kh, corder;
+    std::vector<double> prof;
+    std::vector<uint32_t> pool(qb_max), zrow;
+    std::vector<float> zp;
+    std::vector<std::pair<size_t, size_t>> ws;
+    WordLegs word_legs{x, {}, {}, {}};
+    uint32_t wb_bits;
+    memcpy(&wb_bits, &STRATEGY_WB, 4);
+    rc = timed(x, &dev_ms, [&]() -> yams_status_t {
+        yams_status_t r;
+        float* rows = x->dense.as<float>();
+        for (uint32_t q0 = 0; q0 < nq; q0 += (uint32_t)qb_max) {
+            const uint32_t qb = (uint32_t)std::min<uint64_t>(qb_max, nq - q0);
+            auto qp = [&](uint32_t j) { return reinterpret_cast<const uint8_t*>(queries[q0 + j]); };
+            // the plain scores
+            raw.clear();
+            for (uint32_t j = 0; j < qb; ++j) { qoff[j] = raw.size(); word_legs(qp(j), qlens[q0 + j], 0, raw); }
+            qoff[qb] = raw.size();
+            if ((r = run_legs(x, nullptr, 0.0f, raw, qoff, qb, false, rows)) != YAMS_OK) return r;
+            // the pools
+            for (uint32_t j = 0; j < qb; ++j) pool[j] = strategy;
+            if (strategy == YAMS_BM25_STRATEGY_ROUTED) {
+                prof.resize((uint64_t)qb * 3);
+                bm_route_kernel<<<qb, BM_THREADS, 0, st>>>(rows, n, x->route.as<double>());
+                YB_CUDA(cudaGetLastError());
+                YB_CUDA(cudaMemcpyAsync(prof.data(), x->route.p, (uint64_t)qb * 24, cudaMemcpyDeviceToHost, st));
+                YB_CUDA(cudaStreamSynchronize(st));
+                for (uint32_t j = 0; j < qb; ++j) {
+                    bool rep = false;
+                    const int p = route_pool(prof.data() + 3 * j, rows + (uint64_t)j * n, n, margin, st, &rep);
+                    if (p < 0) { set_last_error("route replay copy failed"); return YAMS_ERR_INTERNAL; }
+                    pool[j] = (uint32_t)p;
+                    x->sstats.replayed += rep;
+                }
+            }
+            // pools 0 and 2: score_bm25f's body scale and aux legs onto the plain rows
+            raw.clear();
+            bool kp = false;
+            for (uint32_t j = 0; j < qb; ++j) {
+                qoff[j] = raw.size();
+                ++x->sstats.queries[pool[j]];
+                if (pool[j] == 1) { kp = true; continue; }
+                size_t aux_len = qlens[q0 + j];
+                if (pool[j] == YAMS_BM25_STRATEGY_BM25) {
+                    aux_len = lead_cut(qp(j), qlens[q0 + j], STRATEGY_LEAD);
+                    bool empty = true;
+                    for (size_t i = 0; i < aux_len && empty; ++i) empty = is_space(qp(j)[i]);
+                    if (empty) continue;
+                }
+                raw.push_back({0, 0, BM_SCALE, wb_bits});
+                word_legs(qp(j), aux_len, BM_AUX, raw);
+            }
+            qoff[qb] = raw.size();
+            if (!raw.empty() && (r = run_legs(x, nullptr, 0.0f, raw, qoff, qb, true, rows)) != YAMS_OK) return r;
+            // pool 1: the entropy gate over the top-10 with its zeros, the matches, the z-score
+            if (kp) {
+                launch_topk_dense(rows, n, qb, K10, x->sel.as<Cand>(), x->seln.as<uint32_t>(), st);
+                YB_CUDA(cudaGetLastError());
+                h_sel.resize((uint64_t)qb * K10);
+                h_n.resize(qb);
+                YB_CUDA(cudaMemcpyAsync(h_sel.data(), x->sel.p, (uint64_t)qb * K10 * sizeof(Cand), cudaMemcpyDeviceToHost, st));
+                YB_CUDA(cudaMemcpyAsync(h_n.data(), x->seln.p, (uint64_t)qb * 4, cudaMemcpyDeviceToHost, st));
+                YB_CUDA(cudaStreamSynchronize(st));
+                raw.clear();
+                zrow.clear();
+                zp.clear();
+                for (uint32_t j = 0; j < qb; ++j) {
+                    qoff[j] = raw.size();
+                    if (pool[j] != 1) continue;
+                    // simeon::top_k(scores, 10): the positives best first, then zeros (every other score is 0)
+                    double vals[10];
+                    uint32_t m = 0;
+                    for (; m < std::min(h_n[j], K10) && h_sel[(uint64_t)j * K10 + m].score > 0.0f; ++m)
+                        vals[m] = (double)h_sel[(uint64_t)j * K10 + m].score;
+                    for (; m < K10; ++m) vals[m] = 0.0;
+                    double ent = 0.0;
+                    if (K10 >= 2) {
+                        double sum_exp = 0.0;
+                        for (uint32_t i = 0; i < K10; ++i) sum_exp += std::exp(vals[i]);
+                        for (uint32_t i = 0; i < K10; ++i) {
+                            const double pr = std::exp(vals[i]) / sum_exp;
+                            if (pr > 1e-12) ent -= pr * std::log(pr);
+                        }
+                        ent /= std::log((double)K10);
+                    }
+                    const float entropy = (float)ent;
+                    if (entropy < 0.30f) continue;
+                    keyphrase_hashes(x, qp(j), qlens[q0 + j], kh);
+                    if (kh.empty()) continue;
+                    for (uint64_t h : kh) raw.push_back({h, h, 0, BM_PRESENCE});
+                    const float lam = 1.0f / (1.0f + std::exp(-(entropy - 0.48f) * 8.0f));
+                    zrow.push_back(j);
+                    zp.push_back(lam * 0.25f);
+                    zp.push_back((float)kh.size());
+                }
+                qoff[qb] = raw.size();
+                if (!zrow.empty()) {
+                    x->sstats.keyphrase_boosted += (uint32_t)zrow.size();
+                    if ((r = run_legs(x, nullptr, 0.0f, raw, qoff, qb, false, x->counts.as<float>())) != YAMS_OK) return r;
+                    YB_CUDA(cudaMemcpyAsync(x->zrow.p, zrow.data(), zrow.size() * 4, cudaMemcpyHostToDevice, st));
+                    YB_CUDA(cudaMemcpyAsync(x->zp.p, zp.data(), zp.size() * 4, cudaMemcpyHostToDevice, st));
+                    YB_CUDA(cudaEventRecord(x->zev[0], st));
+                    bm_zscore_kernel<<<(unsigned)zrow.size(), BM_THREADS, 0, st>>>(rows, x->counts.as<float>(), n, x->zrow.as<uint32_t>(),
+                                                                                   x->zp.as<float>());
+                    YB_CUDA(cudaGetLastError());
+                    YB_CUDA(cudaEventRecord(x->zev[1], st));
+                    YB_CUDA(cudaEventSynchronize(x->zev[1]));
+                    float zms = 0.f;
+                    YB_CUDA(cudaEventElapsedTime(&zms, x->zev[0], x->zev[1]));
+                    x->sstats.zscore_ms += zms;
+                }
+            }
+            // the concept blend onto the strategies' rows
+            if (blend) {
+                raw.clear();
+                for (uint32_t j = 0; j < qb; ++j) {
+                    qoff[j] = raw.size();
+                    concept_order(c, qp(j), qlens[q0 + j], ws, corder);
+                    for (uint64_t bh : corder) raw.push_back({bh, bh, BM_CONCEPT, 0});
+                }
+                qoff[qb] = raw.size();
+                if (!raw.empty() && (r = run_legs(x, c, weight, raw, qoff, qb, true, rows)) != YAMS_OK) return r;
+            }
+            if (out_chosen)
+                for (uint32_t j = 0; j < qb; ++j) out_chosen[q0 + j] = pool[j];
+            if ((r = emit_batch(x, rows, n, q0, qb, nq, K, k, out_scores, out_docs, out_topk, out_counts, h_sel, h_n)) != YAMS_OK) return r;
+        }
+        return YAMS_OK;
+    });
+    if (rc != YAMS_OK) return rc;
+    x->ms[6] = dev_ms;
+    x->ms[7] = (float)(wall_ms() - t0);
+    x->sstats.device_ms = dev_ms;
+    x->sstats.wall_ms = x->ms[7];
     return YAMS_OK;
 }
 
@@ -1459,6 +1975,11 @@ void yams_b200_bm25_default_config(yams_bm25_config* cfg) {
 
 yams_status_t yams_b200_bm25_build(void* self, const yams_bm25_config* cfg_in, const char* const* texts, const size_t* lens,
                                    uint64_t n_docs, yams_b200_bm25** out) {
+    return yams_b200_bm25_build_lead(self, cfg_in, texts, lens, n_docs, 0, out);
+}
+
+yams_status_t yams_b200_bm25_build_lead(void* self, const yams_bm25_config* cfg_in, const char* const* texts, const size_t* lens,
+                                        uint64_t n_docs, uint32_t lead_tokens, yams_b200_bm25** out) {
     YB_TRY
     (void)self;
     DeviceCtx* dev = nullptr;
@@ -1481,8 +2002,10 @@ yams_status_t yams_b200_bm25_build(void* self, const yams_bm25_config* cfg_in, c
     x->dev = dev;
     x->cfg = cfg;
     x->n = n_docs;
+    x->lead = lead_tokens;
     YB_CUDA(cudaStreamCreateWithFlags(&x->st, cudaStreamNonBlocking));
     for (auto& e : x->ev) YB_CUDA(cudaEventCreate(&e));
+    for (auto& e : x->zev) YB_CUDA(cudaEventCreate(&e));
     if ((rc = bm25_build(x.get(), texts, lens)) != YAMS_OK) return rc;
     *out = x.release();
     return YAMS_OK;
@@ -1524,6 +2047,23 @@ yams_status_t yams_b200_bm25_stats(yams_b200_bm25* idx, yams_bm25_stats* out) {
     return YAMS_OK;
 }
 
+yams_status_t yams_b200_bm25_aux_stats(yams_b200_bm25* idx, yams_bm25_stats* out) {
+    DeviceCtx* dev = nullptr;
+    yams_status_t rc = ensure_device(&dev);
+    if (rc != YAMS_OK) return rc;
+    YB_ARG(idx && out, "null argument");
+    out->n_docs = idx->aux_active ? idx->n : 0;
+    out->avg_dl = idx->f[2]->avg;
+    out->ngram_avg_dl = idx->f[3]->avg;
+    out->total_tokens = idx->f[2]->sum;
+    for (int fi = 0; fi < 2; ++fi) {
+        out->terms[fi] = idx->f[2 + fi]->terms;
+        out->postings[fi] = idx->f[2 + fi]->posts;
+    }
+    out->pruned = idx->aux_pruned;
+    return YAMS_OK;
+}
+
 yams_status_t yams_b200_bm25_postings(yams_b200_bm25* idx, uint32_t field, uint64_t term_hash, uint32_t* out_df, float* out_idf,
                                       uint64_t* out_total_tf, uint32_t* out_docs, uint32_t* out_tfs, uint64_t cap) {
     YB_TRY
@@ -1531,7 +2071,7 @@ yams_status_t yams_b200_bm25_postings(yams_b200_bm25* idx, uint32_t field, uint6
     yams_status_t rc = ensure_device(&dev);
     if (rc != YAMS_OK) return rc;
     YB_ARG(idx && out_df && out_idf && out_total_tf, "null argument");
-    YB_ARG(field < 2, "field must be 0 (words) or 1 (n-grams)");
+    YB_ARG(field < 4, "field must be 0 (words), 1 (n-grams), 2 (lead words) or 3 (lead n-grams)");
     YB_ARG(cap == 0 || (out_docs && out_tfs), "null posting output");
     YB_BIND(idx);
     std::lock_guard<std::mutex> g(idx->mu);
@@ -1569,7 +2109,7 @@ yams_status_t yams_b200_bm25_doc_lengths(yams_b200_bm25* idx, uint32_t field, ui
     yams_status_t rc = ensure_device(&dev);
     if (rc != YAMS_OK) return rc;
     YB_ARG(idx, "index is null");
-    YB_ARG(field < 2, "field must be 0 (words) or 1 (n-grams)");
+    YB_ARG(field < 4, "field must be 0 (words), 1 (n-grams), 2 (lead words) or 3 (lead n-grams)");
     YB_ARG(out || idx->n == 0, "out is null");
     if (idx->n) memcpy(out, idx->f[field]->h_dl.data(), idx->n * 4);
     return YAMS_OK;
@@ -1606,9 +2146,14 @@ yams_status_t yams_b200_bm25_atire_view(yams_b200_bm25* idx, yams_b200_bm25** ou
     v->total_tokens = idx->total_tokens;
     v->f[0] = idx->f[0];
     v->f[1]->h_dl.assign(idx->n, 0);
+    v->f[2] = idx->f[2];   // the lead-text words, as an Atire build with the same lead length would have them
+    v->f[3]->h_dl.assign(idx->n, 0);
+    v->lead = idx->lead;
+    v->aux_active = idx->aux_active;
     v->idf = idx->idf;
     YB_CUDA(cudaStreamCreateWithFlags(&v->st, cudaStreamNonBlocking));
     for (auto& e : v->ev) YB_CUDA(cudaEventCreate(&e));
+    for (auto& e : v->zev) YB_CUDA(cudaEventCreate(&e));
     *out = v.release();
     return YAMS_OK;
     YB_CATCH
@@ -1708,6 +2253,45 @@ yams_status_t yams_b200_bm25_score_blended(yams_b200_bm25* idx, const yams_b200_
     YB_CATCH
 }
 
+yams_status_t yams_b200_bm25_score_strategy(yams_b200_bm25* idx, uint32_t strategy, const yams_b200_concepts* concepts, float weight,
+                                            const char* const* queries, const size_t* qlens, uint32_t nq, float* out_scores, uint32_t k,
+                                            uint32_t* out_docs, float* out_topk_scores, uint32_t* out_counts, uint32_t* out_chosen) {
+    YB_TRY
+    DeviceCtx* dev = nullptr;
+    yams_status_t rc = ensure_device(&dev);
+    if (rc != YAMS_OK) return rc;
+    YB_ARG(idx, "index is null");
+    YB_ARG(strategy <= YAMS_BM25_STRATEGY_ROUTED, "strategy must be 0 (BM25), 1 (KEYPHRASE), 2 (LEAD_FIELD) or 3 (ROUTED)");
+    YB_ARG(k <= TOPK_MAX, "k must be <= 4096");
+    YB_ARG(k == 0 || (out_docs && out_topk_scores && out_counts), "null top-k output");
+    if (nq == 0) return YAMS_OK;
+    YB_ARG(queries && qlens, "null argument");
+    for (uint32_t q = 0; q < nq; ++q) YB_ARG(queries[q] || qlens[q] == 0, "null query");
+    YB_BIND(idx);
+    std::lock_guard<std::mutex> g(idx->mu);
+    if (strategy == YAMS_BM25_STRATEGY_KEYPHRASE || strategy == YAMS_BM25_STRATEGY_ROUTED)
+        return bm25_score_staged(idx, concepts, weight, strategy, queries, qlens, nq, out_scores, k, out_docs, out_topk_scores, out_counts,
+                                 out_chosen);
+    // pools 0 and 2: the body, the scale, the aux legs and the concepts in one pass
+    if ((rc = bm25_score(idx, concepts, weight, queries, qlens, nq, out_scores, k, out_docs, out_topk_scores, out_counts, (int)strategy)) != YAMS_OK)
+        return rc;
+    if (out_chosen)
+        for (uint32_t q = 0; q < nq; ++q) out_chosen[q] = strategy;
+    idx->sstats = yams_bm25_strategy_stats{};
+    idx->sstats.queries[strategy] = nq;
+    idx->sstats.device_ms = idx->ms[6];
+    idx->sstats.wall_ms = idx->ms[7];
+    return YAMS_OK;
+    YB_CATCH
+}
+
+yams_status_t yams_b200_bm25_strategy_stats(yams_b200_bm25* idx, yams_bm25_strategy_stats* out) {
+    YB_ARG(idx && out, "null argument");
+    std::lock_guard<std::mutex> g(idx->mu);
+    *out = idx->sstats;
+    return YAMS_OK;
+}
+
 yams_status_t yams_b200_concepts_blend(yams_b200_concepts* c, const char* query, size_t qlen, float weight, float* inout, uint64_t n) {
     YB_TRY
     DeviceCtx* dev = nullptr;
@@ -1735,7 +2319,7 @@ yams_status_t yams_b200_concepts_blend(yams_b200_concepts* c, const char* query,
         YB_CUDA(cudaMemcpyAsync(c->raw.p, raw.data(), nlegs * sizeof(RawLeg), cudaMemcpyHostToDevice, st));
         YB_CUDA(cudaMemcpyAsync(c->qoff.p, qoff, 16, cudaMemcpyHostToDevice, st));
         YB_CUDA(cudaMemcpyAsync(c->dense.p, inout, n * 4, cudaMemcpyHostToDevice, st));
-        bm_plan_kernel<<<bm_grid(nlegs), BM_THREADS, 0, st>>>(c->raw.as<RawLeg>(), nlegs, Dict{}, Dict{}, nullptr, 0, 0.0f,
+        bm_plan_kernel<<<bm_grid(nlegs), BM_THREADS, 0, st>>>(c->raw.as<RawLeg>(), nlegs, FieldDicts{}, nullptr, 0, 0.0f, 0.0f,
                                                               concept_dict(c, weight), c->legs.as<Leg>());
         ScoreArgs a{};
         a.legs = c->legs.as<Leg>();

@@ -951,7 +951,9 @@ class B200ConceptIndex;
 
 class B200Bm25Index {
 public:
-    explicit B200Bm25Index(const yams_bm25_config* cfg = nullptr) {
+    // lead_tokens > 0: every document also gets extract_lead_tokens(text, lead_tokens) as its aux field, as the lexical backend's
+    // add_doc(text, lead) does with the strategy router on (64); finalize builds both fields in one device build
+    explicit B200Bm25Index(const yams_bm25_config* cfg = nullptr, uint32_t lead_tokens = 0) : lead_(lead_tokens) {
         if (cfg) cfg_ = *cfg; else yams_b200_bm25_default_config(&cfg_);
     }
     ~B200Bm25Index() { yams_b200_bm25_destroy(idx_); }
@@ -967,7 +969,7 @@ public:
         std::vector<const char*> ptrs;
         std::vector<size_t> lens;
         for (const auto& t : texts_) { ptrs.push_back(t.data()); lens.push_back(t.size()); }
-        check(yams_b200_bm25_build(nullptr, &cfg_, ptrs.data(), lens.data(), texts_.size(), &idx_), "build");
+        check(yams_b200_bm25_build_lead(nullptr, &cfg_, ptrs.data(), lens.data(), texts_.size(), lead_, &idx_), "build");
         n_ = texts_.size();
         texts_.clear();
         texts_.shrink_to_fit();
@@ -985,11 +987,21 @@ public:
     // SimeonLexicalBackend::score with its concept index: the BM25 scores, then concepts->blend_into(query, scores, weight), fused
     // on the device (a null or empty concept index, or one of another document count, adds nothing)
     void score(std::string_view query, std::span<float> out_scores, const B200ConceptIndex* concepts, float weight) const;
+    // The strategy router's pool (YAMS_BM25_STRATEGY_BM25 / KEYPHRASE / LEAD_FIELD: Bm25Strategy, KeyphraseStrategy and the
+    // "keyphrase" arm, LeadFieldStrategy and the "lead_field" arm) or its routed choice (YAMS_BM25_STRATEGY_ROUTED:
+    // SimeonLexicalBackend::scoreStrategyRouted), then concepts->blend_into(query, scores, weight), in one device call.  Returns the
+    // pool that scored.
+    uint32_t score_strategy(uint32_t strategy, std::string_view query, std::span<float> out_scores,
+                            const B200ConceptIndex* concepts = nullptr, float weight = 0.0f) const;
+    uint32_t score_strategy_routed(std::string_view query, std::span<float> out_scores, const B200ConceptIndex* concepts = nullptr,
+                                   float weight = 0.0f) const {
+        return score_strategy(YAMS_BM25_STRATEGY_ROUTED, query, out_scores, concepts, weight);
+    }
     // The Atire index SimeonLexicalBackend builds beside a SubwordAwareBackoff primary for RRF (and its router), served from this
     // index's word field without a second build (yams_b200_bm25_atire_view).  The view and this index may go in either order.
     std::unique_ptr<B200Bm25Index> atire_view() const {
         if (!idx_) throw std::runtime_error("Bm25Index::atire_view before finalize()");
-        std::unique_ptr<B200Bm25Index> v(new B200Bm25Index(&cfg_));
+        std::unique_ptr<B200Bm25Index> v(new B200Bm25Index(&cfg_, lead_));
         v->cfg_.variant = YAMS_BM25_ATIRE;
         check(yams_b200_bm25_atire_view(idx_, &v->idx_), "atire_view");
         v->n_ = n_;
@@ -1045,6 +1057,7 @@ private:
         if (st != YAMS_OK) throw std::runtime_error(std::string("yams_b200_bm25 ") + what + ": " + yams_b200_last_error());
     }
     yams_bm25_config cfg_{};
+    uint32_t lead_ = 0;
     std::vector<std::string> texts_;
     yams_b200_bm25* idx_ = nullptr;
     uint64_t n_ = 0;
@@ -1127,6 +1140,19 @@ inline B200ConceptIndex mine_concepts(const B200Bm25Index& idx, std::span<const 
     B200ConceptIndex::check(yams_b200_concepts_mine(idx.handle(), &cfg, ptrs.data(), lens.data(), docs.size(), &out.c_), "mine");
     B200ConceptIndex::check(yams_b200_concepts_stats(out.c_, &out.stats_), "stats");
     return out;
+}
+
+inline uint32_t B200Bm25Index::score_strategy(uint32_t strategy, std::string_view query, std::span<float> out_scores,
+                                              const B200ConceptIndex* concepts, float weight) const {
+    if (!idx_) throw std::runtime_error("Bm25Index::score before finalize()");
+    if (out_scores.size() != n_) throw std::runtime_error("Bm25Index::score out_scores size mismatch");
+    const char* q = query.data();
+    const size_t len = query.size();
+    uint32_t chosen = 0;
+    check(yams_b200_bm25_score_strategy(idx_, strategy, concepts ? concepts->handle() : nullptr, weight, &q, &len, 1, out_scores.data(), 0,
+                                        nullptr, nullptr, nullptr, &chosen),
+          "score_strategy");
+    return chosen;
 }
 
 inline void B200Bm25Index::score(std::string_view query, std::span<float> out_scores, const B200ConceptIndex* concepts, float weight) const {
