@@ -596,8 +596,8 @@ YAMS_B200_API void yams_b200_simeon_destroy(yams_b200_encoder* e);
  *          alpha > 0, and (1 - alpha) * bm25plus over the list of each distinct n-gram of the word still in the index when
  *          alpha < 1.  Every float operation is the reference's, in its order, without fused multiply-adds.
  * Scores are bit-identical to the reference.  The concept blend (ConceptIndex::blend_into) is the concepts block below.  The lead-text
- * aux field and the strategy router are yams_b200_bm25_build_lead and yams_b200_bm25_score_strategy.  Out of scope (the
- * caller's, as today): fragment geometry, the query router, SDM / word bigrams, PRF, and the caller's document windowing (buildEnhancementText).  RRF over variants is
+ * aux field and the strategy router are yams_b200_bm25_build_lead and yams_b200_bm25_score_strategy; the query router is
+ * yams_b200_bm25_score_routed.  Out of scope (the caller's, as today): fragment geometry, SDM / word bigrams, PRF, and the caller's document windowing (buildEnhancementText).  RRF over variants is
  * yams_b200_bm25_score_rrf. */
 #define YAMS_BM25_ATIRE 0                    /* simeon::Bm25Variant::Atire */
 #define YAMS_BM25_SUBWORD_AWARE_BACKOFF 7    /* simeon::Bm25Variant::SubwordAwareBackoff */
@@ -795,6 +795,52 @@ typedef struct yams_bm25_strategy_stats {   /* of the index's last yams_b200_bm2
     float device_ms, wall_ms;     /* the call's device and host wall ms */
 } yams_bm25_strategy_stats;
 YAMS_B200_API yams_status_t yams_b200_bm25_strategy_stats(yams_b200_bm25* idx, yams_bm25_strategy_stats* out);
+
+/* ---- the query router (DESIGN.md §4.15) -------------------------------------------------------------------------
+ * SimeonLexicalBackend::scoreRouted with router_enabled (fragment geometry and RRF off): simeon::QueryRouter::features(query) and
+ * choose(features) over the index's field 0 (query_router.cpp:29-117, 222-238), the chosen index's scores -- Atire for
+ * Bm25Atire (an Atire view of idx, yams_b200_bm25_atire_view), idx for Bm25SabSmooth and CascadeLinearAlpha; every recipe scores
+ * Atire when idx is Atire -- then, with concepts, ConceptIndex::blend_into(query, scores, weight), then the projection onto the
+ * caller's candidate pool.
+ *   features  the query's words (maximal runs of [A-Za-z0-9_]) hashed WITHOUT case folding: a word with an uppercase letter is
+ *             out of vocabulary for the router (df 0) although scoring folds it.  n_terms and avg_term_chars count every
+ *             occurrence; scq_sum adds (1 + log(total_tf)) * idf per present occurrence; simplified_clarity sums, over the distinct
+ *             present hashes in first-occurrence order, p_q * log(p_q / p_c), p_q = occurrences / n_terms (OOV words counted in
+ *             n_terms), p_c = total_tf / total_tokens; idf_stddev is computed only with more than one present occurrence.  Every
+ *             operation is the reference's, in its order, in double with glibc log, and so is the route.
+ *   choose    the pool-based signals keep features()'s no-signal defaults (pool_overlap_jaccard 1, score_decay_rate 0) and are
+ *             compared with atire_max_pool_jaccard and atire_min_score_decay as the reference compares them. */
+#define YAMS_BM25_RECIPE_ATIRE 0              /* simeon::Recipe::Bm25Atire */
+#define YAMS_BM25_RECIPE_SAB_SMOOTH 1         /* simeon::Recipe::Bm25SabSmooth */
+#define YAMS_BM25_RECIPE_CASCADE 2            /* simeon::Recipe::CascadeLinearAlpha */
+typedef struct yams_bm25_router_config {      /* simeon::RouterConfig's routing fields */
+    float oov_threshold, high_idf_threshold;  /* 0, 3 */
+    uint32_t atire_min_terms;                 /* 0 */
+    float atire_min_idf_floor, atire_max_pool_jaccard, atire_min_score_decay, atire_min_scq, atire_max_clarity;   /* 0, 1, 0, 0, 3 */
+    uint32_t cascade_min_terms;               /* 4 */
+    float cascade_max_idf;                    /* 5 */
+} yams_bm25_router_config;
+typedef struct yams_bm25_query_features {     /* the fields simeon::QueryRouter::features fills */
+    float oov_rate, avg_idf, max_idf, min_idf, idf_stddev;
+    uint32_t n_terms;
+    float avg_term_chars, scq_sum, simplified_clarity;
+} yams_bm25_query_features;
+/* the lexical backend's RouterPreset (passE: atire_max_clarity 3) over RouterConfig's defaults */
+YAMS_B200_API void yams_b200_bm25_default_router_config(yams_bm25_router_config* cfg);
+/* The routed scores of nq HOST queries: the outputs, top-k rule, limits, locking and 1 GiB batching of
+ * yams_b200_bm25_score_blended; rows of different recipes share a batch.  out_recipe (nullable): [nq] YAMS_BM25_RECIPE_*;
+ * out_features (nullable): [nq].
+ * Candidate pools (cand_offsets nullable: none): query q's pool is cand_docs[cand_offsets[q] .. cand_offsets[q + 1]) (document
+ * indices; 0xFFFFFFFF = a candidate the index does not hold), cand_offsets[0] = 0, non-decreasing; out_cand_scores[j] =
+ * isfinite(row[d]) ? row[d] : 0, 0 for 0xFFFFFFFF -- gathered on the device, so with out_scores NULL and k = 0 only the pools
+ * cross to the host.  A pool may repeat a document and be longer than n_docs.  A candidate index >= n_docs other than
+ * 0xFFFFFFFF: YAMS_ERR_INVALID_ARG. */
+YAMS_B200_API yams_status_t yams_b200_bm25_score_routed(yams_b200_bm25* idx, const yams_bm25_router_config* rcfg /* NULL = default */,
+                                                        const yams_b200_concepts* concepts, float weight, const char* const* queries,
+                                                        const size_t* qlens, uint32_t nq, float* out_scores, uint32_t k, uint32_t* out_docs,
+                                                        float* out_topk_scores, uint32_t* out_counts, const uint64_t* cand_offsets,
+                                                        const uint32_t* cand_docs, float* out_cand_scores, uint32_t* out_recipe,
+                                                        yams_bm25_query_features* out_features);
 
 /* [0] stage-1 scan ms, [1] rescoring+select ms, [2] total device ms of the last yams_b200_search or
  * yams_b200_search_device on this corpus (the latter's once its work is done); [3] unused (0);

@@ -66,6 +66,29 @@ class Bm25StrategyStats(C.Structure):
                 ("device_ms", C.c_float), ("wall_ms", C.c_float)]
 
 
+class RouterConfig(C.Structure):
+    """yams_bm25_router_config: simeon::RouterConfig's routing fields.  RouterConfig.default(**overrides) starts from the lexical
+    backend's preset (yams_b200_bm25_default_router_config)."""
+    _fields_ = [("oov_threshold", C.c_float), ("high_idf_threshold", C.c_float), ("atire_min_terms", C.c_uint32),
+                ("atire_min_idf_floor", C.c_float), ("atire_max_pool_jaccard", C.c_float), ("atire_min_score_decay", C.c_float),
+                ("atire_min_scq", C.c_float), ("atire_max_clarity", C.c_float), ("cascade_min_terms", C.c_uint32),
+                ("cascade_max_idf", C.c_float)]
+
+    @classmethod
+    def default(cls, **overrides) -> "RouterConfig":
+        cfg = cls()
+        lib().yams_b200_bm25_default_router_config(C.byref(cfg))
+        for k, v in overrides.items():
+            setattr(cfg, k, v)
+        return cfg
+
+
+class QueryFeatures(C.Structure):
+    """yams_bm25_query_features: the fields simeon::QueryRouter::features fills"""
+    _fields_ = [("oov_rate", C.c_float), ("avg_idf", C.c_float), ("max_idf", C.c_float), ("min_idf", C.c_float), ("idf_stddev", C.c_float),
+                ("n_terms", C.c_uint32), ("avg_term_chars", C.c_float), ("scq_sum", C.c_float), ("simplified_clarity", C.c_float)]
+
+
 class ConceptConfig(C.Structure):
     _fields_ = [("min_ttf", C.c_uint32), ("pmi_floor", C.c_float), ("max_concepts", C.c_uint32), ("k1", C.c_float), ("b", C.c_float)]
 
@@ -78,6 +101,9 @@ class ConceptStats(C.Structure):
 BM25_ATIRE, BM25_SUBWORD_AWARE_BACKOFF = 0, 7   # simeon::Bm25Variant numbering
 BM25_STRATEGY_BM25, BM25_STRATEGY_KEYPHRASE, BM25_STRATEGY_LEAD_FIELD = 0, 1, 2   # the strategy router's pool numbers
 BM25_STRATEGY_ROUTED = 3
+BM25_RECIPE_ATIRE, BM25_RECIPE_SAB_SMOOTH, BM25_RECIPE_CASCADE = 0, 1, 2   # simeon::Recipe numbering
+BM25_NOT_INDEXED = 0xFFFFFFFF   # a candidate the index does not hold
+QUERY_FEATURES_DTYPE = np.dtype([(n, "<u4" if t is C.c_uint32 else "<f4") for n, t in QueryFeatures._fields_])
 
 SIMEON_WORD_TOKENS = 1        # NGramMode::CharAndWord
 SIMEON_PROJECTION_FWHT = 2    # ProjectionMode::Fwht (default projection: AchlioptasSparse)
@@ -199,6 +225,10 @@ SYMBOLS = {
     "yams_b200_bm25_strategy_stats": (C.c_int, [C.c_void_p, C.POINTER(Bm25StrategyStats)]),
     "yams_b200_bm25_score_strategy": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_float, C.POINTER(C.c_char_p), C.POINTER(C.c_size_t),
                                                 C.c_uint32, f32p, C.c_uint32, u32p, f32p, u32p, u32p]),
+    "yams_b200_bm25_default_router_config": (None, [C.POINTER(RouterConfig)]),
+    "yams_b200_bm25_score_routed": (C.c_int, [C.c_void_p, C.POINTER(RouterConfig), C.c_void_p, C.c_float, C.POINTER(C.c_char_p),
+                                              C.POINTER(C.c_size_t), C.c_uint32, f32p, C.c_uint32, u32p, f32p, u32p, u64p, u32p, f32p, u32p,
+                                              C.c_void_p]),
     "yams_b200_pq_build": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, f32p, u64p, C.POINTER(C.c_void_p)]),
     "yams_b200_pq_search": (C.c_int, [C.c_void_p, f32p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_float, i64p, f32p, u32p, u64p]),
     "yams_b200_pq_search_candidates": (C.c_int, [C.c_void_p, f32p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_float, i64p, u64p, i64p, f32p,
@@ -879,6 +909,36 @@ class Bm25Index:
                                                                                     else None, weight, *args, chosen.ctypes.data_as(u32p)),
                                                "bm25_score_strategy"), self.n, queries, k, full)
         out["chosen"] = chosen[:nq]
+        return out
+
+    def score_routed(self, queries, k: int = 0, full: bool = True, concepts: Optional["ConceptIndex"] = None, weight: float = 0.5,
+                     router: Optional[RouterConfig] = None, candidates=None):
+        """The lexical backend's scoreRouted with router_enabled (yams_b200_bm25_score_routed): QueryRouter's features and recipe of
+        each query over this index, the recipe's scores (Bm25Atire: as this index's Atire view), then with `concepts`
+        blend_into(query, scores, weight).  The outputs of score, and "recipe" [nq] (BM25_RECIPE_*), "features" [nq]
+        (QUERY_FEATURES_DTYPE); with `candidates` (one sequence of document indices per query, BM25_NOT_INDEXED for a candidate the
+        index does not hold), "candidates": per query the finite score of each candidate, else 0, gathered on the device."""
+        nq = len(queries)
+        recipe = np.zeros(max(nq, 1), np.uint32)
+        feats = np.zeros(max(nq, 1), QUERY_FEATURES_DTYPE)
+        off = flat = proj = None
+        if candidates is not None:
+            assert len(candidates) == nq
+            pools = [np.asarray(c, np.uint32).ravel() for c in candidates]
+            off = np.zeros(nq + 1, np.uint64)
+            off[1:] = np.cumsum([len(c) for c in pools], dtype=np.uint64)
+            flat = np.concatenate(pools + [np.zeros(1, np.uint32)]) if pools else np.zeros(1, np.uint32)
+            proj = np.zeros(max(int(off[-1]), 1), np.float32)
+        rcfg = router if router is not None else RouterConfig.default()
+        out = _score_call(lambda *args: _check(lib().yams_b200_bm25_score_routed(
+            self._h, C.byref(rcfg), concepts._h if concepts is not None else None, weight, *args,
+            off.ctypes.data_as(u64p) if off is not None else None, flat.ctypes.data_as(u32p) if flat is not None else None,
+            proj.ctypes.data_as(f32p) if proj is not None else None, recipe.ctypes.data_as(u32p), feats.ctypes.data), "bm25_score_routed"),
+            self.n, queries, k, full)
+        out["recipe"] = recipe[:nq]
+        out["features"] = feats[:nq]
+        if candidates is not None:
+            out["candidates"] = [proj[int(off[i]):int(off[i + 1])] for i in range(nq)]
         return out
 
     def strategy_stats(self) -> dict:

@@ -34,6 +34,11 @@
 // keyphrase strategy counts matches with presence legs and z-scores a row with one lane's sequential double sums; the route
 // reduces each row's profile on the device with a bound on its distance from the reference's, replaying the row on the host
 // when the bound cannot settle it.
+//
+// Query router (QueryRouter::features / choose, the backend's scoreRouted; DESIGN.md §4.15): one kernel looks up the unfolded
+// query words' field-0 statistics, the host computes the features and the recipe in the reference's order, Bm25Atire rows of a
+// SubwordAwareBackoff index score with BM_ATIRE legs in the same launch as the others, and the candidate pools are gathered from
+// each batch's rows on the device.
 #include <cub/cub.cuh>
 #include <thrust/iterator/counting_iterator.h>
 #include <thrust/iterator/transform_iterator.h>
@@ -42,6 +47,7 @@
 #include <chrono>
 #include <cmath>
 #include <functional>
+#include <limits>
 #include <memory>
 #include <mutex>
 #include <new>
@@ -252,18 +258,21 @@ constexpr uint32_t BM_SCALE = 5;
 // A presence leg (RawLeg / Leg pad of a field-0 leg): adds 1.0f to each document of a keyphrase's word list whose single-term
 // score (score_weighted_hashes with weight 1: bm25plus, or score_atire for Atire) is > 0, counting KeyphraseStrategy's matches.
 constexpr uint32_t BM_PRESENCE = 1;
+// An Atire leg (RawLeg / Leg pad of a word leg of a SubwordAwareBackoff index): scored as an Atire build of the same texts would
+// score it (score_atire over the word's list), so rows of both variants share one launch (the query router's Bm25Atire rows).
+constexpr uint32_t BM_ATIRE = 2;
 
 struct RawLeg {        // one query word (field 0 / 2), one distinct n-gram of it (1 / 3), one matched concept, or a scale
     uint64_t hash;
     uint64_t term_hash;
     uint32_t field;
-    uint32_t pad;      // BM_SCALE: the scale's float bits
+    uint32_t pad;      // BM_SCALE: the scale's float bits; BM_PRESENCE, BM_ATIRE: the leg's kind
 };
 struct Leg {           // an addition over documents docs[b, e) of `field`; empty when b == e
     uint64_t b, e;
     float w, idf;
     uint32_t field;
-    uint32_t pad;      // BM_PRESENCE: a presence leg
+    uint32_t pad;      // BM_PRESENCE: a presence leg; BM_ATIRE: an Atire leg
 };
 struct Dict {
     const uint64_t* hashes;
@@ -310,8 +319,8 @@ __global__ void bm_plan_kernel(const RawLeg* __restrict__ raw, uint64_t nlegs, F
             const Dict& w = f.d[r.field & BM_AUX];
             if (r.pad == BM_PRESENCE) {   // a keyphrase's word list, whatever the variant
                 if (dict_find(w, r.hash, &b, &e)) { L.b = b; L.e = e; L.idf = idf[e - b]; L.pad = BM_PRESENCE; }
-            } else if (!sab) {
-                if (dict_find(w, r.hash, &b, &e)) { L.b = b; L.e = e; L.w = aux ? wa : 0.0f; L.idf = idf[e - b]; }
+            } else if (!sab || r.pad == BM_ATIRE) {
+                if (dict_find(w, r.hash, &b, &e)) { L.b = b; L.e = e; L.w = aux ? wa : 0.0f; L.idf = idf[e - b]; L.pad = r.pad; }
             } else {
                 // alpha = float(df) / (float(df) + gamma), 0 when the word is unknown (bm25.cpp:805-807)
                 const uint64_t df = dict_find(w, r.term_hash, &b, &e) ? e - b : 0;
@@ -375,6 +384,7 @@ __global__ void __launch_bounds__(BM_THREADS) bm_score_kernel(ScoreArgs a) {
         const uint32_t* dlv = a.dl[g.field];
         const float avg = a.avg[g.field], k1 = a.k1[g.field], b = a.b[g.field];
         const float k1p1 = __fadd_rn(k1, 1.0f), omb = __fsub_rn(1.0f, b);
+        const bool sab = a.sab && g.pad != BM_ATIRE;   // this leg's arithmetic
         for (uint64_t i = sb + threadIdx.x; i < se; i += BM_THREADS) {
             const uint32_t d = docs[i];
             const float tf = __uint2float_rn(tfs[i]), dl = __uint2float_rn(dlv[d]);
@@ -386,10 +396,10 @@ __global__ void __launch_bounds__(BM_THREADS) bm_score_kernel(ScoreArgs a) {
             const float plus = __fmul_rn(g.idf, __fadd_rn(__fdiv_rn(__fmul_rn(tf, k1p1), denom), a.delta));
             float add;
             if (g.pad == BM_PRESENCE)    // 1.0f * the single-term score > 0
-                add = (a.sab ? plus : atire) > 0.0f ? 1.0f : 0.0f;
-            else if (g.field == BM_CONCEPT || (!a.sab && g.field == BM_AUX))   // wpmi * score_atire; weight_aux * score_atire
+                add = (sab ? plus : atire) > 0.0f ? 1.0f : 0.0f;
+            else if (g.field == BM_CONCEPT || (!sab && g.field == BM_AUX))   // wpmi * score_atire; weight_aux * score_atire
                 add = __fmul_rn(g.w, atire);
-            else if (a.sab)              // alpha * bm25plus
+            else if (sab)                // alpha * bm25plus
                 add = __fmul_rn(g.w, plus);
             else
                 add = atire;
@@ -483,6 +493,21 @@ __global__ void __launch_bounds__(BM_THREADS) bm_zscore_kernel(float* __restrict
         x[i] = __fadd_rn(__double2float_rn(__ddiv_rn(__dsub_rn((double)x[i], mean), sd)), __fmul_rn(lw, __fdiv_rn(cnt[i], nkp)));
 }
 
+// The query router's projection onto the caller's candidate pools (scoreRouted, simeon_lexical_backend.cpp:920-931): out[j] =
+// the row's score of candidate j if finite, else 0; 0 for a candidate the index does not hold (any index >= n).  Block row y is
+// query q0 + y of the batch; its pool is docs[off[q], off[q + 1]).
+__global__ void __launch_bounds__(BM_THREADS) bm_pool_gather_kernel(const float* __restrict__ rows, uint64_t n, uint32_t q0,
+                                                                    const uint64_t* __restrict__ off, const uint32_t* __restrict__ docs,
+                                                                    float* __restrict__ out) {
+    const uint32_t q = q0 + blockIdx.y;
+    const float* row = rows + (uint64_t)blockIdx.y * n;
+    for (uint64_t j = off[q] + (uint64_t)blockIdx.x * BM_THREADS + threadIdx.x; j < off[q + 1]; j += (uint64_t)gridDim.x * BM_THREADS) {
+        const uint32_t d = docs[j];
+        const float v = d < n ? row[d] : 0.0f;
+        out[j] = isfinite(v) ? v : 0.0f;
+    }
+}
+
 inline unsigned bm_grid(uint64_t n) { return (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((n + BM_THREADS - 1) / BM_THREADS, 65535ull * 4)); }
 
 // cub temp storage in a growable buffer
@@ -544,6 +569,7 @@ struct yams_b200_bm25 {
     cudaEvent_t zev[2] = {nullptr, nullptr};
     yams_bm25_strategy_stats sstats{};
     DevBuf fused, keys, keys2, cnt, base;       // RRF workspace (the call runs on its first variant's)
+    DevBuf rwords, rstats, pool_off, pool_docs, pool_out;   // query-router workspace: word lookups, candidate pools
     CubTmp tmp;
     float ms[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     std::mutex mu;
@@ -940,21 +966,22 @@ static size_t lead_cut(const uint8_t* p, size_t len, uint32_t lead) {
     return len;
 }
 
-// The BM25 legs of the words of p[0, len) over fields fw (words) and fw + 1 (n-grams), in Bm25Index::score's order
+// The BM25 legs of the words of p[0, len) over fields fw (words) and fw + 1 (n-grams), in Bm25Index::score's order; with
+// atire, the legs an Atire build of the same texts would score (words only, as BM_ATIRE legs)
 struct WordLegs {
     const yams_b200_bm25* x;
     std::vector<std::pair<size_t, size_t>> ws;
     std::vector<uint8_t> low;
     std::unordered_set<uint64_t> seen;
-    void operator()(const uint8_t* p, size_t len, uint32_t fw, std::vector<RawLeg>& raw) {
-        const bool sab = x->cfg.variant == YAMS_BM25_SUBWORD_AWARE_BACKOFF;
+    void operator()(const uint8_t* p, size_t len, uint32_t fw, std::vector<RawLeg>& raw, bool atire = false) {
+        const bool sab = x->cfg.variant == YAMS_BM25_SUBWORD_AWARE_BACKOFF && !atire;
         const uint64_t h0 = gram_hash_h0(x->cfg.hash_seed);
         query_words(p, len, ws);
         for (const auto& [s, l] : ws) {
             low.resize(l);
             for (size_t i = 0; i < l; ++i) low[i] = ascii_lower(p[s + i]);
             const uint64_t th = gram_hash(low.data(), l, h0);
-            raw.push_back({th, th, fw, 0});
+            raw.push_back({th, th, fw, atire ? BM_ATIRE : 0u});
             if (!sab) continue;
             // collect_unique_query_ngrams (bm25.cpp:151-161): k ascending, position ascending, first occurrence of each hash
             seen.clear();
@@ -974,10 +1001,11 @@ constexpr uint32_t STRATEGY_LEAD = 64;
 constexpr float STRATEGY_WB = 0.85f, STRATEGY_WA = 0.15f;
 
 // The legs of queries [0, nq), in the reference's order, appended to raw: the BM25 legs of index x (nullable: none) -- with
-// strategy >= 0, score_bm25f's: the body's, the body scale, the aux query's over the aux fields -- then, with a concept index c,
-// the concepts each query matches in blend_into's order.  qoff[q] .. qoff[q + 1] are query q's (absolute).
+// strategy >= 0, score_bm25f's: the body's, the body scale, the aux query's over the aux fields; with atire[q] != 0, an Atire
+// build's -- then, with a concept index c, the concepts each query matches in blend_into's order.  qoff[q] .. qoff[q + 1] are
+// query q's (absolute).
 static void query_legs(const yams_b200_bm25* x, const yams_b200_concepts* c, const char* const* queries, const size_t* qlens,
-                       uint32_t nq, std::vector<RawLeg>& raw, uint64_t* qoff, int strategy = -1) {
+                       uint32_t nq, std::vector<RawLeg>& raw, uint64_t* qoff, int strategy = -1, const uint8_t* atire = nullptr) {
     WordLegs word_legs{x, {}, {}, {}};
     std::vector<std::pair<size_t, size_t>> ws;
     std::vector<uint64_t> corder;
@@ -986,7 +1014,7 @@ static void query_legs(const yams_b200_bm25* x, const yams_b200_concepts* c, con
     qoff[0] = raw.size();
     for (uint32_t q = 0; q < nq; ++q) {
         const uint8_t* p = reinterpret_cast<const uint8_t*>(queries[q]);
-        if (x) word_legs(p, qlens[q], 0, raw);
+        if (x) word_legs(p, qlens[q], 0, raw, atire && atire[q]);
         if (x && strategy >= 0) {
             // the aux query: the query's lead prefix (Bm25Strategy) or the query (LeadFieldStrategy)
             size_t aux_len = qlens[q];
@@ -1079,12 +1107,21 @@ static void clear_topk(uint32_t nq, uint32_t k, uint32_t* out_docs, float* out_t
     for (uint32_t q = 0; q < nq; ++q) out_counts[q] = 0;
 }
 
+// The query router's part of a score call: rows scored as Atire, and the candidate pools projected from the rows
+struct Routed {
+    const uint8_t* atire;        // [nq]: 1 = the row scores as an Atire build of the same texts
+    const uint64_t* cand_off;    // nullable: [nq + 1] pool offsets, cand_off[0] = 0
+    const uint32_t* cand_docs;   // [cand_off[nq]]
+    float* out_cand;             // [cand_off[nq]]
+};
+
 // Bm25Index::score of every query; with a concept index `c` of the same document count, then ConceptIndex::blend_into(query,
 // scores, weight) of each (SimeonLexicalBackend::score).
-// With strategy >= 0, the strategy's score_bm25f replaces Bm25Index::score (the strategy router's pools 0 and 2).
+// With strategy >= 0, the strategy's score_bm25f replaces Bm25Index::score (the strategy router's pools 0 and 2).  With rt, its
+// Atire rows score as Atire and its pools are gathered from each batch's rows and copied back once.
 static yams_status_t bm25_score(yams_b200_bm25* x, const yams_b200_concepts* c, float weight, const char* const* queries,
                                 const size_t* qlens, uint32_t nq, float* out_scores, uint32_t k, uint32_t* out_docs, float* out_topk,
-                                uint32_t* out_counts, int strategy = -1) {
+                                uint32_t* out_counts, int strategy = -1, const Routed* rt = nullptr) {
     const double t0 = wall_ms();
     cudaStream_t st = x->st;
     const uint64_t n = x->n;
@@ -1094,7 +1131,7 @@ static yams_status_t bm25_score(yams_b200_bm25* x, const yams_b200_concepts* c, 
     const bool blend = c && c->size && c->n == n;
     std::vector<RawLeg> raw;
     std::vector<uint64_t> qoff(nq + 1, 0);
-    query_legs(x, blend ? c : nullptr, queries, qlens, nq, raw, qoff.data(), strategy);
+    query_legs(x, blend ? c : nullptr, queries, qlens, nq, raw, qoff.data(), strategy, rt ? rt->atire : nullptr);
     const uint64_t nlegs = raw.size();
     const uint32_t K = std::min<uint64_t>(k, n);
     if ((rc = x->raw.reserve(std::max<uint64_t>(nlegs, 1) * sizeof(RawLeg))) != YAMS_OK) return rc;
@@ -1104,8 +1141,13 @@ static yams_status_t bm25_score(yams_b200_bm25* x, const yams_b200_concepts* c, 
     if (n && (rc = x->dense.reserve(qb_max * n * 4)) != YAMS_OK) return rc;
     if (K && (rc = x->sel.reserve(qb_max * K * sizeof(Cand))) != YAMS_OK) return rc;
     if (K && (rc = x->seln.reserve(qb_max * 4)) != YAMS_OK) return rc;
+    const uint64_t npool = rt && rt->cand_off ? rt->cand_off[nq] : 0;
+    if (npool && (rc = x->pool_off.reserve((nq + 1) * 8)) != YAMS_OK) return rc;
+    if (npool && (rc = x->pool_docs.reserve(npool * 4)) != YAMS_OK) return rc;
+    if (npool && (rc = x->pool_out.reserve(npool * 4)) != YAMS_OK) return rc;
     clear_topk(nq, k, out_docs, out_topk, out_counts);
     if (n == 0) {
+        for (uint64_t j = 0; j < npool; ++j) rt->out_cand[j] = 0.0f;   // no candidate is indexed
         x->ms[6] = 0.f;
         x->ms[7] = (float)(wall_ms() - t0);
         return YAMS_OK;
@@ -1115,6 +1157,10 @@ static yams_status_t bm25_score(yams_b200_bm25* x, const yams_b200_concepts* c, 
     std::vector<uint32_t> h_n;
     rc = timed(x, &dev_ms, [&]() -> yams_status_t {
         yams_status_t r;
+        if (npool) {
+            YB_CUDA(cudaMemcpyAsync(x->pool_off.p, rt->cand_off, (nq + 1) * 8, cudaMemcpyHostToDevice, st));
+            YB_CUDA(cudaMemcpyAsync(x->pool_docs.p, rt->cand_docs, npool * 4, cudaMemcpyHostToDevice, st));
+        }
         if (nlegs) {
             YB_CUDA(cudaMemcpyAsync(x->raw.p, raw.data(), nlegs * sizeof(RawLeg), cudaMemcpyHostToDevice, st));
             if ((r = plan_legs(x, blend ? c : nullptr, weight, x->raw.as<RawLeg>(), nlegs, x->legs.as<Leg>(), st)) != YAMS_OK) return r;
@@ -1131,9 +1177,18 @@ static yams_status_t bm25_score(yams_b200_bm25* x, const yams_b200_concepts* c, 
             a.q0 = q0;
             bm_score_kernel<<<dim3(tiles, qb), BM_THREADS, 0, st>>>(a);
             YB_CUDA(cudaGetLastError());
+            if (npool && rt->cand_off[q0 + qb] > rt->cand_off[q0]) {
+                uint64_t longest = 0;
+                for (uint32_t j = q0; j < q0 + qb; ++j) longest = std::max(longest, rt->cand_off[j + 1] - rt->cand_off[j]);
+                const unsigned gx = (unsigned)std::min<uint64_t>((longest + BM_THREADS - 1) / BM_THREADS, 64);
+                bm_pool_gather_kernel<<<dim3(gx, qb), BM_THREADS, 0, st>>>(x->dense.as<float>(), n, q0, x->pool_off.as<uint64_t>(),
+                                                                          x->pool_docs.as<uint32_t>(), x->pool_out.as<float>());
+                YB_CUDA(cudaGetLastError());
+            }
             if ((r = emit_batch(x, x->dense.as<float>(), n, q0, qb, nq, K, k, out_scores, out_docs, out_topk, out_counts, h_sel, h_n)) != YAMS_OK)
                 return r;
         }
+        if (npool) YB_CUDA(cudaMemcpyAsync(rt->out_cand, x->pool_out.p, npool * 4, cudaMemcpyDeviceToHost, st));
         return YAMS_OK;
     });
     if (rc != YAMS_OK) return rc;
@@ -1955,6 +2010,141 @@ __global__ void bm_lookup_kernel(Dict D, const uint64_t* __restrict__ ttf, uint6
     out[2] = found ? ttf[last_le(D.hashes, D.terms, h)] : 0;
 }
 
+// ---- the query router (simeon::QueryRouter over the index's field 0, query_router.cpp; DESIGN.md §4.15) ----
+struct TermStat {   // Bm25Index::df / idf / total_tf of one hash: 0, 0.0f, 0 when absent
+    uint64_t ttf;
+    uint32_t df;
+    float idf;
+};
+
+// df, idf and total_tf of every word hash of a batch of queries
+__global__ void bm_term_stats_kernel(Dict D, const uint64_t* __restrict__ ttf, const float* __restrict__ idf, const uint64_t* __restrict__ h,
+                                     uint64_t m, TermStat* __restrict__ out) {
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < m; i += (uint64_t)gridDim.x * blockDim.x) {
+        uint64_t b = 0, e = 0, t = 0;
+        out[i] = dict_find(D, h[i], &b, &e, &t) ? TermStat{ttf[t], (uint32_t)(e - b), idf[e - b]} : TermStat{0, 0, 0.0f};
+    }
+}
+
+// QueryRouter::features (query_router.cpp:29-117) of one query from its words' lengths, unfolded hashes and field-0 statistics,
+// every operation the reference's, in its order (double, glibc log)
+static yams_bm25_query_features router_features(const uint64_t* wlen, const uint64_t* h, const TermStat* ts, uint32_t nw,
+                                                uint64_t total_tokens) {
+    yams_bm25_query_features f{};
+    f.n_terms = nw;
+    if (nw == 0) return f;
+    uint32_t oov = 0, present = 0;
+    double idf_sum = 0.0, idf_sq_sum = 0.0, scq = 0.0;
+    uint64_t char_sum = 0;
+    float min_idf_seen = std::numeric_limits<float>::infinity();
+    std::unordered_map<uint64_t, uint32_t> q_count;
+    for (uint32_t i = 0; i < nw; ++i) {
+        char_sum += wlen[i];
+        if (ts[i].df == 0) { ++oov; continue; }
+        const float v = ts[i].idf;
+        idf_sum += (double)v;
+        idf_sq_sum += (double)v * (double)v;
+        if (v > f.max_idf) f.max_idf = v;
+        if (v < min_idf_seen) min_idf_seen = v;
+        ++present;
+        if (ts[i].ttf > 0) scq += (1.0 + std::log((double)ts[i].ttf)) * (double)v;
+        ++q_count[h[i]];
+    }
+    f.oov_rate = (float)oov / (float)nw;
+    if (present > 0) {
+        f.avg_idf = (float)(idf_sum / present);
+        f.min_idf = min_idf_seen;
+        if (present > 1) {
+            const double mean = idf_sum / present;
+            const double var = (idf_sq_sum / present) - (mean * mean);
+            f.idf_stddev = (float)(var > 0.0 ? std::sqrt(var) : 0.0);
+        }
+    }
+    f.avg_term_chars = (float)((double)char_sum / (double)nw);
+    f.scq_sum = (float)scq;
+    if (!q_count.empty() && total_tokens > 0) {
+        const double q_norm = (double)nw, c_norm = (double)total_tokens;
+        double acc = 0.0;
+        std::unordered_set<uint64_t> visited;
+        for (uint32_t i = 0; i < nw; ++i) {   // distinct hashes in first-occurrence order
+            if (!visited.insert(h[i]).second || ts[i].ttf == 0) continue;
+            const double p_q = (double)q_count[h[i]] / q_norm, p_c = (double)ts[i].ttf / c_norm;
+            acc += p_q * std::log(p_q / p_c);
+        }
+        f.simplified_clarity = (float)acc;
+    }
+    return f;
+}
+
+// QueryRouter::choose (query_router.cpp:222-238); features() leaves the pool signals at pool_overlap_jaccard 1, score_decay_rate 0
+static uint32_t router_choose(const yams_bm25_query_features& f, const yams_bm25_router_config& c) {
+    const float jaccard = 1.0f, decay = 0.0f;
+    if (f.n_terms == 0 || f.oov_rate > c.oov_threshold) return YAMS_BM25_RECIPE_SAB_SMOOTH;
+    if (f.avg_idf > c.high_idf_threshold && f.n_terms >= c.atire_min_terms && f.min_idf >= c.atire_min_idf_floor &&
+        jaccard <= c.atire_max_pool_jaccard && decay >= c.atire_min_score_decay && f.scq_sum >= c.atire_min_scq &&
+        f.simplified_clarity <= c.atire_max_clarity)
+        return YAMS_BM25_RECIPE_ATIRE;
+    if (f.n_terms >= c.cascade_min_terms && f.avg_idf <= c.cascade_max_idf) return YAMS_BM25_RECIPE_CASCADE;
+    return YAMS_BM25_RECIPE_SAB_SMOOTH;
+}
+
+// SimeonLexicalBackend::scoreRouted with router_enabled: the router's words of every query (unfolded hashes) looked up on the
+// device in one kernel, features and choose on the host, then one score call whose Bm25Atire rows score as Atire, the blend
+// and the pools' projection
+static yams_status_t bm25_score_routed(yams_b200_bm25* x, const yams_bm25_router_config& rc, const yams_b200_concepts* c, float weight,
+                                      const char* const* queries, const size_t* qlens, uint32_t nq, float* out_scores, uint32_t k,
+                                      uint32_t* out_docs, float* out_topk, uint32_t* out_counts, const uint64_t* cand_off,
+                                      const uint32_t* cand_docs, float* out_cand, uint32_t* out_recipe,
+                                      yams_bm25_query_features* out_features) {
+    const double t0 = wall_ms();
+    cudaStream_t st = x->st;
+    const uint64_t h0 = gram_hash_h0(x->cfg.hash_seed);
+    std::vector<std::pair<size_t, size_t>> ws;
+    std::vector<uint64_t> h, woff(nq + 1, 0);
+    std::vector<uint64_t> wlen;
+    for (uint32_t q = 0; q < nq; ++q) {
+        const uint8_t* p = reinterpret_cast<const uint8_t*>(queries[q]);
+        query_words(p, qlens[q], ws);
+        for (const auto& [s, l] : ws) {
+            h.push_back(gram_hash(p + s, l, h0));
+            wlen.push_back(l);
+        }
+        woff[q + 1] = h.size();
+    }
+    std::vector<TermStat> ts(h.size());
+    if (!h.empty()) {
+        yams_status_t r;
+        if ((r = x->rwords.reserve(h.size() * 8)) != YAMS_OK || (r = x->rstats.reserve(h.size() * sizeof(TermStat))) != YAMS_OK) return r;
+        const Bm25Field& F = *x->f[0];
+        YB_CUDA(cudaMemcpyAsync(x->rwords.p, h.data(), h.size() * 8, cudaMemcpyHostToDevice, st));
+        bm_term_stats_kernel<<<bm_grid(h.size()), BM_THREADS, 0, st>>>(Dict{F.hashes.as<uint64_t>(), F.offs.as<uint64_t>(), F.terms},
+                                                                       F.ttf.as<uint64_t>(), x->idf->as<float>(), x->rwords.as<uint64_t>(),
+                                                                       h.size(), x->rstats.as<TermStat>());
+        YB_CUDA(cudaGetLastError());
+        YB_CUDA(cudaMemcpyAsync(ts.data(), x->rstats.p, h.size() * sizeof(TermStat), cudaMemcpyDeviceToHost, st));
+        YB_CUDA(cudaStreamSynchronize(st));
+    }
+    std::vector<uint8_t> atire(nq);
+    for (uint32_t q = 0; q < nq; ++q) {
+        const uint64_t w0 = woff[q];
+        const yams_bm25_query_features f =
+            router_features(wlen.data() + w0, h.data() + w0, ts.data() + w0, (uint32_t)(woff[q + 1] - w0), x->total_tokens);
+        const uint32_t recipe = router_choose(f, rc);
+        atire[q] = recipe == YAMS_BM25_RECIPE_ATIRE;
+        if (out_recipe) out_recipe[q] = recipe;
+        if (out_features) out_features[q] = f;
+    }
+    if (!out_scores && k == 0 && !(cand_off && cand_off[nq])) {   // the route alone: nothing of the scores is asked for
+        x->ms[6] = 0.f;
+        x->ms[7] = (float)(wall_ms() - t0);
+        return YAMS_OK;
+    }
+    const Routed rt{atire.data(), cand_off, cand_docs, out_cand};
+    const yams_status_t r = bm25_score(x, c, weight, queries, qlens, nq, out_scores, k, out_docs, out_topk, out_counts, -1, &rt);
+    x->ms[7] = (float)(wall_ms() - t0);
+    return r;
+}
+
 }  // namespace yb
 
 extern "C" {
@@ -2282,6 +2472,53 @@ yams_status_t yams_b200_bm25_score_strategy(yams_b200_bm25* idx, uint32_t strate
     idx->sstats.device_ms = idx->ms[6];
     idx->sstats.wall_ms = idx->ms[7];
     return YAMS_OK;
+    YB_CATCH
+}
+
+void yams_b200_bm25_default_router_config(yams_bm25_router_config* cfg) {
+    if (!cfg) return;
+    // RouterConfig's defaults (include/simeon/query_router.hpp:14-65) under the backend's RouterPreset (passE_scq0_clar3,
+    // simeon_lexical_backend.h:75-85, applied by toRouterConfig)
+    cfg->oov_threshold = 0.0f;
+    cfg->high_idf_threshold = 3.0f;
+    cfg->atire_min_terms = 0;
+    cfg->atire_min_idf_floor = 0.0f;
+    cfg->atire_max_pool_jaccard = 1.0f;
+    cfg->atire_min_score_decay = 0.0f;
+    cfg->atire_min_scq = 0.0f;
+    cfg->atire_max_clarity = 3.0f;
+    cfg->cascade_min_terms = 4;
+    cfg->cascade_max_idf = 5.0f;
+}
+
+yams_status_t yams_b200_bm25_score_routed(yams_b200_bm25* idx, const yams_bm25_router_config* rcfg, const yams_b200_concepts* concepts,
+                                          float weight, const char* const* queries, const size_t* qlens, uint32_t nq, float* out_scores,
+                                          uint32_t k, uint32_t* out_docs, float* out_topk_scores, uint32_t* out_counts,
+                                          const uint64_t* cand_offsets, const uint32_t* cand_docs, float* out_cand_scores,
+                                          uint32_t* out_recipe, yams_bm25_query_features* out_features) {
+    YB_TRY
+    DeviceCtx* dev = nullptr;
+    yams_status_t rc = ensure_device(&dev);
+    if (rc != YAMS_OK) return rc;
+    YB_ARG(idx, "index is null");
+    YB_ARG(k <= TOPK_MAX, "k must be <= 4096");
+    YB_ARG(k == 0 || (out_docs && out_topk_scores && out_counts), "null top-k output");
+    if (nq == 0) return YAMS_OK;
+    YB_ARG(queries && qlens, "null argument");
+    for (uint32_t q = 0; q < nq; ++q) YB_ARG(queries[q] || qlens[q] == 0, "null query");
+    if (cand_offsets) {
+        YB_ARG(cand_offsets[0] == 0, "cand_offsets[0] must be 0");
+        for (uint32_t q = 0; q < nq; ++q) YB_ARG(cand_offsets[q + 1] >= cand_offsets[q], "cand_offsets must not decrease");
+        YB_ARG(cand_offsets[nq] == 0 || (cand_docs && out_cand_scores), "null candidate pool");
+        for (uint64_t j = 0; j < cand_offsets[nq]; ++j)
+            YB_ARG(cand_docs[j] < idx->n || cand_docs[j] == 0xFFFFFFFFu, "a candidate index is >= n_docs (0xFFFFFFFF: not indexed)");
+    }
+    yams_bm25_router_config cfg;
+    if (rcfg) cfg = *rcfg; else yams_b200_bm25_default_router_config(&cfg);
+    YB_BIND(idx);
+    std::lock_guard<std::mutex> g(idx->mu);
+    return bm25_score_routed(idx, cfg, concepts, weight, queries, qlens, nq, out_scores, k, out_docs, out_topk_scores, out_counts,
+                             cand_offsets, cand_docs, out_cand_scores, out_recipe, out_features);
     YB_CATCH
 }
 

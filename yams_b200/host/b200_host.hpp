@@ -997,6 +997,19 @@ public:
                                    float weight = 0.0f) const {
         return score_strategy(YAMS_BM25_STRATEGY_ROUTED, query, out_scores, concepts, weight);
     }
+    // SimeonLexicalBackend::scoreRouted with router_enabled, in one device call: QueryRouter::features and choose over this index
+    // (router: NULL = the backend's preset), the recipe's scores -- Bm25Atire as this index's Atire view, so no second index and
+    // no QueryRouter are needed -- then concepts->blend_into(query, scores, weight).  Returns the recipe (YAMS_BM25_RECIPE_*).
+    uint32_t score_routed(std::string_view query, std::span<float> out_scores, const B200ConceptIndex* concepts = nullptr,
+                          float weight = 0.0f, const yams_bm25_router_config* router = nullptr) const;
+    // The same, projected onto the backend's candidate pool (its RescoreDecision scores): out[i] = the finite score of document
+    // index candidates[i], else 0, 0 for NOT_INDEXED; gathered on the device, so only the pool crosses PCIe.
+    static constexpr uint32_t NOT_INDEXED = 0xFFFFFFFFu;
+    uint32_t score_routed(std::string_view query, std::span<const uint32_t> candidates, std::span<float> out,
+                          const B200ConceptIndex* concepts = nullptr, float weight = 0.0f,
+                          const yams_bm25_router_config* router = nullptr) const;
+    // QueryRouter::features(query) over this index (no scoring)
+    yams_bm25_query_features router_features(std::string_view query, const yams_bm25_router_config* router = nullptr) const;
     // The Atire index SimeonLexicalBackend builds beside a SubwordAwareBackoff primary for RRF (and its router), served from this
     // index's word field without a second build (yams_b200_bm25_atire_view).  The view and this index may go in either order.
     std::unique_ptr<B200Bm25Index> atire_view() const {
@@ -1153,6 +1166,44 @@ inline uint32_t B200Bm25Index::score_strategy(uint32_t strategy, std::string_vie
                                         nullptr, nullptr, nullptr, &chosen),
           "score_strategy");
     return chosen;
+}
+
+inline uint32_t B200Bm25Index::score_routed(std::string_view query, std::span<float> out_scores, const B200ConceptIndex* concepts,
+                                            float weight, const yams_bm25_router_config* router) const {
+    if (!idx_) throw std::runtime_error("Bm25Index::score before finalize()");
+    if (out_scores.size() != n_) throw std::runtime_error("Bm25Index::score out_scores size mismatch");
+    const char* q = query.data();
+    const size_t len = query.size();
+    uint32_t recipe = 0;
+    check(yams_b200_bm25_score_routed(idx_, router, concepts ? concepts->handle() : nullptr, weight, &q, &len, 1, out_scores.data(), 0,
+                                      nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, &recipe, nullptr),
+          "score_routed");
+    return recipe;
+}
+
+inline uint32_t B200Bm25Index::score_routed(std::string_view query, std::span<const uint32_t> candidates, std::span<float> out,
+                                            const B200ConceptIndex* concepts, float weight, const yams_bm25_router_config* router) const {
+    if (!idx_) throw std::runtime_error("Bm25Index::score before finalize()");
+    if (out.size() != candidates.size()) throw std::runtime_error("Bm25Index::score_routed out size mismatch");
+    const char* q = query.data();
+    const size_t len = query.size();
+    const uint64_t off[2] = {0, candidates.size()};
+    uint32_t recipe = 0;
+    check(yams_b200_bm25_score_routed(idx_, router, concepts ? concepts->handle() : nullptr, weight, &q, &len, 1, nullptr, 0, nullptr,
+                                      nullptr, nullptr, off, candidates.data(), out.data(), &recipe, nullptr),
+          "score_routed");
+    return recipe;
+}
+
+inline yams_bm25_query_features B200Bm25Index::router_features(std::string_view query, const yams_bm25_router_config* router) const {
+    if (!idx_) throw std::runtime_error("Bm25Index::router_features before finalize()");
+    const char* q = query.data();
+    const size_t len = query.size();
+    yams_bm25_query_features f{};
+    check(yams_b200_bm25_score_routed(idx_, router, nullptr, 0.0f, &q, &len, 1, nullptr, 0, nullptr, nullptr, nullptr, nullptr, nullptr,
+                                      nullptr, nullptr, &f),
+          "router_features");
+    return f;
 }
 
 inline void B200Bm25Index::score(std::string_view query, std::span<float> out_scores, const B200ConceptIndex* concepts, float weight) const {
