@@ -12,7 +12,7 @@
 //                                   with the per-query threshold and appends survivors
 //
 // A CTA owns whole row tiles and runs every query tile against each: the corpus tile comes from HBM once and is
-// re-read from L2 by the same SM; the next row tile is prefetched into L2 meanwhile.
+// re-read from L2 by the same SM; the next row tile is prefetched into L2 during the last query tile.
 //
 // Queries are pre-scaled by 1/|q| and rounded to fp16; the resulting ~1e-5 score error only affects which
 // rows reach stage 2, where the survivors are re-scored exactly in fp64 (knn.cu).
@@ -151,7 +151,8 @@ __device__ __forceinline__ void mbar_arrive_u(uint32_t bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
 
-__device__ __noinline__ void append_candidate(uint32_t* counts, Cand* cands, uint32_t cap, uint32_t q, uint32_t row, float sc) {
+// inlined: a call from the filter epilogue would have to save the live accumulators around it
+__device__ __forceinline__ void append_candidate(uint32_t* counts, Cand* cands, uint32_t cap, uint32_t q, uint32_t row, float sc) {
     uint32_t pos = atomicAdd(&counts[q], 1u);
     if (pos < cap) {
         Cand cd;
@@ -219,7 +220,8 @@ stage1_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
             const int block_k = UM_BLOCK_K_BYTES / (TF32 ? 4 : 2);
             // A corpus tile is read from L2 once per query tile.  Its last read marks its lines evict-first: with every
             // CTA's current and prefetched next tile (~50 MB at C2) the L2 is full, and a dead tile should leave before a
-            // live one is pushed out and fetched from HBM again.
+            // live one is pushed out and fetched from HBM again.  The next tile is prefetched during the current tile's last
+            // query tile, not its first: from the first on, it would share the L2 with the current tile for the whole tile.
             uint64_t last_use;
             asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(last_use));
             for (uint32_t rt = blockIdx.x; rt < u.nrt; rt += gridDim.x) {
@@ -228,7 +230,7 @@ stage1_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
                 const bool have_next = rt + gridDim.x < u.nrt;
                 for (uint32_t qt = 0; qt < u.nqt; ++qt) {
                     const int b_row = (int)(qt * N);
-                    const bool pf = qt == 0 && have_next;
+                    const bool pf = qt + 1 == u.nqt && have_next;
                     const bool a_last = qt + 1 == u.nqt;
                     int kc = 0;
                     for (uint32_t kb = 0; kb < u.kblocks; ++kb, kc += block_k) {
@@ -327,10 +329,10 @@ stage1_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
 
                 const long long t_epi0 = PROF ? clock64() : 0;
                 if (FILTER) {
-                    // common path: the maximum of each (group, row) against its bound, one branch for the whole tile
+                    // common path: the maximum of each (group, row) against its bound, one branch for the whole tile.  The
+                    // outcomes are kept as one bit each (bit 2 h + r) for the cold path, not as 16 maxima in registers.
                     constexpr int J = TG / 8;   // accumulator column pairs per group
-                    float gmax[G][2];
-                    bool any = false;
+                    uint32_t pass = 0;
 #pragma unroll
                     for (int h = 0; h < G; ++h) {
 #pragma unroll
@@ -338,19 +340,16 @@ stage1_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
                             float m = acc[4 * J * h + 2 * r];
 #pragma unroll
                             for (int j = J * h; j < J * (h + 1); ++j) m = fmaxf(m, fmaxf(acc[4 * j + 2 * r], acc[4 * j + 2 * r + 1]));
-                            gmax[h][r] = m;
-                            any |= m > bound[h][r];
+                            pass |= (m > bound[h][r] ? 1u : 0u) << (2 * h + r);
                         }
                     }
-                    if (any) {   // rare: some column of a group of this thread may survive
+                    if (pass) {   // rare: some column of a group of this thread may survive
                         const float* tau_t = tau_all + q0;
 #pragma unroll
                         for (int h = 0; h < G; ++h) {
 #pragma unroll
                             for (int r = 0; r < 2; ++r) {
-                                // the common path's test, m > bound, in a form the compiler does not merge with it: it would
-                                // otherwise carry the 16 outcomes through the common path in a bit mask
-                                if (!(gmax[h][r] - bound[h][r] > 0.f)) continue;
+                                if (!((pass >> (2 * h + r)) & 1u)) continue;
 #pragma unroll
                                 for (int j = J * h; j < J * (h + 1); ++j) {
 #pragma unroll
