@@ -22,7 +22,10 @@
 // CTA per (query, tile of documents) keeps the tile's scores in shared memory and walks the legs in order; per leg it finds the
 // part of the posting list inside the tile by binary search and adds each document's contribution -- a document appears once
 // per leg, so no atomics, and each document receives its additions in the reference's order.  Every float operation is an
-// explicit _rn intrinsic: the reference is compiled without -mfma, so nothing may be fused.
+// explicit _rn intrinsic: the reference is compiled without -mfma, so nothing may be fused.  Every score call takes one host
+// path: its legs go into a host leg list (LegList, one appender per leg kind), one staging step uploads and plans a list
+// (stage_legs) and one launches the score kernel over a batch's rows (score_rows), and one driver (run_batches) sizes the
+// batches from the bytes a query's rows take, carves them from one arena, and emits each batch's rows and top-k.
 //
 // RRF (score_bm25_variants_rrf, fusion.cpp; DESIGN.md §4.13): the variants' score rows, their ranked entries as sortable keys,
 // one segmented sort per batch, one scatter of 1 / (k + r) per variant in order.  An Atire view shares its parent's word field
@@ -517,6 +520,12 @@ struct CubTmp {
     yams_status_t grow() { return buf.reserve(std::max<size_t>(bytes, 256)); }
 };
 
+// The score calls' workspace: the staged legs (raw, planned, per-query offsets), the arena of a batch's rows (and whatever a
+// path carves from it) and the top-k selection
+struct ScoreWs {
+    DevBuf raw, legs, qoff, rows, sel, seln;
+};
+
 template <typename Pred>
 yams_status_t select_indices(CubTmp& tmp, uint64_t lo, uint64_t n, Pred pred, DevBuf& out, DevBuf& cnt, uint64_t* h_cnt, cudaStream_t st) {
     yams_status_t rc;
@@ -564,11 +573,11 @@ struct yams_b200_bm25 {
     std::shared_ptr<DevBuf> idf = std::make_shared<DevBuf>();   // n + 1 floats: idf of df = 0..n
     cudaStream_t st = nullptr;
     cudaEvent_t ev[2] = {nullptr, nullptr};
-    DevBuf raw, legs, qoff, dense, sel, seln;   // score workspace
-    DevBuf counts, route, zrow, zp;             // strategy workspace: keyphrase matches, route profiles, z-score rows
+    ScoreWs ws;
+    DevBuf route, zrow, zp;                     // strategy workspace: route profiles, z-score rows
     cudaEvent_t zev[2] = {nullptr, nullptr};
     yams_bm25_strategy_stats sstats{};
-    DevBuf fused, keys, keys2, cnt, base;       // RRF workspace (the call runs on its first variant's)
+    DevBuf cnt, base;                           // RRF workspace: ranked entries per tile, their scan (on the first variant's)
     DevBuf rwords, rstats, pool_off, pool_docs, pool_out;   // query-router workspace: word lookups, candidate pools
     CubTmp tmp;
     float ms[8] = {0, 0, 0, 0, 0, 0, 0, 0};
@@ -601,7 +610,7 @@ struct yams_b200_concepts {
     std::vector<float> h_pmi, h_idf;
     cudaStream_t st = nullptr;
     cudaEvent_t ev[2] = {nullptr, nullptr};
-    DevBuf raw, legs, qoff, dense;   // standalone blend workspace
+    ScoreWs ws;                      // the standalone blend's
     float ms[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     std::mutex mu;
     ~yams_b200_concepts() {
@@ -914,42 +923,6 @@ static void query_words(const uint8_t* p, size_t len, std::vector<std::pair<size
     }
 }
 
-// ConceptIndex::blend_into's concept order for one query: its unfolded words' adjacent bigrams that are kept concepts, emplaced
-// into an unordered_map reserved for the word count, in that map's iteration order (concept_mining.cpp:82-104).  The additions
-// of a document in several matched concepts are made in this order.
-static void concept_order(const yams_b200_concepts* c, const uint8_t* p, size_t len, std::vector<std::pair<size_t, size_t>>& ws,
-                          std::vector<uint64_t>& out) {
-    out.clear();
-    query_words(p, len, ws);
-    if (c->size == 0 || ws.size() < 2) return;
-    std::vector<uint64_t> qw(ws.size());
-    for (size_t i = 0; i < ws.size(); ++i) qw[i] = gram_hash(p + ws[i].first, ws[i].second, c->h0);
-    std::unordered_map<uint64_t, uint32_t> matched;
-    matched.reserve(qw.size());
-    for (size_t i = 1; i < qw.size(); ++i) {
-        const uint64_t bh = hash_bigram(qw[i - 1], qw[i]);
-        const auto it = std::lower_bound(c->h_hashes.begin(), c->h_hashes.end(), bh);
-        if (it != c->h_hashes.end() && *it == bh) matched.emplace(bh, (uint32_t)(it - c->h_hashes.begin()));
-    }
-    for (const auto& [bh, j] : matched) {
-        (void)j;
-        out.push_back(bh);
-    }
-}
-
-// the concept field of the score kernel's arguments, and the plan kernel's concept dictionary
-static void concept_field(const yams_b200_concepts* c, ScoreArgs& a) {
-    a.docs[BM_CONCEPT] = c->docs.as<uint32_t>();
-    a.tfs[BM_CONCEPT] = c->tfs.as<uint32_t>();
-    a.dl[BM_CONCEPT] = c->bdl.as<uint32_t>();
-    a.avg[BM_CONCEPT] = c->avg;
-    a.k1[BM_CONCEPT] = c->cfg.k1;
-    a.b[BM_CONCEPT] = c->cfg.b;
-}
-static ConceptDict concept_dict(const yams_b200_concepts* c, float weight) {
-    return ConceptDict{Dict{c->hashes.as<uint64_t>(), c->offs.as<uint64_t>(), c->size}, c->pmi.as<float>(), c->idf.as<float>(), weight};
-}
-
 // The end of the lead prefix of p[0, len): the whitespace byte that ends its lead-th token, else len (extract_lead_tokens,
 // corpus_adapter.cpp:16-39).  The prefix's words are the lead text's: the reference only turns whitespace into ' ' and trims.
 static size_t lead_cut(const uint8_t* p, size_t len, uint32_t lead) {
@@ -966,14 +939,31 @@ static size_t lead_cut(const uint8_t* p, size_t len, uint32_t lead) {
     return len;
 }
 
-// The BM25 legs of the words of p[0, len) over fields fw (words) and fw + 1 (n-grams), in Bm25Index::score's order; with
-// atire, the legs an Atire build of the same texts would score (words only, as BM_ATIRE legs)
-struct WordLegs {
-    const yams_b200_bm25* x;
-    std::vector<std::pair<size_t, size_t>> ws;
+// The lexical backend's strategies over its primary index (SimeonLexicalBackend, simeon_lexical_backend.cpp:563-580): Bm25Strategy
+// scores score_bm25f(q, lead(q, 64), 0.85, 0.15), or score(q) when that lead text is empty; LeadFieldStrategy scores
+// score_bm25f(q, q, 0.85, 0.15) (retrieval_strategy.cpp:84-127).
+constexpr uint32_t STRATEGY_LEAD = 64;
+constexpr float STRATEGY_WB = 0.85f, STRATEGY_WA = 0.15f;
+
+// The raw legs of a run of queries in the reference's order: query j's are raw[qoff[j], qoff[j + 1]).  Each appender adds one
+// kind of leg to the open query; end_query closes it.
+struct LegList {
+    std::vector<RawLeg> raw;
+    std::vector<uint64_t> qoff{0};
+    std::vector<std::pair<size_t, size_t>> ws;   // the appenders' scratch
     std::vector<uint8_t> low;
     std::unordered_set<uint64_t> seen;
-    void operator()(const uint8_t* p, size_t len, uint32_t fw, std::vector<RawLeg>& raw, bool atire = false) {
+    std::vector<uint64_t> qw;
+
+    void clear() {
+        raw.clear();
+        qoff.assign(1, 0);
+    }
+    void end_query() { qoff.push_back(raw.size()); }
+
+    // The BM25 legs of the words of p[0, len) over fields fw (words) and fw + 1 (n-grams) of index x, in Bm25Index::score's
+    // order; with atire, the legs an Atire build of the same texts would score (words only, as BM_ATIRE legs)
+    void words(const yams_b200_bm25* x, const uint8_t* p, size_t len, uint32_t fw, bool atire = false) {
         const bool sab = x->cfg.variant == YAMS_BM25_SUBWORD_AWARE_BACKOFF && !atire;
         const uint64_t h0 = gram_hash_h0(x->cfg.hash_seed);
         query_words(p, len, ws);
@@ -992,107 +982,153 @@ struct WordLegs {
                 }
         }
     }
+    // score_bm25f's legs after the body's, for strategy pool 0 or 2: the body scale, then the aux query's legs over the aux
+    // fields.  The aux query is the query's lead prefix (Bm25Strategy) or the query (LeadFieldStrategy); a lead prefix of
+    // whitespace alone is no evidence, and the query scores as Bm25Index::score alone.
+    void bm25f(const yams_b200_bm25* x, const uint8_t* p, size_t len, uint32_t pool) {
+        size_t aux = len;
+        if (pool == YAMS_BM25_STRATEGY_BM25) {
+            aux = lead_cut(p, len, STRATEGY_LEAD);
+            if (std::all_of(p, p + aux, [](uint8_t ch) { return is_space(ch); })) return;
+        }
+        uint32_t wb_bits;
+        memcpy(&wb_bits, &STRATEGY_WB, 4);
+        raw.push_back({0, 0, BM_SCALE, wb_bits});   // weight_body != 1 (bm25.cpp:993-996)
+        words(x, p, aux, BM_AUX);
+    }
+    // one presence leg per keyphrase hash
+    void presence(const std::vector<uint64_t>& kh) {
+        for (uint64_t h : kh) raw.push_back({h, h, 0, BM_PRESENCE});
+    }
+    // The concepts of concept index c that p[0, len) matches, in ConceptIndex::blend_into's order: its unfolded words' adjacent
+    // bigrams that are kept concepts, emplaced into an unordered_map reserved for the word count, in that map's iteration order
+    // (concept_mining.cpp:82-104).  The additions of a document in several matched concepts are made in this order.
+    void concepts(const yams_b200_concepts* c, const uint8_t* p, size_t len) {
+        query_words(p, len, ws);
+        if (c->size == 0 || ws.size() < 2) return;
+        qw.resize(ws.size());
+        for (size_t i = 0; i < ws.size(); ++i) qw[i] = gram_hash(p + ws[i].first, ws[i].second, c->h0);
+        std::unordered_map<uint64_t, uint32_t> matched;
+        matched.reserve(qw.size());
+        for (size_t i = 1; i < qw.size(); ++i) {
+            const uint64_t bh = hash_bigram(qw[i - 1], qw[i]);
+            const auto it = std::lower_bound(c->h_hashes.begin(), c->h_hashes.end(), bh);
+            if (it != c->h_hashes.end() && *it == bh) matched.emplace(bh, (uint32_t)(it - c->h_hashes.begin()));
+        }
+        for (const auto& m : matched) raw.push_back({m.first, m.first, BM_CONCEPT, 0});
+    }
 };
 
-// The lexical backend's strategies over its primary index (SimeonLexicalBackend, simeon_lexical_backend.cpp:563-580): Bm25Strategy
-// scores score_bm25f(q, lead(q, 64), 0.85, 0.15), or score(q) when that lead text is empty; LeadFieldStrategy scores
-// score_bm25f(q, q, 0.85, 0.15) (retrieval_strategy.cpp:84-127).
-constexpr uint32_t STRATEGY_LEAD = 64;
-constexpr float STRATEGY_WB = 0.85f, STRATEGY_WA = 0.15f;
+// What a leg list is planned and scored against: index x's fields and concept index c's concepts at the blend's weight.  Either
+// may be null when the list has none of its legs.
+struct Scorer {
+    const yams_b200_bm25* x;
+    const yams_b200_concepts* c;
+    float weight;
+};
 
-// The legs of queries [0, nq), in the reference's order, appended to raw: the BM25 legs of index x (nullable: none) -- with
-// strategy >= 0, score_bm25f's: the body's, the body scale, the aux query's over the aux fields; with atire[q] != 0, an Atire
-// build's -- then, with a concept index c, the concepts each query matches in blend_into's order.  qoff[q] .. qoff[q + 1] are
-// query q's (absolute).
-static void query_legs(const yams_b200_bm25* x, const yams_b200_concepts* c, const char* const* queries, const size_t* qlens,
-                       uint32_t nq, std::vector<RawLeg>& raw, uint64_t* qoff, int strategy = -1, const uint8_t* atire = nullptr) {
-    WordLegs word_legs{x, {}, {}, {}};
-    std::vector<std::pair<size_t, size_t>> ws;
-    std::vector<uint64_t> corder;
-    uint32_t wb_bits;
-    memcpy(&wb_bits, &STRATEGY_WB, 4);
-    qoff[0] = raw.size();
-    for (uint32_t q = 0; q < nq; ++q) {
-        const uint8_t* p = reinterpret_cast<const uint8_t*>(queries[q]);
-        if (x) word_legs(p, qlens[q], 0, raw, atire && atire[q]);
-        if (x && strategy >= 0) {
-            // the aux query: the query's lead prefix (Bm25Strategy) or the query (LeadFieldStrategy)
-            size_t aux_len = qlens[q];
-            if (strategy == YAMS_BM25_STRATEGY_BM25) {
-                aux_len = lead_cut(p, qlens[q], STRATEGY_LEAD);
-                bool empty = true;
-                for (size_t i = 0; i < aux_len && empty; ++i) empty = is_space(p[i]);
-                if (empty) aux_len = SIZE_MAX;   // no evidence: Bm25Index::score alone
-            }
-            if (aux_len != SIZE_MAX) {
-                raw.push_back({0, 0, BM_SCALE, wb_bits});   // weight_body != 1 (bm25.cpp:993-996)
-                word_legs(p, aux_len, BM_AUX, raw);
-            }
-        }
-        if (c) {
-            concept_order(c, p, qlens[q], ws, corder);
-            for (uint64_t bh : corder) raw.push_back({bh, bh, BM_CONCEPT, 0});
-        }
-        qoff[q + 1] = raw.size();
+// Uploads leg list L to w, one copy of its legs and one of its offsets, and plans it.  L's queries form ns blocks of equal count,
+// block i planned against s[i] (RRF: one block per variant, each against its own dictionaries, then the concepts').
+static yams_status_t stage_legs(ScoreWs& w, const LegList& L, const Scorer* s, uint32_t ns, cudaStream_t st) {
+    const uint64_t nlegs = L.raw.size(), per = (L.qoff.size() - 1) / ns;
+    if (nlegs == 0) return YAMS_OK;
+    yams_status_t rc;
+    if ((rc = w.raw.reserve(nlegs * sizeof(RawLeg))) != YAMS_OK || (rc = w.legs.reserve(nlegs * sizeof(Leg))) != YAMS_OK ||
+        (rc = w.qoff.reserve(L.qoff.size() * 8)) != YAMS_OK)
+        return rc;
+    YB_CUDA(cudaMemcpyAsync(w.raw.p, L.raw.data(), nlegs * sizeof(RawLeg), cudaMemcpyHostToDevice, st));
+    YB_CUDA(cudaMemcpyAsync(w.qoff.p, L.qoff.data(), L.qoff.size() * 8, cudaMemcpyHostToDevice, st));
+    for (uint32_t i = 0; i < ns; ++i) {
+        const uint64_t lb = L.qoff[i * per], le = L.qoff[(i + 1) * per];
+        if (lb == le) continue;
+        const yams_b200_bm25* x = s[i].x;
+        FieldDicts f{};
+        for (int fi = 0; x && fi < 4; ++fi) f.d[fi] = Dict{x->f[fi]->hashes.as<uint64_t>(), x->f[fi]->offs.as<uint64_t>(), x->f[fi]->terms};
+        const yams_b200_concepts* c = s[i].c;
+        const ConceptDict cd = c ? ConceptDict{Dict{c->hashes.as<uint64_t>(), c->offs.as<uint64_t>(), c->size}, c->pmi.as<float>(),
+                                               c->idf.as<float>(), s[i].weight}
+                                 : ConceptDict{};
+        bm_plan_kernel<<<bm_grid(le - lb), BM_THREADS, 0, st>>>(w.raw.as<RawLeg>() + lb, le - lb, f, x ? x->idf->as<float>() : nullptr,
+                                                               x && x->cfg.variant == YAMS_BM25_SUBWORD_AWARE_BACKOFF,
+                                                               x ? x->cfg.subword_gamma : 0.0f, STRATEGY_WA, cd, w.legs.as<Leg>() + lb);
+        YB_CUDA(cudaGetLastError());
     }
+    return YAMS_OK;
 }
 
-// the plan kernel over raw legs [0, nlegs) of index x (nullable: concept legs only) and concept index c (nullable)
-static yams_status_t plan_legs(const yams_b200_bm25* x, const yams_b200_concepts* c, float weight, const RawLeg* raw, uint64_t nlegs,
-                               Leg* legs, cudaStream_t st) {
-    if (nlegs == 0) return YAMS_OK;
-    FieldDicts f{};
-    for (int fi = 0; x && fi < 4; ++fi) f.d[fi] = Dict{x->f[fi]->hashes.as<uint64_t>(), x->f[fi]->offs.as<uint64_t>(), x->f[fi]->terms};
-    const ConceptDict cd = c ? concept_dict(c, weight) : ConceptDict{};
-    bm_plan_kernel<<<bm_grid(nlegs), BM_THREADS, 0, st>>>(raw, nlegs, f, x ? x->idf->as<float>() : nullptr,
-                                                          x && x->cfg.variant == YAMS_BM25_SUBWORD_AWARE_BACKOFF,
-                                                          x ? x->cfg.subword_gamma : 0.0f, STRATEGY_WA, cd, legs);
+// Scores queries [q0, q0 + qb) of the staged list L against s onto rows[qb][n]: from zero, or (in_place) onto the rows' own
+// scores, each CTA reading and writing its tile
+static yams_status_t score_rows(const ScoreWs& w, const LegList& L, const Scorer& s, uint64_t n, uint64_t q0, uint32_t qb, bool in_place,
+                                float* rows, cudaStream_t st) {
+    if (L.qoff[q0] == L.qoff[q0 + qb]) {   // no leg: zeros, or the rows as they are
+        if (!in_place) YB_CUDA(cudaMemsetAsync(rows, 0, (uint64_t)qb * n * 4, st));
+        return YAMS_OK;
+    }
+    ScoreArgs a{};
+    if (const yams_b200_bm25* x = s.x) {
+        for (int fi = 0; fi < 4; ++fi) {
+            a.docs[fi] = x->f[fi]->docs.as<uint32_t>();
+            a.tfs[fi] = x->f[fi]->tfs.as<uint32_t>();
+            a.dl[fi] = x->f[fi]->dl.as<uint32_t>();
+            a.avg[fi] = x->f[fi]->avg > 0.0f ? x->f[fi]->avg : 1.0f;
+            a.k1[fi] = x->cfg.k1;
+            a.b[fi] = x->cfg.b;
+        }
+        a.delta = x->cfg.delta;
+        a.sab = x->cfg.variant == YAMS_BM25_SUBWORD_AWARE_BACKOFF;
+    }
+    if (const yams_b200_concepts* c = s.c) {
+        a.docs[BM_CONCEPT] = c->docs.as<uint32_t>();
+        a.tfs[BM_CONCEPT] = c->tfs.as<uint32_t>();
+        a.dl[BM_CONCEPT] = c->bdl.as<uint32_t>();
+        a.avg[BM_CONCEPT] = c->avg;
+        a.k1[BM_CONCEPT] = c->cfg.k1;
+        a.b[BM_CONCEPT] = c->cfg.b;
+    }
+    a.legs = w.legs.as<Leg>();
+    a.qoff = w.qoff.as<uint64_t>() + q0;
+    a.n = n;
+    a.init = in_place ? rows : nullptr;
+    a.out = rows;
+    bm_score_kernel<<<dim3((unsigned)((n + BM_TILE - 1) / BM_TILE), qb), BM_THREADS, 0, st>>>(a);
     YB_CUDA(cudaGetLastError());
     return YAMS_OK;
 }
 
-// the score kernel's arguments of index x's four fields
-static ScoreArgs bm25_args(const yams_b200_bm25* x) {
-    ScoreArgs a{};
-    for (int fi = 0; fi < 4; ++fi) {
-        a.docs[fi] = x->f[fi]->docs.as<uint32_t>();
-        a.tfs[fi] = x->f[fi]->tfs.as<uint32_t>();
-        a.dl[fi] = x->f[fi]->dl.as<uint32_t>();
-        a.avg[fi] = x->f[fi]->avg > 0.0f ? x->f[fi]->avg : 1.0f;
-        a.k1[fi] = x->cfg.k1;
-        a.b[fi] = x->cfg.b;
-    }
-    a.n = x->n;
-    a.delta = x->cfg.delta;
-    a.sab = x->cfg.variant == YAMS_BM25_SUBWORD_AWARE_BACKOFF;
-    return a;
-}
+// What a score call returns: the full score rows, and the best k (k <= 4096) of score > 0 of each query, best first
+struct ScoreOut {
+    float* scores;      // nullable: [nq][n]
+    uint32_t k;
+    uint32_t* docs;     // [nq][k], padded with 0xFFFFFFFF
+    float* topk;        // [nq][k], padded with 0
+    uint32_t* counts;   // [nq]
+};
 
 // The outputs of one batch: queries q0 .. q0 + qb, whose score rows are rows[qb][n] on x's stream -- the full vectors, and the
 // best K (k <= 4096 asked) of score > 0 through x's selection workspace.  Returns with the rows free for the next batch.
-static yams_status_t emit_batch(yams_b200_bm25* x, const float* rows, uint64_t n, uint32_t q0, uint32_t qb, uint32_t nq, uint32_t K,
-                                uint32_t k, float* out_scores, uint32_t* out_docs, float* out_topk, uint32_t* out_counts,
+static yams_status_t emit_batch(yams_b200_bm25* x, const float* rows, uint32_t q0, uint32_t qb, uint32_t nq, uint32_t K, const ScoreOut& o,
                                 std::vector<Cand>& h_sel, std::vector<uint32_t>& h_n) {
     cudaStream_t st = x->st;
-    if (out_scores) YB_CUDA(cudaMemcpyAsync(out_scores + (uint64_t)q0 * n, rows, (uint64_t)qb * n * 4, cudaMemcpyDeviceToHost, st));
+    const uint64_t n = x->n;
+    if (o.scores) YB_CUDA(cudaMemcpyAsync(o.scores + (uint64_t)q0 * n, rows, (uint64_t)qb * n * 4, cudaMemcpyDeviceToHost, st));
     if (K) {
-        launch_topk_dense(rows, n, qb, K, x->sel.as<Cand>(), x->seln.as<uint32_t>(), st);
+        launch_topk_dense(rows, n, qb, K, x->ws.sel.as<Cand>(), x->ws.seln.as<uint32_t>(), st);
         YB_CUDA(cudaGetLastError());
         h_sel.resize((uint64_t)qb * K);
         h_n.resize(qb);
-        YB_CUDA(cudaMemcpyAsync(h_sel.data(), x->sel.p, (uint64_t)qb * K * sizeof(Cand), cudaMemcpyDeviceToHost, st));
-        YB_CUDA(cudaMemcpyAsync(h_n.data(), x->seln.p, (uint64_t)qb * 4, cudaMemcpyDeviceToHost, st));
+        YB_CUDA(cudaMemcpyAsync(h_sel.data(), x->ws.sel.p, (uint64_t)qb * K * sizeof(Cand), cudaMemcpyDeviceToHost, st));
+        YB_CUDA(cudaMemcpyAsync(h_n.data(), x->ws.seln.p, (uint64_t)qb * 4, cudaMemcpyDeviceToHost, st));
         YB_CUDA(cudaStreamSynchronize(st));
         // best first: the documents of score > 0 lead the selection
         for (uint32_t j = 0; j < qb; ++j) {
             uint32_t c = 0;
             const uint32_t m = std::min(h_n[j], K);
             while (c < m && h_sel[(uint64_t)j * K + c].score > 0.0f) {
-                out_docs[(uint64_t)(q0 + j) * k + c] = h_sel[(uint64_t)j * K + c].row;
-                out_topk[(uint64_t)(q0 + j) * k + c] = h_sel[(uint64_t)j * K + c].score;
+                o.docs[(uint64_t)(q0 + j) * o.k + c] = h_sel[(uint64_t)j * K + c].row;
+                o.topk[(uint64_t)(q0 + j) * o.k + c] = h_sel[(uint64_t)j * K + c].score;
                 ++c;
             }
-            out_counts[q0 + j] = c;
+            o.counts[q0 + j] = c;
         }
     } else if (q0 + qb < nq) {
         YB_CUDA(cudaStreamSynchronize(st));   // the next batch overwrites the score rows
@@ -1101,10 +1137,54 @@ static yams_status_t emit_batch(yams_b200_bm25* x, const float* rows, uint64_t n
 }
 
 // the top-k outputs before any batch: padding, counts 0
-static void clear_topk(uint32_t nq, uint32_t k, uint32_t* out_docs, float* out_topk, uint32_t* out_counts) {
-    if (!k) return;
-    for (uint64_t i = 0; i < (uint64_t)nq * k; ++i) { out_docs[i] = 0xFFFFFFFFu; out_topk[i] = 0.0f; }
-    for (uint32_t q = 0; q < nq; ++q) out_counts[q] = 0;
+static void clear_topk(uint32_t nq, const ScoreOut& o) {
+    if (!o.k) return;
+    for (uint64_t i = 0; i < (uint64_t)nq * o.k; ++i) { o.docs[i] = 0xFFFFFFFFu; o.topk[i] = 0.0f; }
+    for (uint32_t q = 0; q < nq; ++q) o.counts[q] = 0;
+}
+
+// the next buffer carved from a row arena: the first 256-byte boundary at or after p
+template <typename T>
+static T* carve(const void* p) {
+    return reinterpret_cast<T*>((reinterpret_cast<uintptr_t>(p) + 255) & ~uintptr_t(255));
+}
+
+// The batches of one score call on x's stream and workspace.  A query's rows take bytes_per_q, so a batch holds
+// max(1, min(BM_DENSE_BYTES / bytes_per_q, nq, 4096)) queries, and the row arena one batch's rows with room to align three
+// buffers carved from it.  The top-k is cleared first; an empty index scores nothing.  body(q0, qb, arena, &rows) computes
+// queries q0 .. q0 + qb and sets the rows to emit; ksel is the widest top-k a body selects itself.  ms[6] gets the device time,
+// ms[7] the wall time since t0.
+template <typename Body>
+static yams_status_t run_batches(yams_b200_bm25* x, double t0, uint32_t nq, uint64_t bytes_per_q, uint32_t ksel, const ScoreOut& o,
+                                 Body&& body) {
+    const uint64_t n = x->n;
+    const uint32_t K = (uint32_t)std::min<uint64_t>(o.k, n);
+    ksel = (uint32_t)std::min<uint64_t>(std::max(o.k, ksel), n);
+    const uint64_t qb_max = n ? std::max<uint64_t>(1, std::min<uint64_t>({BM_DENSE_BYTES / bytes_per_q, (uint64_t)nq, 4096})) : 0;
+    yams_status_t rc;
+    if (n && (rc = x->ws.rows.reserve(qb_max * bytes_per_q + 3 * 256)) != YAMS_OK) return rc;
+    if (ksel && ((rc = x->ws.sel.reserve(qb_max * ksel * sizeof(Cand))) != YAMS_OK || (rc = x->ws.seln.reserve(qb_max * 4)) != YAMS_OK))
+        return rc;
+    clear_topk(nq, o);
+    float dev_ms = 0.f;
+    if (n) {
+        std::vector<Cand> h_sel;
+        std::vector<uint32_t> h_n;
+        rc = timed(x, &dev_ms, [&]() -> yams_status_t {
+            for (uint32_t q0 = 0; q0 < nq; q0 += (uint32_t)qb_max) {
+                const uint32_t qb = (uint32_t)std::min<uint64_t>(qb_max, nq - q0);
+                const float* rows = nullptr;
+                yams_status_t r;
+                if ((r = body(q0, qb, x->ws.rows.p, &rows)) != YAMS_OK || (r = emit_batch(x, rows, q0, qb, nq, K, o, h_sel, h_n)) != YAMS_OK)
+                    return r;
+            }
+            return YAMS_OK;
+        });
+        if (rc != YAMS_OK) return rc;
+    }
+    x->ms[6] = dev_ms;
+    x->ms[7] = (float)(wall_ms() - t0);
+    return YAMS_OK;
 }
 
 // The query router's part of a score call: rows scored as Atire, and the candidate pools projected from the rows
@@ -1120,81 +1200,50 @@ struct Routed {
 // With strategy >= 0, the strategy's score_bm25f replaces Bm25Index::score (the strategy router's pools 0 and 2).  With rt, its
 // Atire rows score as Atire and its pools are gathered from each batch's rows and copied back once.
 static yams_status_t bm25_score(yams_b200_bm25* x, const yams_b200_concepts* c, float weight, const char* const* queries,
-                                const size_t* qlens, uint32_t nq, float* out_scores, uint32_t k, uint32_t* out_docs, float* out_topk,
-                                uint32_t* out_counts, int strategy = -1, const Routed* rt = nullptr) {
+                                const size_t* qlens, uint32_t nq, const ScoreOut& o, int strategy = -1, const Routed* rt = nullptr) {
     const double t0 = wall_ms();
     cudaStream_t st = x->st;
     const uint64_t n = x->n;
     yams_status_t rc;
     // ---- host: the legs of every query, in the reference's order ----
     // the blend is a no-op when the concept index is empty or of another document count (blend_into's size test)
-    const bool blend = c && c->size && c->n == n;
-    std::vector<RawLeg> raw;
-    std::vector<uint64_t> qoff(nq + 1, 0);
-    query_legs(x, blend ? c : nullptr, queries, qlens, nq, raw, qoff.data(), strategy, rt ? rt->atire : nullptr);
-    const uint64_t nlegs = raw.size();
-    const uint32_t K = std::min<uint64_t>(k, n);
-    if ((rc = x->raw.reserve(std::max<uint64_t>(nlegs, 1) * sizeof(RawLeg))) != YAMS_OK) return rc;
-    if ((rc = x->legs.reserve(std::max<uint64_t>(nlegs, 1) * sizeof(Leg))) != YAMS_OK) return rc;
-    if ((rc = x->qoff.reserve((nq + 1) * 8)) != YAMS_OK) return rc;
-    const uint64_t qb_max = n ? std::max<uint64_t>(1, std::min<uint64_t>({BM_DENSE_BYTES / (n * 4), (uint64_t)nq, 4096})) : 0;
-    if (n && (rc = x->dense.reserve(qb_max * n * 4)) != YAMS_OK) return rc;
-    if (K && (rc = x->sel.reserve(qb_max * K * sizeof(Cand))) != YAMS_OK) return rc;
-    if (K && (rc = x->seln.reserve(qb_max * 4)) != YAMS_OK) return rc;
+    const Scorer s{x, c && c->size && c->n == n ? c : nullptr, weight};
+    LegList L;
+    for (uint32_t q = 0; q < nq; ++q, L.end_query()) {
+        const uint8_t* p = reinterpret_cast<const uint8_t*>(queries[q]);
+        L.words(x, p, qlens[q], 0, rt && rt->atire[q]);
+        if (strategy >= 0) L.bm25f(x, p, qlens[q], (uint32_t)strategy);
+        if (s.c) L.concepts(s.c, p, qlens[q]);
+    }
     const uint64_t npool = rt && rt->cand_off ? rt->cand_off[nq] : 0;
     if (npool && (rc = x->pool_off.reserve((nq + 1) * 8)) != YAMS_OK) return rc;
     if (npool && (rc = x->pool_docs.reserve(npool * 4)) != YAMS_OK) return rc;
     if (npool && (rc = x->pool_out.reserve(npool * 4)) != YAMS_OK) return rc;
-    clear_topk(nq, k, out_docs, out_topk, out_counts);
-    if (n == 0) {
+    if (n == 0)
         for (uint64_t j = 0; j < npool; ++j) rt->out_cand[j] = 0.0f;   // no candidate is indexed
-        x->ms[6] = 0.f;
-        x->ms[7] = (float)(wall_ms() - t0);
-        return YAMS_OK;
-    }
-    float dev_ms = 0.f;
-    std::vector<Cand> h_sel;
-    std::vector<uint32_t> h_n;
-    rc = timed(x, &dev_ms, [&]() -> yams_status_t {
+    return run_batches(x, t0, nq, n * 4, 0, o, [&](uint32_t q0, uint32_t qb, void* arena, const float** out) -> yams_status_t {
+        float* rows = static_cast<float*>(arena);
         yams_status_t r;
-        if (npool) {
-            YB_CUDA(cudaMemcpyAsync(x->pool_off.p, rt->cand_off, (nq + 1) * 8, cudaMemcpyHostToDevice, st));
-            YB_CUDA(cudaMemcpyAsync(x->pool_docs.p, rt->cand_docs, npool * 4, cudaMemcpyHostToDevice, st));
-        }
-        if (nlegs) {
-            YB_CUDA(cudaMemcpyAsync(x->raw.p, raw.data(), nlegs * sizeof(RawLeg), cudaMemcpyHostToDevice, st));
-            if ((r = plan_legs(x, blend ? c : nullptr, weight, x->raw.as<RawLeg>(), nlegs, x->legs.as<Leg>(), st)) != YAMS_OK) return r;
-        }
-        YB_CUDA(cudaMemcpyAsync(x->qoff.p, qoff.data(), (nq + 1) * 8, cudaMemcpyHostToDevice, st));
-        ScoreArgs a = bm25_args(x);
-        a.legs = x->legs.as<Leg>();
-        a.qoff = x->qoff.as<uint64_t>();
-        if (blend) concept_field(c, a);
-        a.out = x->dense.as<float>();
-        const unsigned tiles = (unsigned)((n + BM_TILE - 1) / BM_TILE);
-        for (uint32_t q0 = 0; q0 < nq; q0 += (uint32_t)qb_max) {
-            const uint32_t qb = (uint32_t)std::min<uint64_t>(qb_max, nq - q0);
-            a.q0 = q0;
-            bm_score_kernel<<<dim3(tiles, qb), BM_THREADS, 0, st>>>(a);
-            YB_CUDA(cudaGetLastError());
-            if (npool && rt->cand_off[q0 + qb] > rt->cand_off[q0]) {
-                uint64_t longest = 0;
-                for (uint32_t j = q0; j < q0 + qb; ++j) longest = std::max(longest, rt->cand_off[j + 1] - rt->cand_off[j]);
-                const unsigned gx = (unsigned)std::min<uint64_t>((longest + BM_THREADS - 1) / BM_THREADS, 64);
-                bm_pool_gather_kernel<<<dim3(gx, qb), BM_THREADS, 0, st>>>(x->dense.as<float>(), n, q0, x->pool_off.as<uint64_t>(),
-                                                                          x->pool_docs.as<uint32_t>(), x->pool_out.as<float>());
-                YB_CUDA(cudaGetLastError());
+        if (q0 == 0) {   // the call's pools and legs, staged once
+            if (npool) {
+                YB_CUDA(cudaMemcpyAsync(x->pool_off.p, rt->cand_off, (nq + 1) * 8, cudaMemcpyHostToDevice, st));
+                YB_CUDA(cudaMemcpyAsync(x->pool_docs.p, rt->cand_docs, npool * 4, cudaMemcpyHostToDevice, st));
             }
-            if ((r = emit_batch(x, x->dense.as<float>(), n, q0, qb, nq, K, k, out_scores, out_docs, out_topk, out_counts, h_sel, h_n)) != YAMS_OK)
-                return r;
+            if ((r = stage_legs(x->ws, L, &s, 1, st)) != YAMS_OK) return r;
         }
-        if (npool) YB_CUDA(cudaMemcpyAsync(rt->out_cand, x->pool_out.p, npool * 4, cudaMemcpyDeviceToHost, st));
+        if ((r = score_rows(x->ws, L, s, n, q0, qb, false, rows, st)) != YAMS_OK) return r;
+        if (npool && rt->cand_off[q0 + qb] > rt->cand_off[q0]) {
+            uint64_t longest = 0;
+            for (uint32_t j = q0; j < q0 + qb; ++j) longest = std::max(longest, rt->cand_off[j + 1] - rt->cand_off[j]);
+            const unsigned gx = (unsigned)std::min<uint64_t>((longest + BM_THREADS - 1) / BM_THREADS, 64);
+            bm_pool_gather_kernel<<<dim3(gx, qb), BM_THREADS, 0, st>>>(rows, n, q0, x->pool_off.as<uint64_t>(), x->pool_docs.as<uint32_t>(),
+                                                                      x->pool_out.as<float>());
+            YB_CUDA(cudaGetLastError());
+        }
+        if (npool && q0 + qb == nq) YB_CUDA(cudaMemcpyAsync(rt->out_cand, x->pool_out.p, npool * 4, cudaMemcpyDeviceToHost, st));
+        *out = rows;
         return YAMS_OK;
     });
-    if (rc != YAMS_OK) return rc;
-    x->ms[6] = dev_ms;
-    x->ms[7] = (float)(wall_ms() - t0);
-    return YAMS_OK;
 }
 
 // ---- the keyphrase strategy and the entropy route (DESIGN.md §4.14) ----
@@ -1261,202 +1310,158 @@ static int route_pool(const double* prof, const float* row_dev, uint64_t n, doub
     return e < 0.05f ? 0 : e > 0.50f ? 2 : 1;
 }
 
-// raw legs [qoff[j], qoff[j + 1]) of the batch's rows j = 0 .. qb: planned and scored onto rows (init: in place; null: from 0)
-static yams_status_t run_legs(yams_b200_bm25* x, const yams_b200_concepts* c, float weight, const std::vector<RawLeg>& raw,
-                              const std::vector<uint64_t>& qoff, uint32_t qb, bool init, float* rows) {
-    cudaStream_t st = x->st;
-    yams_status_t rc;
-    const uint64_t nlegs = raw.size();
-    if (nlegs == 0) {
-        if (!init) YB_CUDA(cudaMemsetAsync(rows, 0, (uint64_t)qb * x->n * 4, st));
-        return YAMS_OK;
-    }
-    if ((rc = x->raw.reserve(nlegs * sizeof(RawLeg))) != YAMS_OK || (rc = x->legs.reserve(nlegs * sizeof(Leg))) != YAMS_OK ||
-        (rc = x->qoff.reserve((qb + 1) * 8)) != YAMS_OK)
-        return rc;
-    YB_CUDA(cudaMemcpyAsync(x->raw.p, raw.data(), nlegs * sizeof(RawLeg), cudaMemcpyHostToDevice, st));
-    YB_CUDA(cudaMemcpyAsync(x->qoff.p, qoff.data(), (qb + 1) * 8, cudaMemcpyHostToDevice, st));
-    if ((rc = plan_legs(x, c, weight, x->raw.as<RawLeg>(), nlegs, x->legs.as<Leg>(), st)) != YAMS_OK) return rc;
-    ScoreArgs a = bm25_args(x);
-    a.legs = x->legs.as<Leg>();
-    a.qoff = x->qoff.as<uint64_t>();
-    if (c) concept_field(c, a);
-    a.init = init ? rows : nullptr;
-    a.out = rows;
-    bm_score_kernel<<<dim3((unsigned)((x->n + BM_TILE - 1) / BM_TILE), qb), BM_THREADS, 0, st>>>(a);
-    YB_CUDA(cudaGetLastError());
-    YB_CUDA(cudaStreamSynchronize(st));   // raw and qoff are the caller's until here
-    return YAMS_OK;
-}
-
 // The strategy router's KEYPHRASE pool or its ROUTED choice for every query, then ConceptIndex::blend_into.  Per batch: the
 // plain score rows; with ROUTED, each row's profile and pool; the BM25F legs of rows routed to pools 0 and 2 onto their rows; for
 // rows of pool 1 the top-10 (padded with zero scores as simeon::top_k keeps them), the gate, the matches of each gated row's
 // keyphrases and the z-score; the concept legs; the outputs.
 static yams_status_t bm25_score_staged(yams_b200_bm25* x, const yams_b200_concepts* c, float weight, uint32_t strategy,
-                                       const char* const* queries, const size_t* qlens, uint32_t nq, float* out_scores, uint32_t k,
-                                       uint32_t* out_docs, float* out_topk, uint32_t* out_counts, uint32_t* out_chosen) {
+                                       const char* const* queries, const size_t* qlens, uint32_t nq, const ScoreOut& o,
+                                       uint32_t* out_chosen) {
     const double t0 = wall_ms();
     cudaStream_t st = x->st;
     const uint64_t n = x->n;
-    yams_status_t rc;
-    const bool blend = c && c->size && c->n == n;
-    const uint32_t K = std::min<uint64_t>(k, n), K10 = (uint32_t)std::min<uint64_t>(10, n);
+    const Scorer plain{x, nullptr, 0.0f}, blend{x, c && c->size && c->n == n ? c : nullptr, weight};
+    const uint32_t K10 = (uint32_t)std::min<uint64_t>(10, n);
     double margin = 0.0;   // YAMS_B200_BM25_ROUTE_MARGIN = w > 0 widens the certified interval by w, read at every call
     if (const char* e = getenv("YAMS_B200_BM25_ROUTE_MARGIN")) margin = std::max(0.0, strtod(e, nullptr));
-    // per query: its score row and its row of keyphrase matches
-    const uint64_t qb_max = n ? std::max<uint64_t>(1, std::min<uint64_t>({BM_DENSE_BYTES / (n * 8), (uint64_t)nq, 4096})) : 0;
-    x->sstats = yams_bm25_strategy_stats{};
-    clear_topk(nq, k, out_docs, out_topk, out_counts);
-    if (n == 0) {
-        if (out_chosen)
-            for (uint32_t q = 0; q < nq; ++q) out_chosen[q] = strategy == YAMS_BM25_STRATEGY_ROUTED ? 0 : strategy;
-        x->ms[6] = 0.f;
-        x->ms[7] = (float)(wall_ms() - t0);
-        return YAMS_OK;
-    }
-    if ((rc = x->dense.reserve(qb_max * n * 4)) != YAMS_OK || (rc = x->counts.reserve(qb_max * n * 4)) != YAMS_OK ||
-        (rc = x->route.reserve(qb_max * 24)) != YAMS_OK || (rc = x->zrow.reserve(qb_max * 4)) != YAMS_OK ||
-        (rc = x->zp.reserve(qb_max * 8)) != YAMS_OK || (rc = x->sel.reserve(qb_max * std::max<uint32_t>(std::max(K, K10), 1) * sizeof(Cand))) != YAMS_OK ||
-        (rc = x->seln.reserve(qb_max * 4)) != YAMS_OK)
-        return rc;
-    float dev_ms = 0.f;
+    if (n == 0 && out_chosen) std::fill(out_chosen, out_chosen + nq, strategy == YAMS_BM25_STRATEGY_ROUTED ? 0u : strategy);
+    // A batch's plain, BM25F, presence and concept legs: each list outlives its copy, and the next batch starts after emit_batch
+    // has synchronised, so the sub-passes need no synchronisation of their own.
+    LegList plain_legs, f_legs, kp_legs, concept_legs;
+    std::vector<uint64_t> kh;
+    std::vector<double> prof;
+    std::vector<uint32_t> pool, zrow;
+    std::vector<float> zp;
     std::vector<Cand> h_sel;
     std::vector<uint32_t> h_n;
-    std::vector<RawLeg> raw;
-    std::vector<uint64_t> qoff(qb_max + 1), kh, corder;
-    std::vector<double> prof;
-    std::vector<uint32_t> pool(qb_max), zrow;
-    std::vector<float> zp;
-    std::vector<std::pair<size_t, size_t>> ws;
-    WordLegs word_legs{x, {}, {}, {}};
-    uint32_t wb_bits;
-    memcpy(&wb_bits, &STRATEGY_WB, 4);
-    rc = timed(x, &dev_ms, [&]() -> yams_status_t {
+    // per query: its score row and its row of keyphrase matches
+    return run_batches(x, t0, nq, n * 8, 10, o, [&](uint32_t q0, uint32_t qb, void* arena, const float** out) -> yams_status_t {
+        float* rows = static_cast<float*>(arena);
+        float* counts = carve<float>(rows + (uint64_t)qb * n);
+        auto qp = [&](uint32_t j) { return reinterpret_cast<const uint8_t*>(queries[q0 + j]); };
         yams_status_t r;
-        float* rows = x->dense.as<float>();
-        for (uint32_t q0 = 0; q0 < nq; q0 += (uint32_t)qb_max) {
-            const uint32_t qb = (uint32_t)std::min<uint64_t>(qb_max, nq - q0);
-            auto qp = [&](uint32_t j) { return reinterpret_cast<const uint8_t*>(queries[q0 + j]); };
-            // the plain scores
-            raw.clear();
-            for (uint32_t j = 0; j < qb; ++j) { qoff[j] = raw.size(); word_legs(qp(j), qlens[q0 + j], 0, raw); }
-            qoff[qb] = raw.size();
-            if ((r = run_legs(x, nullptr, 0.0f, raw, qoff, qb, false, rows)) != YAMS_OK) return r;
-            // the pools
-            for (uint32_t j = 0; j < qb; ++j) pool[j] = strategy;
-            if (strategy == YAMS_BM25_STRATEGY_ROUTED) {
-                prof.resize((uint64_t)qb * 3);
-                bm_route_kernel<<<qb, BM_THREADS, 0, st>>>(rows, n, x->route.as<double>());
-                YB_CUDA(cudaGetLastError());
-                YB_CUDA(cudaMemcpyAsync(prof.data(), x->route.p, (uint64_t)qb * 24, cudaMemcpyDeviceToHost, st));
-                YB_CUDA(cudaStreamSynchronize(st));
-                for (uint32_t j = 0; j < qb; ++j) {
-                    bool rep = false;
-                    const int p = route_pool(prof.data() + 3 * j, rows + (uint64_t)j * n, n, margin, st, &rep);
-                    if (p < 0) { set_last_error("route replay copy failed"); return YAMS_ERR_INTERNAL; }
-                    pool[j] = (uint32_t)p;
-                    x->sstats.replayed += rep;
-                }
-            }
-            // pools 0 and 2: score_bm25f's body scale and aux legs onto the plain rows
-            raw.clear();
-            bool kp = false;
+        if ((r = x->route.reserve((uint64_t)qb * 24)) != YAMS_OK || (r = x->zrow.reserve((uint64_t)qb * 4)) != YAMS_OK ||
+            (r = x->zp.reserve((uint64_t)qb * 8)) != YAMS_OK)
+            return r;
+        // the plain scores
+        plain_legs.clear();
+        for (uint32_t j = 0; j < qb; ++j, plain_legs.end_query()) plain_legs.words(x, qp(j), qlens[q0 + j], 0);
+        if ((r = stage_legs(x->ws, plain_legs, &plain, 1, st)) != YAMS_OK ||
+            (r = score_rows(x->ws, plain_legs, plain, n, 0, qb, false, rows, st)) != YAMS_OK)
+            return r;
+        // the pools
+        pool.assign(qb, strategy);
+        if (strategy == YAMS_BM25_STRATEGY_ROUTED) {
+            prof.resize((uint64_t)qb * 3);
+            bm_route_kernel<<<qb, BM_THREADS, 0, st>>>(rows, n, x->route.as<double>());
+            YB_CUDA(cudaGetLastError());
+            YB_CUDA(cudaMemcpyAsync(prof.data(), x->route.p, (uint64_t)qb * 24, cudaMemcpyDeviceToHost, st));
+            YB_CUDA(cudaStreamSynchronize(st));
             for (uint32_t j = 0; j < qb; ++j) {
-                qoff[j] = raw.size();
-                ++x->sstats.queries[pool[j]];
-                if (pool[j] == 1) { kp = true; continue; }
-                size_t aux_len = qlens[q0 + j];
-                if (pool[j] == YAMS_BM25_STRATEGY_BM25) {
-                    aux_len = lead_cut(qp(j), qlens[q0 + j], STRATEGY_LEAD);
-                    bool empty = true;
-                    for (size_t i = 0; i < aux_len && empty; ++i) empty = is_space(qp(j)[i]);
-                    if (empty) continue;
-                }
-                raw.push_back({0, 0, BM_SCALE, wb_bits});
-                word_legs(qp(j), aux_len, BM_AUX, raw);
+                bool rep = false;
+                const int p = route_pool(prof.data() + 3 * j, rows + (uint64_t)j * n, n, margin, st, &rep);
+                if (p < 0) { set_last_error("route replay copy failed"); return YAMS_ERR_INTERNAL; }
+                pool[j] = (uint32_t)p;
+                x->sstats.replayed += rep;
             }
-            qoff[qb] = raw.size();
-            if (!raw.empty() && (r = run_legs(x, nullptr, 0.0f, raw, qoff, qb, true, rows)) != YAMS_OK) return r;
-            // pool 1: the entropy gate over the top-10 with its zeros, the matches, the z-score
-            if (kp) {
-                launch_topk_dense(rows, n, qb, K10, x->sel.as<Cand>(), x->seln.as<uint32_t>(), st);
-                YB_CUDA(cudaGetLastError());
-                h_sel.resize((uint64_t)qb * K10);
-                h_n.resize(qb);
-                YB_CUDA(cudaMemcpyAsync(h_sel.data(), x->sel.p, (uint64_t)qb * K10 * sizeof(Cand), cudaMemcpyDeviceToHost, st));
-                YB_CUDA(cudaMemcpyAsync(h_n.data(), x->seln.p, (uint64_t)qb * 4, cudaMemcpyDeviceToHost, st));
-                YB_CUDA(cudaStreamSynchronize(st));
-                raw.clear();
-                zrow.clear();
-                zp.clear();
-                for (uint32_t j = 0; j < qb; ++j) {
-                    qoff[j] = raw.size();
-                    if (pool[j] != 1) continue;
-                    // simeon::top_k(scores, 10): the positives best first, then zeros (every other score is 0)
-                    double vals[10];
-                    uint32_t m = 0;
-                    for (; m < std::min(h_n[j], K10) && h_sel[(uint64_t)j * K10 + m].score > 0.0f; ++m)
-                        vals[m] = (double)h_sel[(uint64_t)j * K10 + m].score;
-                    for (; m < K10; ++m) vals[m] = 0.0;
-                    double ent = 0.0;
-                    if (K10 >= 2) {
-                        double sum_exp = 0.0;
-                        for (uint32_t i = 0; i < K10; ++i) sum_exp += std::exp(vals[i]);
-                        for (uint32_t i = 0; i < K10; ++i) {
-                            const double pr = std::exp(vals[i]) / sum_exp;
-                            if (pr > 1e-12) ent -= pr * std::log(pr);
-                        }
-                        ent /= std::log((double)K10);
-                    }
-                    const float entropy = (float)ent;
-                    if (entropy < 0.30f) continue;
-                    keyphrase_hashes(x, qp(j), qlens[q0 + j], kh);
-                    if (kh.empty()) continue;
-                    for (uint64_t h : kh) raw.push_back({h, h, 0, BM_PRESENCE});
-                    const float lam = 1.0f / (1.0f + std::exp(-(entropy - 0.48f) * 8.0f));
-                    zrow.push_back(j);
-                    zp.push_back(lam * 0.25f);
-                    zp.push_back((float)kh.size());
-                }
-                qoff[qb] = raw.size();
-                if (!zrow.empty()) {
-                    x->sstats.keyphrase_boosted += (uint32_t)zrow.size();
-                    if ((r = run_legs(x, nullptr, 0.0f, raw, qoff, qb, false, x->counts.as<float>())) != YAMS_OK) return r;
-                    YB_CUDA(cudaMemcpyAsync(x->zrow.p, zrow.data(), zrow.size() * 4, cudaMemcpyHostToDevice, st));
-                    YB_CUDA(cudaMemcpyAsync(x->zp.p, zp.data(), zp.size() * 4, cudaMemcpyHostToDevice, st));
-                    YB_CUDA(cudaEventRecord(x->zev[0], st));
-                    bm_zscore_kernel<<<(unsigned)zrow.size(), BM_THREADS, 0, st>>>(rows, x->counts.as<float>(), n, x->zrow.as<uint32_t>(),
-                                                                                   x->zp.as<float>());
-                    YB_CUDA(cudaGetLastError());
-                    YB_CUDA(cudaEventRecord(x->zev[1], st));
-                    YB_CUDA(cudaEventSynchronize(x->zev[1]));
-                    float zms = 0.f;
-                    YB_CUDA(cudaEventElapsedTime(&zms, x->zev[0], x->zev[1]));
-                    x->sstats.zscore_ms += zms;
-                }
-            }
-            // the concept blend onto the strategies' rows
-            if (blend) {
-                raw.clear();
-                for (uint32_t j = 0; j < qb; ++j) {
-                    qoff[j] = raw.size();
-                    concept_order(c, qp(j), qlens[q0 + j], ws, corder);
-                    for (uint64_t bh : corder) raw.push_back({bh, bh, BM_CONCEPT, 0});
-                }
-                qoff[qb] = raw.size();
-                if (!raw.empty() && (r = run_legs(x, c, weight, raw, qoff, qb, true, rows)) != YAMS_OK) return r;
-            }
-            if (out_chosen)
-                for (uint32_t j = 0; j < qb; ++j) out_chosen[q0 + j] = pool[j];
-            if ((r = emit_batch(x, rows, n, q0, qb, nq, K, k, out_scores, out_docs, out_topk, out_counts, h_sel, h_n)) != YAMS_OK) return r;
         }
+        // pools 0 and 2: score_bm25f's body scale and aux legs onto the plain rows
+        f_legs.clear();
+        bool kp = false;
+        for (uint32_t j = 0; j < qb; ++j, f_legs.end_query()) {
+            ++x->sstats.queries[pool[j]];
+            if (pool[j] == YAMS_BM25_STRATEGY_KEYPHRASE) kp = true;
+            else f_legs.bm25f(x, qp(j), qlens[q0 + j], pool[j]);
+        }
+        if ((r = stage_legs(x->ws, f_legs, &plain, 1, st)) != YAMS_OK || (r = score_rows(x->ws, f_legs, plain, n, 0, qb, true, rows, st)) != YAMS_OK)
+            return r;
+        // pool 1: the entropy gate over the top-10 with its zeros, the matches, the z-score
+        if (kp) {
+            launch_topk_dense(rows, n, qb, K10, x->ws.sel.as<Cand>(), x->ws.seln.as<uint32_t>(), st);
+            YB_CUDA(cudaGetLastError());
+            h_sel.resize((uint64_t)qb * K10);
+            h_n.resize(qb);
+            YB_CUDA(cudaMemcpyAsync(h_sel.data(), x->ws.sel.p, (uint64_t)qb * K10 * sizeof(Cand), cudaMemcpyDeviceToHost, st));
+            YB_CUDA(cudaMemcpyAsync(h_n.data(), x->ws.seln.p, (uint64_t)qb * 4, cudaMemcpyDeviceToHost, st));
+            YB_CUDA(cudaStreamSynchronize(st));
+            kp_legs.clear();
+            zrow.clear();
+            zp.clear();
+            for (uint32_t j = 0; j < qb; ++j, kp_legs.end_query()) {
+                if (pool[j] != 1) continue;
+                // simeon::top_k(scores, 10): the positives best first, then zeros (every other score is 0)
+                double vals[10];
+                uint32_t m = 0;
+                for (; m < std::min(h_n[j], K10) && h_sel[(uint64_t)j * K10 + m].score > 0.0f; ++m)
+                    vals[m] = (double)h_sel[(uint64_t)j * K10 + m].score;
+                for (; m < K10; ++m) vals[m] = 0.0;
+                double ent = 0.0;
+                if (K10 >= 2) {
+                    double sum_exp = 0.0;
+                    for (uint32_t i = 0; i < K10; ++i) sum_exp += std::exp(vals[i]);
+                    for (uint32_t i = 0; i < K10; ++i) {
+                        const double pr = std::exp(vals[i]) / sum_exp;
+                        if (pr > 1e-12) ent -= pr * std::log(pr);
+                    }
+                    ent /= std::log((double)K10);
+                }
+                const float entropy = (float)ent;
+                if (entropy < 0.30f) continue;
+                keyphrase_hashes(x, qp(j), qlens[q0 + j], kh);
+                if (kh.empty()) continue;
+                kp_legs.presence(kh);
+                const float lam = 1.0f / (1.0f + std::exp(-(entropy - 0.48f) * 8.0f));
+                zrow.push_back(j);
+                zp.push_back(lam * 0.25f);
+                zp.push_back((float)kh.size());
+            }
+            if (!zrow.empty()) {
+                x->sstats.keyphrase_boosted += (uint32_t)zrow.size();
+                if ((r = stage_legs(x->ws, kp_legs, &plain, 1, st)) != YAMS_OK ||
+                    (r = score_rows(x->ws, kp_legs, plain, n, 0, qb, false, counts, st)) != YAMS_OK)
+                    return r;
+                YB_CUDA(cudaMemcpyAsync(x->zrow.p, zrow.data(), zrow.size() * 4, cudaMemcpyHostToDevice, st));
+                YB_CUDA(cudaMemcpyAsync(x->zp.p, zp.data(), zp.size() * 4, cudaMemcpyHostToDevice, st));
+                YB_CUDA(cudaEventRecord(x->zev[0], st));
+                bm_zscore_kernel<<<(unsigned)zrow.size(), BM_THREADS, 0, st>>>(rows, counts, n, x->zrow.as<uint32_t>(), x->zp.as<float>());
+                YB_CUDA(cudaGetLastError());
+                YB_CUDA(cudaEventRecord(x->zev[1], st));
+                YB_CUDA(cudaEventSynchronize(x->zev[1]));
+                float zms = 0.f;
+                YB_CUDA(cudaEventElapsedTime(&zms, x->zev[0], x->zev[1]));
+                x->sstats.zscore_ms += zms;
+            }
+        }
+        // the concept blend onto the strategies' rows
+        if (blend.c) {
+            concept_legs.clear();
+            for (uint32_t j = 0; j < qb; ++j, concept_legs.end_query()) concept_legs.concepts(blend.c, qp(j), qlens[q0 + j]);
+            if ((r = stage_legs(x->ws, concept_legs, &blend, 1, st)) != YAMS_OK ||
+                (r = score_rows(x->ws, concept_legs, blend, n, 0, qb, true, rows, st)) != YAMS_OK)
+                return r;
+        }
+        if (out_chosen) std::copy(pool.begin(), pool.end(), out_chosen + q0);
+        *out = rows;
         return YAMS_OK;
     });
-    if (rc != YAMS_OK) return rc;
-    x->ms[6] = dev_ms;
-    x->ms[7] = (float)(wall_ms() - t0);
-    x->sstats.device_ms = dev_ms;
+}
+
+// The strategy router's score call and its stats.  Pools 0 and 2 score every query in one pass: the body, the scale, the aux
+// legs and the concepts.  KEYPHRASE and ROUTED are staged per batch and count the pool of each row they score, so an empty
+// index counts none of their queries and reports no time.
+static yams_status_t bm25_score_strategy(yams_b200_bm25* x, uint32_t strategy, const yams_b200_concepts* c, float weight,
+                                         const char* const* queries, const size_t* qlens, uint32_t nq, const ScoreOut& o,
+                                         uint32_t* out_chosen) {
+    yams_status_t rc;
+    x->sstats = yams_bm25_strategy_stats{};
+    if (strategy == YAMS_BM25_STRATEGY_KEYPHRASE || strategy == YAMS_BM25_STRATEGY_ROUTED) {
+        if ((rc = bm25_score_staged(x, c, weight, strategy, queries, qlens, nq, o, out_chosen)) != YAMS_OK || x->n == 0) return rc;
+    } else {
+        if ((rc = bm25_score(x, c, weight, queries, qlens, nq, o, (int)strategy)) != YAMS_OK) return rc;
+        if (out_chosen) std::fill(out_chosen, out_chosen + nq, strategy);
+        x->sstats.queries[strategy] = nq;
+    }
+    x->sstats.device_ms = x->ms[6];
     x->sstats.wall_ms = x->ms[7];
     return YAMS_OK;
 }
@@ -1525,125 +1530,72 @@ __global__ void rrf_scatter_kernel(const uint64_t* __restrict__ keys, const uint
 // workspace.  Per batch of queries: every variant's score rows, their ranked keys, one segmented sort of the (variant, query)
 // segments, one scatter per variant in order onto zeroed fused rows, the blend's concept legs, the outputs.
 static yams_status_t bm25_score_rrf(const yams_b200_bm25* const* v, uint32_t nv, float k_rrf, const yams_b200_concepts* c, float weight,
-                                    const char* const* queries, const size_t* qlens, uint32_t nq, float* out_scores, uint32_t k,
-                                    uint32_t* out_docs, float* out_topk, uint32_t* out_counts) {
+                                    const char* const* queries, const size_t* qlens, uint32_t nq, const ScoreOut& o) {
     const double t0 = wall_ms();
     yams_b200_bm25* x = const_cast<yams_b200_bm25*>(v[0]);
     cudaStream_t st = x->st;
     const uint64_t n = x->n;
-    yams_status_t rc;
-    const bool blend = c && c->size && c->n == n;
-    // ---- host: each variant's legs, then the concepts' (offsets: nv + 1 blocks of nq + 1) ----
-    std::vector<RawLeg> raw;
-    std::vector<uint64_t> qoff((uint64_t)(nv + 1) * (nq + 1), 0);
-    for (uint32_t j = 0; j < nv; ++j) query_legs(v[j], nullptr, queries, qlens, nq, raw, qoff.data() + (uint64_t)j * (nq + 1));
-    if (blend) query_legs(nullptr, c, queries, qlens, nq, raw, qoff.data() + (uint64_t)nv * (nq + 1));
-    const uint64_t nlegs = raw.size();
-    const uint32_t K = std::min<uint64_t>(k, n);
+    // ---- host: each variant's legs of every query, then the concepts' ----
+    std::vector<Scorer> s;
+    for (uint32_t j = 0; j < nv; ++j) s.push_back({v[j], nullptr, 0.0f});
+    if (c && c->size && c->n == n) s.push_back({nullptr, c, weight});
+    LegList L;
+    for (const Scorer& b : s)
+        for (uint32_t q = 0; q < nq; ++q, L.end_query()) {
+            const uint8_t* p = reinterpret_cast<const uint8_t*>(queries[q]);
+            if (b.x) L.words(b.x, p, qlens[q], 0);
+            else L.concepts(b.c, p, qlens[q]);
+        }
     const uint64_t tiles = (n + BM_TILE - 1) / BM_TILE;
     // per query: nv score rows (4 bytes a document), at most n keys per row twice (the sort's double buffer), one fused row
-    const uint64_t per_q = n * (20ull * nv + 4);
-    const uint64_t qb_max = n ? std::max<uint64_t>(1, std::min<uint64_t>({BM_DENSE_BYTES / per_q, (uint64_t)nq, 4096})) : 0;
-    if ((rc = x->raw.reserve(std::max<uint64_t>(nlegs, 1) * sizeof(RawLeg))) != YAMS_OK) return rc;
-    if ((rc = x->legs.reserve(std::max<uint64_t>(nlegs, 1) * sizeof(Leg))) != YAMS_OK) return rc;
-    if ((rc = x->qoff.reserve(qoff.size() * 8)) != YAMS_OK) return rc;
-    if (n) {
-        if ((rc = x->dense.reserve(qb_max * nv * n * 4)) != YAMS_OK || (rc = x->fused.reserve(qb_max * n * 4)) != YAMS_OK ||
-            (rc = x->keys.reserve(qb_max * nv * n * 8)) != YAMS_OK || (rc = x->keys2.reserve(qb_max * nv * n * 8)) != YAMS_OK ||
-            (rc = x->cnt.reserve((qb_max * nv * tiles + 1) * 4)) != YAMS_OK || (rc = x->base.reserve((qb_max * nv * tiles + 1) * 4)) != YAMS_OK)
-            return rc;
-    }
-    if (K && (rc = x->sel.reserve(qb_max * K * sizeof(Cand))) != YAMS_OK) return rc;
-    if (K && (rc = x->seln.reserve(qb_max * 4)) != YAMS_OK) return rc;
-    clear_topk(nq, k, out_docs, out_topk, out_counts);
-    if (n == 0) {
-        x->ms[6] = 0.f;
-        x->ms[7] = (float)(wall_ms() - t0);
-        return YAMS_OK;
-    }
-    float dev_ms = 0.f;
-    std::vector<Cand> h_sel;
-    std::vector<uint32_t> h_n;
-    rc = timed(x, &dev_ms, [&]() -> yams_status_t {
+    return run_batches(x, t0, nq, n * (20ull * nv + 4), 0, o, [&](uint32_t q0, uint32_t qb, void* arena, const float** out) -> yams_status_t {
         yams_status_t r;
-        if (nlegs) {
-            YB_CUDA(cudaMemcpyAsync(x->raw.p, raw.data(), nlegs * sizeof(RawLeg), cudaMemcpyHostToDevice, st));
-            for (uint32_t j = 0; j <= nv; ++j) {
-                if (j == nv && !blend) break;
-                const uint64_t lb = qoff[(uint64_t)j * (nq + 1)], le = qoff[(uint64_t)j * (nq + 1) + nq];
-                if ((r = plan_legs(j < nv ? v[j] : nullptr, j < nv ? nullptr : c, weight, x->raw.as<RawLeg>() + lb, le - lb,
-                                   x->legs.as<Leg>() + lb, st)) != YAMS_OK)
-                    return r;
-            }
-        }
-        YB_CUDA(cudaMemcpyAsync(x->qoff.p, qoff.data(), qoff.size() * 8, cudaMemcpyHostToDevice, st));
-        for (uint32_t q0 = 0; q0 < nq; q0 += (uint32_t)qb_max) {
-            const uint32_t qb = (uint32_t)std::min<uint64_t>(qb_max, nq - q0);
-            const uint64_t rows = (uint64_t)nv * qb, blocks = rows * tiles;
-            // every variant's rows: variant j's queries at rows j * qb ..
-            for (uint32_t j = 0; j < nv; ++j) {
-                ScoreArgs a = bm25_args(v[j]);
-                a.legs = x->legs.as<Leg>();
-                a.qoff = x->qoff.as<uint64_t>() + (uint64_t)j * (nq + 1);
-                a.q0 = q0;
-                a.out = x->dense.as<float>() + (uint64_t)j * qb * n;
-                bm_score_kernel<<<dim3((unsigned)tiles, qb), BM_THREADS, 0, st>>>(a);
-                YB_CUDA(cudaGetLastError());
-            }
-            // the ranked keys of each row, the rows' segments, one segmented sort
-            rrf_count_kernel<<<(unsigned)blocks, BM_THREADS, 0, st>>>(x->dense.as<float>(), n, (uint32_t)tiles, x->cnt.as<uint32_t>());
-            YB_CUDA(cudaGetLastError());
-            YB_CUDA(cudaMemsetAsync(x->cnt.as<uint32_t>() + blocks, 0, 4, st));
+        const uint64_t rows = (uint64_t)nv * qb, blocks = rows * tiles;
+        if (q0 == 0 && (r = stage_legs(x->ws, L, s.data(), (uint32_t)s.size(), st)) != YAMS_OK) return r;   // the call's legs, once
+        if ((r = x->cnt.reserve((blocks + 1) * 4)) != YAMS_OK || (r = x->base.reserve((blocks + 1) * 4)) != YAMS_OK) return r;
+        float* dense = static_cast<float*>(arena);
+        uint64_t* keys = carve<uint64_t>(dense + rows * n);
+        uint64_t* keys2 = carve<uint64_t>(keys + rows * n);
+        float* fused = carve<float>(keys2 + rows * n);
+        // every variant's rows: variant j's queries at rows j * qb ..
+        for (uint32_t j = 0; j < nv; ++j)
+            if ((r = score_rows(x->ws, L, s[j], n, (uint64_t)j * nq + q0, qb, false, dense + (uint64_t)j * qb * n, st)) != YAMS_OK) return r;
+        // the ranked keys of each row, the rows' segments, one segmented sort
+        rrf_count_kernel<<<(unsigned)blocks, BM_THREADS, 0, st>>>(dense, n, (uint32_t)tiles, x->cnt.as<uint32_t>());
+        YB_CUDA(cudaGetLastError());
+        YB_CUDA(cudaMemsetAsync(x->cnt.as<uint32_t>() + blocks, 0, 4, st));
+        x->tmp.bytes = 0;
+        YB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, x->tmp.bytes, x->cnt.as<uint32_t>(), x->base.as<uint32_t>(), (int64_t)blocks + 1, st));
+        if ((r = x->tmp.grow()) != YAMS_OK) return r;
+        YB_CUDA(cub::DeviceScan::ExclusiveSum(x->tmp.buf.p, x->tmp.bytes, x->cnt.as<uint32_t>(), x->base.as<uint32_t>(), (int64_t)blocks + 1, st));
+        uint32_t items = 0;
+        YB_CUDA(cudaMemcpyAsync(&items, x->base.as<uint32_t>() + blocks, 4, cudaMemcpyDeviceToHost, st));
+        rrf_keys_kernel<<<(unsigned)blocks, BM_THREADS, 0, st>>>(dense, n, (uint32_t)tiles, x->base.as<uint32_t>(), keys);
+        YB_CUDA(cudaGetLastError());
+        YB_CUDA(cudaStreamSynchronize(st));   // items
+        const uint64_t* sorted = keys;
+        if (items) {
+            cub::DoubleBuffer<uint64_t> db(keys, keys2);
+            const auto begins = thrust::make_transform_iterator(thrust::counting_iterator<uint64_t>(0), RowStart{x->base.as<uint32_t>(), (uint32_t)tiles});
             x->tmp.bytes = 0;
-            YB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, x->tmp.bytes, x->cnt.as<uint32_t>(), x->base.as<uint32_t>(), (int64_t)blocks + 1, st));
+            YB_CUDA(cub::DeviceSegmentedSort::SortKeys(nullptr, x->tmp.bytes, db, (int64_t)items, (int64_t)rows, begins, begins + 1, st));
             if ((r = x->tmp.grow()) != YAMS_OK) return r;
-            YB_CUDA(cub::DeviceScan::ExclusiveSum(x->tmp.buf.p, x->tmp.bytes, x->cnt.as<uint32_t>(), x->base.as<uint32_t>(), (int64_t)blocks + 1, st));
-            uint32_t items = 0;
-            YB_CUDA(cudaMemcpyAsync(&items, x->base.as<uint32_t>() + blocks, 4, cudaMemcpyDeviceToHost, st));
-            rrf_keys_kernel<<<(unsigned)blocks, BM_THREADS, 0, st>>>(x->dense.as<float>(), n, (uint32_t)tiles, x->base.as<uint32_t>(),
-                                                                     x->keys.as<uint64_t>());
-            YB_CUDA(cudaGetLastError());
-            YB_CUDA(cudaStreamSynchronize(st));   // items
-            const uint64_t* sorted = x->keys.as<uint64_t>();
-            if (items) {
-                cub::DoubleBuffer<uint64_t> db(x->keys.as<uint64_t>(), x->keys2.as<uint64_t>());
-                const auto begins = thrust::make_transform_iterator(thrust::counting_iterator<uint64_t>(0), RowStart{x->base.as<uint32_t>(), (uint32_t)tiles});
-                x->tmp.bytes = 0;
-                YB_CUDA(cub::DeviceSegmentedSort::SortKeys(nullptr, x->tmp.bytes, db, (int64_t)items, (int64_t)rows, begins, begins + 1, st));
-                if ((r = x->tmp.grow()) != YAMS_OK) return r;
-                YB_CUDA(cub::DeviceSegmentedSort::SortKeys(x->tmp.buf.p, x->tmp.bytes, db, (int64_t)items, (int64_t)rows, begins, begins + 1, st));
-                sorted = db.Current();
-            }
-            // the fusion: zeros, then each variant's ranks in order
-            YB_CUDA(cudaMemsetAsync(x->fused.p, 0, (uint64_t)qb * n * 4, st));
-            const unsigned gx = (unsigned)std::min<uint64_t>((n + 4 * BM_THREADS - 1) / (4 * BM_THREADS), 64);
-            for (uint32_t j = 0; items && j < nv; ++j) {
-                rrf_scatter_kernel<<<dim3(gx, qb), BM_THREADS, 0, st>>>(sorted, x->base.as<uint32_t>(), (uint32_t)tiles, (uint64_t)j * qb,
-                                                                        k_rrf, n, x->fused.as<float>());
-                YB_CUDA(cudaGetLastError());
-            }
-            // the blend adds onto the fused rows in place (its init rows)
-            if (blend) {
-                ScoreArgs a{};
-                a.legs = x->legs.as<Leg>();
-                a.qoff = x->qoff.as<uint64_t>() + (uint64_t)nv * (nq + 1);
-                a.q0 = q0;
-                concept_field(c, a);
-                a.n = n;
-                a.init = x->fused.as<float>();
-                a.out = x->fused.as<float>();
-                bm_score_kernel<<<dim3((unsigned)tiles, qb), BM_THREADS, 0, st>>>(a);
-                YB_CUDA(cudaGetLastError());
-            }
-            if ((r = emit_batch(x, x->fused.as<float>(), n, q0, qb, nq, K, k, out_scores, out_docs, out_topk, out_counts, h_sel, h_n)) != YAMS_OK)
-                return r;
+            YB_CUDA(cub::DeviceSegmentedSort::SortKeys(x->tmp.buf.p, x->tmp.bytes, db, (int64_t)items, (int64_t)rows, begins, begins + 1, st));
+            sorted = db.Current();
         }
+        // the fusion: zeros, then each variant's ranks in order
+        YB_CUDA(cudaMemsetAsync(fused, 0, (uint64_t)qb * n * 4, st));
+        const unsigned gx = (unsigned)std::min<uint64_t>((n + 4 * BM_THREADS - 1) / (4 * BM_THREADS), 64);
+        for (uint32_t j = 0; items && j < nv; ++j) {
+            rrf_scatter_kernel<<<dim3(gx, qb), BM_THREADS, 0, st>>>(sorted, x->base.as<uint32_t>(), (uint32_t)tiles, (uint64_t)j * qb, k_rrf, n,
+                                                                    fused);
+            YB_CUDA(cudaGetLastError());
+        }
+        // the blend adds onto the fused rows in place
+        if (s.size() > nv && (r = score_rows(x->ws, L, s[nv], n, (uint64_t)nv * nq + q0, qb, true, fused, st)) != YAMS_OK) return r;
+        *out = fused;
         return YAMS_OK;
     });
-    if (rc != YAMS_OK) return rc;
-    x->ms[6] = dev_ms;
-    x->ms[7] = (float)(wall_ms() - t0);
-    return YAMS_OK;
 }
 
 // ---- concept mining (mine_concepts, concept_mining.cpp:117-258) ----
@@ -2092,9 +2044,8 @@ static uint32_t router_choose(const yams_bm25_query_features& f, const yams_bm25
 // device in one kernel, features and choose on the host, then one score call whose Bm25Atire rows score as Atire, the blend
 // and the pools' projection
 static yams_status_t bm25_score_routed(yams_b200_bm25* x, const yams_bm25_router_config& rc, const yams_b200_concepts* c, float weight,
-                                      const char* const* queries, const size_t* qlens, uint32_t nq, float* out_scores, uint32_t k,
-                                      uint32_t* out_docs, float* out_topk, uint32_t* out_counts, const uint64_t* cand_off,
-                                      const uint32_t* cand_docs, float* out_cand, uint32_t* out_recipe,
+                                      const char* const* queries, const size_t* qlens, uint32_t nq, const ScoreOut& o,
+                                      const uint64_t* cand_off, const uint32_t* cand_docs, float* out_cand, uint32_t* out_recipe,
                                       yams_bm25_query_features* out_features) {
     const double t0 = wall_ms();
     cudaStream_t st = x->st;
@@ -2134,15 +2085,25 @@ static yams_status_t bm25_score_routed(yams_b200_bm25* x, const yams_bm25_router
         if (out_recipe) out_recipe[q] = recipe;
         if (out_features) out_features[q] = f;
     }
-    if (!out_scores && k == 0 && !(cand_off && cand_off[nq])) {   // the route alone: nothing of the scores is asked for
+    if (!o.scores && o.k == 0 && !(cand_off && cand_off[nq])) {   // the route alone: nothing of the scores is asked for
         x->ms[6] = 0.f;
         x->ms[7] = (float)(wall_ms() - t0);
         return YAMS_OK;
     }
     const Routed rt{atire.data(), cand_off, cand_docs, out_cand};
-    const yams_status_t r = bm25_score(x, c, weight, queries, qlens, nq, out_scores, k, out_docs, out_topk, out_counts, -1, &rt);
+    const yams_status_t r = bm25_score(x, c, weight, queries, qlens, nq, o, -1, &rt);
     x->ms[7] = (float)(wall_ms() - t0);
     return r;
+}
+
+// the argument checks every score call makes after its handles': k, the top-k outputs and, when there are queries, the queries
+static yams_status_t check_score_args(const char* const* queries, const size_t* qlens, uint32_t nq, const ScoreOut& o) {
+    YB_ARG(o.k <= TOPK_MAX, "k must be <= 4096");
+    YB_ARG(o.k == 0 || (o.docs && o.topk && o.counts), "null top-k output");
+    if (nq == 0) return YAMS_OK;
+    YB_ARG(queries && qlens, "null argument");
+    for (uint32_t q = 0; q < nq; ++q) YB_ARG(queries[q] || qlens[q] == 0, "null query");
+    return YAMS_OK;
 }
 
 }  // namespace yb
@@ -2204,20 +2165,7 @@ yams_status_t yams_b200_bm25_build_lead(void* self, const yams_bm25_config* cfg_
 
 yams_status_t yams_b200_bm25_score(yams_b200_bm25* idx, const char* const* queries, const size_t* qlens, uint32_t nq, float* out_scores,
                                    uint32_t k, uint32_t* out_docs, float* out_topk_scores, uint32_t* out_counts) {
-    YB_TRY
-    DeviceCtx* dev = nullptr;
-    yams_status_t rc = ensure_device(&dev);
-    if (rc != YAMS_OK) return rc;
-    YB_ARG(idx, "index is null");
-    YB_ARG(k <= TOPK_MAX, "k must be <= 4096");
-    YB_ARG(k == 0 || (out_docs && out_topk_scores && out_counts), "null top-k output");
-    if (nq == 0) return YAMS_OK;
-    YB_ARG(queries && qlens, "null argument");
-    for (uint32_t q = 0; q < nq; ++q) YB_ARG(queries[q] || qlens[q] == 0, "null query");
-    YB_BIND(idx);
-    std::lock_guard<std::mutex> g(idx->mu);
-    return bm25_score(idx, nullptr, 0.0f, queries, qlens, nq, out_scores, k, out_docs, out_topk_scores, out_counts);
-    YB_CATCH
+    return yams_b200_bm25_score_blended(idx, nullptr, 0.0f, queries, qlens, nq, out_scores, k, out_docs, out_topk_scores, out_counts);
 }
 
 yams_status_t yams_b200_bm25_stats(yams_b200_bm25* idx, yams_bm25_stats* out) {
@@ -2365,14 +2313,11 @@ yams_status_t yams_b200_bm25_score_rrf(const yams_b200_bm25* const* variants, ui
             return YAMS_ERR_UNSUPPORTED;
         }
     YB_ARG(std::isfinite(k_rrf) && k_rrf >= 0.0f, "k_rrf must be finite and >= 0");
-    YB_ARG(k <= TOPK_MAX, "k must be <= 4096");
-    YB_ARG(k == 0 || (out_docs && out_topk_scores && out_counts), "null top-k output");
     YB_ARG(nv == 0 || (uint64_t)nv * variants[0]->n < (1ull << 32), "more than 2^32 - 1 ranked entries per query");
-    if (nq == 0) return YAMS_OK;
-    YB_ARG(queries && qlens, "null argument");
-    for (uint32_t q = 0; q < nq; ++q) YB_ARG(queries[q] || qlens[q] == 0, "null query");
+    const ScoreOut o{out_scores, k, out_docs, out_topk_scores, out_counts};
+    if ((rc = check_score_args(queries, qlens, nq, o)) != YAMS_OK || nq == 0) return rc;
     if (nv == 0) {   // nothing ranks a document; there is no document count, so no score row
-        clear_topk(nq, k, out_docs, out_topk_scores, out_counts);
+        clear_topk(nq, o);
         return YAMS_OK;
     }
     YB_BIND(variants[0]);
@@ -2383,7 +2328,7 @@ yams_status_t yams_b200_bm25_score_rrf(const yams_b200_bm25* const* variants, ui
     hs.erase(std::unique(hs.begin(), hs.end()), hs.end());
     std::vector<std::unique_lock<std::mutex>> locks;
     for (yams_b200_bm25* h : hs) locks.emplace_back(h->mu);
-    return bm25_score_rrf(variants, nv, k_rrf, concepts, weight, queries, qlens, nq, out_scores, k, out_docs, out_topk_scores, out_counts);
+    return bm25_score_rrf(variants, nv, k_rrf, concepts, weight, queries, qlens, nq, o);
     YB_CATCH
 }
 
@@ -2432,14 +2377,11 @@ yams_status_t yams_b200_bm25_score_blended(yams_b200_bm25* idx, const yams_b200_
     yams_status_t rc = ensure_device(&dev);
     if (rc != YAMS_OK) return rc;
     YB_ARG(idx, "index is null");
-    YB_ARG(k <= TOPK_MAX, "k must be <= 4096");
-    YB_ARG(k == 0 || (out_docs && out_topk_scores && out_counts), "null top-k output");
-    if (nq == 0) return YAMS_OK;
-    YB_ARG(queries && qlens, "null argument");
-    for (uint32_t q = 0; q < nq; ++q) YB_ARG(queries[q] || qlens[q] == 0, "null query");
+    const ScoreOut o{out_scores, k, out_docs, out_topk_scores, out_counts};
+    if ((rc = check_score_args(queries, qlens, nq, o)) != YAMS_OK || nq == 0) return rc;
     YB_BIND(idx);
     std::lock_guard<std::mutex> g(idx->mu);
-    return bm25_score(idx, concepts, weight, queries, qlens, nq, out_scores, k, out_docs, out_topk_scores, out_counts);
+    return bm25_score(idx, concepts, weight, queries, qlens, nq, o);
     YB_CATCH
 }
 
@@ -2452,26 +2394,11 @@ yams_status_t yams_b200_bm25_score_strategy(yams_b200_bm25* idx, uint32_t strate
     if (rc != YAMS_OK) return rc;
     YB_ARG(idx, "index is null");
     YB_ARG(strategy <= YAMS_BM25_STRATEGY_ROUTED, "strategy must be 0 (BM25), 1 (KEYPHRASE), 2 (LEAD_FIELD) or 3 (ROUTED)");
-    YB_ARG(k <= TOPK_MAX, "k must be <= 4096");
-    YB_ARG(k == 0 || (out_docs && out_topk_scores && out_counts), "null top-k output");
-    if (nq == 0) return YAMS_OK;
-    YB_ARG(queries && qlens, "null argument");
-    for (uint32_t q = 0; q < nq; ++q) YB_ARG(queries[q] || qlens[q] == 0, "null query");
+    const ScoreOut o{out_scores, k, out_docs, out_topk_scores, out_counts};
+    if ((rc = check_score_args(queries, qlens, nq, o)) != YAMS_OK || nq == 0) return rc;
     YB_BIND(idx);
     std::lock_guard<std::mutex> g(idx->mu);
-    if (strategy == YAMS_BM25_STRATEGY_KEYPHRASE || strategy == YAMS_BM25_STRATEGY_ROUTED)
-        return bm25_score_staged(idx, concepts, weight, strategy, queries, qlens, nq, out_scores, k, out_docs, out_topk_scores, out_counts,
-                                 out_chosen);
-    // pools 0 and 2: the body, the scale, the aux legs and the concepts in one pass
-    if ((rc = bm25_score(idx, concepts, weight, queries, qlens, nq, out_scores, k, out_docs, out_topk_scores, out_counts, (int)strategy)) != YAMS_OK)
-        return rc;
-    if (out_chosen)
-        for (uint32_t q = 0; q < nq; ++q) out_chosen[q] = strategy;
-    idx->sstats = yams_bm25_strategy_stats{};
-    idx->sstats.queries[strategy] = nq;
-    idx->sstats.device_ms = idx->ms[6];
-    idx->sstats.wall_ms = idx->ms[7];
-    return YAMS_OK;
+    return bm25_score_strategy(idx, strategy, concepts, weight, queries, qlens, nq, o, out_chosen);
     YB_CATCH
 }
 
@@ -2501,11 +2428,8 @@ yams_status_t yams_b200_bm25_score_routed(yams_b200_bm25* idx, const yams_bm25_r
     yams_status_t rc = ensure_device(&dev);
     if (rc != YAMS_OK) return rc;
     YB_ARG(idx, "index is null");
-    YB_ARG(k <= TOPK_MAX, "k must be <= 4096");
-    YB_ARG(k == 0 || (out_docs && out_topk_scores && out_counts), "null top-k output");
-    if (nq == 0) return YAMS_OK;
-    YB_ARG(queries && qlens, "null argument");
-    for (uint32_t q = 0; q < nq; ++q) YB_ARG(queries[q] || qlens[q] == 0, "null query");
+    const ScoreOut o{out_scores, k, out_docs, out_topk_scores, out_counts};
+    if ((rc = check_score_args(queries, qlens, nq, o)) != YAMS_OK || nq == 0) return rc;
     if (cand_offsets) {
         YB_ARG(cand_offsets[0] == 0, "cand_offsets[0] must be 0");
         for (uint32_t q = 0; q < nq; ++q) YB_ARG(cand_offsets[q + 1] >= cand_offsets[q], "cand_offsets must not decrease");
@@ -2517,8 +2441,8 @@ yams_status_t yams_b200_bm25_score_routed(yams_b200_bm25* idx, const yams_bm25_r
     if (rcfg) cfg = *rcfg; else yams_b200_bm25_default_router_config(&cfg);
     YB_BIND(idx);
     std::lock_guard<std::mutex> g(idx->mu);
-    return bm25_score_routed(idx, cfg, concepts, weight, queries, qlens, nq, out_scores, k, out_docs, out_topk_scores, out_counts,
-                             cand_offsets, cand_docs, out_cand_scores, out_recipe, out_features);
+    return bm25_score_routed(idx, cfg, concepts, weight, queries, qlens, nq, o, cand_offsets, cand_docs, out_cand_scores, out_recipe,
+                             out_features);
     YB_CATCH
 }
 
@@ -2540,34 +2464,20 @@ yams_status_t yams_b200_concepts_blend(yams_b200_concepts* c, const char* query,
     if (n != c->n || c->size == 0) return YAMS_OK;
     YB_BIND(c);
     std::lock_guard<std::mutex> g(c->mu);
-    std::vector<std::pair<size_t, size_t>> ws;
-    std::vector<uint64_t> order;
-    concept_order(c, reinterpret_cast<const uint8_t*>(query), qlen, ws, order);
-    if (order.empty()) return YAMS_OK;
-    std::vector<RawLeg> raw;
-    for (uint64_t bh : order) raw.push_back({bh, bh, BM_CONCEPT, 0});
-    const uint64_t nlegs = raw.size(), qoff[2] = {0, nlegs};
-    cudaStream_t st = c->st;
-    if ((rc = c->raw.reserve(nlegs * sizeof(RawLeg))) != YAMS_OK || (rc = c->legs.reserve(nlegs * sizeof(Leg))) != YAMS_OK ||
-        (rc = c->qoff.reserve(16)) != YAMS_OK || (rc = c->dense.reserve(n * 4)) != YAMS_OK)
-        return rc;
+    LegList L;
+    L.concepts(c, reinterpret_cast<const uint8_t*>(query), qlen);
+    L.end_query();
+    if (L.raw.empty()) return YAMS_OK;
+    const Scorer s{nullptr, c, weight};
+    if ((rc = c->ws.rows.reserve(n * 4)) != YAMS_OK) return rc;
+    float* row = c->ws.rows.as<float>();
     float dev_ms = 0.f;   // timed() also waits for the copy back
     return timed(c, &dev_ms, [&]() -> yams_status_t {
-        YB_CUDA(cudaMemcpyAsync(c->raw.p, raw.data(), nlegs * sizeof(RawLeg), cudaMemcpyHostToDevice, st));
-        YB_CUDA(cudaMemcpyAsync(c->qoff.p, qoff, 16, cudaMemcpyHostToDevice, st));
-        YB_CUDA(cudaMemcpyAsync(c->dense.p, inout, n * 4, cudaMemcpyHostToDevice, st));
-        bm_plan_kernel<<<bm_grid(nlegs), BM_THREADS, 0, st>>>(c->raw.as<RawLeg>(), nlegs, FieldDicts{}, nullptr, 0, 0.0f, 0.0f,
-                                                              concept_dict(c, weight), c->legs.as<Leg>());
-        ScoreArgs a{};
-        a.legs = c->legs.as<Leg>();
-        a.qoff = c->qoff.as<uint64_t>();
-        concept_field(c, a);
-        a.n = n;
-        a.init = c->dense.as<float>();   // in place: each CTA reads and writes its own tile
-        a.out = c->dense.as<float>();
-        bm_score_kernel<<<dim3((unsigned)((n + BM_TILE - 1) / BM_TILE), 1), BM_THREADS, 0, st>>>(a);
-        YB_CUDA(cudaGetLastError());
-        YB_CUDA(cudaMemcpyAsync(inout, c->dense.p, n * 4, cudaMemcpyDeviceToHost, st));
+        yams_status_t r;
+        YB_CUDA(cudaMemcpyAsync(row, inout, n * 4, cudaMemcpyHostToDevice, c->st));
+        if ((r = stage_legs(c->ws, L, &s, 1, c->st)) != YAMS_OK || (r = score_rows(c->ws, L, s, n, 0, 1, true, row, c->st)) != YAMS_OK)
+            return r;
+        YB_CUDA(cudaMemcpyAsync(inout, row, n * 4, cudaMemcpyDeviceToHost, c->st));
         return YAMS_OK;
     });
     YB_CATCH
